@@ -1,12 +1,12 @@
 #!/usr/bin/env python
 """Headline benchmark: NSF-NPE training samples/s (+ posterior log_prob evals/s) on the
 linear-Gaussian workload of BASELINE.json configs[1]:
-    posterior_nn("nsf"), dim 10, 100 000 sims, training batch 4096, fp32, 1..8 x B200.
+    posterior_nn("nsf"), dim 10, 100 000 sims, training batch 4096, fp32, 1..8 x H100.
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--impl b200|reference]
-                    [--workload cfg2|cfg3|cfg4|cfg5]
+                    [--workload cfg2|cfg3|cfg4|cfg5] [--dump-outputs DIR]
 
-Default workload (cfg2, the line the driver records).  A "step" is one optimisation step (fused
+Default workload (cfg2, the headline line).  A "step" is one optimisation step (fused
 forward+backward kernel -> partial-gradient reduce -> [gradient sum over the ranks] -> clip+Adam
 kernel) on one batch of 4096 rows per GPU gathered from the HBM-resident simulation set.
 * `value`  = rows of all ranks / device time (CUDA events, max over ranks), weak scaling
@@ -18,11 +18,14 @@ kernel) on one batch of 4096 rows per GPU gathered from the HBM-resident simulat
   through `sbi_b200.inference.NPE.train()` (validation included);
 * `secondary` = posterior log_prob evals/s at one x_o, with its own CPU baseline.
 `--impl reference` times the reference's own CPU training loop on the same workload: the UNMODIFIED
-reference package (baseline/_ref or /root/reference, imported through oracle.ref_shim; its nflows
+reference package (oracle/_ref, imported through oracle.ref_shim; its nflows
 dependency is the oracle's port) when present, else the oracle port of that loop.
 `--workload cfg3|cfg4|cfg5` print one line each for the other BASELINE configs (slice-sampling
 potential evals/s, FMPE training samples/s, rejection proposals/s); they are secondary measurements
 kept under profiles/.
+`--dump-outputs DIR` (cfg2) writes what the last timed training step left behind -- the updated flat
+parameters, their gradient and that step's loss accumulator -- as DIR/<name>.npy (float32), so that two builds
+can be compared output for output on the same seeded inputs.
 """
 from __future__ import annotations
 
@@ -32,6 +35,7 @@ import json
 import math
 import os
 import sys
+import tempfile
 import threading
 import time
 
@@ -202,21 +206,28 @@ def cpu_reference_train(steps, warmup, threads):
     epochs = warm_ep + max(1, math.ceil(steps / spe))
     prior = MultivariateNormal(torch.zeros(DIM), 0.1 * torch.eye(DIM))
     torch.manual_seed(0)
-    with warnings.catch_warnings():
+    # the reference trainer writes TensorBoard logs under ./sbi-logs: run it from a temporary directory
+    # so that the benchmark writes nothing into the (possibly read-only) tree
+    cwd = os.getcwd()
+    with warnings.catch_warnings(), tempfile.TemporaryDirectory(prefix="sbi_bench_") as tmp:
         warnings.simplefilter("ignore")
-        inf = NPE(prior, density_estimator=posterior_nn("nsf"), device="cpu", show_progress_bars=False)
-        t_train = []
-        orig = inf._train_epoch
+        os.chdir(tmp)
+        try:
+            inf = NPE(prior, density_estimator=posterior_nn("nsf"), device="cpu", show_progress_bars=False)
+            t_train = []
+            orig = inf._train_epoch
 
-        def timed(*a, **k):
-            t0 = time.perf_counter()
-            out = orig(*a, **k)
-            t_train.append(time.perf_counter() - t0)
-            return out
+            def timed(*a, **k):
+                t0 = time.perf_counter()
+                out = orig(*a, **k)
+                t_train.append(time.perf_counter() - t0)
+                return out
 
-        inf._train_epoch = timed
-        inf.append_simulations(theta, x).train(training_batch_size=BATCH, max_num_epochs=epochs - 1,
-                                               stop_after_epochs=10 ** 6)
+            inf._train_epoch = timed
+            inf.append_simulations(theta, x).train(training_batch_size=BATCH, max_num_epochs=epochs - 1,
+                                                   stop_after_epochs=10 ** 6)
+        finally:
+            os.chdir(cwd)
     dur = inf._summary["epoch_durations_sec"]
     e = len(dur) - warm_ep
     step_s = sum(t_train[warm_ep:]) / (e * spe)
@@ -421,6 +432,8 @@ class StepRunner:
         cx.barrier()
         for i in range(K):
             flush.zero_()
+            if i == K - 1:
+                self.loss_acc.zero_()      # the loss accumulator then holds the last step's loss alone
             ev[i][0].record()
             if self.graphs is not None:
                 self.graphs[i % len(self.graphs)].replay()
@@ -449,7 +462,7 @@ def run_cfg2(args):
     P = lay.n_params
     theta_d, x_d = theta.to(dev), x.to(dev)
     B = BATCH
-    flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)   # > 126 MB L2
+    flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)   # > 50 MB L2
     # N > 1: the flat gradients are summed over NVLink peer memory by our own kernel (csrc/peer.cu);
     # SBI_B200_NCCL=1 keeps the NCCL all-reduce instead (no CUDA graph then)
     peer = None
@@ -462,6 +475,8 @@ def run_cfg2(args):
     run = StepRunner(cx, est, theta_d, x_d, n_train, B, peer)
     run.prepare(W)
     ms_steps = run.timed(K, flush)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, params=est.flat.data, grad=run.grad, loss_acc=run.loss_acc)
     ms_step = cx.max_over_ranks(sum(ms_steps) / K)
     train_sps = world * B / (ms_step * 1e-3)
     n_launch = K * run.launches_per_step
@@ -693,7 +708,7 @@ def run_cfg2(args):
                          "peak_source": peaks["source"],
                          "alg_bytes_per_launch": alg_bytes, "kernel_ms": vjp_ms,
                          "compute": {"achieved_tflops": flops / (vjp_ms * 1e-3) / 1e12,
-                                     "fp32_fma_nominal_tflops": 74.5,
+                                     "fp32_fma_nominal_tflops": 67.0,
                                      "tf32_tensor_peak_tflops": peaks["bf16_tflops"] / 2.0,
                                      "note": "the fused kernel is compute/latency bound (SURVEY 8d): algorithmic "
                                              "flops = 2 x 3 x conditioner MACs per row (fwd + dX + dW)"}},
@@ -710,10 +725,18 @@ def run_cfg2(args):
     cx.finish()
 
 
+def dump_outputs(out_dir, **arrays):
+    """Write each array as out_dir/<name>.npy in float32."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    for name, t in arrays.items():
+        np.save(os.path.join(out_dir, name + ".npy"), t.detach().float().cpu().numpy())
+
+
 def _vjp_kernel_info(est=None, B=BATCH):
     """Which VJP kernels the library dispatches to at B rows (names for the roofline entry)."""
     if est is not None and est._vjp_uses_tc(B, True):
-        return {"kernel": "nsf_logprob_tc_kernel<50,10,false,SAVE> + nsf_vjp_tc_kernel<50,10> (tcgen05 forward + "
+        return {"kernel": "nsf_logprob_tc_kernel<50,10,false,SAVE> + nsf_vjp_tc_kernel<50,10> (wgmma forward + "
                           "backward pair; operand re-pack included in the timing)",
                 "traffic_key": "nsf_vjp_tc", "tc": True}
     return {"kernel": "nsf_vjp_kernel<32,2,2,true>", "traffic_key": "nsf_vjp_kernel", "tc": False}
@@ -763,9 +786,9 @@ def _peaks():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         d = json.load(open(p))
-        return {"hbm_gbs": d["hbm_gbs"], "bf16_tflops": d.get("bf16_tflops", 1590.0),
+        return {"hbm_gbs": d["hbm_gbs"], "bf16_tflops": d.get("bf16_tflops", 989.0),
                 "source": "MEASURED_PEAKS.json (measured)"}
-    return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "source": "fallback (B200_PROFILING.md)"}
+    return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0, "source": "H100 SXM data sheet (dense, 700 W), not measured"}
 
 
 # ------------------------------------------------------------------------------------ other BASELINE configs
@@ -793,8 +816,10 @@ def run_cfg4(args):
     inf = FMPE(prior, device=cx.dev)
     if cx.world > 1:
         inf.data_parallel("global")
-    epochs = max(3, args.steps // 54)
-    inf.append_simulations(theta, x).train(training_batch_size=B, max_num_epochs=epochs - 1, stop_after_epochs=10 ** 6)
+    # the trainer runs whole epochs of 54 steps: --steps is rounded up to whole epochs (the first, untimed
+    # epoch comes on top)
+    epochs = max(1, math.ceil(args.steps / 54))
+    inf.append_simulations(theta, x).train(training_batch_size=B, max_num_epochs=epochs, stop_after_epochs=10 ** 6)
     dur = inf.summary["epoch_durations_sec"][1:]
     sec = cx.max_over_ranks(sum(dur))
     n_train = int(0.9 * N)
@@ -871,7 +896,7 @@ def run_cfg5(args):
     est = inf._neural_net
     pot, _ = ratio_estimator_based_potential(est, prior, x_o=x[:1])
     from sbi_b200.posteriors import prior_to_device
-    prior_d = prior_to_device(prior, cx.dev)      # log_prob as one matmul (torch's triangular solve: 5.4 s per 1M rows)
+    prior_d = prior_to_device(prior, cx.dev)      # log_prob as one matmul instead of torch's triangular solve
     chol = math.sqrt(0.1)
     NP = 1_000_000
 
@@ -886,7 +911,7 @@ def run_cfg5(args):
     if cx.world > 1:
         cx.dist.broadcast(t, 0)
     log_bound = float(t.item())
-    K = max(5, min(args.steps, 20))
+    K = max(1, args.steps)
     times, n_acc = [], None
     for i in range(3 + K):
         cx.barrier()
@@ -982,7 +1007,11 @@ def main():
     ap.add_argument("--workload", default="cfg2", choices=["cfg2", "cfg3", "cfg4", "cfg5"])
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-trainer", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the last timed step's outputs as DIR/<name>.npy (cfg2)")
     args = ap.parse_args()
+    if args.dump_outputs and (args.impl != "b200" or args.workload != "cfg2"):
+        ap.error("--dump-outputs is implemented for the default workload (cfg2) of --impl b200")
     if args.impl == "reference":
         run_reference(args)
     else:

@@ -1,7 +1,7 @@
-/* sbi_b200 -- C ABI of the B200-native hot path of sbi (density-estimator training and
+/* sbi_b200 -- C ABI of the H100-native hot path of sbi (density-estimator training and
  * posterior evaluation).  Plain pointers and sizes only; no torch types.
  *
- * Every pointer named d_* is a DEVICE pointer (sm_100a), every h_* a HOST pointer.
+ * Every pointer named d_* is a DEVICE pointer (sm_90a), every h_* a HOST pointer.
  * `stream` is a cudaStream_t passed as void* (NULL = legacy default stream).
  * All functions return 0 on success, a negative SBI_E* code on argument errors, or a
  * positive cudaError_t value if a CUDA call failed.  Nothing here synchronises unless the
@@ -29,7 +29,7 @@ extern "C" {
 
 #define SBI_EINVAL (-1)   /* bad argument */
 #define SBI_ESMEM (-2)    /* model does not fit the shared-memory budget of one CTA */
-#define SBI_ENOGPU (-3)   /* no sm_100 device */
+#define SBI_ENOGPU (-3)   /* no sm_90 device */
 
 /* per-layer descriptor table: SBI_NSF_LAYER_STRIDE ints per coupling layer */
 #define SBI_NSF_LAYER_STRIDE 64
@@ -94,7 +94,7 @@ typedef struct {
 } sbi_rows;
 
 int sbi_b200_abi_version(void);
-int sbi_b200_device_ok(void);      /* 1 if device 0 is sm_100, else 0 */
+int sbi_b200_device_ok(void);      /* 1 if device 0 is sm_90, else 0 */
 
 /* log q(input | cond) for R rows.  d_logp (R,) ; d_noise (R, D) optional (the base-space
  * point z, i.e. NFlowsFlow.inverse_transform). */

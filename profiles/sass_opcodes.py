@@ -1,10 +1,10 @@
-"""SASS opcode summary per kernel of the shipped library (evidence that the tcgen05 / TMEM / TMA-bulk
+"""SASS opcode summary per kernel of the shipped library (evidence that the wgmma / TMA-bulk
 instructions are where DESIGN.md says they are):  python profiles/sass_opcodes.py > profiles/r02_sass_opcodes.md"""
 import collections, os, re, subprocess, sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 lib = os.path.join(ROOT, "sbi_b200", "lib", "libsbi_b200.so")
 out = subprocess.run(["cuobjdump", "-sass", lib], capture_output=True, text=True).stdout
-WANT = ["UTCHMMA", "UTCBAR", "LDTM", "STTM", "UBLKCP", "UBLKRED", "SYNCS", "FFMA", "MUFU", "LDS", "STS", "LDG", "STG",
+WANT = ["HGMMA", "UBLKCP", "UBLKRED", "SYNCS", "FFMA", "MUFU", "LDS", "STS", "LDG", "STG",
         "LDL", "STL", "BAR"]
 fn, cnt, tot = None, collections.OrderedDict(), {}
 for line in out.splitlines():
@@ -21,8 +21,8 @@ for line in out.splitlines():
         if op in WANT:
             cnt[fn][op] += 1
 dem = subprocess.run(["cu++filt"] + list(cnt), capture_output=True, text=True).stdout.splitlines()
-print("# SASS opcode counts per kernel (`cuobjdump -sass sbi_b200/lib/libsbi_b200.so`, sm_100a)\n")
-print("UTCHMMA = tcgen05.mma, LDTM / STTM = tcgen05.ld / st (TMEM), UBLKCP = cp.async.bulk (TMA bulk copy), "
+print("# SASS opcode counts per kernel (`cuobjdump -sass sbi_b200/lib/libsbi_b200.so`, sm_90a)\n")
+print("HGMMA = wgmma.mma_async, UBLKCP = cp.async.bulk (TMA bulk copy), "
       "UBLKRED = cp.reduce.async.bulk, SYNCS = mbarrier ops, LDL / STL = local-memory (spill) traffic.\n")
 print("| kernel | SASS instr | " + " | ".join(WANT) + " |")
 print("|---|---|" + "---|" * len(WANT))

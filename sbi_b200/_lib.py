@@ -1,6 +1,6 @@
 """ctypes binding of the C-ABI library (include/sbi_b200.h).
 
-The product path has NO CPU fallback: if the shared library is missing or no sm_100 device
+The product path has NO CPU fallback: if the shared library is missing or no sm_90 device
 is present, calls raise.  PyTorch is used only for device memory and streams; kernels are
 launched through the C ABI with raw device pointers on torch's current CUDA stream.
 """
@@ -301,7 +301,7 @@ def require_cuda(t: torch.Tensor, name: str):
     global _active_device
     if not t.is_cuda:
         raise RuntimeError(
-            f"sbi_b200: `{name}` lives on {t.device}; the kernels only run on a CUDA (sm_100a) "
+            f"sbi_b200: `{name}` lives on {t.device}; the kernels only run on a CUDA (sm_90a) "
             "device and there is no CPU fallback")
     _active_device = t.device
     return t

@@ -62,7 +62,7 @@ def hop_device():
     if not torch.cuda.is_available():
         raise RuntimeError(
             "sbi_b200: the estimator's parameters are on the CPU and no CUDA device is available; "
-            "the kernels only run on a CUDA (sm_100a) device and there is no CPU fallback")
+            "the kernels only run on a CUDA (sm_90a) device and there is no CPU fallback")
     return torch.device("cuda", torch.cuda.current_device())
 
 

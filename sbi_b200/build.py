@@ -1,7 +1,8 @@
-"""Build the C-ABI CUDA library in-tree: sbi_b200/lib/libsbi_b200.so (sm_100a only).
+"""Build the C-ABI CUDA library in-tree: sbi_b200/lib/libsbi_b200.so (sm_90a, H100).
 
-nvcc cross-compiles without a GPU; the .so is git-ignored but travels to the GPU box.
+nvcc cross-compiles without a GPU; everything under sbi_b200/lib/ is a git-ignored build product.
 """
+import concurrent.futures
 import hashlib
 import os
 import shutil
@@ -15,7 +16,7 @@ LIB = os.path.join(LIBDIR, "libsbi_b200.so")
 INCLUDE = os.path.join(os.path.dirname(HERE), "include")
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-lineinfo", "-O3", "-std=c++17",
     "-Xcompiler", "-fPIC",
     "--expt-relaxed-constexpr",
@@ -60,7 +61,7 @@ def build_variant(name, defines):
             sys.stderr.write(r.stdout + r.stderr)
             raise RuntimeError(f"nvcc failed on {src}")
         objs.append(obj)
-    subprocess.check_call([_nvcc(), "-shared", "-o", out, *objs, "-gencode", "arch=compute_100a,code=sm_100a"])
+    subprocess.check_call([_nvcc(), "-shared", "-o", out, *objs, "-gencode", "arch=compute_90a,code=sm_90a"])
     return out
 
 
@@ -71,18 +72,21 @@ def build(force=False, verbose=False):
     if not force and os.path.exists(LIB) and os.path.exists(stamp):
         if open(stamp).read().strip() == fp:
             return LIB
-    objs = []
-    log = []
-    for src in sources():
+    def compile_one(src):
         obj = os.path.join(LIBDIR, os.path.basename(src)[:-3] + ".o")
         cmd = [_nvcc(), *NVCC_FLAGS, "-I", INCLUDE, "-c", src, "-o", obj]
-        r = subprocess.run(cmd, capture_output=True, text=True)
-        log.append(r.stderr)
-        if r.returncode != 0:
-            sys.stderr.write(r.stdout + r.stderr)
-            raise RuntimeError(f"nvcc failed on {src}")
-        objs.append(obj)
-    cmd = [_nvcc(), "-shared", "-o", LIB, *objs, "-gencode", "arch=compute_100a,code=sm_100a"]
+        return src, obj, subprocess.run(cmd, capture_output=True, text=True)
+
+    objs = []
+    log = []
+    with concurrent.futures.ThreadPoolExecutor(max_workers=min(8, os.cpu_count() or 1)) as pool:
+        for src, obj, r in pool.map(compile_one, sources()):
+            log.append(r.stderr)
+            if r.returncode != 0:
+                sys.stderr.write(r.stdout + r.stderr)
+                raise RuntimeError(f"nvcc failed on {src}")
+            objs.append(obj)
+    cmd = [_nvcc(), "-shared", "-o", LIB, *objs, "-gencode", "arch=compute_90a,code=sm_90a"]
     r = subprocess.run(cmd, capture_output=True, text=True)
     if r.returncode != 0:
         sys.stderr.write(r.stdout + r.stderr)

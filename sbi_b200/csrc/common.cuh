@@ -1,4 +1,4 @@
-// Shared device helpers for the sbi_b200 kernels (sm_100a).
+// Shared device helpers for the sbi_b200 kernels (sm_90a).
 //
 //  * mbarrier + cp.async.bulk (TMA bulk copy, SASS UBLKCP) wrappers used by the
 //    warp-specialised weight pipeline: one producer warp streams weight chunks from

@@ -39,7 +39,7 @@ inline int dev_num_sms() {
   const int d = cur_dev();
   if (n[d] == 0) {
     cudaDeviceProp p;
-    n[d] = (cudaGetDeviceProperties(&p, d) == cudaSuccess) ? p.multiProcessorCount : 148;
+    n[d] = (cudaGetDeviceProperties(&p, d) == cudaSuccess) ? p.multiProcessorCount : 132;
   }
   return n[d];
 }

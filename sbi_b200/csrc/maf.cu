@@ -586,7 +586,7 @@ extern "C" int sbi_b200_maf_logprob(const sbi_maf_model* m, const sbi_rows* rows
   if (rc) return rc;
   if (!rows || !rows->d_input || !rows->d_cond || rows->R < 0 || !d_logp) return SBI_EINVAL;
   if (rows->R == 0) return 0;
-  if (rows->R >= (int64_t)64 * 148 * 2)
+  if (rows->R >= (int64_t)64 * sbi::dev_num_sms() * 2)
     return maf_launch_rows<0, 64, 4>(maf_logprob_kernel<64, 4>, m, rows, d_logp, d_noise, (cudaStream_t)stream);
   return maf_launch_rows<1, 32, 2>(maf_logprob_kernel<32, 2>, m, rows, d_logp, d_noise, (cudaStream_t)stream);
 }
@@ -598,7 +598,7 @@ extern "C" int sbi_b200_maf_inverse(const sbi_maf_model* m, const sbi_rows* rows
   if (rc) return rc;
   if (!rows || !rows->d_input || !rows->d_cond || rows->R < 0 || !d_out) return SBI_EINVAL;
   if (rows->R == 0) return 0;
-  if (rows->R >= (int64_t)64 * 148 * 2)
+  if (rows->R >= (int64_t)64 * sbi::dev_num_sms() * 2)
     return maf_launch_rows<2, 64, 4>(maf_inverse_kernel<64, 4>, m, rows, d_out, d_logabsdet, (cudaStream_t)stream);
   return maf_launch_rows<3, 32, 2>(maf_inverse_kernel<32, 2>, m, rows, d_out, d_logabsdet, (cudaStream_t)stream);
 }

@@ -663,10 +663,10 @@ extern "C" int sbi_b200_device_ok(void) {
   if (cudaGetDeviceCount(&n) != cudaSuccess || n < 1) return 0;
   cudaDeviceProp p;
   if (cudaGetDeviceProperties(&p, 0) != cudaSuccess) return 0;
-  return p.major == 10 ? 1 : 0;
+  return (p.major == 9 && p.minor == 0) ? 1 : 0;
 }
 
-static bool use_big_tile(int64_t R) { return R >= (int64_t)64 * 148 * 2; }
+static bool use_big_tile(int64_t R) { return R >= (int64_t)64 * sbi::dev_num_sms() * 2; }
 
 extern "C" int sbi_b200_nsf_logprob(const sbi_nsf_model* m, const sbi_rows* rows, float* d_logp,
                                     float* d_noise, void* stream) {

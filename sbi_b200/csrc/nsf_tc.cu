@@ -4,28 +4,26 @@
 //
 // Same function, same parameter buffer and same evaluation order outside the linears as
 // nsf_logprob_kernel (nsf.cu); the ResidualNet linears (nflows ResidualNet, restated in
-// oracle/nflows_port/nn/nets/resnet.py; built at flow.py:411-419) run on the 5th-generation
-// tensor cores:
+// oracle/nflows_port/nn/nets/resnet.py; built at flow.py:411-419) run on the tensor cores:
 //
-//   * one CTA = 8 warps (128 rows = 128 TMEM lanes, two threads per row splitting the columns
-//     of every epilogue), two CTAs per SM (256 TMEM columns each); the warps take turns issuing
-//     the MMAs of a stage (whole warp converged, one elected lane) and the TMA copies of the
-//     weight stages (tc_common.cuh);
-//   * tcgen05.mma kind::tf32, M = 128; A (activations) is read from TMEM,
-//     where the row threads put it with tcgen05.st after splitting every fp32 value into
-//     hi = tf32(x) and lo = x - hi; B (weights, pre-split hi/lo and pre-arranged in the K-major
-//     no-swizzle UMMA layout by tc_pack_kernel) is streamed by TMA bulk copies into a
-//     shared-memory ring; D = A_hi B_hi + A_lo B_hi + A_hi B_lo (3xTF32) accumulates in TMEM in
-//     fp32 and comes back with tcgen05.ld for the bias / relu / GLU / spline epilogues;
+//   * one CTA = 8 warps (128 rows = 128 lanes of the accumulator store, two threads per row
+//     splitting the columns of every epilogue), two CTAs per SM (256 store columns each); the
+//     warps take turns issuing the TMA copies of the weight stages (tc_common.cuh);
+//   * wgmma.mma_async kind tf32, both warpgroups together (64 rows each), synchronously: the row
+//     threads put A (activations) into the accumulator store (tc_common.cuh) after splitting every
+//     fp32 value into hi = tf32(x) and lo = x - hi, the warpgroups load their A fragments from it;
+//     B (weights, pre-split hi/lo and pre-arranged in the K-major no-swizzle layout by
+//     tc_pack_kernel) is streamed by TMA bulk copies into a shared-memory ring;
+//     D = A_hi B_hi + A_lo B_hi + A_hi B_lo (3xTF32) accumulates in fp32 registers and goes back
+//     to the store for the bias / relu / GLU / spline epilogues;
 //   * the context is a K-extension of the hidden operand: A columns are
 //     [ hidden (H) | context (C) | 0 ], so the GLU gate W_c ctx is one more small MMA on the
 //     same operand and the context never has to be re-staged;
 //   * spline, LU (register-resident row against zero-padded 16x16 factors) and base density are
-//     per-thread code on the thread's own row; the gate's sigmoid is evaluated while W_1 relu(h)
-//     is on the tensor core and the spline of final-layer pass p while pass p+1 is computed;
+//     per-thread code on the thread's own row;
 //   * the same kernel template runs the sampling direction (layers T-1..0, LU^-1, inverse spline).
 //
-// TMEM columns of a CTA:  [0,64) A_hi | [64,128) A_lo | [128,192) D | [192,256) G (GLU gate);
+// Store columns of a CTA:  [0,64) A_hi | [64,128) A_lo | [128,192) D | [192,256) G (GLU gate);
 // the final layer's spline parameters P (32 columns per feature, 2 features per pass)
 // alternate between D and G.
 #include <cuda_runtime.h>
@@ -70,10 +68,9 @@ __host__ __device__ inline TcSmem tc_smem_layout(const sbi_nsf_model& m, int sta
 //
 // Per coupling layer the tensor core sees these stages (accumulator barrier in brackets):
 //   initial layer -> D [0]
-//   per block:  W_c ctx -> G [1],  W_1 relu(h) -> D [0]   (issued together: the gate's sigmoid is
-//               evaluated while W_1 runs),  W_2 relu(.) -> D [0]
-//   final layer in passes of <= 2 spline features, pass p -> P_(p&1) [p&1]; two passes are in
-//               flight, so the spline of pass p runs while pass p+1 is computed.
+//   per block:  W_c ctx -> G [1],  W_1 relu(h) -> D [0],  W_2 relu(.) -> D [0]
+//   final layer in passes of <= 2 spline features, pass p -> P_(p&1) [p&1] (two result regions, so
+//               pass p + 1 may be computed before the spline of pass p has read its parameters).
 //
 // INV = false: log_prob (logp (R,), optional base-space point `noise` (R,D)).
 // INV = true : sampling direction x = T^{-1}(noise | cond): rows.d_input holds the noise, the
@@ -88,7 +85,7 @@ template <int H, int KB, bool INV, bool SAVE = false>
 __global__ void __launch_bounds__(kThreads, 2)
 nsf_logprob_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_constant__ sbi_nsf_tc tc,
                       const __grid_constant__ sbi_rows rows, float* __restrict__ logp,
-                      float* __restrict__ noise, float* __restrict__ save) {
+                      float* __restrict__ noise, float* __restrict__ save, const StoreArgs sa) {
   constexpr int HP8 = (H + 7) & ~7;
   constexpr int NCH = HP8 / 8;      // K-steps / 8-column chunks of the hidden operand
   constexpr int KC0 = H / 8;        // first chunk that holds context columns
@@ -114,11 +111,7 @@ nsf_logprob_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_cons
     fence_barrier_init();
   }
   if (warp == 0) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(
-                     smem_u32(tbase_s)),
-                 "r"(kCols)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
+    store_alloc(tbase_s, kCols, sa);
   }
   fence_before();
   __syncthreads();
@@ -131,7 +124,7 @@ nsf_logprob_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_cons
   float* lds = sm + L.lds;
   const float* bias_s = sm + L.bias;
   const int half = warp >> 2;                          // which column half of the row
-  const int row = ((warp & 3) << 5) | (tid & 31);      // row of the tile = TMEM lane
+  const int row = ((warp & 3) << 5) | (tid & 31);      // row of the tile = store lane
   const uint32_t tlane = tbase + ((uint32_t)((warp & 3) * 32) << 16);
   const int cbase = half * NC;                          // first hidden column of this thread
   const uint32_t tmine = tlane + cbase;
@@ -190,7 +183,7 @@ nsf_logprob_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_cons
     ld_const = INV ? (-tot - m.ld_zscore) : (tot + m.ld_zscore - 0.5f * (float)D * 1.8378770664093453f);
   }
 
-  // operands written / accumulators read: hand TMEM over to the issuing thread
+  // operands written / accumulators read: hand the store over to the MMAs
   auto hand_over = [&]() {
     wait_st();
     fence_before();
@@ -600,8 +593,25 @@ nsf_logprob_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_cons
   fence_before();
   group_sync();
   if (warp == 0)
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tbase), "r"(kCols)
-                 : "memory");
+    store_dealloc(tbase, kCols, sa);
+}
+
+// the accumulator store of every tensor-core kernel of the library (tc_common.cuh)
+static __device__ float g_store[kStoreSlots][kStoreCols * kStoreLanes];
+static __device__ unsigned int g_store_mask[kStoreSlots];
+
+int store_args(StoreArgs* out) {
+  static StoreArgs cache[kMaxDev];
+  static bool ready[kMaxDev] = {false};
+  const int d = cur_dev();
+  if (!ready[d]) {
+    cudaError_t e = cudaGetSymbolAddress(reinterpret_cast<void**>(&cache[d].slab), g_store);
+    if (e == cudaSuccess) e = cudaGetSymbolAddress(reinterpret_cast<void**>(&cache[d].mask), g_store_mask);
+    if (e != cudaSuccess) return (int)e;
+    ready[d] = true;
+  }
+  *out = cache[d];
+  return 0;
 }
 
 }  // namespace tc
@@ -651,6 +661,8 @@ extern "C" int sbi_b200_nsf_logprob_tc(const sbi_nsf_model* m, const sbi_nsf_tc*
   if (!sbi_b200_nsf_tc_supported(m, tc)) return SBI_ESMEM;
   if (rows->R == 0) return 0;
   const int nslot = tc_plan_slots(m, tc);
+  tc::StoreArgs sa;
+  if (int e = tc::store_args(&sa)) return e;
   const tc::TcSmem L = tc::tc_smem_layout(*m, tc->stage_cap, nslot);
   auto k = tc::nsf_logprob_tc_kernel<50, 10, false>;
   static int smem_set_[sbi::kMaxDev] = {0};
@@ -662,13 +674,15 @@ extern "C" int sbi_b200_nsf_logprob_tc(const sbi_nsf_model* m, const sbi_nsf_tc*
   }
   const int64_t ntiles = (rows->R + tc::kRows - 1) / tc::kRows;
   const int grid = (int)std::min<int64_t>(ntiles, (int64_t)tc_num_sms() * 2);
-  k<<<grid, tc::kThreads, L.total_bytes, (cudaStream_t)stream>>>(*m, *tc, *rows, d_logp, d_noise, nullptr);
+  k<<<grid, tc::kThreads, L.total_bytes, (cudaStream_t)stream>>>(*m, *tc, *rows, d_logp, d_noise, nullptr, sa);
   return (int)cudaGetLastError();
 }
 
 int sbi::tc::launch_forward_save(const sbi_nsf_model* m, const sbi_nsf_tc* tc, const sbi_rows* rows, float* d_logp,
                                  float* d_save, cudaStream_t s) {
   const int nslot = tc_plan_slots(m, tc);
+  tc::StoreArgs sa;
+  if (int e = tc::store_args(&sa)) return e;
   const tc::TcSmem L = tc::tc_smem_layout(*m, tc->stage_cap, nslot);
   auto k = tc::nsf_logprob_tc_kernel<50, 10, false, true>;
   static int smem_set_[sbi::kMaxDev] = {0};
@@ -679,7 +693,7 @@ int sbi::tc::launch_forward_save(const sbi_nsf_model* m, const sbi_nsf_tc* tc, c
     smem_set = L.total_bytes;
   }
   const int grid = (int)((rows->R + tc::kRows - 1) / tc::kRows);      // one tile per CTA: `d_save` slab = blockIdx
-  k<<<grid, tc::kThreads, L.total_bytes, s>>>(*m, *tc, *rows, d_logp, nullptr, d_save);
+  k<<<grid, tc::kThreads, L.total_bytes, s>>>(*m, *tc, *rows, d_logp, nullptr, d_save, sa);
   return (int)cudaGetLastError();
 }
 
@@ -693,6 +707,8 @@ extern "C" int sbi_b200_nsf_inverse_tc(const sbi_nsf_model* m, const sbi_nsf_tc*
   if (!sbi_b200_nsf_tc_supported(m, tc)) return SBI_ESMEM;
   if (rows->R == 0) return 0;
   const int nslot = tc_plan_slots(m, tc);
+  tc::StoreArgs sa;
+  if (int e = tc::store_args(&sa)) return e;
   const tc::TcSmem L = tc::tc_smem_layout(*m, tc->stage_cap, nslot);
   auto k = tc::nsf_logprob_tc_kernel<50, 10, true>;
   static int smem_set_[sbi::kMaxDev] = {0};
@@ -704,7 +720,7 @@ extern "C" int sbi_b200_nsf_inverse_tc(const sbi_nsf_model* m, const sbi_nsf_tc*
   }
   const int64_t ntiles = (rows->R + tc::kRows - 1) / tc::kRows;
   const int grid = (int)std::min<int64_t>(ntiles, (int64_t)tc_num_sms() * 2);
-  k<<<grid, tc::kThreads, L.total_bytes, (cudaStream_t)stream>>>(*m, *tc, *rows, d_logabsdet, d_out, nullptr);
+  k<<<grid, tc::kThreads, L.total_bytes, (cudaStream_t)stream>>>(*m, *tc, *rows, d_logabsdet, d_out, nullptr, sa);
   return (int)cudaGetLastError();
 }
 

@@ -7,11 +7,12 @@
 // (nsf_tc_save.cuh).  Replaces nsf_vjp_kernel (nsf.cu, FP32 SIMT) when only parameter gradients
 // are asked for -- the trainer's case.
 //
-// One CTA = 8 warps owns a tile of 128 rows (row = TMEM lane, two threads per row splitting the
+// One CTA = 8 warps owns a tile of 128 rows (row = store lane, two threads per row splitting the
 // columns), walks the layers T-1 .. 0 and, per layer, the linears of the conditioner
 // (nflows ResidualNet, restated in oracle/nflows_port/nn/nets/resnet.py) in reverse:
 //
-//   * input-gradient chain  dX = dY W  on tcgen05.mma kind::tf32, M = 128: A = dY from TMEM (written
+//   * input-gradient chain  dX = dY W  on wgmma kind tf32 (both warpgroups, 64 rows each): A = dY from
+//     the accumulator store of tc_common.cuh (written
 //     by the row threads, 3xTF32 hi/lo split), B = W^T streamed by TMA bulk copies from the
 //     pre-transposed operand blocks (pack.NsfLayout.tc_bwd_plan) through a 2-slot ring; relu / GLU
 //     masks, the spline backward (rqs.cuh) and the LULinear backward are per-thread code on the
@@ -20,12 +21,12 @@
 //     operands from shared memory: the row threads write dY^T and X^T into K-major staging buffers
 //     ([row/4][feature][row%4], one padding row per slab so that the 32 rows of a warp hit 32 banks),
 //     one M = 64 MMA chain of 16 K-steps per linear (single TF32 pass: the sum over rows averages the
-//     operand rounding), accumulators in TMEM, read back by the 16 lanes per warp that hold them and
-//     written to this CTA's partial-gradient slab; a ones row appended to X^T yields the bias
-//     gradient in the same MMA.  Staging buffers and accumulators are double buffered, so a weight
-//     gradient runs on the tensor core while the chain's next epilogue executes.
+//     operand rounding; the two warpgroups split N), accumulators stored in the accumulator store,
+//     read back by the 16 lanes per warp that hold them and written to this CTA's partial-gradient
+//     slab; a ones row appended to X^T yields the bias gradient in the same MMA.  Staging buffers and
+//     accumulators are double buffered; every MMA completes before the code after it runs.
 //
-// TMEM columns (512): [0,64) A_hi | [64,128) A_lo | [128,192) D | [192,256) G |
+// Store columns (512): [0,64) A_hi | [64,128) A_lo | [128,192) D | [192,256) G |
 //                     [256,320) A2_hi | [320,384) A2_lo (second A set: spline passes alternate) |
 //                     [384,448) dW slot 0 | [448,512) dW slot 1
 #include <cuda_runtime.h>
@@ -45,6 +46,7 @@ namespace tc {
 
 constexpr int kBwdSlots = 2;
 constexpr int kBwdCols = 512;
+static_assert(kBwdCols <= kStoreCols, "one CTA's columns must fit one slab");
 constexpr int cA2 = 256;
 constexpr int cW = 384;
 constexpr int kStLd = 65;                       // feature rows per K-slab of a staging buffer (64 + 1 pad)
@@ -119,7 +121,7 @@ __global__ void __launch_bounds__(kThreads, 1)
 nsf_vjp_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_constant__ sbi_nsf_tc tcb,
                   const __grid_constant__ sbi_rows rows, const float* __restrict__ gout, float g_const,
                   float* __restrict__ gpart, float* __restrict__ loss_acc,
-                  const float* __restrict__ save, int accum_first) {
+                  const float* __restrict__ save, int accum_first, const StoreArgs sa) {
   constexpr int HP8 = (H + 7) & ~7;
   constexpr int NCH = HP8 / 8;
   constexpr int NC = HP8 / 2;
@@ -147,11 +149,7 @@ nsf_vjp_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_constant
     fence_barrier_init();
   }
   if (warp == 0) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(
-                     smem_u32(tbase_s)),
-                 "r"(kBwdCols)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
+    store_alloc(tbase_s, kBwdCols, sa);
   }
   fence_before();
   __syncthreads();
@@ -253,22 +251,14 @@ nsf_vjp_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_constant
   };
   // dW = A'^T-staged dY (M = 64 feature rows) x B'-staged X (N feature rows), K = 128 tile rows
   auto dw_issue = [&](int slot, const DwGeo& g) {
-    if ((int)(dwn & 7u) == warp) {
-      fence_after();
-      const uint32_t a_s = __shfl_sync(0xffffffffu, smem_u32(stg + (2 * slot) * kStFloats), 0);
-      const uint32_t b_s = __shfl_sync(0xffffffffu, smem_u32(stg + (2 * slot + 1) * kStFloats), 0);
-      const int N = __shfl_sync(0xffffffffu, g.N, 0);
-      const uint32_t idesc = make_idesc_mn(64, N);
-      uint64_t da = make_bdesc(a_s, kStLd * 16u, 128u);
-      uint64_t db = make_bdesc(b_s, kStLd * 16u, 128u);
+    {
+      const uint32_t a_s = smem_u32(stg + (2 * slot) * kStFloats);
+      const uint32_t b_s = smem_u32(stg + (2 * slot + 1) * kStFloats);
+      const uint64_t da = make_bdesc(a_s, kStLd * 16u, 128u);
+      const uint64_t db = make_bdesc(b_s, kStLd * 16u, 128u);
       const uint64_t dstep = (uint64_t)((2u * kStLd * 16u) >> 4);
-      const uint32_t d = iss.tbase + cW + 64 * slot;
-#pragma unroll 4
-      for (int kk = 0; kk < kRows / 8; ++kk) {
-        if (iss.leader) mma_tf32_ss(d, da, db, idesc, kk > 0 ? 1u : 0u);
-        da += dstep; db += dstep;
-      }
-      if (iss.leader) commit(&dwbar[slot]);
+      mma_ss64(g.N, store_col(iss.tbase) + cW + 64 * slot, da, db, dstep, kRows / 8);
+      commit(&dwbar[slot]);
     }
     if (slot) { pend1 = true; geo1 = g; } else { pend0 = true; geo0 = g; }
     ++dwn;
@@ -759,8 +749,7 @@ nsf_vjp_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_constant
   fence_before();
   group_sync();
   if (warp == 0)
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tbase), "r"(kBwdCols)
-                 : "memory");
+    store_dealloc(tbase, kBwdCols, sa);
 }
 
 }  // namespace tc
@@ -823,6 +812,8 @@ extern "C" int sbi_b200_nsf_vjp_tc(const sbi_nsf_model* m, const sbi_nsf_tc* tc_
   }
   // chunks of one tile per SM: forward sweep (saves activations) then backward sweep of the same rows;
   // later chunks accumulate into the partial-gradient slabs
+  tc::StoreArgs sa;
+  if (int e = tc::store_args(&sa)) return e;
   const int64_t chunk = vjp_tc_chunk_rows();
   for (int64_t r0 = 0; r0 < rows->R; r0 += chunk) {
     sbi_rows rr = *rows;
@@ -836,7 +827,7 @@ extern "C" int sbi_b200_nsf_vjp_tc(const sbi_nsf_model* m, const sbi_nsf_tc* tc_
     const int rc = tc::launch_forward_save(m, tc_fwd, &rr, d_logp ? d_logp + r0 : nullptr, d_save, s);
     if (rc) return rc;
     kb<<<grid, tc::kThreads, Lb.total_bytes, s>>>(*m, *tc_bwd, rr, d_gout ? d_gout + r0 : nullptr, g_const,
-                                                  d_gpart, d_loss_acc, d_save, r0 > 0 ? 1 : 0);
+                                                  d_gpart, d_loss_acc, d_save, r0 > 0 ? 1 : 0, sa);
   }
   return (int)cudaGetLastError();
 }

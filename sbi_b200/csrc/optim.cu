@@ -124,8 +124,7 @@ adam_clip_kernel(float* __restrict__ params, const float* __restrict__ grad,
   }
   if (threadIdx.x == 0) {
     // bias corrections 1 - beta^t in double like torch (python floats), by repeated squaring: ~2 log2(t)
-    // FP64 multiplies instead of a software pow() (which cost ~10 of this kernel's 15 us on sm_100a's
-    // reduced-rate FP64 pipe)
+    // FP64 multiplies instead of a software pow()
     const int t = d_step[0] + 1;
     double p1 = 1.0, p2 = 1.0, b1 = (double)beta1, b2 = (double)beta2;
     for (int e = t; e > 0; e >>= 1) {
@@ -237,7 +236,7 @@ extern "C" int sbi_b200_adam_clip_step_norm(float* d_params, const float* d_grad
   if (!d_params || !d_grad || !d_state || !d_step || n < 1) return SBI_EINVAL;
   if (d_sumsq_part != nullptr && n_sumsq < 1) return SBI_EINVAL;
   int grid = (int)((n + 1023) / 1024);
-  if (grid > 148) grid = 148;
+  if (grid > sbi::dev_num_sms()) grid = sbi::dev_num_sms();
   sbi::adam_clip_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(
       d_params, d_grad, d_state, d_step, d_mask, n, lr, beta1, beta2, eps, max_norm, grad_scale,
       d_sumsq_part, n_sumsq);

@@ -4,9 +4,9 @@
 // ResidualNet(in = D_theta + D_x, out = 1, hidden 50, 2 blocks, relu, no context)) for large
 // numbers of (theta, x) pairs — the potential of rejection sampling and MCMC at a fixed x_o.
 //
-// Same machinery as nsf_tc.cu (tc_common.cuh): 128 pairs per CTA = 128 TMEM lanes, two threads per
-// pair splitting the hidden columns, tcgen05.mma kind::tf32 with the 3xTF32 split, A from TMEM,
-// weights streamed by TMA in the UMMA canonical layout, the warps taking turns to issue.
+// Same machinery as nsf_tc.cu (tc_common.cuh): 128 pairs per CTA = 128 lanes of the accumulator
+// store, two threads per pair splitting the hidden columns, wgmma kind tf32 with the 3xTF32 split on
+// both warpgroups, A from the store, weights streamed by TMA in the no-swizzle K-major layout.
 //   stages: initial layer (A = [theta | x] standardised, K = round8(Dt + Dx)),
 //           per block W_1 relu(h), W_2 relu(.), final layer as an N = 16 MMA whose column 0 is
 //           the logit.
@@ -40,7 +40,7 @@ __host__ __device__ inline RatioTcSmem ratio_tc_smem_layout(const sbi_ratio_mode
 template <int H>
 __global__ void __launch_bounds__(kThreads, 2)
 ratio_forward_tc_kernel(const __grid_constant__ sbi_ratio_model m, const __grid_constant__ sbi_nsf_tc tc,
-                        const __grid_constant__ sbi_pairs pr, float* __restrict__ logits) {
+                        const __grid_constant__ sbi_pairs pr, float* __restrict__ logits, const StoreArgs sa) {
   constexpr int HP8 = (H + 7) & ~7;
   constexpr int NCH = HP8 / 8;
   constexpr int NC = HP8 / 2;       // hidden columns per thread
@@ -61,11 +61,7 @@ ratio_forward_tc_kernel(const __grid_constant__ sbi_ratio_model m, const __grid_
     fence_barrier_init();
   }
   if (warp == 0) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(
-                     smem_u32(tbase_s)),
-                 "r"(kCols)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
+    store_alloc(tbase_s, kCols, sa);
   }
   fence_before();
   __syncthreads();
@@ -246,8 +242,7 @@ ratio_forward_tc_kernel(const __grid_constant__ sbi_ratio_model m, const __grid_
   fence_before();
   group_sync();
   if (warp == 0)
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tbase), "r"(kCols)
-                 : "memory");
+    store_dealloc(tbase, kCols, sa);
 }
 
 }  // namespace tc
@@ -284,6 +279,8 @@ extern "C" int sbi_b200_ratio_forward_tc(const sbi_ratio_model* m, const sbi_nsf
   if (!sbi_b200_ratio_tc_supported(m, tc)) return SBI_ESMEM;
   if (pairs->R == 0) return 0;
   const tc::RatioTcSmem L = tc::ratio_tc_smem_layout(*m, tc->stage_cap);
+  tc::StoreArgs sa;
+  if (int e = tc::store_args(&sa)) return e;
   auto k = tc::ratio_forward_tc_kernel<50>;
   static int smem_set_[sbi::kMaxDev] = {0};
   int& smem_set = smem_set_[sbi::cur_dev()];
@@ -294,6 +291,6 @@ extern "C" int sbi_b200_ratio_forward_tc(const sbi_ratio_model* m, const sbi_nsf
   }
   const int64_t ntiles = (pairs->R + tc::kRows - 1) / tc::kRows;
   const int grid = (int)std::min<int64_t>(ntiles, (int64_t)rtc_num_sms() * 2);
-  k<<<grid, tc::kThreads, L.total_bytes, (cudaStream_t)stream>>>(*m, *tc, *pairs, d_logits);
+  k<<<grid, tc::kThreads, L.total_bytes, (cudaStream_t)stream>>>(*m, *tc, *pairs, d_logits, sa);
   return (int)cudaGetLastError();
 }

@@ -1,12 +1,13 @@
-// Building blocks of the tensor-core (tcgen05) row-tile kernels: PTX wrappers, the 3xTF32 split,
-// the weight-stage ring and its issuing logic.  Used by nsf_tc.cu and ratio_tc.cu; see the header of
-// nsf_tc.cu for the design.
+// Building blocks of the tensor-core (wgmma) row-tile kernels: the accumulator store, the MMAs, the
+// 3xTF32 split, the weight-stage ring and its issuing logic.  Used by nsf_tc.cu, nsf_vjp_tc.cu and
+// ratio_tc.cu; see the header of nsf_tc.cu for the design.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
 
 #include "../../include/sbi_b200.h"
 #include "common.cuh"
+#include "wgmma.cuh"
 
 namespace sbi {
 namespace tc {
@@ -33,84 +34,232 @@ constexpr int kRowThreads = 256;  // two threads per row (column halves)
 constexpr int kThreads = 256;     // 8 row warps, which also take turns issuing MMAs and TMA copies
 constexpr int kLuMax = 16;        // LULinear runs on register-resident rows of <= 16 features
 constexpr int kSlots = 3;         // weight ring: up to two stages in use + one prefetched
-constexpr int kCols = 256;        // TMEM columns per CTA
+constexpr int kCols = 256;        // accumulator-store columns per CTA
 constexpr int cAhi = 0, cAlo = 64, cD = 128, cG = 192;
 
-// ---- tcgen05 wrappers -------------------------------------------------------------------------
-__device__ __forceinline__ void fence_before() {
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
+// ---- accumulator store --------------------------------------------------------------------------
+// The kernels address their MMA operands and accumulators as (slot << 23) | (lane << 16) | column,
+// lane = tile row (128 lanes).  Hopper keeps wgmma accumulators in registers, and an SM's shared memory
+// is taken by the weight ring and the staging buffers, so the operand / accumulator columns live in
+// global memory: kStoreSlots slabs of kStoreCols columns x 128 lanes (lane-contiguous, so the 32 threads
+// of a warp touch one 128-byte line per column; 34.6 MB per device, defined once in nsf_tc.cu and
+// mostly L2-resident while a kernel runs), handed out in 64-column units through one mask per slab.
+// A CTA picks the slab of the SM it starts on (for locality only) and records the slot in its column
+// base; every later address comes from that record, so a CTA that resumes on another SM keeps its slab.
+constexpr int kStoreCols = 512;
+constexpr int kStoreLanes = 128;
+constexpr int kStoreSlots = 132;  // one per H100 SXM SM; SMs with larger ids share slabs through the masks
+struct StoreArgs {
+  float* slab;              // [kStoreSlots][kStoreCols * kStoreLanes]
+  unsigned int* mask;       // [kStoreSlots]: bit u = columns [64u, 64u + 64) are taken
+};
+// the device's slabs and masks (host; defined in nsf_tc.cu); returns a cudaError_t
+int store_args(StoreArgs* out);
+
+static __shared__ float* s_store_slab;     // this CTA's slab, set by store_alloc
+
+__device__ __forceinline__ float* store_slab() { return s_store_slab; }
+// element (column, lane) of this CTA's slab
+__device__ __forceinline__ float* store_at(uint32_t col, uint32_t lane) {
+  return s_store_slab + (size_t)col * kStoreLanes + lane;
 }
-__device__ __forceinline__ void fence_after() {
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
+// warp 0 of the CTA, before the CTA barrier that publishes *dst: reserve `ncols` (multiple of 64,
+// <= kStoreCols) columns of a slab; the column base (slot in bits 23+) goes to *dst.  Spins while
+// other CTAs hold the columns.  A waiting CTA holds no columns (a reservation is one CAS of all its
+// units), and a holder waits on no other CTA before it releases, so the wait cannot form a cycle.
+__device__ __forceinline__ void store_alloc(uint32_t* dst, int ncols, const StoreArgs& sa) {
+  if ((threadIdx.x & 31) == 0) {
+    uint32_t sm;
+    asm volatile("mov.u32 %0, %%smid;" : "=r"(sm));
+    const uint32_t slot = sm % kStoreSlots;
+    unsigned int* mk = sa.mask + slot;
+    const int units = ncols / 64;
+    const unsigned int want = (1u << units) - 1u;
+    for (;;) {
+      const unsigned int cur = atomicAdd(mk, 0u);
+      int pos = -1;
+      for (int p = 0; p + units <= kStoreCols / 64; p += units)
+        if (!(cur & (want << p))) { pos = p; break; }
+      if (pos >= 0 && atomicCAS(mk, cur, cur | (want << pos)) == cur) {
+        __threadfence();
+        *dst = (slot << 23) | ((uint32_t)pos * 64u);
+        s_store_slab = sa.slab + (size_t)slot * kStoreCols * kStoreLanes;
+        break;
+      }
+      __nanosleep(200);
+    }
+  }
+  __syncwarp();
 }
-__device__ __forceinline__ void wait_ld() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void wait_st() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void store_dealloc(uint32_t base, int ncols, const StoreArgs& sa) {
+  if ((threadIdx.x & 31) == 0) {
+    __threadfence();
+    atomicAnd(sa.mask + (base >> 23), ~(((1u << (ncols / 64)) - 1u) << ((base & 0xffffu) / 64)));
+  }
+  __syncwarp();
+}
+// column and lane fields of a store address
+__device__ __forceinline__ uint32_t store_col(uint32_t taddr) { return taddr & 0xffffu; }
+__device__ __forceinline__ uint32_t store_lane(uint32_t taddr) { return (taddr >> 16) & 0x7fu; }
+
+// ordering points of the row-tile protocol: the accumulator store is ordinary global memory, which the
+// CTA barriers and mbarriers around these calls already order
+__device__ __forceinline__ void fence_before() { asm volatile("" ::: "memory"); }
+__device__ __forceinline__ void fence_after() { asm volatile("" ::: "memory"); }
+__device__ __forceinline__ void wait_ld() { asm volatile("" ::: "memory"); }
+__device__ __forceinline__ void wait_st() { asm volatile("" ::: "memory"); }
+// completion of the MMAs issued since the last one: they ran synchronously on all 256 threads, so one
+// CTA barrier and one arrival make their accumulators visible to whoever waits on `bar`
 __device__ __forceinline__ void commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(
-                   smem_u32(bar))
-               : "memory");
+  asm volatile("bar.sync 1, 256;" ::: "memory");
+  if (threadIdx.x == 0) mbar_arrive(bar);
 }
-// D[tmem] (+)= A[tmem] * B[smem]^T : one K = 8 step of kind::tf32
-__device__ __forceinline__ void mma_tf32(uint32_t d, uint32_t a, uint64_t bdesc, uint32_t idesc,
-                                         uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], [%1], %2, %3, p;\n\t}"
-      ::"r"(d),
-      "r"(a), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// instruction descriptor (cute/arch/mma_sm100_desc.hpp InstrDescriptor): fp32 accumulate @4,
-// A/B format tf32 @7/@10, both K-major, N>>3 @17, M>>4 @24
-__device__ __forceinline__ uint32_t make_idesc(int N) {
-  return (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
-}
-// shared-memory operand descriptor, SWIZZLE_NONE, K-major: core matrix = 8 rows x 16 B contiguous;
-// LBO = byte distance of K-adjacent core matrices, SBO = byte distance of 8-row groups
-// (field positions: cute/arch/mma_sm100_desc.hpp SmemDescriptor; the assignment was pinned on
-// hardware with profiles/micro/umma_probe.cu)
+
+// shared-memory operand descriptor of wgmma, no swizzle (interleave), K-major: core matrix = 8 rows x
+// 16 B contiguous; LBO = byte distance of K-adjacent core matrices, SBO = byte distance of 8-row groups
 __device__ __forceinline__ uint64_t make_bdesc(uint32_t saddr, uint32_t lbo, uint32_t sbo) {
   uint64_t d = 0;
   d |= (uint64_t)((saddr >> 4) & 0x3fff);
   d |= (uint64_t)((lbo >> 4) & 0x3fff) << 16;
   d |= (uint64_t)((sbo >> 4) & 0x3fff) << 32;
-  d |= (uint64_t)1 << 46;
   return d;
 }
+// 8 / 4 consecutive columns of the thread's lane (lane = taddr's lane field + lane id)
 __device__ __forceinline__ void st8(uint32_t taddr, const float (&v)[8]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x8.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8};" ::"r"(taddr),
-      "r"(__float_as_uint(v[0])), "r"(__float_as_uint(v[1])), "r"(__float_as_uint(v[2])),
-      "r"(__float_as_uint(v[3])), "r"(__float_as_uint(v[4])), "r"(__float_as_uint(v[5])),
-      "r"(__float_as_uint(v[6])), "r"(__float_as_uint(v[7]))
-      : "memory");
-}
-// 8 consecutive columns of the thread's lane -> v[0..8)   (no wait inside)
-__device__ __forceinline__ void ld8(uint32_t taddr, float* v) {
-  uint32_t r[8];
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]),
-                 "=r"(r[7])
-               : "r"(taddr)
-               : "memory");
+  float* p = store_at(store_col(taddr), store_lane(taddr) + (threadIdx.x & 31));
 #pragma unroll
-  for (int i = 0; i < 8; ++i) v[i] = __uint_as_float(r[i]);
+  for (int i = 0; i < 8; ++i) p[i * kStoreLanes] = v[i];
+}
+__device__ __forceinline__ void ld8(uint32_t taddr, float* v) {
+  const float* p = store_at(store_col(taddr), store_lane(taddr) + (threadIdx.x & 31));
+#pragma unroll
+  for (int i = 0; i < 8; ++i) v[i] = p[i * kStoreLanes];
 }
 __device__ __forceinline__ void st4(uint32_t taddr, const float (&v)[4]) {
-  asm volatile("tcgen05.st.sync.aligned.32x32b.x4.b32 [%0], {%1,%2,%3,%4};" ::"r"(taddr),
-               "r"(__float_as_uint(v[0])), "r"(__float_as_uint(v[1])), "r"(__float_as_uint(v[2])),
-               "r"(__float_as_uint(v[3]))
-               : "memory");
+  float* p = store_at(store_col(taddr), store_lane(taddr) + (threadIdx.x & 31));
+#pragma unroll
+  for (int i = 0; i < 4; ++i) p[i * kStoreLanes] = v[i];
 }
 __device__ __forceinline__ void ld4(uint32_t taddr, float* v) {
-  uint32_t r[4];
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x4.b32 {%0,%1,%2,%3}, [%4];"
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3])
-               : "r"(taddr)
-               : "memory");
+  const float* p = store_at(store_col(taddr), store_lane(taddr) + (threadIdx.x & 31));
 #pragma unroll
-  for (int i = 0; i < 4; ++i) v[i] = __uint_as_float(r[i]);
+  for (int i = 0; i < 4; ++i) v[i] = p[i * kStoreLanes];
+}
+
+// ---- the MMAs: both warpgroups of the CTA, synchronously ------------------------------------------
+// Accumulator fragment of wgmma m64nNk8 (f32): warp w of the warpgroup holds rows 16w + g and
+// 16w + g + 8 (g = lane / 4), columns 8j + 2t and 8j + 2t + 1 (t = lane % 4) in d[4j .. 4j+3].
+//
+// D[store, M = 128] (+)= A[store] * B[smem]^T over nk K-steps, 3xTF32 (A_hi B_hi + A_lo B_hi + A_hi B_lo):
+// warpgroup wg computes rows 64 wg .. 64 wg + 63; A_hi / A_lo fragments come straight from the store.
+template <int N>
+__device__ __forceinline__ void mma_rows_n(uint32_t dcol, uint32_t ahcol, uint32_t alcol, uint64_t dh,
+                                           uint64_t dl, uint64_t dstep, int nk, uint32_t acc) {
+  const int lane = threadIdx.x & 31, g = lane >> 2, t = lane & 3;
+  const uint32_t r0 = (threadIdx.x >> 7) * 64 + ((threadIdx.x >> 5) & 3) * 16 + g;
+  float* slab = store_slab();
+  float d[N / 2];
+#pragma unroll
+  for (int j = 0; j < N / 8; ++j) {
+    const uint32_t c = dcol + 8 * j + 2 * t;
+    d[4 * j + 0] = acc ? slab[c * kStoreLanes + r0] : 0.f;
+    d[4 * j + 1] = acc ? slab[(c + 1) * kStoreLanes + r0] : 0.f;
+    d[4 * j + 2] = acc ? slab[c * kStoreLanes + r0 + 8] : 0.f;
+    d[4 * j + 3] = acc ? slab[(c + 1) * kStoreLanes + r0 + 8] : 0.f;
+  }
+  for (int kk = 0; kk < nk; ++kk) {
+    uint32_t ah[4], al[4];
+    const uint32_t ch = ahcol + 8 * kk + t, cl = alcol + 8 * kk + t;
+    ah[0] = __float_as_uint(slab[ch * kStoreLanes + r0]);
+    ah[1] = __float_as_uint(slab[ch * kStoreLanes + r0 + 8]);
+    ah[2] = __float_as_uint(slab[(ch + 4) * kStoreLanes + r0]);
+    ah[3] = __float_as_uint(slab[(ch + 4) * kStoreLanes + r0 + 8]);
+    al[0] = __float_as_uint(slab[cl * kStoreLanes + r0]);
+    al[1] = __float_as_uint(slab[cl * kStoreLanes + r0 + 8]);
+    al[2] = __float_as_uint(slab[(cl + 4) * kStoreLanes + r0]);
+    al[3] = __float_as_uint(slab[(cl + 4) * kStoreLanes + r0 + 8]);
+    // each K-step into a fresh accumulator, correction terms first; the running sum is then carried
+    // with round-to-nearest adds (the tensor core's own fp32 accumulation truncates)
+    float p[N / 2];
+#pragma unroll
+    for (int i = 0; i < N / 2; ++i) p[i] = 0.f;
+    wgmma_fence();
+    wgmma_rs<N>(p, al, dh, 0u);
+    wgmma_rs<N>(p, ah, dl, 1u);
+    wgmma_rs<N>(p, ah, dh, 1u);
+    wgmma_commit();
+    wgmma_wait_all();
+#pragma unroll
+    for (int i = 0; i < N / 2; ++i) d[i] += p[i];
+    dh += dstep; dl += dstep;
+  }
+#pragma unroll
+  for (int j = 0; j < N / 8; ++j) {
+    const uint32_t c = dcol + 8 * j + 2 * t;
+    slab[c * kStoreLanes + r0] = d[4 * j + 0];
+    slab[(c + 1) * kStoreLanes + r0] = d[4 * j + 1];
+    slab[c * kStoreLanes + r0 + 8] = d[4 * j + 2];
+    slab[(c + 1) * kStoreLanes + r0 + 8] = d[4 * j + 3];
+  }
+}
+__device__ __forceinline__ void mma_rows(int N, uint32_t dcol, uint32_t ahcol, uint32_t alcol, uint64_t dh,
+                                         uint64_t dl, uint64_t dstep, int nk, uint32_t acc) {
+  switch (N) {
+    case 8: mma_rows_n<8>(dcol, ahcol, alcol, dh, dl, dstep, nk, acc); break;
+    case 16: mma_rows_n<16>(dcol, ahcol, alcol, dh, dl, dstep, nk, acc); break;
+    case 24: mma_rows_n<24>(dcol, ahcol, alcol, dh, dl, dstep, nk, acc); break;
+    case 32: mma_rows_n<32>(dcol, ahcol, alcol, dh, dl, dstep, nk, acc); break;
+    case 40: mma_rows_n<40>(dcol, ahcol, alcol, dh, dl, dstep, nk, acc); break;
+    case 48: mma_rows_n<48>(dcol, ahcol, alcol, dh, dl, dstep, nk, acc); break;
+    case 56: mma_rows_n<56>(dcol, ahcol, alcol, dh, dl, dstep, nk, acc); break;
+    case 64: mma_rows_n<64>(dcol, ahcol, alcol, dh, dl, dstep, nk, acc); break;
+    default: __trap();      // operand blocks are planned with N in {8, ..., 64}
+  }
+}
+
+// D[store, M = 64] = A[smem]^T-staged * B[smem]^T over nk K-steps, single TF32 pass.  Row r of D sits
+// in lane 32 (r / 16) + r % 16 (the lane map of an M = 64 tensor-memory accumulator); warpgroup wg
+// computes columns [wg N/2, (wg + 1) N/2) (N % 16 == 0).
+template <int NH>
+__device__ __forceinline__ void mma_ss64_n(uint32_t dcol, uint64_t da, uint64_t db, uint64_t dstep, int nk) {
+  const int lane = threadIdx.x & 31, g = lane >> 2, t = lane & 3;
+  const int wg = threadIdx.x >> 7;
+  const uint32_t l0 = ((threadIdx.x >> 5) & 3) * 32 + g;
+  db += (uint64_t)((wg * NH / 8) * 128 >> 4);      // 8-row groups of B are 128 B apart
+  dcol += wg * NH;
+  float* slab = store_slab();
+  float d[NH / 2];
+#pragma unroll
+  for (int i = 0; i < NH / 2; ++i) d[i] = 0.f;
+  for (int kk = 0; kk < nk; ++kk) {
+    float p[NH / 2];
+#pragma unroll
+    for (int i = 0; i < NH / 2; ++i) p[i] = 0.f;
+    wgmma_fence();
+    wgmma_ss<NH>(p, da, db, 0u);
+    wgmma_commit();
+    wgmma_wait_all();
+#pragma unroll
+    for (int i = 0; i < NH / 2; ++i) d[i] += p[i];
+    da += dstep; db += dstep;
+  }
+#pragma unroll
+  for (int j = 0; j < NH / 8; ++j) {
+    const uint32_t c = dcol + 8 * j + 2 * t;
+    slab[c * kStoreLanes + l0] = d[4 * j + 0];
+    slab[(c + 1) * kStoreLanes + l0] = d[4 * j + 1];
+    slab[c * kStoreLanes + l0 + 8] = d[4 * j + 2];
+    slab[(c + 1) * kStoreLanes + l0 + 8] = d[4 * j + 3];
+  }
+}
+__device__ __forceinline__ void mma_ss64(int N, uint32_t dcol, uint64_t da, uint64_t db, uint64_t dstep, int nk) {
+  switch (N) {
+    case 16: mma_ss64_n<8>(dcol, da, db, dstep, nk); break;
+    case 32: mma_ss64_n<16>(dcol, da, db, dstep, nk); break;
+    case 48: mma_ss64_n<24>(dcol, da, db, dstep, nk); break;
+    case 64: mma_ss64_n<32>(dcol, da, db, dstep, nk); break;
+    default: __trap();      // weight-gradient blocks are planned with N in {16, 32, 48, 64}
+  }
 }
 template <int NCHUNK>
 __device__ __forceinline__ void ld_cols(uint32_t taddr, float* v) {
@@ -119,8 +268,7 @@ __device__ __forceinline__ void ld_cols(uint32_t taddr, float* v) {
 }
 
 // hi = x rounded to tf32 (10 explicit mantissa bits, round half away in the integer domain),
-// lo = x - hi (exact in fp32).  cvt.rna.tf32.f32 computes the same hi but expands to a longer
-// sequence on sm_100a.
+// lo = x - hi (exact in fp32).  Same hi as cvt.rna.tf32.f32.
 __device__ __forceinline__ void split_tf32(float x, float& hi, float& lo) {
   hi = __uint_as_float((__float_as_uint(x) + 0x1000u) & 0xffffe000u);
   lo = x - hi;
@@ -142,7 +290,7 @@ __device__ __forceinline__ void store_a4(uint32_t tlane, int col, const float (&
 }
 __device__ __forceinline__ void group_sync() { asm volatile("bar.sync 1, 256;" ::: "memory"); }
 
-// ---- weight re-pack: flat fp32 parameters -> [hi | lo] UMMA operand blocks ---------------------
+// ---- weight re-pack: flat fp32 parameters -> [hi | lo] wgmma operand blocks --------------------
 static __global__ void tc_pack_kernel(const float* __restrict__ params, const int32_t* __restrict__ src,
                                    float* __restrict__ tcw, int n) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -162,21 +310,18 @@ static __global__ void tc_pack_kernel(const float* __restrict__ params, const in
 }
 
 // ---- the kernel ------------------------------------------------------------------------------------
-// The warps of the CTA take turns driving the tensor core and the weight stream (stage k is
-// issued by warp k % 8, so the issue work is spread evenly): the whole warp runs this code
-// converged (so the descriptor arithmetic stays in the uniform datapath and the MMAs go out at
-// the tensor pipe's own cadence; a single divergent thread issues 2x slower, see
-// profiles/micro/umma_probe.cu), one elected lane executes the tcgen05 / TMA instructions.
-// Stage k lives in ring slot
-// k % kSlots.  A stage is fetched (TMA bulk copy, completion on full[slot]) as soon as the stage
-// that used its slot kSlots stages earlier is known to be complete, which every warp learns each
-// time it passes an accumulator barrier (a tcgen05.commit covers every MMA issued before it).
+// Every thread runs begin / block / end: the MMAs of a stage take both warpgroups and complete
+// before end() returns.  The weight stream rotates between the warps (stage k is fetched by the
+// elected lane of warp (k + 4) % 8).  Stage k lives in ring slot k % kSlots.  A stage is fetched
+// (TMA bulk copy, completion on full[slot]) as soon as the stage that used its slot kSlots stages
+// earlier is known to be complete, which every warp learns each time it passes an accumulator
+// barrier.
 template <int NSLOT>
 struct IssuerT {
-  uint32_t tbase;       // TMEM base (lane 0, column 0)
+  uint32_t tbase;       // accumulator-store base (slot, lane 0, column 0)
   bool leader;          // the elected lane of this warp
-  int warp;             // this warp; stage k is issued by warp k % 8, fetched by warp (k+4) % 8
-  bool mine;            // this warp issues the current stage
+  int warp;             // this warp; stage k is fetched by warp (k+4) % 8
+  bool mine;            // (kept true: every warp takes part in every stage)
   float* ring;
   uint64_t *full, *bars;
   const float* tcw;
@@ -207,44 +352,28 @@ struct IssuerT {
       }
     }
   }
+  // every thread of the CTA runs begin / block / end: the MMAs take both warpgroups
   __device__ __forceinline__ void begin(int stage_floats) {
-    mine = (int)(it & 7u) == warp;
-    if (!mine) return;
+    mine = true;
     const uint32_t s = it % NSLOT;
     mbar_wait(&full[s], (it / NSLOT) & 1u);
-    // (the shuffles only tell the compiler that these values are warp-uniform)
-    sbase = __shfl_sync(0xffffffffu, smem_u32(ring + (size_t)s * cap), 0);
-    lo_off = __shfl_sync(0xffffffffu, (uint32_t)stage_floats * 2u, 0);   // (floats / 2) * 4 bytes
-    fence_after();
+    sbase = smem_u32(ring + (size_t)s * cap);
+    lo_off = (uint32_t)stage_floats * 2u;   // (floats / 2) * 4 bytes
   }
   // one operand block of N rows starting `blk_floats` into the half: nk K-steps, A columns from a0
   __device__ __forceinline__ void block(int dcol, int a0, int nk, int blk_floats, int N, uint32_t& acc) {
-    if (!mine) return;
-    N = __shfl_sync(0xffffffffu, N, 0);
-    nk = __shfl_sync(0xffffffffu, nk, 0);
-    blk_floats = __shfl_sync(0xffffffffu, blk_floats, 0);
-    const uint32_t idesc = make_idesc(N);
     const uint32_t slab = (uint32_t)N * 16u;
     const uint32_t bh = sbase + (uint32_t)blk_floats * 4u;
-    uint64_t dh = make_bdesc(bh, slab, 128u);
-    uint64_t dl = make_bdesc(bh + lo_off, slab, 128u);
+    const uint64_t dh = make_bdesc(bh, slab, 128u);
+    const uint64_t dl = make_bdesc(bh + lo_off, slab, 128u);
     const uint64_t dstep = (uint64_t)((2u * slab) >> 4);    // start-address field advance per K-step
-    uint32_t ah = tbase + cAhi + a0, al = tbase + cAlo + a0;
-    const uint32_t d = tbase + dcol;
-#pragma unroll 8
-    for (int kk = 0; kk < nk; ++kk) {
-      if (leader) {
-        mma_tf32(d, ah, dh, idesc, acc);
-        mma_tf32(d, al, dh, idesc, 1u);
-        mma_tf32(d, ah, dl, idesc, 1u);
-      }
-      acc = 1u;
-      dh += dstep; dl += dstep; ah += 8; al += 8;
-    }
+    const uint32_t col0 = store_col(tbase);
+    if (nk > 0) mma_rows(N, col0 + dcol, col0 + cAhi + a0, col0 + cAlo + a0, dh, dl, dstep, nk, acc);
+    if (nk > 0) acc = 1u;
   }
   // close the stage: its accumulators are signalled on accumulator barrier `b`
   __device__ __forceinline__ void end(int b) {
-    if (mine && leader) commit(&bars[b]);
+    commit(&bars[b]);
     ++it;
     if (b == 0) cov0 = it; else cov1 = it;
   }
@@ -257,22 +386,7 @@ struct IssuerT {
 };
 using Issuer = IssuerT<kSlots>;
 
-// instruction descriptor with an explicit M (64 or 128)
-__device__ __forceinline__ uint32_t make_idesc_mn(int M, int N) {
-  return (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
-}
-// D[tmem] (+)= A[smem] * B[smem]^T : one K = 8 step of kind::tf32, both operands from shared memory
-__device__ __forceinline__ void mma_tf32_ss(uint32_t d, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                            uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(d),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// generic-proxy shared-memory writes -> visible to the async proxy (tcgen05.mma operand reads)
+// generic-proxy shared-memory writes -> visible to the async proxy (wgmma operand reads)
 __device__ __forceinline__ void fence_async_smem() {
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
 }

@@ -1,4 +1,4 @@
-"""Estimator modules at sbi's estimator boundary, backed by the sm_100a kernels.
+"""Estimator modules at sbi's estimator boundary, backed by the sm_90a kernels.
 
 `NSFEstimator` mirrors `sbi.neural_nets.estimators.NFlowsFlow`
 (/root/reference/sbi/neural_nets/estimators/nflows_flow.py:14-151) on the shape rules of
@@ -122,7 +122,7 @@ def _is_identity(m: nn.Module) -> bool:
 
 
 class FlowEstimator(nn.Module):
-    r"""Normalizing flow q(input | condition) evaluated by hand-written sm_100a kernels
+    r"""Normalizing flow q(input | condition) evaluated by hand-written sm_90a kernels
     (families: neural spline flow `nsf`, masked autoregressive flow `maf`)."""
 
     def __init__(self, layout, input_shape, condition_shape, shift: Tensor,
@@ -381,9 +381,9 @@ class FlowEstimator(nn.Module):
         return out, lad
 
     # ---- tensor-core bulk path (nsf only) --------------------------------------------------------
-    #: rows from which log_prob / sampling go through the tcgen05 kernel (csrc/nsf_tc.cu).
-    #: Measured crossover (profiles/tc_cross.py): one 128-row tile takes ~90 us end to end
-    #: including the operand re-pack, the SIMT kernel 116 us at 2048 rows and 250 us at 10 000.
+    #: rows from which log_prob / sampling go through the wgmma kernel (csrc/nsf_tc.cu).  The
+    #: crossover against the SIMT kernel has not been measured for the wgmma kernel (profiles/tc_cross.py
+    #: measures it); 1024 is carried over from the earlier tensor-core design.
     #: SBI_B200_TC=0 disables, =1 forces.
     TC_MIN_ROWS = int(os.environ.get("SBI_B200_TC_MIN_ROWS", 1024))
 
@@ -419,7 +419,8 @@ class FlowEstimator(nn.Module):
 
     # ---- fused forward+backward of a batch (parameter / input / condition gradients) --------------
     #: rows from which the training VJP runs on the tensor cores (csrc/nsf_vjp_tc.cu) when only parameter
-    #: gradients are wanted; SBI_B200_VJP_TC=0 disables, =1 forces
+    #: gradients are wanted (threshold not measured for the wgmma kernels; profiles/vjp_cross.py measures
+    #: it); SBI_B200_VJP_TC=0 disables, =1 forces
     VJP_TC_MIN_ROWS = int(os.environ.get("SBI_B200_VJP_TC_MIN_ROWS", 256))
 
     def _tc_train_state(self, m, pack: bool = True):

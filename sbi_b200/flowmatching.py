@@ -1,4 +1,4 @@
-"""Flow-matching posterior estimation (FMPE) on the sm_100a kernels.
+"""Flow-matching posterior estimation (FMPE) on the sm_90a kernels.
 
 `FlowMatchingEstimator` mirrors /root/reference/sbi/neural_nets/estimators/flowmatching_estimator.py
 (loss :270-347, forward :205-268, ode_fn :349-372) for the default `VectorFieldMLP`
@@ -76,7 +76,7 @@ class FlowMatchingEstimator(nn.Module):
         self._input_shape, self._condition_shape = torch.Size(input_shape), torch.Size(condition_shape)
         user = embedding_net if embedding_net is not None else nn.Identity()
         if not isinstance(user, nn.Identity):
-            raise NotImplementedError("the sm_100a flow-matching kernels take nn.Identity() embedding nets")
+            raise NotImplementedError("the sm_90a flow-matching kernels take nn.Identity() embedding nets")
         self._embedding_net = nn.Sequential(Standardize(*cond_stats), user) if cond_stats else user
         self.noise_scale = noise_scale
         self.register_buffer("mean_0", torch.as_tensor(mean_0, dtype=torch.float32).expand(input_shape).clone())

@@ -40,7 +40,7 @@ def _process_device(device: str) -> str:
         device = "cuda:0"
     if not str(device).startswith("cuda"):
         raise RuntimeError(
-            f"sbi_b200 trains on a CUDA (sm_100a) device only; got device={device!r}. "
+            f"sbi_b200 trains on a CUDA (sm_90a) device only; got device={device!r}. "
             "There is no CPU fallback.")
     if not torch.cuda.is_available():
         raise RuntimeError("sbi_b200: no CUDA device available (no CPU fallback)")

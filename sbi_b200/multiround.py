@@ -1,4 +1,4 @@
-"""Multi-round losses on top of the sm_100a estimators (SURVEY 8f-2).
+"""Multi-round losses on top of the sm_90a estimators (SURVEY 8f-2).
 
 * `atomic_log_prob_proposal_posterior` -- NPE-C / APT atomic proposal correction
   (/root/reference/sbi/inference/trainers/npe/npe_c.py:356-440): every row of the batch is classified

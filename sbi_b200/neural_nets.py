@@ -4,7 +4,7 @@ Same names, argument meaning and defaults as the reference factories
 (/root/reference/sbi/neural_nets/factory.py:323-430 `posterior_nn`, :244-320
 `likelihood_nn`) and builders (/root/reference/sbi/neural_nets/net_builders/flow.py:333-460
 `build_nsf`).  Each factory returns `build_fn(batch_theta, batch_x)`; the returned estimator
-implements sbi's ConditionalDensityEstimator interface on the sm_100a kernels, so it can be
+implements sbi's ConditionalDensityEstimator interface on the sm_90a kernels, so it can be
 passed to the reference trainers (`NPE(prior, density_estimator=posterior_nn("nsf"))`) or to
 this package's device-resident trainers (`sbi_b200.inference`).
 """
@@ -110,7 +110,7 @@ def build_nsf(
     if z_score_x == "transform_to_unconstrained":
         raise ValueError("`transform_to_unconstrained` is not supported by build_nsf.")
     if dropout_probability != 0.0 or use_batch_norm:
-        raise NotImplementedError("dropout / batch norm are not implemented in the sm_100a "
+        raise NotImplementedError("dropout / batch norm are not implemented in the sm_90a "
                                   "NSF kernels (reference defaults are 0.0 / False)")
     x_numel = batch_x[0].numel()
     with torch.no_grad():
@@ -203,7 +203,7 @@ def build_maf(
     if z_score_x == "transform_to_unconstrained":
         raise ValueError("`transform_to_unconstrained` is not supported by build_maf.")
     if dropout_probability != 0.0 or use_batch_norm:
-        raise NotImplementedError("dropout / batch norm are not implemented in the sm_100a MAF kernels")
+        raise NotImplementedError("dropout / batch norm are not implemented in the sm_90a MAF kernels")
     x_numel = batch_x[0].numel()
     with torch.no_grad():
         y_numel = embedding_net(batch_y[:1]).numel()
@@ -253,9 +253,9 @@ def build_maf_rqs(
     if z_score_x == "transform_to_unconstrained":
         raise ValueError("`transform_to_unconstrained` is not supported by build_maf_rqs.")
     if dropout_probability != 0.0 or use_batch_norm:
-        raise NotImplementedError("dropout / batch norm are not implemented in the sm_100a MAF kernels")
+        raise NotImplementedError("dropout / batch norm are not implemented in the sm_90a MAF kernels")
     if tails != "linear":
-        raise NotImplementedError("the sm_100a spline code implements tails='linear' (the reference default)")
+        raise NotImplementedError("the sm_90a spline code implements tails='linear' (the reference default)")
     x_numel = batch_x[0].numel()
     with torch.no_grad():
         y_numel = embedding_net(batch_y[:1]).numel()
@@ -351,7 +351,7 @@ _BUILDERS = {"nsf": build_nsf, "maf": build_maf, "maf_rqs": build_maf_rqs, "made
 def _density_build_fn(model: str, input_is_theta: bool, **kw) -> Callable:
     if model not in _BUILDERS:
         raise NotImplementedError(
-            f"sbi_b200 implements {sorted(_BUILDERS)} density estimators on sm_100a; "
+            f"sbi_b200 implements {sorted(_BUILDERS)} density estimators on sm_90a; "
             f"got model={model!r}.")
     builder = _BUILDERS[model]
 

@@ -208,12 +208,12 @@ class NsfLayout(_LayoutOps):
 
     # ------------------------------------------------------------- tensor-core operand plan
     def tc_plan(self):
-        """Gather map + stage table for the tcgen05 evaluation path (include/sbi_b200.h,
+        """Gather map + stage table for the wgmma evaluation path (include/sbi_b200.h,
         `sbi_nsf_tc`; kernel sbi_b200/csrc/nsf_tc.cu), or None when the model is outside what
         that kernel instantiates.
 
         Every linear of the conditioner (nflows ResidualNet) becomes one or two K-major
-        no-swizzle UMMA operand blocks [K/4 slabs][N rows][4 floats].  The hidden operand's
+        no-swizzle (interleaved) wgmma operand blocks [K/4 slabs][N rows][4 floats].  The hidden operand's
         columns are [hidden (H) | context (C) | 0] so that the context never needs its own
         staging: the GLU gate reads the K-steps that cover columns H..H+C-1.
         Returns dict(src=int32 (n_words,), tab=int32 (T*STRIDE,), stage_cap=int, n_words=int).
@@ -301,7 +301,7 @@ class NsfLayout(_LayoutOps):
                     stage_cap=int((stage_cap + 31) & ~31), n_words=int(off))
 
     def tc_bwd_plan(self):
-        """Gather map + stage table of the TRANSPOSED linears for the tcgen05 training kernel's
+        """Gather map + stage table of the TRANSPOSED linears for the wgmma training kernel's
         input-gradient chain (kernel sbi_b200/csrc/nsf_vjp_tc.cu): dX = dY W needs, as the B operand
         [N = in-features][K = out-features] in the same K-major no-swizzle layout, B[n][k] = W[k][n].
         Stages of a layer in the order the backward sweep uses them (aux = number of K-steps):
@@ -854,7 +854,7 @@ class RatioLayout(_LayoutOps):
         self.buffers = {}
 
     def tc_plan(self):
-        """Gather map + stage table for the tcgen05 evaluation path (csrc/ratio_tc.cu), or None."""
+        """Gather map + stage table for the wgmma evaluation path (csrc/ratio_tc.cu), or None."""
         Dt, Dx, H, NB = self.Dt, self.Dx, self.H, self.NB
         if H != 50 or Dt + Dx > 56:
             return None

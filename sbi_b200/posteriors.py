@@ -37,8 +37,7 @@ def within_support(distribution: Any, samples: Tensor) -> Tensor:
 class DeviceMultivariateNormal(torch.distributions.MultivariateNormal):
     """MultivariateNormal whose `log_prob` is one (rows, D) x (D, D) product with the inverse Cholesky factor.
     torch's implementation solves a triangular system with the rows as right-hand sides, which on CUDA takes
-    seconds for the 10^6-row batches of the rejection / MCMC potentials (measured 5.4 s per call at
-    1 M x 10 on a B200, bench cfg5); same value to fp32 rounding."""
+    a long time for the 10^6-row batches of the rejection / MCMC potentials; same value to fp32 rounding."""
 
     def __init__(self, loc, covariance_matrix=None, scale_tril=None, validate_args=None):
         super().__init__(loc, covariance_matrix=covariance_matrix, scale_tril=scale_tril, validate_args=validate_args)

@@ -1,4 +1,4 @@
-"""Ratio estimator (NRE) at sbi's estimator boundary, backed by the sm_100a kernels.
+"""Ratio estimator (NRE) at sbi's estimator boundary, backed by the sm_90a kernels.
 
 `RatioEstimator` mirrors /root/reference/sbi/neural_nets/ratio_estimators.py:11-157 for the
 `resnet` classifier of /root/reference/sbi/neural_nets/net_builders/classifier.py:172-235:
@@ -68,7 +68,7 @@ class RatioEstimator(nn.Module):
         et = embedding_net_theta if embedding_net_theta is not None else nn.Identity()
         ex = embedding_net_x if embedding_net_x is not None else nn.Identity()
         if not isinstance(et, nn.Identity) or not isinstance(ex, nn.Identity):
-            raise NotImplementedError("the sm_100a ratio kernels take nn.Identity() embedding nets")
+            raise NotImplementedError("the sm_90a ratio kernels take nn.Identity() embedding nets")
         self.embedding_net_theta = nn.Sequential(Standardize(*theta_stats), et) if theta_stats else et
         self.embedding_net_x = nn.Sequential(Standardize(*x_stats), ex) if x_stats else ex
         self.net = _RatioNet(layout)
@@ -182,8 +182,8 @@ class RatioEstimator(nn.Module):
         L.check(lib.sbi_b200_ratio_forward(C.byref(m), C.byref(pr), L.ptr(out), L.stream_ptr()), "ratio_forward")
         return out
 
-    #: pairs from which the logits go through the tcgen05 kernel (csrc/ratio_tc.cu); measured
-    #: (profiles/tc_ratio_time.py): 10 k pairs 29 us SIMT vs 35 us, 131 k pairs 140 vs 58 us
+    #: pairs from which the logits go through the wgmma kernel (csrc/ratio_tc.cu); the crossover against
+    #: the SIMT kernel has not been measured for the wgmma kernel (profiles/tc_ratio_time.py measures it)
     TC_MIN_ROWS = int(os.environ.get("SBI_B200_RATIO_TC_MIN_ROWS", 32768))
 
     def _tc_state(self, m):
@@ -259,7 +259,7 @@ def build_resnet_classifier(
     if z_score_x == "transform_to_unconstrained":
         raise ValueError("Ratio-based classifiers (NRE) do not implement `transform_to_unconstrained`.")
     if dropout_probability != 0.0 or use_batch_norm:
-        raise NotImplementedError("dropout / batch norm are not implemented in the sm_100a ratio kernels")
+        raise NotImplementedError("dropout / batch norm are not implemented in the sm_90a ratio kernels")
     Dt, Dx, H = batch_x[0].numel(), batch_y[0].numel(), hidden_features
     lay = RatioLayout(Dt=Dt, Dx=Dx, H=H, NB=num_blocks)
     state = {}
@@ -289,7 +289,7 @@ def classifier_nn(
 ) -> Callable:
     """factory.py:174-241: build function for the NRE classifier."""
     if model != "resnet":
-        raise NotImplementedError(f"sbi_b200 implements the 'resnet' classifier on sm_100a; got {model!r}.")
+        raise NotImplementedError(f"sbi_b200 implements the 'resnet' classifier on sm_90a; got {model!r}.")
 
     def build_fn(batch_theta, batch_x):
         from ._refabc import register_with_reference

@@ -1,4 +1,4 @@
-"""Neural posterior score estimation (NPSE, SURVEY 8f-3) on the sm_100a kernels.
+"""Neural posterior score estimation (NPSE, SURVEY 8f-3) on the sm_90a kernels.
 
 The score network is the same `VectorFieldMLP` as FMPE's (vector_field_nets.py:610-719), so it runs on the
 flow-matching kernels in their bare-network mode (`sbi_fm_model.raw = 1`): forward = `sbi_b200_fm_forward`,
@@ -434,7 +434,7 @@ def build_score_estimator(batch_x: Tensor, batch_y: Tensor, sde_type: str = "ve"
     if sde_type not in _SDE:
         raise ValueError(f"Unknown SDE type: {sde_type}")
     if net != "mlp":
-        raise NotImplementedError("sbi_b200 implements net='mlp' score networks on sm_100a")
+        raise NotImplementedError("sbi_b200 implements net='mlp' score networks on sm_90a")
     fm = build_vector_field_estimator(batch_x, batch_y, estimator_type="flow", z_score_x=z_score_x, z_score_y=z_score_y,
                                       embedding_net=embedding_net, hidden_features=hidden_features,
                                       time_embedding_dim=time_embedding_dim, num_layers=num_layers, net="mlp")

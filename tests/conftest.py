@@ -9,7 +9,7 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a real B200 (sm_100a); run with -m gpu")
+    config.addinivalue_line("markers", "gpu: needs a real H100 (sm_90a); run with -m gpu")
     config.addinivalue_line("markers", "slow: long-running")
 
 
@@ -33,5 +33,5 @@ def cuda_lib(lib):
     import torch
     if not torch.cuda.is_available():
         pytest.fail("GPU test selected but torch.cuda.is_available() is False")
-    assert lib.sbi_b200_device_ok() == 1, "device 0 is not sm_100"
+    assert lib.sbi_b200_device_ok() == 1, "device 0 is not sm_90 (H100)"
     return lib

@@ -1,4 +1,4 @@
-"""CPU checks of the boundary: the library builds for sm_100a, loads, and exports every symbol
+"""CPU checks of the boundary: the library builds for sm_90a, loads, and exports every symbol
 include/sbi_b200.h declares; argument errors surface as the documented codes; the product path
 refuses to run without a CUDA device (no CPU fallback)."""
 import os
@@ -22,7 +22,8 @@ def test_header_symbols_exported(lib):
 
 
 def test_sass_has_tma_bulk_copy(lib):
-    """The weight pipeline must be the TMA bulk-copy path (UBLKCP) for sm_100a."""
+    """The weight pipeline must be the TMA bulk-copy path (UBLKCP) for sm_90a, and the tensor-core
+    kernels must run on warpgroup MMAs (HGMMA)."""
     import shutil
     import subprocess
     from sbi_b200 import _lib
@@ -30,8 +31,9 @@ def test_sass_has_tma_bulk_copy(lib):
     if not os.path.exists(cuobjdump):
         pytest.skip("cuobjdump not available")
     out = subprocess.run([cuobjdump, "-sass", _lib.LIB_PATH], capture_output=True, text=True).stdout
-    assert "sm_100a" in out or "SM100" in out.upper()
+    assert "sm_90a" in out
     assert "UBLKCP" in out
+    assert "HGMMA" in out
 
 
 def test_argument_errors(lib):

@@ -1,6 +1,6 @@
 """The estimators bind to the UNMODIFIED reference's ABCs (trainers/base.py:690,985,999 gates) and
-refuse CPU compute.  Runs wherever a copy of the reference exists (/root/reference in the build
-container, baseline/_ref on the GPU box)."""
+refuse CPU compute.  Runs wherever build() staged a copy of the reference
+(oracle/_ref)."""
 import pytest
 import torch
 

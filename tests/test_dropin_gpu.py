@@ -1,8 +1,8 @@
 """Drop-in at the estimator boundary: the UNMODIFIED reference trainers / posteriors
-(`sbi.inference.NPE / NLE / NRE_B / FMPE`, from baseline/_ref on the GPU box) run end to end on
+(`sbi.inference.NPE / NLE / NRE_B / FMPE`, from the copy staged under oracle/_ref) run end to end on
 estimators built by sbi_b200's build functions -- the reference's DataLoader loop, Adam, clipping,
 convergence check, `build_posterior`, `sample`, `log_prob`, with every estimator call going through
-the sm_100a kernels.  Acceptance: the analytic linear-Gaussian posterior (as
+the sm_90a kernels.  Acceptance: the analytic linear-Gaussian posterior (as
 tests/linearGaussian_snpe_test.py:53-152 does with c2st; here mean / std bars)."""
 import math
 import warnings
@@ -92,7 +92,7 @@ def test_reference_nre_b_rejection_on_b200_resnet(cuda_lib, ref):
 
 
 def test_reference_fmpe_on_b200_mlp(cuda_lib, ref):
-    """The reference's FMPE trainer (base_vf_inference.py:206-350) on the sm_100a flow-matching
+    """The reference's FMPE trainer (base_vf_inference.py:206-350) on the sm_90a flow-matching
     estimator.  The reference's VectorFieldPosterior needs zuko's ODE solver at construction (absent
     offline), so the trained estimator is sampled through sbi_b200's posterior (SDE and ODE)."""
     from sbi.inference import FMPE

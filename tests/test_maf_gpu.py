@@ -1,4 +1,4 @@
-"""Parity of the sm_100a MAF kernels (BASELINE configs[0]: posterior_nn='maf', dim 3) against the
+"""Parity of the sm_90a MAF kernels (BASELINE configs[0]: posterior_nn='maf', dim 3) against the
 CPU oracle, through the C ABI.  Tolerances as in test_nsf_gpu.py."""
 import math
 

@@ -1,4 +1,4 @@
-"""Parity of the sm_100a NSF kernels against the CPU oracle (through the C ABI).
+"""Parity of the sm_90a NSF kernels against the CPU oracle (through the C ABI).
 
 Tolerances (fp32 kernels vs. the fp64 oracle; the fp32 oracle's own error against fp64 is
 printed next to it):  |dlogp| <= 2e-3 absolute on log-probs of magnitude O(10..50),

@@ -1,4 +1,4 @@
-"""Parity of the tensor-core (tcgen05, 3xTF32) NSF log_prob kernel, through the C ABI.
+"""Parity of the tensor-core (wgmma, 3xTF32) NSF log_prob kernel, through the C ABI.
 
 Bars: against the fp64 oracle the same LOGP_TOL as the SIMT kernel (2e-3 absolute on
 log-probs of magnitude O(10..50)); against the SIMT fp32 kernel 5e-4 (the 3xTF32 split keeps

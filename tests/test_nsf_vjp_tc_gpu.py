@@ -1,5 +1,5 @@
 """Tensor-core training step (csrc/nsf_tc.cu forward with activation save + csrc/nsf_vjp_tc.cu backward;
-tcgen05 for every conditioner linear: forward, input gradient and weight gradient) against the fp64
+wgmma for every conditioner linear: forward, input gradient and weight gradient) against the fp64
 oracle autograd, against the SIMT VJP kernel, and as a training step."""
 import ctypes as C
 import math

@@ -1,5 +1,5 @@
 """Cross-check of oracle.sbi_port against the UNMODIFIED reference sbi (imported through
-oracle.ref_shim).  Skipped where /root/reference is absent (the GPU box)."""
+oracle.ref_shim).  Skipped where no copy of the reference was staged (oracle/_ref)."""
 import warnings
 
 import pytest
@@ -7,7 +7,7 @@ import torch
 
 from oracle import ref_shim, sbi_port
 
-pytestmark = pytest.mark.skipif(not ref_shim.available(), reason="/root/reference not present")
+pytestmark = pytest.mark.skipif(not ref_shim.available(), reason="no copy of the reference sbi (oracle/_ref)")
 
 
 @pytest.fixture(scope="module")

@@ -1,5 +1,5 @@
 """Parity of the callers around the estimator kernels with the UNMODIFIED reference (imported through
-oracle.ref_shim from baseline/_ref on the GPU box): potentials, mcmc_transform /
+oracle.ref_shim from the copy staged under oracle/_ref): potentials, mcmc_transform /
 transformed_potential, the rejection accept set on fixed seeds (BASELINE north_star), gradient
 ascent, leakage correction, and BASELINE configs[2] (two-moons NLE + vectorized slice sampling,
 c2st against the reference's own posterior samples).
@@ -131,7 +131,7 @@ def test_rejection_accept_set_identity_1m_proposals(cuda_lib, ref):
     """BASELINE north_star: "identical accepted-index sets for rejection on fixed seeds"; cfg5 size
     (resnet classifier, D = 10, 1 000 000 prior proposals).  Candidates and the uniforms come from
     the CPU generator exactly as rejection.py:170-200 draws them; the reference side evaluates its
-    own RatioBasedPotential (CPU fp32), ours the tcgen05 ratio kernel.  The accept decision is
+    own RatioBasedPotential (CPU fp32), ours the wgmma ratio kernel.  The accept decision is
     exp(potential - log q - log_bound) > u, so a draw can only differ when the two fp32 evaluations
     straddle u: every such flip is reported with its margin, and the margin must be rounding-sized."""
     from sbi.inference.potentials.ratio_based_potential import ratio_estimator_based_potential as ref_rat
@@ -175,7 +175,7 @@ def test_rejection_accept_set_identity_1m_proposals(cuda_lib, ref):
     a, b = set(acc_ref.tolist()), set(idx.tolist())
     flips = sorted(a ^ b)
     margins = [(i, float(ratio_ref[i] - u[i]) / max(float(u[i]), 1e-30)) for i in flips]
-    print(f"rejection accept set: reference {len(a)} accepted, sm_100a {len(b)}, flips {len(flips)}: {margins[:20]}")
+    print(f"rejection accept set: reference {len(a)} accepted, sm_90a {len(b)}, flips {len(flips)}: {margins[:20]}")
     assert len(a) > 1000
     # identical sets up to draws whose acceptance ratio equals u within fp32 rounding of the logit
     assert len(flips) <= max(3, int(2e-5 * N)), margins
@@ -236,7 +236,7 @@ def test_leakage_correction_matches_reference(cuda_lib, ref):
         a = float(RefDirect(r_est, prior).leakage_correction(x_o, num_rejection_samples=n, show_progress_bars=False))
         b = float(DirectPosterior(est.cuda(), prior, device="cuda").leakage_correction(x_o.cuda(), num_rejection_samples=n))
     sigma = math.sqrt(max(a * (1 - a), 1e-4) / n)
-    print(f"leakage correction: reference {a:.4f}, sm_100a {b:.4f} (sigma {sigma:.4f})")
+    print(f"leakage correction: reference {a:.4f}, sm_90a {b:.4f} (sigma {sigma:.4f})")
     assert 0.02 < a < 0.98 and abs(a - b) < 6 * sigma + 2e-3, (a, b)
     # and the normalised log-prob uses it: log q - log(acceptance)  (direct_posterior.py:370-386)
     th = theta[:50]

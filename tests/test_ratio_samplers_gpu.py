@@ -123,7 +123,7 @@ def test_nle_mcmc_and_nre_rejection_linear_gaussian(cuda_lib):
 @pytest.mark.parametrize("Dt,Dx,R,shared", [(10, 10, 5000, False), (10, 10, 129, True), (4, 6, 2048, False),
                                             (1, 1, 33, False), (2, 3, 20000, True)])
 def test_ratio_tensor_core_matches_simt_and_oracle(cuda_lib, monkeypatch, Dt, Dx, R, shared):
-    """Logits through the tcgen05 kernel (csrc/ratio_tc.cu, 3xTF32) vs the SIMT kernel (<= 2e-4) and
+    """Logits through the wgmma kernel (csrc/ratio_tc.cu, 3xTF32) vs the SIMT kernel (<= 2e-4) and
     the fp64 oracle (<= 1e-3, the bar of the SIMT test); pairs given directly, by index, or with a
     shared x."""
     ref, est, theta, x = _ratio_pair(Dt, Dx)

@@ -1,6 +1,6 @@
 """Score estimators of sbi_b200/score.py (NPSE, SURVEY 8f-3) against the UNMODIFIED reference classes on the CPU
 (through oracle.ref_shim).  Everything around the network is element-wise torch arithmetic that runs unchanged on
-the device; the network call itself (the sm_100a kernel) is replaced by the reference's own `VectorFieldMLP` with
+the device; the network call itself (the sm_90a kernel) is replaced by the reference's own `VectorFieldMLP` with
 the same weights, so forward / loss / schedules / SDE coefficients must agree exactly, and the divergence algebra
 of `ode_fn_and_divergence` is checked against an autograd trace.  (GPU side: tests/test_score_gpu.py.)"""
 import warnings

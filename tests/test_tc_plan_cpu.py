@@ -1,5 +1,5 @@
 """Host logic of the tensor-core operand packing (pack.NsfLayout.tc_plan / RatioLayout.tc_plan):
-the gather map must reproduce every linear of the network in the K-major no-swizzle UMMA layout
+the gather map must reproduce every linear of the network in the K-major no-swizzle wgmma layout
 [K/4 slabs][N rows][4 floats], hi half then lo half (CPU only; the device side is
 tests/test_nsf_tc_gpu.py / test_ratio_samplers_gpu.py)."""
 import numpy as np
