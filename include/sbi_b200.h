@@ -157,15 +157,15 @@ int sbi_b200_adam_clip_step_norm(float* d_params, const float* d_grad, float* d_
                                  float grad_scale, const float* d_sumsq_part, int n_sumsq,
                                  void* stream);
 
-/* ---- tensor-core bulk evaluation of the NSF (tcgen05 kind::tf32, 3xTF32 split, accumulators in
- * TMEM).  Same function as sbi_b200_nsf_logprob (NFlowsFlow.log_prob,
+/* ---- tensor-core bulk evaluation of the NSF (wgmma tf32, 3xTF32 split, fp32 accumulation).
+ * Same function as sbi_b200_nsf_logprob (NFlowsFlow.log_prob,
  * sbi/neural_nets/estimators/nflows_flow.py:77-97) for large row counts: the ResidualNet linears
  * (nflows ResidualNet; call site sbi/neural_nets/net_builders/flow.py:411-419) run on the tensor
- * cores, one row per TMEM lane, everything else (spline, LU, base density) per thread.
+ * cores, 128 rows per thread block, everything else (spline, LU, base density) per thread.
  *
  * The linears' weights are re-packed from the flat parameter buffer into d_tcw by
  * sbi_b200_nsf_tc_pack (call it whenever d_params changed): per coupling layer a sequence of
- * stages [hi | lo], each half a concatenation of K-major no-swizzle UMMA operand blocks
+ * stages [hi | lo], each half a concatenation of K-major no-swizzle wgmma operand blocks
  * [K/4 slabs][N rows][4 floats] (hi = tf32-rounded weight, lo = weight - hi).
  *   d_src   (n_words,) gather map built by the host (sbi_b200/pack.py NsfLayout.tc_plan):
  *           -1 -> 0 ; s >= 0 -> hi(params[s]) ; s <= -2 -> lo(params[-2-s])
@@ -199,7 +199,7 @@ int sbi_b200_nsf_inverse_tc(const sbi_nsf_model* m, const sbi_nsf_tc* tc, const 
  * backward sweep): the parameter gradients of  sum_r g_r log q(input_r | cond_r)  -- what
  * sbi_b200_nsf_vjp computes with d_ginput == d_gcond == NULL, i.e. NFlowsFlow.loss + autograd backward of a
  * training batch (sbi/neural_nets/estimators/nflows_flow.py:99-109, sbi/inference/trainers/base.py:1171-1180)
- * -- with every conditioner linear (forward, input gradient, weight gradient) on tcgen05.mma kind::tf32.
+ * -- with every conditioner linear (forward, input gradient, weight gradient) on wgmma tf32.
  *   tc_fwd: operand plan of the forward linears (pack.NsfLayout.tc_plan), as for sbi_b200_nsf_logprob_tc;
  *   tc_bwd: operand plan of the transposed linears (pack.NsfLayout.tc_bwd_plan), same descriptor format;
  *           both must have been packed from the current parameters (sbi_b200_nsf_tc_pack);

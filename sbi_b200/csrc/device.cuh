@@ -4,6 +4,8 @@
 #pragma once
 #include <cuda_runtime.h>
 
+#include "../../include/sbi_b200.h"
+
 namespace sbi {
 
 constexpr int kMaxDev = 32;
@@ -42,6 +44,21 @@ inline int dev_num_sms() {
     n[d] = (cudaGetDeviceProperties(&p, d) == cudaSuccess) ? p.multiProcessorCount : 132;
   }
   return n[d];
+}
+
+// Raise the dynamic shared-memory limit of a kernel once per (kernel, size): steady-state
+// launches -- and launches recorded during CUDA-graph capture -- make no attribute calls.  Kernels of
+// the same signature share a type, so each kernel of a translation unit takes its own ID.
+template <int ID, class K>
+static int set_smem(K kernel, int bytes) {
+  static int granted_[kMaxDev] = {0};
+  int& granted = granted_[cur_dev()];
+  if (bytes > 227 * 1024) return SBI_ESMEM;
+  if (bytes <= granted) return 0;
+  cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
+  if (e != cudaSuccess) return (int)e;
+  granted = bytes;
+  return 0;
 }
 
 }  // namespace sbi

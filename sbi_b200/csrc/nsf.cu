@@ -642,20 +642,6 @@ static int check_model(const sbi_nsf_model* m) {
   return 0;
 }
 
-// Raise the dynamic shared-memory limit of a kernel once per (kernel, size): steady-state
-// launches -- and launches recorded during CUDA-graph capture -- make no attribute calls.
-template <int ID, class K>
-static int set_smem(K kernel, int bytes) {
-  static int granted_[sbi::kMaxDev] = {0};
-  int& granted = granted_[sbi::cur_dev()];   // one instance per kernel id (same-signature kernels share a type)
-  if (bytes > 227 * 1024) return SBI_ESMEM;
-  if (bytes <= granted) return 0;
-  cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
-  if (e != cudaSuccess) return (int)e;
-  granted = bytes;
-  return 0;
-}
-
 extern "C" int sbi_b200_abi_version(void) { return SBI_B200_ABI_VERSION; }
 
 extern "C" int sbi_b200_device_ok(void) {

@@ -46,7 +46,7 @@ struct TcSmem {
   int zs, ctx, lds, lum, bias, bias_stride, ring;   // float offsets
   int bar_bytes, total_bytes;
 };
-__host__ __device__ inline TcSmem tc_smem_layout(const sbi_nsf_model& m, int stage_cap, int nslot) {
+__host__ __device__ inline TcSmem tc_smem_layout(const sbi_nsf_model& m, int stage_cap) {
   TcSmem L;
   int fl = 0;
   L.zs = fl;  fl += m.Dp * kRows;
@@ -56,9 +56,9 @@ __host__ __device__ inline TcSmem tc_smem_layout(const sbi_nsf_model& m, int sta
   L.bias_stride = 64 + m.NB * 192 + m.TRmax * 32;
   L.bias = fl; fl += m.T * L.bias_stride;
   fl = (fl + 31) & ~31;
-  L.ring = fl; fl += nslot * stage_cap;
+  L.ring = fl; fl += kSlots * stage_cap;
   L.bar_bytes = fl * 4;
-  L.total_bytes = L.bar_bytes + (nslot + 2) * 8 + 16;
+  L.total_bytes = L.bar_bytes + kSlots * 8;
   return L;
 }
 
@@ -66,10 +66,10 @@ __host__ __device__ inline TcSmem tc_smem_layout(const sbi_nsf_model& m, int sta
 // (which end in the first context columns).  All epilogues are column-wise, so the
 // halves never exchange activations; the spline features of a layer alternate between them.
 //
-// Per coupling layer the tensor core sees these stages (accumulator barrier in brackets):
-//   initial layer -> D [0]
-//   per block:  W_c ctx -> G [1],  W_1 relu(h) -> D [0],  W_2 relu(.) -> D [0]
-//   final layer in passes of <= 2 spline features, pass p -> P_(p&1) [p&1] (two result regions, so
+// Per coupling layer the tensor core sees these stages (result columns after the arrow):
+//   initial layer -> D
+//   per block:  W_c ctx -> G,  W_1 relu(h) -> D,  W_2 relu(.) -> D
+//   final layer in passes of <= 2 spline features, pass p -> P_(p&1) (two result regions, so
 //               pass p + 1 may be computed before the spline of pass p has read its parameters).
 //
 // INV = false: log_prob (logp (R,), optional base-space point `noise` (R,D)).
@@ -94,29 +94,15 @@ nsf_logprob_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_cons
   constexpr int QC = H - NC;        // first column offset of half 1 that is a context column
   static_assert(HP8 % 8 == 0 && NC % 4 == 0 && H > NC && H <= 64, "hidden width");
   extern __shared__ __align__(128) float sm[];
-  const TcSmem L = tc_smem_layout(m, tc.stage_cap, kSlots);
+  const TcSmem L = tc_smem_layout(m, tc.stage_cap);
   uint64_t* full = reinterpret_cast<uint64_t*>(reinterpret_cast<char*>(sm) + L.bar_bytes);
-  uint64_t* bars = full + kSlots;             // two accumulator barriers
-  uint32_t* tbase_s = reinterpret_cast<uint32_t*>(bars + 2);
   const int tid = threadIdx.x, warp = tid >> 5;
   const int C = m.C;
   const int nkc = (H + C + 7) / 8 - KC0;     // K-steps that cover the context columns
   const int64_t ntiles = (rows.R + kRows - 1) / kRows;
   const TcSave SV = tc_save_layout(m.NB, m.TRmax, m.T);
 
-  if (tid == 0) {
-    for (int s = 0; s < kSlots; ++s) mbar_init(&full[s], 1);
-    mbar_init(&bars[0], 1);
-    mbar_init(&bars[1], 1);
-    fence_barrier_init();
-  }
-  if (warp == 0) {
-    store_alloc(tbase_s, kCols, sa);
-  }
-  fence_before();
-  __syncthreads();
-  fence_after();
-  const uint32_t tbase = *tbase_s;
+  Issuer iss = tc_begin<kSlots>(full, sm + L.ring, tc, m.T, ntiles, INV, kCols, sa);
 
   const float* __restrict__ P = m.d_params;
   float* zs = sm + L.zs;
@@ -125,34 +111,16 @@ nsf_logprob_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_cons
   const float* bias_s = sm + L.bias;
   const int half = warp >> 2;                          // which column half of the row
   const int row = ((warp & 3) << 5) | (tid & 31);      // row of the tile = store lane
-  const uint32_t tlane = tbase + ((uint32_t)((warp & 3) * 32) << 16);
   const int cbase = half * NC;                          // first hidden column of this thread
-  const uint32_t tmine = tlane + cbase;
   RqsConst rc = rqs_const(m);
   rc.K = KB;
   const int D = m.D;
-
-  Issuer iss;
-  iss.tbase = __shfl_sync(0xffffffffu, tbase, 0); iss.ring = sm + L.ring; iss.full = full; iss.bars = bars;
-  iss.tcw = tc.d_tcw; iss.tab = tc.d_tab; iss.cap = tc.stage_cap; iss.T = m.T;
-  iss.it = 0; iss.done = 0; iss.fetched = 0; iss.cov0 = iss.cov1 = 0;
-  iss.sbase = 0; iss.lo_off = 0;
-  iss.f_tile = blockIdx.x; iss.ntiles = ntiles; iss.tile_step = gridDim.x; iss.f_l = 0; iss.f_s = 0;
-  iss.reverse = INV;
-  {
-    uint32_t el = 0;
-    asm volatile("{\n\t.reg .pred p;\n\telect.sync _|p, 0xffffffff;\n\tselp.u32 %0, 1, 0, p;\n\t}" : "=r"(el));
-    iss.leader = el != 0;
-  }
-  iss.warp = warp; iss.mine = false;
-  iss.pump();     // first kSlots stages
-  uint32_t bpar = 0u;          // phase parity of the two accumulator barriers (bit b)
 
   // all biases of the conditioners, once per CTA (zero beyond the real widths):
   //   per layer [b0 64 | per block: b1 64, b2 64, bc 64 | bf TRmax*32]
   {
     float* bs = sm + L.bias;
-    for (int e = tid; e < m.T * L.bias_stride; e += kRowThreads) {
+    for (int e = tid; e < m.T * L.bias_stride; e += kThreads) {
       const int l = e / L.bias_stride, o = e % L.bias_stride;
       const int* LT = m.d_layer_tab + l * SBI_NSF_LAYER_STRIDE;
       float v = 0.f;
@@ -183,49 +151,10 @@ nsf_logprob_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_cons
     ld_const = INV ? (-tot - m.ld_zscore) : (tot + m.ld_zscore - 0.5f * (float)D * 1.8378770664093453f);
   }
 
-  // operands written / accumulators read: hand the store over to the MMAs
-  auto hand_over = [&]() {
-    wait_st();
-    fence_before();
-    group_sync();
-  };
-  // wait for the accumulators signalled on barrier b
-  auto wait_acc = [&](int b) {
-    mbar_wait(&bars[b], (bpar >> b) & 1u);
-    bpar ^= 1u << b;
-    __syncwarp();
-    fence_after();
-    iss.passed(b);
-  };
   // A-operand column j of a hidden layer: activation (j < H), context (H <= j < H+C), zero
   auto acol = [&](int j, float act) -> float {
     const int c = j - H;
     return j < H ? act : ((c < C) ? ctx_s[c * kRows + row] : 0.f);
-  };
-
-  // dense LU factors of layer l, zero-padded to 16x16: [U | L | bias 16 | diag 16]
-  auto prep_lu = [&](int l) {
-    const int* LT = m.d_layer_tab + l * SBI_NSF_LAYER_STRIDE;
-    if (!__ldg(LT + SBI_L_HAS_LU)) return;
-    const float* lo = P + __ldg(LT + SBI_L_LU_LOWER);
-    const float* up = P + __ldg(LT + SBI_L_LU_UPPER);
-    const float* dg = P + __ldg(LT + SBI_L_LU_DIAG);
-    const float* bi = P + __ldg(LT + SBI_L_LU_BIAS);
-    float* U = sm + L.lum;
-    float* Lw = U + kLuMax * kLuMax;
-    for (int t = tid; t < kLuMax * kLuMax; t += kRowThreads) {
-      const int i = t / kLuMax, j = t % kLuMax;
-      float u = 0.f, lv = 0.f;
-      if (i < D && j < D) {
-        if (j > i) u = __ldg(up + i * D - i * (i + 1) / 2 + (j - i - 1));
-        else if (j < i) lv = __ldg(lo + i * (i - 1) / 2 + j);
-        else u = softplus_f(__ldg(dg + i)) + 1e-3f;
-      }
-      U[t] = u;
-      Lw[t] = lv;
-      if (j == 0) Lw[kLuMax * kLuMax + i] = (i < D) ? __ldg(bi + i) : 0.f;
-      if (j == i) Lw[kLuMax * kLuMax + kLuMax + i] = (i < D) ? u : 1.f;
-    }
   };
   // this thread's NC columns of a hidden-layer A operand; half 1's last columns are context
   auto write_a = [&](const float (&act)[NC]) {
@@ -238,13 +167,12 @@ nsf_logprob_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_cons
         if (q < QC) a[i] = act[q];
         else a[i] = half ? ((q - QC < C) ? ctx_s[(q - QC) * kRows + row] : 0.f) : act[q];
       }
-      store_a4(tlane, cbase + 4 * g, a);
+      store_a4(row, cbase + 4 * g, a);
     }
   };
   auto read_acc = [&](int region, float (&d)[NC]) {
 #pragma unroll
-    for (int g = 0; g < NG; ++g) ld4(tmine + region + 4 * g, d + 4 * g);
-    wait_ld();
+    for (int g = 0; g < NG; ++g) ld4(row, region + cbase + 4 * g, d + 4 * g);
   };
 
   for (int64_t tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
@@ -253,7 +181,7 @@ nsf_logprob_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_cons
     {
       const float* st = m.d_stats;
       const int Dp = m.Dp, Cp = m.Cp;
-      for (int e = tid; e < kRows * Dp; e += kRowThreads) {
+      for (int e = tid; e < kRows * Dp; e += kThreads) {
         const int r = e / Dp, d = e % Dp;
         const int64_t gr = row0 + r;
         float val = 0.f;
@@ -264,7 +192,7 @@ nsf_logprob_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_cons
         }
         zs[d * kRows + r] = val;
       }
-      for (int e = tid; e < kRows * Cp; e += kRowThreads) {
+      for (int e = tid; e < kRows * Cp; e += kThreads) {
         const int r = e / Cp, c = e % Cp;
         const int64_t gr = row0 + r;
         float val = 0.f;
@@ -274,7 +202,7 @@ nsf_logprob_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_cons
         }
         ctx_s[c * kRows + r] = val;
       }
-      if (INV) prep_lu(m.T - 1);
+      if (INV) prep_lu(m, m.T - 1, sm + L.lum);
       group_sync();
     }
     // context tail columns [HP8, 64) never change within a tile
@@ -284,7 +212,7 @@ nsf_logprob_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_cons
         float v[8];
 #pragma unroll
         for (int i = 0; i < 8; ++i) v[i] = acol(8 * c + i, 0.f);
-        store_a8(tlane, 8 * c, v);
+        store_a8(row, 8 * c, v);
       }
     }
     float ldacc = 0.f;
@@ -352,7 +280,7 @@ nsf_logprob_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_cons
             const int j = 8 * kk + i;
             a[i] = (j < v.n_id) ? zs[__ldg(v.idf + j) * kRows + row] : 0.f;
           }
-          store_a8(tlane, 8 * kk, a);
+          store_a8(row, 8 * kk, a);
         }
       } else {
 #pragma unroll
@@ -360,25 +288,24 @@ nsf_logprob_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_cons
           float a[8];
 #pragma unroll
           for (int i = 0; i < 8; ++i) a[i] = acol(8 * c + i, 0.f);
-          store_a8(tlane, 8 * c, a);
+          store_a8(row, 8 * c, a);
         }
       }
-      hand_over();
+      group_sync();
       {
         iss.begin(__ldg(tab + 5 + 4 * stage));
         uint32_t acc = 0u;
         iss.block(cD, 0, kid8 / 8, 0, 64, acc);
         iss.block(cD, 8 * KC0, nkc, 64 * kid8, 64, acc);
-        iss.end(0);
+        iss.end();
       }
       ++stage;
       SBI_TL(1000 * (li + 1) + 1);
       // dense LU factors: forward needs this layer's after the spline, sampling needs the next
       // processed layer's before its conditioner; either way the previous contents were last
       // read before the barrier above
-      if (!INV) prep_lu(l);
-      else if (l > 0) prep_lu(l - 1);
-      wait_acc(0);
+      if (!INV) prep_lu(m, l, sm + L.lum);
+      else if (l > 0) prep_lu(m, l - 1, sm + L.lum);
       const float* blh = bl + cbase;
       {
         float d[NC];
@@ -401,22 +328,21 @@ nsf_logprob_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_cons
           for (int q = 0; q < NC; ++q) a[q] = relu_f(h[q]);
           write_a(a);
         }
-        hand_over();
+        group_sync();
         {
           uint32_t accg = 0u;
           iss.begin(__ldg(tab + 5 + 4 * stage));
           iss.block(cG, 8 * KC0, nkc, 0, 64, accg);
-          iss.end(1);
+          iss.end();
           uint32_t acc = 0u;
           iss.begin(__ldg(tab + 5 + 4 * (stage + 1)));
           iss.block(cD, 0, NCH, 0, 64, acc);
-          iss.end(0);
+          iss.end();
         }
         stage += 2;
         SBI_TL(1000 * (li + 1) + 10 * b + 13);
-        // gate = sigmoid(Wc ctx + bc) while W1 relu(h) is on the tensor core
+        // gate = sigmoid(Wc ctx + bc)
         float sg[NC];
-        wait_acc(1);
         {
           float g[NC];
           read_acc(cG, g);
@@ -425,7 +351,6 @@ nsf_logprob_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_cons
           if (SAVE) tc_save_cols<NC>(svl + SV.s(b), row, half, sg);
         }
         SBI_TL(1000 * (li + 1) + 10 * b + 14);
-        wait_acc(0);
         {
           float d[NC];
           read_acc(cD, d);
@@ -434,16 +359,15 @@ nsf_logprob_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_cons
           if (SAVE) tc_save_cols<NC>(svl + SV.a1(b), row, half, d);
           write_a(d);
         }
-        hand_over();
+        group_sync();
         {
           uint32_t acc = 0u;
           iss.begin(__ldg(tab + 5 + 4 * stage));
           iss.block(cD, 0, NCH, 0, 64, acc);
-          iss.end(0);
+          iss.end();
         }
         ++stage;
         SBI_TL(1000 * (li + 1) + 10 * b + 15);
-        wait_acc(0);
         {
           // h += (W2 a + b2) * gate
           float d[NC];
@@ -469,25 +393,23 @@ nsf_logprob_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_cons
         const float* bf = bl + 64 + m.NB * 192;
         const int ns = __ldg(tab);
         const int np = ns - stage;            // passes
-        hand_over();
+        group_sync();
         {
           for (int p = 0; p < 2 && p < np; ++p) {
             uint32_t acc = 0u;
             iss.begin(__ldg(tab + 5 + 4 * (stage + p)));
             iss.block(cD + 64 * p, 0, NCH, 0, __ldg(tab + 6 + 4 * (stage + p)), acc);
-            iss.end(p);
+            iss.end();
           }
         }
         SBI_TL(1000 * (li + 1) + 40);
         for (int p = 0; p < np; ++p) {
           const int aux = __ldg(tab + 7 + 4 * (stage + p));
           const int f0 = aux & 0xffff, nf = aux >> 16;
-          wait_acc(p & 1);
           for (int f = 0; f < nf; ++f) {
             if (((f0 + f) & 1) != half) continue;     // warp-uniform: features alternate between halves
             float q[32];
-            ld_cols<4>(tlane + cD + 64 * (p & 1) + 32 * f, q);
-            wait_ld();
+            ld_cols<4>(row, cD + 64 * (p & 1) + 32 * f, q);
             const float* bff = bf + (f0 + f) * 32;
 #pragma unroll
             for (int i = 0; i < 32; ++i) q[i] = (i < 3 * KB - 1) ? q[i] + bff[i] : 0.f;
@@ -503,12 +425,12 @@ nsf_logprob_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_cons
           SBI_TL(1000 * (li + 1) + 41 + p);
           if (p + 2 < np) {
             // region p&1 has been read by everyone: pass p+2 may overwrite it
-            hand_over();
+            group_sync();
             {
               uint32_t acc = 0u;
               iss.begin(__ldg(tab + 5 + 4 * (stage + p + 2)));
               iss.block(cD + 64 * (p & 1), 0, NCH, 0, __ldg(tab + 6 + 4 * (stage + p + 2)), acc);
-              iss.end(p & 1);
+              iss.end();
             }
           }
         }
@@ -590,10 +512,7 @@ nsf_logprob_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_cons
     group_sync();   // rows of the next tile are written cooperatively
   }
 
-  fence_before();
-  group_sync();
-  if (warp == 0)
-    store_dealloc(tbase, kCols, sa);
+  tc_end(kCols, sa);
 }
 
 // the accumulator store of every tensor-core kernel of the library (tc_common.cuh)
@@ -624,12 +543,6 @@ using namespace sbi;
 
 static int tc_num_sms() { return sbi::dev_num_sms(); }
 
-// the weight ring has to fit next to a second CTA on the SM
-static int tc_plan_slots(const sbi_nsf_model* m, const sbi_nsf_tc* tc) {
-  const tc::TcSmem L = tc::tc_smem_layout(*m, tc->stage_cap, tc::kSlots);
-  return L.total_bytes <= 112 * 1024 ? tc::kSlots : 0;
-}
-
 extern "C" int sbi_b200_nsf_tc_supported(const sbi_nsf_model* m, const sbi_nsf_tc* tc) {
   sbi::DeviceGuard dev_guard_(m ? m->d_params : nullptr);
   if (!m || !tc) return 0;
@@ -639,7 +552,8 @@ extern "C" int sbi_b200_nsf_tc_supported(const sbi_nsf_model* m, const sbi_nsf_t
   if (m->IDp > 48 || m->PR > 32 || m->D > tc::kLuMax) return 0;
   if (m->NB < 1 || m->NB > SBI_NSF_MAX_BLOCKS) return 0;
   if (tc->stage_cap <= 0 || (tc->stage_cap & 31) || tc->n_words <= 0) return 0;
-  return tc_plan_slots(m, tc) >= 2 ? 1 : 0;
+  // the weight ring has to fit next to a second CTA on the SM
+  return tc::tc_smem_layout(*m, tc->stage_cap).total_bytes <= 112 * 1024 ? 1 : 0;
 }
 
 extern "C" int sbi_b200_nsf_tc_pack(const sbi_nsf_model* m, const sbi_nsf_tc* tc, void* stream) {
@@ -660,18 +574,11 @@ extern "C" int sbi_b200_nsf_logprob_tc(const sbi_nsf_model* m, const sbi_nsf_tc*
   if (!tc->d_tab || !tc->d_tcw) return SBI_EINVAL;
   if (!sbi_b200_nsf_tc_supported(m, tc)) return SBI_ESMEM;
   if (rows->R == 0) return 0;
-  const int nslot = tc_plan_slots(m, tc);
   tc::StoreArgs sa;
   if (int e = tc::store_args(&sa)) return e;
-  const tc::TcSmem L = tc::tc_smem_layout(*m, tc->stage_cap, nslot);
+  const tc::TcSmem L = tc::tc_smem_layout(*m, tc->stage_cap);
   auto k = tc::nsf_logprob_tc_kernel<50, 10, false>;
-  static int smem_set_[sbi::kMaxDev] = {0};
-  int& smem_set = smem_set_[sbi::cur_dev()];
-  if (smem_set < L.total_bytes) {
-    cudaError_t e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, L.total_bytes);
-    if (e != cudaSuccess) return SBI_ESMEM;
-    smem_set = L.total_bytes;
-  }
+  if (int e = sbi::set_smem<0>(k, L.total_bytes)) return e;
   const int64_t ntiles = (rows->R + tc::kRows - 1) / tc::kRows;
   const int grid = (int)std::min<int64_t>(ntiles, (int64_t)tc_num_sms() * 2);
   k<<<grid, tc::kThreads, L.total_bytes, (cudaStream_t)stream>>>(*m, *tc, *rows, d_logp, d_noise, nullptr, sa);
@@ -680,18 +587,11 @@ extern "C" int sbi_b200_nsf_logprob_tc(const sbi_nsf_model* m, const sbi_nsf_tc*
 
 int sbi::tc::launch_forward_save(const sbi_nsf_model* m, const sbi_nsf_tc* tc, const sbi_rows* rows, float* d_logp,
                                  float* d_save, cudaStream_t s) {
-  const int nslot = tc_plan_slots(m, tc);
   tc::StoreArgs sa;
   if (int e = tc::store_args(&sa)) return e;
-  const tc::TcSmem L = tc::tc_smem_layout(*m, tc->stage_cap, nslot);
+  const tc::TcSmem L = tc::tc_smem_layout(*m, tc->stage_cap);
   auto k = tc::nsf_logprob_tc_kernel<50, 10, false, true>;
-  static int smem_set_[sbi::kMaxDev] = {0};
-  int& smem_set = smem_set_[sbi::cur_dev()];
-  if (smem_set < L.total_bytes) {
-    if (cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, L.total_bytes) != cudaSuccess)
-      return SBI_ESMEM;
-    smem_set = L.total_bytes;
-  }
+  if (int e = sbi::set_smem<1>(k, L.total_bytes)) return e;
   const int grid = (int)((rows->R + tc::kRows - 1) / tc::kRows);      // one tile per CTA: `d_save` slab = blockIdx
   k<<<grid, tc::kThreads, L.total_bytes, s>>>(*m, *tc, *rows, d_logp, nullptr, d_save, sa);
   return (int)cudaGetLastError();
@@ -706,18 +606,11 @@ extern "C" int sbi_b200_nsf_inverse_tc(const sbi_nsf_model* m, const sbi_nsf_tc*
   if (!tc->d_tab || !tc->d_tcw) return SBI_EINVAL;
   if (!sbi_b200_nsf_tc_supported(m, tc)) return SBI_ESMEM;
   if (rows->R == 0) return 0;
-  const int nslot = tc_plan_slots(m, tc);
   tc::StoreArgs sa;
   if (int e = tc::store_args(&sa)) return e;
-  const tc::TcSmem L = tc::tc_smem_layout(*m, tc->stage_cap, nslot);
+  const tc::TcSmem L = tc::tc_smem_layout(*m, tc->stage_cap);
   auto k = tc::nsf_logprob_tc_kernel<50, 10, true>;
-  static int smem_set_[sbi::kMaxDev] = {0};
-  int& smem_set = smem_set_[sbi::cur_dev()];
-  if (smem_set < L.total_bytes) {
-    cudaError_t e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, L.total_bytes);
-    if (e != cudaSuccess) return SBI_ESMEM;
-    smem_set = L.total_bytes;
-  }
+  if (int e = sbi::set_smem<2>(k, L.total_bytes)) return e;
   const int64_t ntiles = (rows->R + tc::kRows - 1) / tc::kRows;
   const int grid = (int)std::min<int64_t>(ntiles, (int64_t)tc_num_sms() * 2);
   k<<<grid, tc::kThreads, L.total_bytes, (cudaStream_t)stream>>>(*m, *tc, *rows, d_logabsdet, d_out, nullptr, sa);

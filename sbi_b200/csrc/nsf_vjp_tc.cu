@@ -71,7 +71,7 @@ __host__ __device__ inline BwdSmem bwd_smem_layout(int stage_cap, int ldmax) {
   fl = (fl + 31) & ~31;
   L.ring = fl; fl += kBwdSlots * stage_cap;
   L.bar_bytes = fl * 4;
-  L.total_bytes = L.bar_bytes + (kBwdSlots + 2 + 2 + 1) * 8 + 16;
+  L.total_bytes = L.bar_bytes + (kBwdSlots + 1) * 8;
   return L;
 }
 __host__ __device__ inline int bwd_ldmax(const sbi_nsf_model& m) {
@@ -87,18 +87,17 @@ struct DwGeo {
   int Mv, N;       // rows of the block incl. zero padding rows (Mv % 4 == 0); accumulator columns (multiple of 16)
 };
 
-// accumulators of one weight-gradient MMA (M = 64: rows 16q .. 16q+15 sit in lanes 0..15 of lane quarter q)
+// accumulators of one weight-gradient MMA (M = 64: rows 16q .. 16q+15 sit in lanes 32q .. 32q+15, mma_ss64)
 // -> the shared-memory image of the block, laid out exactly like the block in the parameter buffer
 // ([Mv][ldw] weights, then the Mv bias entries), from where ONE thread sends it to the CTA's
 // partial-gradient slab with two TMA bulk copies (coalesced, asynchronous; scattered per-lane global
 // stores of the same data cost 1.3 us per weight gradient).  Columns >= nX of a row are padding and take
 // a zero gradient.  One copy of the code for all call sites (the kernel is instruction-fetch bound).
-__device__ __noinline__ void dw_read_fn(uint32_t taddr, const DwGeo g, float* obuf, int mrow, int col0,
+__device__ __noinline__ void dw_read_fn(uint32_t row, uint32_t col, const DwGeo g, float* obuf, int mrow, int col0,
                                         bool holds_rows) {
   if (col0 >= g.N) return;                          // warp-uniform
   float v[32];
-  ld_cols<4>(taddr + col0, v);
-  wait_ld();
+  ld_cols<4>(row, col + col0, v);
   if (holds_rows && mrow < g.Mv) {
     float4* orow = reinterpret_cast<float4*>(obuf + mrow * g.ldw + col0);
     float bv = 0.f;
@@ -130,31 +129,14 @@ nsf_vjp_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_constant
   extern __shared__ __align__(128) float sm[];
   const BwdSmem L = bwd_smem_layout(tcb.stage_cap, bwd_ldmax(m));
   uint64_t* full = reinterpret_cast<uint64_t*>(reinterpret_cast<char*>(sm) + L.bar_bytes);
-  uint64_t* bars = full + kBwdSlots;          // two accumulator barriers of the dX chain
-  uint64_t* dwbar = bars + 2;                 // one barrier per weight-gradient slot
-  uint64_t* obar = dwbar + 2;                 // the output image has been read by its bulk copies
-  uint32_t* tbase_s = reinterpret_cast<uint32_t*>(obar + 1);
+  uint64_t* obar = full + kBwdSlots;          // the output image has been read by its bulk copies
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int C = m.C, D = m.D, Cp = m.Cp, Hp = m.Hp;
   const int64_t ntiles = (rows.R + kRows - 1) / kRows;
   const TcSave SV = tc_save_layout(m.NB, m.TRmax, m.T);
 
-  if (tid == 0) {
-    for (int s = 0; s < kBwdSlots; ++s) mbar_init(&full[s], 1);
-    mbar_init(&bars[0], 1);
-    mbar_init(&bars[1], 1);
-    mbar_init(&dwbar[0], 1);
-    mbar_init(&dwbar[1], 1);
-    mbar_init(obar, 1);
-    fence_barrier_init();
-  }
-  if (warp == 0) {
-    store_alloc(tbase_s, kBwdCols, sa);
-  }
-  fence_before();
-  __syncthreads();
-  fence_after();
-  const uint32_t tbase = *tbase_s;
+  if (tid == 0) mbar_init(obar, 1);
+  IssuerT<kBwdSlots> iss = tc_begin<kBwdSlots>(full, sm + L.ring, tcb, m.T, ntiles, true, kBwdCols, sa);
   SBI_TL(100);
 
   const float* __restrict__ P = m.d_params;
@@ -164,29 +146,12 @@ nsf_vjp_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_constant
   float* stg = sm + L.stg;
   const int half = warp >> 2;
   const int row = ((warp & 3) << 5) | lane;
-  const uint32_t tlane = tbase + ((uint32_t)((warp & 3) * 32) << 16);
   const int cbase = half * NC;
-  const uint32_t tmine = tlane + cbase;
   const int q_one = H - cbase;                 // this thread's column that is X column H (the ones column)
   RqsConst rc = rqs_const(m);
   rc.K = KB;
   float* gp = gpart + (size_t)blockIdx.x * m.n_params;
 
-  IssuerT<kBwdSlots> iss;
-  iss.tbase = __shfl_sync(0xffffffffu, tbase, 0); iss.ring = sm + L.ring; iss.full = full; iss.bars = bars;
-  iss.tcw = tcb.d_tcw; iss.tab = tcb.d_tab; iss.cap = tcb.stage_cap; iss.T = m.T;
-  iss.it = 0; iss.done = 0; iss.fetched = 0; iss.cov0 = iss.cov1 = 0;
-  iss.sbase = 0; iss.lo_off = 0;
-  iss.f_tile = blockIdx.x; iss.ntiles = ntiles; iss.tile_step = gridDim.x; iss.f_l = 0; iss.f_s = 0;
-  iss.reverse = true;
-  {
-    uint32_t el = 0;
-    asm volatile("{\n\t.reg .pred p;\n\telect.sync _|p, 0xffffffff;\n\tselp.u32 %0, 1, 0, p;\n\t}" : "=r"(el));
-    iss.leader = el != 0;
-  }
-  iss.warp = warp; iss.mine = false;
-  iss.pump();
-  uint32_t bpar = 0u;          // phase parity of bars[0], bars[1] (bits 0,1) and dwbar[0], dwbar[1] (bits 2,3)
   uint32_t dwn = 0u;           // weight-gradient MMAs issued so far (slot = dwn & 1, issuing warp = dwn & 7)
   bool pend0 = false, pend1 = false;
   DwGeo geo0, geo1;
@@ -194,18 +159,10 @@ nsf_vjp_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_constant
   geo1 = geo0;
   bool accum = accum_first != 0;
 
+  // operands written (the staging buffers through the generic proxy): hand them over to the MMAs
   auto hand_over = [&]() {
-    wait_st();
     fence_async_smem();
-    fence_before();
     group_sync();
-  };
-  auto wait_acc = [&](int b) {
-    mbar_wait(&bars[b], (bpar >> b) & 1u);
-    bpar ^= 1u << b;
-    __syncwarp();
-    fence_after();
-    iss.passed(b);
   };
   // element (feature n, row) of a transposed staging buffer
   auto st_put = [&](float* buf, int n, float v) { buf[((row >> 2) * kStLd + n) * 4 + (row & 3)] = v; };
@@ -214,14 +171,12 @@ nsf_vjp_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_constant
   bool opend = false;          // the output image holds a block that has not been sent yet
   uint32_t nflush = 0u;        // blocks sent so far (phase of obar)
   DwGeo ogeo = geo0;
-  // make `slot` reusable: wait for the MMA chain that last used it and move its accumulators into the
-  // output image (whose previous block has been read out by then).  The caller passes a CTA barrier
+  // make `slot` reusable: move the accumulators of the MMA chain that last used it into the output
+  // image, once the previous block's bulk copies have read the image.  The caller passes a CTA barrier
   // (hand_over / fence_async_smem + group_sync) and then dw_flush() before the next dw_free.
   auto dw_free = [&](int slot) {
     const bool pend = slot ? pend1 : pend0;
     if (!pend) return;
-    mbar_wait(&dwbar[slot], (bpar >> (2 + slot)) & 1u);
-    bpar ^= 1u << (2 + slot);
     if (nflush > 0u) {
       // the previous block's copies were issued a whole stage ago: they have read the image by now
       if (tid == 0) {
@@ -230,11 +185,8 @@ nsf_vjp_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_constant
       }
       mbar_wait(obar, (nflush - 1u) & 1u);
     }
-    __syncwarp();
-    fence_after();
     ogeo = slot ? geo1 : geo0;
-    dw_read_fn(tlane + cW + 64 * slot, ogeo, obuf, (warp & 3) * 16 + lane, half * 32, lane < 16);
-    fence_before();        // the accumulator reads are ordered before the next MMA into this region
+    dw_read_fn(row, cW + 64 * slot, ogeo, obuf, (warp & 3) * 16 + lane, half * 32, lane < 16);
     if (slot) pend1 = false; else pend0 = false;
     opend = true;
   };
@@ -257,8 +209,8 @@ nsf_vjp_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_constant
       const uint64_t da = make_bdesc(a_s, kStLd * 16u, 128u);
       const uint64_t db = make_bdesc(b_s, kStLd * 16u, 128u);
       const uint64_t dstep = (uint64_t)((2u * kStLd * 16u) >> 4);
-      mma_ss64(g.N, store_col(iss.tbase) + cW + 64 * slot, da, db, dstep, kRows / 8);
-      commit(&dwbar[slot]);
+      mma_ss64(g.N, cW + 64 * slot, da, db, dstep, kRows / 8);
+      group_sync();
     }
     if (slot) { pend1 = true; geo1 = g; } else { pend0 = true; geo0 = g; }
     ++dwn;
@@ -269,35 +221,12 @@ nsf_vjp_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_constant
       float a[4];
 #pragma unroll
       for (int i = 0; i < 4; ++i) a[i] = act[4 * g + i];
-      store_a4(tlane, col0 + cbase + 4 * g, a);
+      store_a4(row, col0 + cbase + 4 * g, a);
     }
   };
   auto read_acc = [&](int region, float (&d)[NC]) {
 #pragma unroll
-    for (int g = 0; g < NG; ++g) ld4(tmine + region + 4 * g, d + 4 * g);
-    wait_ld();
-  };
-  // dense LU factors of layer l, zero-padded to 16x16: [U | L | bias 16 | diag 16]   (as nsf_tc.cu)
-  auto prep_lu = [&](int l) {
-    const int* LT = m.d_layer_tab + l * SBI_NSF_LAYER_STRIDE;
-    if (!__ldg(LT + SBI_L_HAS_LU)) return;
-    const float* lo = P + __ldg(LT + SBI_L_LU_LOWER);
-    const float* up = P + __ldg(LT + SBI_L_LU_UPPER);
-    const float* dg = P + __ldg(LT + SBI_L_LU_DIAG);
-    float* U = sm + L.lum;
-    float* Lw = U + kLuMax * kLuMax;
-    for (int t = tid; t < kLuMax * kLuMax; t += kRowThreads) {
-      const int i = t / kLuMax, j = t % kLuMax;
-      float u = 0.f, lv = 0.f;
-      if (i < D && j < D) {
-        if (j > i) u = __ldg(up + i * D - i * (i + 1) / 2 + (j - i - 1));
-        else if (j < i) lv = __ldg(lo + i * (i - 1) / 2 + j);
-        else u = softplus_f(__ldg(dg + i)) + 1e-3f;
-      }
-      U[t] = u;
-      Lw[t] = lv;
-      if (j == i) Lw[kLuMax * kLuMax + kLuMax + i] = (i < D) ? u : 1.f;
-    }
+    for (int g = 0; g < NG; ++g) ld4(row, region + cbase + 4 * g, d + 4 * g);
   };
 
   int iter = 0;
@@ -310,7 +239,7 @@ nsf_vjp_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_constant
     {
       const float* st = m.d_stats;
       const int Dp = m.Dp;
-      for (int e = tid; e < kRows * Cp; e += kRowThreads) {
+      for (int e = tid; e < kRows * Cp; e += kThreads) {
         const int r = e / Cp, c = e % Cp;
         const int64_t gr = row0 + r;
         float val = 0.f;
@@ -348,7 +277,7 @@ nsf_vjp_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_constant
           dzs[(4 * i + 3) * kRows + row] = live ? -g * t.w : 0.f;
         }
       }
-      prep_lu(m.T - 1);
+      prep_lu(m, m.T - 1, sm + L.lum);
       group_sync();
     }
     SBI_TL(101);
@@ -427,7 +356,7 @@ nsf_vjp_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_constant
         {
           const int o_lo = __ldg(v.LT + SBI_L_LU_LOWER), o_up = __ldg(v.LT + SBI_L_LU_UPPER);
           const int o_dg = __ldg(v.LT + SBI_L_LU_DIAG), o_bi = __ldg(v.LT + SBI_L_LU_BIAS);
-          for (int t = tid; t < D * D + D; t += kRowThreads) {
+          for (int t = tid; t < D * D + D; t += kThreads) {
             float a = 0.f;
             float* dst;
             // dot products over the 128 tile rows, four independent partial sums; every lane reads a
@@ -477,8 +406,8 @@ nsf_vjp_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_constant
           }
           // the arrays are padded to a multiple of 4 entries: padding takes a zero gradient (every
           // entry of the slab is written by this kernel; nothing is zero-filled beforehand)
-          if (!accum && tid >= kRowThreads - 4) {
-            const int k = tid - (kRowThreads - 4);
+          if (!accum && tid >= kThreads - 4) {
+            const int k = tid - (kThreads - 4);
             const int ntri = D * (D - 1) / 2;
             const int o = k == 0 ? o_lo : k == 1 ? o_up : k == 2 ? o_dg : o_bi;
             const int n = k < 2 ? ntri : D;
@@ -502,7 +431,7 @@ nsf_vjp_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_constant
         }
         group_sync();
       }
-      if (l > 0) prep_lu(l - 1);     // next layer's dense factors: first read a whole layer of barriers later
+      if (l > 0) prep_lu(m, l - 1, sm + L.lum);     // next layer's dense factors: first read a whole layer of barriers later
       SBI_TL(1000 * (li + 1) + 1);
 
       // ================= final layer + spline backward, passes of <= 2 features =================
@@ -525,7 +454,6 @@ nsf_vjp_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_constant
             jn = __ldg(v.trf + f + 2);
             xn = tc_load_row16_at(svl + SV.zin, row, jn);
           }
-          if (p >= 2) wait_acc(p & 1);                     // the MMA that read this A set is done
           const int slot = (int)(dwn & 1u);
           dw_free(slot);
           float* As = stg + (2 * slot) * kStFloats;
@@ -539,7 +467,7 @@ nsf_vjp_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_constant
               float a[8];
 #pragma unroll
               for (int i = 0; i < 8; ++i) a[i] = dq[8 * c + i];
-              store_a8(tlane, aset + 32 * half + 8 * c, a);
+              store_a8(row, aset + 32 * half + 8 * c, a);
             }
 #pragma unroll
             for (int i = 0; i < 32; ++i) st_put(As, 32 * half + i, dq[i]);
@@ -553,13 +481,12 @@ nsf_vjp_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_constant
             uint32_t acc = p > 0 ? 1u : 0u;
             iss.begin(__ldg(tab + 5 + 4 * (stage + p)));
             iss.block(cD, aset, 4 * nf, 0, 64, acc);
-            iss.end(p & 1);
+            iss.end();
           }
           DwGeo g;
           g.oW = oWF + 2 * p * m.PR * Hp; g.ldw = Hp; g.oB = oBF + 2 * p * m.PR;
           g.nX = H; g.ones = H; g.Mv = 32 * nf; g.N = 64;
           dw_issue(slot, g);
-        dw_flush();
           dw_flush();
           SBI_TL(1000 * (li + 1) + 10 + p);
         }
@@ -571,7 +498,6 @@ nsf_vjp_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_constant
         tc_load_cols<NC>(svl + SV.s(m.NB - 1), row, half, sv);
         tc_load_cols<NC>(svl + SV.t2(m.NB - 1), row, half, t2);
       }
-      for (int p = max(0, np - 2); p < np; ++p) wait_acc(p & 1);
       float dh[NC];
       read_acc(cD, dh);
       SBI_TL(1000 * (li + 1) + 20);
@@ -601,7 +527,6 @@ nsf_vjp_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_constant
           DwGeo g;
           g.oW = __ldg(BT + 4); g.ldw = Cp; g.oB = __ldg(BT + 5); g.nX = Cp; g.ones = Cp; g.Mv = Hp; g.N = Nc;
           dw_issue(slot, g);
-        dw_flush();
           dw_flush();
         }
         SBI_TL(1000 * (li + 1) + 30 + 10 * b);
@@ -626,20 +551,18 @@ nsf_vjp_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_constant
             uint32_t acc = 0u;
             iss.begin(__ldg(tab + 5 + 4 * stage));
             iss.block(cD, 0, NCH, 0, 64, acc);
-            iss.end(0);
+            iss.end();
           }
           SBI_TL(1000 * (li + 1) + 74 + 10 * b);
           ++stage;
           DwGeo g;
           g.oW = __ldg(BT + 2); g.ldw = Hp; g.oB = __ldg(BT + 3); g.nX = H; g.ones = H; g.Mv = Hp; g.N = 64;
           dw_issue(slot, g);
-        dw_flush();
           dw_flush();
         }
         SBI_TL(1000 * (li + 1) + 31 + 10 * b);
         float hb[NC];
         tc_load_cols<NC>(svl + SV.h(b), row, half, hb);
-        wait_acc(0);
         float dA[NC];
         read_acc(cD, dA);
 #pragma unroll
@@ -662,13 +585,12 @@ nsf_vjp_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_constant
             uint32_t acc = 0u;
             iss.begin(__ldg(tab + 5 + 4 * stage));
             iss.block(cG, 0, NCH, 0, 64, acc);
-            iss.end(1);
+            iss.end();
           }
           ++stage;
           DwGeo g;
           g.oW = __ldg(BT + 0); g.ldw = Hp; g.oB = __ldg(BT + 1); g.nX = H; g.ones = H; g.Mv = Hp; g.N = 64;
           dw_issue(slot, g);
-        dw_flush();
           dw_flush();
         }
         SBI_TL(1000 * (li + 1) + 33 + 10 * b);
@@ -676,7 +598,6 @@ nsf_vjp_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_constant
           tc_load_cols<NC>(svl + SV.s(b - 1), row, half, sv);
           tc_load_cols<NC>(svl + SV.t2(b - 1), row, half, t2);
         }
-        wait_acc(1);
         {
           float d[NC];
           read_acc(cG, d);
@@ -711,7 +632,7 @@ nsf_vjp_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_constant
           uint32_t acc = 0u;
           iss.begin(__ldg(tab + 5 + 4 * stage));
           iss.block(cD, 0, NCH, 0, 16, acc);
-          iss.end(0);
+          iss.end();
         }
         ++stage;
         DwGeo g;
@@ -720,17 +641,14 @@ nsf_vjp_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_constant
         dw_issue(slot, g);
         dw_flush();
         SBI_TL(1000 * (li + 1) + 60);
-        wait_acc(0);
         if (half == 0) {
           float d[16];
-          ld8(tlane + cD, d);
-          ld8(tlane + cD + 8, d + 8);
-          wait_ld();
+          ld8(row, cD, d);
+          ld8(row, cD + 8, d + 8);
 #pragma unroll
           for (int j = 0; j < 16; ++j)
             if (j < v.n_id) dzs[__ldg(v.idf + j) * kRows + row] += d[j];
         }
-        fence_before();
         group_sync();
       }
     }
@@ -746,10 +664,7 @@ nsf_vjp_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_constant
   SBI_TL(9001);
 
   if (tid == 0) bulk_wait_all();
-  fence_before();
-  group_sync();
-  if (warp == 0)
-    store_dealloc(tbase, kBwdCols, sa);
+  tc_end(kBwdCols, sa);
 }
 
 }  // namespace tc
@@ -801,15 +716,7 @@ extern "C" int sbi_b200_nsf_vjp_tc(const sbi_nsf_model* m, const sbi_nsf_tc* tc_
   cudaStream_t s = (cudaStream_t)stream;
   const tc::BwdSmem Lb = tc::bwd_smem_layout(tc_bwd->stage_cap, tc::bwd_ldmax(*m));
   auto kb = tc::nsf_vjp_tc_kernel<50, 10>;
-  {
-    static int set_b_[sbi::kMaxDev] = {0};
-    int& set_b = set_b_[sbi::cur_dev()];
-    if (set_b < Lb.total_bytes) {
-      if (cudaFuncSetAttribute(kb, cudaFuncAttributeMaxDynamicSharedMemorySize, Lb.total_bytes) != cudaSuccess)
-        return SBI_ESMEM;
-      set_b = Lb.total_bytes;
-    }
-  }
+  if (int e = sbi::set_smem<0>(kb, Lb.total_bytes)) return e;
   // chunks of one tile per SM: forward sweep (saves activations) then backward sweep of the same rows;
   // later chunks accumulate into the partial-gradient slabs
   tc::StoreArgs sa;

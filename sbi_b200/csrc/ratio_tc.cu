@@ -33,7 +33,7 @@ __host__ __device__ inline RatioTcSmem ratio_tc_smem_layout(const sbi_ratio_mode
   fl = (fl + 31) & ~31;
   L.ring = fl; fl += kSlots * stage_cap;
   L.bar_bytes = fl * 4;
-  L.total_bytes = L.bar_bytes + (kSlots + 2) * 8 + 16;
+  L.total_bytes = L.bar_bytes + kSlots * 8;
   return L;
 }
 
@@ -49,56 +49,24 @@ ratio_forward_tc_kernel(const __grid_constant__ sbi_ratio_model m, const __grid_
   extern __shared__ __align__(128) float sm[];
   const RatioTcSmem L = ratio_tc_smem_layout(m, tc.stage_cap);
   uint64_t* full = reinterpret_cast<uint64_t*>(reinterpret_cast<char*>(sm) + L.bar_bytes);
-  uint64_t* bars = full + kSlots;
-  uint32_t* tbase_s = reinterpret_cast<uint32_t*>(bars + 2);
   const int tid = threadIdx.x, warp = tid >> 5;
   const int64_t ntiles = (pr.R + kRows - 1) / kRows;
 
-  if (tid == 0) {
-    for (int s = 0; s < kSlots; ++s) mbar_init(&full[s], 1);
-    mbar_init(&bars[0], 1);
-    mbar_init(&bars[1], 1);
-    fence_barrier_init();
-  }
-  if (warp == 0) {
-    store_alloc(tbase_s, kCols, sa);
-  }
-  fence_before();
-  __syncthreads();
-  fence_after();
-  const uint32_t tbase = *tbase_s;
+  Issuer iss = tc_begin<kSlots>(full, sm + L.ring, tc, 1, ntiles, false, kCols, sa);
 
   const float* __restrict__ P = m.d_params;
   const int* T = m.d_tab;
   float* us = sm + L.us;
   const int half = warp >> 2;
   const int row = ((warp & 3) << 5) | (tid & 31);
-  const uint32_t tlane = tbase + ((uint32_t)((warp & 3) * 32) << 16);
   const int cbase = half * NC;
-  const uint32_t tmine = tlane + cbase;
   const int K0 = m.Dt + m.Dx;
   const int k0p8 = __ldg(tc.d_tab + 1);
-
-  Issuer iss;
-  iss.tbase = __shfl_sync(0xffffffffu, tbase, 0); iss.ring = sm + L.ring; iss.full = full; iss.bars = bars;
-  iss.tcw = tc.d_tcw; iss.tab = tc.d_tab; iss.cap = tc.stage_cap; iss.T = 1;
-  iss.it = 0; iss.done = 0; iss.fetched = 0; iss.cov0 = iss.cov1 = 0;
-  iss.sbase = 0; iss.lo_off = 0;
-  iss.f_tile = blockIdx.x; iss.ntiles = ntiles; iss.tile_step = gridDim.x; iss.f_l = 0; iss.f_s = 0;
-  iss.reverse = false;
-  {
-    uint32_t el = 0;
-    asm volatile("{\n\t.reg .pred p;\n\telect.sync _|p, 0xffffffff;\n\tselp.u32 %0, 1, 0, p;\n\t}" : "=r"(el));
-    iss.leader = el != 0;
-  }
-  iss.warp = warp; iss.mine = false;
-  iss.pump();
-  uint32_t bpar = 0u;
 
   // biases once per CTA (zero beyond the real width): [b0 64 | per block b1 64, b2 64 | bf]
   {
     float* bs = sm + L.bias;
-    for (int e = tid; e < 64 + m.NB * 128 + 1; e += kRowThreads) {
+    for (int e = tid; e < 64 + m.NB * 128 + 1; e += kThreads) {
       float v = 0.f;
       if (e < 64) {
         if (e < H) v = __ldg(P + __ldg(T + SBI_R_B0) + e);
@@ -113,37 +81,24 @@ ratio_forward_tc_kernel(const __grid_constant__ sbi_ratio_model m, const __grid_
   }
   const float* bl = sm + L.bias + cbase;
 
-  auto hand_over = [&]() {
-    wait_st();
-    fence_before();
-    group_sync();
-  };
-  auto wait_acc = [&](int b) {
-    mbar_wait(&bars[b], (bpar >> b) & 1u);
-    bpar ^= 1u << b;
-    __syncwarp();
-    fence_after();
-    iss.passed(b);
-  };
   auto write_a = [&](const float (&act)[NC]) {
 #pragma unroll
     for (int g = 0; g < NG; ++g) {
       float a[4];
 #pragma unroll
       for (int i = 0; i < 4; ++i) a[i] = act[4 * g + i];
-      store_a4(tlane, cbase + 4 * g, a);
+      store_a4(row, cbase + 4 * g, a);
     }
   };
   auto read_acc = [&](float (&d)[NC]) {
 #pragma unroll
-    for (int g = 0; g < NG; ++g) ld4(tmine + cD + 4 * g, d + 4 * g);
-    wait_ld();
+    for (int g = 0; g < NG; ++g) ld4(row, cD + cbase + 4 * g, d + 4 * g);
   };
   auto run_stage = [&](int stage, int nk, int N) {
     uint32_t acc = 0u;
     iss.begin(__ldg(tc.d_tab + 5 + 4 * stage));
     iss.block(cD, 0, nk, 0, N, acc);
-    iss.end(0);
+    iss.end();
   };
 
   for (int64_t tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
@@ -152,7 +107,7 @@ ratio_forward_tc_kernel(const __grid_constant__ sbi_ratio_model m, const __grid_
     {
       const float* __restrict__ st = m.d_stats;
       const int Dt = m.Dt, Dx = m.Dx, Dtp = m.Dtp, Dxp = m.Dxp;
-      for (int e = tid; e < kRows * Dtp; e += kRowThreads) {
+      for (int e = tid; e < kRows * Dtp; e += kThreads) {
         const int r = e / Dtp, d = e % Dtp;
         const int64_t gr = row0 + r;
         float val = 0.f;
@@ -162,7 +117,7 @@ ratio_forward_tc_kernel(const __grid_constant__ sbi_ratio_model m, const __grid_
         }
         if (d < Dt) us[d * kRows + r] = val;
       }
-      for (int e = tid; e < kRows * Dxp; e += kRowThreads) {
+      for (int e = tid; e < kRows * Dxp; e += kThreads) {
         const int r = e / Dxp, d = e % Dxp;
         const int64_t gr = row0 + r;
         float val = 0.f;
@@ -182,11 +137,10 @@ ratio_forward_tc_kernel(const __grid_constant__ sbi_ratio_model m, const __grid_
         const int j = 8 * c + i;
         a[i] = (j < K0) ? us[j * kRows + row] : 0.f;
       }
-      store_a8(tlane, 8 * c, a);
+      store_a8(row, 8 * c, a);
     }
-    hand_over();
+    group_sync();
     run_stage(0, k0p8 / 8, 64);
-    wait_acc(0);
     float h[NC];
     {
       float d[NC];
@@ -204,9 +158,8 @@ ratio_forward_tc_kernel(const __grid_constant__ sbi_ratio_model m, const __grid_
         for (int q = 0; q < NC; ++q) a[q] = relu_f(h[q]);
         write_a(a);
       }
-      hand_over();
+      group_sync();
       run_stage(stage++, NCH, 64);
-      wait_acc(0);
       {
         float d[NC];
         read_acc(d);
@@ -214,9 +167,8 @@ ratio_forward_tc_kernel(const __grid_constant__ sbi_ratio_model m, const __grid_
         for (int q = 0; q < NC; ++q) d[q] = relu_f(d[q] + b1[q]);
         write_a(d);
       }
-      hand_over();
+      group_sync();
       run_stage(stage++, NCH, 64);
-      wait_acc(0);
       {
         float d[NC];
         read_acc(d);
@@ -226,23 +178,17 @@ ratio_forward_tc_kernel(const __grid_constant__ sbi_ratio_model m, const __grid_
     }
     // ---- final layer: logit = w_f . h + b_f as column 0 of an N = 16 MMA ----
     write_a(h);
-    hand_over();
+    group_sync();
     run_stage(stage, NCH, 16);
-    wait_acc(0);
     if (half == 0) {
       float d[4];
-      ld4(tlane + cD, d);
-      wait_ld();
+      ld4(row, cD, d);
       if (row0 + row < pr.R) logits[row0 + row] = d[0] + sm[L.bias + 64 + m.NB * 128];
     }
-    fence_before();
     group_sync();   // us and the accumulators are reused by the next tile
   }
 
-  fence_before();
-  group_sync();
-  if (warp == 0)
-    store_dealloc(tbase, kCols, sa);
+  tc_end(kCols, sa);
 }
 
 }  // namespace tc
@@ -282,13 +228,7 @@ extern "C" int sbi_b200_ratio_forward_tc(const sbi_ratio_model* m, const sbi_nsf
   tc::StoreArgs sa;
   if (int e = tc::store_args(&sa)) return e;
   auto k = tc::ratio_forward_tc_kernel<50>;
-  static int smem_set_[sbi::kMaxDev] = {0};
-  int& smem_set = smem_set_[sbi::cur_dev()];
-  if (smem_set < L.total_bytes) {
-    if (cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, L.total_bytes) != cudaSuccess)
-      return SBI_ESMEM;
-    smem_set = L.total_bytes;
-  }
+  if (int e = sbi::set_smem<0>(k, L.total_bytes)) return e;
   const int64_t ntiles = (pairs->R + tc::kRows - 1) / tc::kRows;
   const int grid = (int)std::min<int64_t>(ntiles, (int64_t)rtc_num_sms() * 2);
   k<<<grid, tc::kThreads, L.total_bytes, (cudaStream_t)stream>>>(*m, *tc, *pairs, d_logits, sa);

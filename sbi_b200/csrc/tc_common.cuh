@@ -30,22 +30,22 @@ static __device__ int g_tl_n;
 #endif
 
 constexpr int kRows = 128;        // rows per tile
-constexpr int kRowThreads = 256;  // two threads per row (column halves)
-constexpr int kThreads = 256;     // 8 row warps, which also take turns issuing MMAs and TMA copies
+constexpr int kThreads = 256;     // 8 warps, two threads per row (column halves); all issue the MMAs
 constexpr int kLuMax = 16;        // LULinear runs on register-resident rows of <= 16 features
 constexpr int kSlots = 3;         // weight ring: up to two stages in use + one prefetched
 constexpr int kCols = 256;        // accumulator-store columns per CTA
 constexpr int cAhi = 0, cAlo = 64, cD = 128, cG = 192;
 
 // ---- accumulator store --------------------------------------------------------------------------
-// The kernels address their MMA operands and accumulators as (slot << 23) | (lane << 16) | column,
-// lane = tile row (128 lanes).  Hopper keeps wgmma accumulators in registers, and an SM's shared memory
-// is taken by the weight ring and the staging buffers, so the operand / accumulator columns live in
-// global memory: kStoreSlots slabs of kStoreCols columns x 128 lanes (lane-contiguous, so the 32 threads
-// of a warp touch one 128-byte line per column; 34.6 MB per device, defined once in nsf_tc.cu and
-// mostly L2-resident while a kernel runs), handed out in 64-column units through one mask per slab.
-// A CTA picks the slab of the SM it starts on (for locality only) and records the slot in its column
-// base; every later address comes from that record, so a CTA that resumes on another SM keeps its slab.
+// The kernels keep their MMA A operands and accumulators in columns of 128 lanes, lane = tile row.
+// Hopper keeps wgmma accumulators in registers, and an SM's shared memory is taken by the weight ring
+// and the staging buffers, so the columns live in global memory: kStoreSlots slabs of kStoreCols
+// columns x 128 lanes (lane-contiguous, so the 32 threads of a warp touch one 128-byte line per column;
+// 34.6 MB per device, defined once in nsf_tc.cu and mostly L2-resident while a kernel runs), handed out
+// in 64-column units through one mask per slab.  A CTA picks the slab of the SM it starts on (for
+// locality only) and records the slab and its first column in s_store / s_store_col; every later address
+// comes from that record, so a CTA that resumes on another SM keeps its columns.  The kernels index
+// columns relative to their first column.
 constexpr int kStoreCols = 512;
 constexpr int kStoreLanes = 128;
 constexpr int kStoreSlots = 132;  // one per H100 SXM SM; SMs with larger ids share slabs through the masks
@@ -56,18 +56,18 @@ struct StoreArgs {
 // the device's slabs and masks (host; defined in nsf_tc.cu); returns a cudaError_t
 int store_args(StoreArgs* out);
 
-static __shared__ float* s_store_slab;     // this CTA's slab, set by store_alloc
+static __shared__ float* s_store;          // this CTA's slab, set by store_alloc
+static __shared__ uint32_t s_store_col;    // first column of this CTA in its slab, set by store_alloc
 
-__device__ __forceinline__ float* store_slab() { return s_store_slab; }
-// element (column, lane) of this CTA's slab
-__device__ __forceinline__ float* store_at(uint32_t col, uint32_t lane) {
-  return s_store_slab + (size_t)col * kStoreLanes + lane;
+// element (row, column) of this CTA's columns
+__device__ __forceinline__ float* store_at(uint32_t row, uint32_t col) {
+  return s_store + ((s_store_col + col) * kStoreLanes + row);
 }
-// warp 0 of the CTA, before the CTA barrier that publishes *dst: reserve `ncols` (multiple of 64,
-// <= kStoreCols) columns of a slab; the column base (slot in bits 23+) goes to *dst.  Spins while
-// other CTAs hold the columns.  A waiting CTA holds no columns (a reservation is one CAS of all its
-// units), and a holder waits on no other CTA before it releases, so the wait cannot form a cycle.
-__device__ __forceinline__ void store_alloc(uint32_t* dst, int ncols, const StoreArgs& sa) {
+// warp 0 of the CTA, before the CTA barrier that publishes s_store / s_store_col: reserve `ncols`
+// (multiple of 64, <= kStoreCols) columns of a slab.  Spins while other CTAs hold the columns.  A
+// waiting CTA holds no columns (a reservation is one CAS of all its units), and a holder waits on no
+// other CTA before it releases, so the wait cannot form a cycle.
+__device__ __forceinline__ void store_alloc(int ncols, const StoreArgs& sa) {
   if ((threadIdx.x & 31) == 0) {
     uint32_t sm;
     asm volatile("mov.u32 %0, %%smid;" : "=r"(sm));
@@ -82,8 +82,8 @@ __device__ __forceinline__ void store_alloc(uint32_t* dst, int ncols, const Stor
         if (!(cur & (want << p))) { pos = p; break; }
       if (pos >= 0 && atomicCAS(mk, cur, cur | (want << pos)) == cur) {
         __threadfence();
-        *dst = (slot << 23) | ((uint32_t)pos * 64u);
-        s_store_slab = sa.slab + (size_t)slot * kStoreCols * kStoreLanes;
+        s_store = sa.slab + (size_t)slot * kStoreCols * kStoreLanes;
+        s_store_col = (uint32_t)pos * 64u;
         break;
       }
       __nanosleep(200);
@@ -91,28 +91,14 @@ __device__ __forceinline__ void store_alloc(uint32_t* dst, int ncols, const Stor
   }
   __syncwarp();
 }
-__device__ __forceinline__ void store_dealloc(uint32_t base, int ncols, const StoreArgs& sa) {
+// warp 0 of the CTA, after the CTA barrier that ends the last use of the columns: release them
+__device__ __forceinline__ void store_dealloc(int ncols, const StoreArgs& sa) {
   if ((threadIdx.x & 31) == 0) {
+    const size_t slot = (size_t)(s_store - sa.slab) / ((size_t)kStoreCols * kStoreLanes);
     __threadfence();
-    atomicAnd(sa.mask + (base >> 23), ~(((1u << (ncols / 64)) - 1u) << ((base & 0xffffu) / 64)));
+    atomicAnd(sa.mask + slot, ~(((1u << (ncols / 64)) - 1u) << (s_store_col / 64)));
   }
   __syncwarp();
-}
-// column and lane fields of a store address
-__device__ __forceinline__ uint32_t store_col(uint32_t taddr) { return taddr & 0xffffu; }
-__device__ __forceinline__ uint32_t store_lane(uint32_t taddr) { return (taddr >> 16) & 0x7fu; }
-
-// ordering points of the row-tile protocol: the accumulator store is ordinary global memory, which the
-// CTA barriers and mbarriers around these calls already order
-__device__ __forceinline__ void fence_before() { asm volatile("" ::: "memory"); }
-__device__ __forceinline__ void fence_after() { asm volatile("" ::: "memory"); }
-__device__ __forceinline__ void wait_ld() { asm volatile("" ::: "memory"); }
-__device__ __forceinline__ void wait_st() { asm volatile("" ::: "memory"); }
-// completion of the MMAs issued since the last one: they ran synchronously on all 256 threads, so one
-// CTA barrier and one arrival make their accumulators visible to whoever waits on `bar`
-__device__ __forceinline__ void commit(uint64_t* bar) {
-  asm volatile("bar.sync 1, 256;" ::: "memory");
-  if (threadIdx.x == 0) mbar_arrive(bar);
 }
 
 // shared-memory operand descriptor of wgmma, no swizzle (interleave), K-major: core matrix = 8 rows x
@@ -124,24 +110,24 @@ __device__ __forceinline__ uint64_t make_bdesc(uint32_t saddr, uint32_t lbo, uin
   d |= (uint64_t)((sbo >> 4) & 0x3fff) << 32;
   return d;
 }
-// 8 / 4 consecutive columns of the thread's lane (lane = taddr's lane field + lane id)
-__device__ __forceinline__ void st8(uint32_t taddr, const float (&v)[8]) {
-  float* p = store_at(store_col(taddr), store_lane(taddr) + (threadIdx.x & 31));
+// 8 / 4 consecutive columns [col, col + 8 / 4) of tile row `row`
+__device__ __forceinline__ void st8(uint32_t row, uint32_t col, const float (&v)[8]) {
+  float* p = store_at(row, col);
 #pragma unroll
   for (int i = 0; i < 8; ++i) p[i * kStoreLanes] = v[i];
 }
-__device__ __forceinline__ void ld8(uint32_t taddr, float* v) {
-  const float* p = store_at(store_col(taddr), store_lane(taddr) + (threadIdx.x & 31));
+__device__ __forceinline__ void ld8(uint32_t row, uint32_t col, float* v) {
+  const float* p = store_at(row, col);
 #pragma unroll
   for (int i = 0; i < 8; ++i) v[i] = p[i * kStoreLanes];
 }
-__device__ __forceinline__ void st4(uint32_t taddr, const float (&v)[4]) {
-  float* p = store_at(store_col(taddr), store_lane(taddr) + (threadIdx.x & 31));
+__device__ __forceinline__ void st4(uint32_t row, uint32_t col, const float (&v)[4]) {
+  float* p = store_at(row, col);
 #pragma unroll
   for (int i = 0; i < 4; ++i) p[i * kStoreLanes] = v[i];
 }
-__device__ __forceinline__ void ld4(uint32_t taddr, float* v) {
-  const float* p = store_at(store_col(taddr), store_lane(taddr) + (threadIdx.x & 31));
+__device__ __forceinline__ void ld4(uint32_t row, uint32_t col, float* v) {
+  const float* p = store_at(row, col);
 #pragma unroll
   for (int i = 0; i < 4; ++i) v[i] = p[i * kStoreLanes];
 }
@@ -157,7 +143,9 @@ __device__ __forceinline__ void mma_rows_n(uint32_t dcol, uint32_t ahcol, uint32
                                            uint64_t dl, uint64_t dstep, int nk, uint32_t acc) {
   const int lane = threadIdx.x & 31, g = lane >> 2, t = lane & 3;
   const uint32_t r0 = (threadIdx.x >> 7) * 64 + ((threadIdx.x >> 5) & 3) * 16 + g;
-  float* slab = store_slab();
+  const uint32_t c0 = s_store_col;
+  dcol += c0; ahcol += c0; alcol += c0;
+  float* slab = s_store;
   float d[N / 2];
 #pragma unroll
   for (int j = 0; j < N / 8; ++j) {
@@ -217,17 +205,18 @@ __device__ __forceinline__ void mma_rows(int N, uint32_t dcol, uint32_t ahcol, u
   }
 }
 
-// D[store, M = 64] = A[smem]^T-staged * B[smem]^T over nk K-steps, single TF32 pass.  Row r of D sits
-// in lane 32 (r / 16) + r % 16 (the lane map of an M = 64 tensor-memory accumulator); warpgroup wg
-// computes columns [wg N/2, (wg + 1) N/2) (N % 16 == 0).
+// D[store, M = 64] = A[smem]^T-staged * B[smem]^T over nk K-steps, single TF32 pass.  Rows 16q .. 16q+15
+// of D go to lanes 32q .. 32q+15 of the store, so that lanes 0..15 of warp q of each warpgroup read
+// them back as their own tile rows (dw_read_fn, nsf_vjp_tc.cu); warpgroup wg computes columns
+// [wg N/2, (wg + 1) N/2) (N % 16 == 0).
 template <int NH>
 __device__ __forceinline__ void mma_ss64_n(uint32_t dcol, uint64_t da, uint64_t db, uint64_t dstep, int nk) {
   const int lane = threadIdx.x & 31, g = lane >> 2, t = lane & 3;
   const int wg = threadIdx.x >> 7;
   const uint32_t l0 = ((threadIdx.x >> 5) & 3) * 32 + g;
   db += (uint64_t)((wg * NH / 8) * 128 >> 4);      // 8-row groups of B are 128 B apart
-  dcol += wg * NH;
-  float* slab = store_slab();
+  dcol += s_store_col + wg * NH;
+  float* slab = s_store;
   float d[NH / 2];
 #pragma unroll
   for (int i = 0; i < NH / 2; ++i) d[i] = 0.f;
@@ -262,9 +251,9 @@ __device__ __forceinline__ void mma_ss64(int N, uint32_t dcol, uint64_t da, uint
   }
 }
 template <int NCHUNK>
-__device__ __forceinline__ void ld_cols(uint32_t taddr, float* v) {
+__device__ __forceinline__ void ld_cols(uint32_t row, uint32_t col, float* v) {
 #pragma unroll
-  for (int c = 0; c < NCHUNK; ++c) ld8(taddr + 8 * c, v + 8 * c);
+  for (int c = 0; c < NCHUNK; ++c) ld8(row, col + 8 * c, v + 8 * c);
 }
 
 // hi = x rounded to tf32 (10 explicit mantissa bits, round half away in the integer domain),
@@ -273,22 +262,49 @@ __device__ __forceinline__ void split_tf32(float x, float& hi, float& lo) {
   hi = __uint_as_float((__float_as_uint(x) + 0x1000u) & 0xffffe000u);
   lo = x - hi;
 }
-// split 8 values and put them into A_hi / A_lo columns [col, col+8) of the thread's lane
-__device__ __forceinline__ void store_a8(uint32_t tlane, int col, const float (&v)[8]) {
+// split 8 values and put them into A_hi / A_lo columns [col, col+8) of tile row `row`
+__device__ __forceinline__ void store_a8(uint32_t row, int col, const float (&v)[8]) {
   float hi[8], lo[8];
 #pragma unroll
   for (int i = 0; i < 8; ++i) split_tf32(v[i], hi[i], lo[i]);
-  st8(tlane + cAhi + col, hi);
-  st8(tlane + cAlo + col, lo);
+  st8(row, cAhi + col, hi);
+  st8(row, cAlo + col, lo);
 }
-__device__ __forceinline__ void store_a4(uint32_t tlane, int col, const float (&v)[4]) {
+__device__ __forceinline__ void store_a4(uint32_t row, int col, const float (&v)[4]) {
   float hi[4], lo[4];
 #pragma unroll
   for (int i = 0; i < 4; ++i) split_tf32(v[i], hi[i], lo[i]);
-  st4(tlane + cAhi + col, hi);
-  st4(tlane + cAlo + col, lo);
+  st4(row, cAhi + col, hi);
+  st4(row, cAlo + col, lo);
 }
 __device__ __forceinline__ void group_sync() { asm volatile("bar.sync 1, 256;" ::: "memory"); }
+
+// dense LU factors of NSF layer l, zero-padded to 16x16, into lum = [U | L | bias 16 | diag 16]
+// (all threads; the unit diagonal of L is implicit)
+__device__ __forceinline__ void prep_lu(const sbi_nsf_model& m, int l, float* lum) {
+  const int* LT = m.d_layer_tab + l * SBI_NSF_LAYER_STRIDE;
+  if (!__ldg(LT + SBI_L_HAS_LU)) return;
+  const int D = m.D;
+  const float* lo = m.d_params + __ldg(LT + SBI_L_LU_LOWER);
+  const float* up = m.d_params + __ldg(LT + SBI_L_LU_UPPER);
+  const float* dg = m.d_params + __ldg(LT + SBI_L_LU_DIAG);
+  const float* bi = m.d_params + __ldg(LT + SBI_L_LU_BIAS);
+  float* U = lum;
+  float* Lw = U + kLuMax * kLuMax;
+  for (int t = threadIdx.x; t < kLuMax * kLuMax; t += kThreads) {
+    const int i = t / kLuMax, j = t % kLuMax;
+    float u = 0.f, lv = 0.f;
+    if (i < D && j < D) {
+      if (j > i) u = __ldg(up + i * D - i * (i + 1) / 2 + (j - i - 1));
+      else if (j < i) lv = __ldg(lo + i * (i - 1) / 2 + j);
+      else u = softplus_f(__ldg(dg + i)) + 1e-3f;
+    }
+    U[t] = u;
+    Lw[t] = lv;
+    if (j == 0) Lw[kLuMax * kLuMax + i] = (i < D) ? __ldg(bi + i) : 0.f;
+    if (j == i) Lw[kLuMax * kLuMax + kLuMax + i] = (i < D) ? u : 1.f;
+  }
+}
 
 // ---- weight re-pack: flat fp32 parameters -> [hi | lo] wgmma operand blocks --------------------
 static __global__ void tc_pack_kernel(const float* __restrict__ params, const int32_t* __restrict__ src,
@@ -310,34 +326,29 @@ static __global__ void tc_pack_kernel(const float* __restrict__ params, const in
 }
 
 // ---- the kernel ------------------------------------------------------------------------------------
-// Every thread runs begin / block / end: the MMAs of a stage take both warpgroups and complete
-// before end() returns.  The weight stream rotates between the warps (stage k is fetched by the
-// elected lane of warp (k + 4) % 8).  Stage k lives in ring slot k % kSlots.  A stage is fetched
-// (TMA bulk copy, completion on full[slot]) as soon as the stage that used its slot kSlots stages
-// earlier is known to be complete, which every warp learns each time it passes an accumulator
-// barrier.
+// Every thread runs begin / block / end: the MMAs of a stage take both warpgroups and are complete
+// once end() returns.  The weight stream rotates between the warps (stage k is fetched by the
+// elected lane of warp (k + 4) % 8).  Stage k lives in ring slot k % NSLOT.  A stage is fetched
+// (TMA bulk copy, completion on full[slot]) by the end() of the stage that used its slot NSLOT stages
+// earlier.
 template <int NSLOT>
 struct IssuerT {
-  uint32_t tbase;       // accumulator-store base (slot, lane 0, column 0)
   bool leader;          // the elected lane of this warp
   int warp;             // this warp; stage k is fetched by warp (k+4) % 8
-  bool mine;            // (kept true: every warp takes part in every stage)
   float* ring;
-  uint64_t *full, *bars;
+  uint64_t* full;
   const float* tcw;
   const int32_t* tab;   // stage table (all layers)
   int cap, T;
-  uint32_t it;          // stages issued
-  uint32_t done;        // stages known complete
+  uint32_t it;          // stages issued (and complete)
   uint32_t fetched;     // stages fetched
-  uint32_t cov0, cov1;  // stages covered by the last commit on each accumulator barrier
   uint32_t sbase, lo_off;   // current stage: shared address of the hi half, byte offset of lo half
   int64_t f_tile, ntiles, tile_step;   // next stage to fetch
   int f_l, f_s;
   bool reverse;         // layers are walked T-1 .. 0 (sampling direction)
 
   __device__ __forceinline__ void pump() {
-    while (fetched < done + NSLOT && f_tile < ntiles) {
+    while (fetched < it + NSLOT && f_tile < ntiles) {
       const int32_t* t = tab + (reverse ? T - 1 - f_l : f_l) * SBI_NSF_TC_STRIDE;
       const int off = __ldg(t + 4 + 4 * f_s), nfl = __ldg(t + 5 + 4 * f_s);
       const uint32_t slot = fetched % NSLOT;
@@ -352,9 +363,7 @@ struct IssuerT {
       }
     }
   }
-  // every thread of the CTA runs begin / block / end: the MMAs take both warpgroups
   __device__ __forceinline__ void begin(int stage_floats) {
-    mine = true;
     const uint32_t s = it % NSLOT;
     mbar_wait(&full[s], (it / NSLOT) & 1u);
     sbase = smem_u32(ring + (size_t)s * cap);
@@ -367,24 +376,49 @@ struct IssuerT {
     const uint64_t dh = make_bdesc(bh, slab, 128u);
     const uint64_t dl = make_bdesc(bh + lo_off, slab, 128u);
     const uint64_t dstep = (uint64_t)((2u * slab) >> 4);    // start-address field advance per K-step
-    const uint32_t col0 = store_col(tbase);
-    if (nk > 0) mma_rows(N, col0 + dcol, col0 + cAhi + a0, col0 + cAlo + a0, dh, dl, dstep, nk, acc);
+    if (nk > 0) mma_rows(N, dcol, cAhi + a0, cAlo + a0, dh, dl, dstep, nk, acc);
     if (nk > 0) acc = 1u;
   }
-  // close the stage: its accumulators are signalled on accumulator barrier `b`
-  __device__ __forceinline__ void end(int b) {
-    commit(&bars[b]);
+  // close the stage: after the CTA barrier its accumulators are in the store and its ring slot is free
+  __device__ __forceinline__ void end() {
+    group_sync();
     ++it;
-    if (b == 0) cov0 = it; else cov1 = it;
-  }
-  // the warp has just passed accumulator barrier b
-  __device__ __forceinline__ void passed(int b) {
-    const uint32_t c = (b == 0) ? cov0 : cov1;
-    if (c > done) done = c;
     pump();
   }
 };
 using Issuer = IssuerT<kSlots>;
+
+// Kernel prologue, all threads: thread 0 initialises the ring's mbarriers full[0 .. NSLOT) (and any
+// other mbarrier the kernel initialised before the call), warp 0 reserves `ncols` store columns, and
+// after the CTA barrier the issuer starts fetching the first NSLOT stages of the CTA's first tile.
+template <int NSLOT>
+__device__ __forceinline__ IssuerT<NSLOT> tc_begin(uint64_t* full, float* ring, const sbi_nsf_tc& tc, int T,
+                                                   int64_t ntiles, bool reverse, int ncols, const StoreArgs& sa) {
+  if (threadIdx.x == 0) {
+    for (int s = 0; s < NSLOT; ++s) mbar_init(&full[s], 1);
+    fence_barrier_init();
+  }
+  if (threadIdx.x < 32) store_alloc(ncols, sa);
+  __syncthreads();
+  IssuerT<NSLOT> iss;
+  uint32_t el = 0;
+  asm volatile("{\n\t.reg .pred p;\n\telect.sync _|p, 0xffffffff;\n\tselp.u32 %0, 1, 0, p;\n\t}" : "=r"(el));
+  iss.leader = el != 0;
+  iss.warp = threadIdx.x >> 5;
+  iss.ring = ring; iss.full = full;
+  iss.tcw = tc.d_tcw; iss.tab = tc.d_tab; iss.cap = tc.stage_cap; iss.T = T;
+  iss.it = 0; iss.fetched = 0;
+  iss.sbase = 0; iss.lo_off = 0;
+  iss.f_tile = blockIdx.x; iss.ntiles = ntiles; iss.tile_step = gridDim.x; iss.f_l = 0; iss.f_s = 0;
+  iss.reverse = reverse;
+  iss.pump();
+  return iss;
+}
+// Kernel epilogue, all threads: release the store columns once every thread is done with them.
+__device__ __forceinline__ void tc_end(int ncols, const StoreArgs& sa) {
+  group_sync();
+  if (threadIdx.x < 32) store_dealloc(ncols, sa);
+}
 
 // generic-proxy shared-memory writes -> visible to the async proxy (wgmma operand reads)
 __device__ __forceinline__ void fence_async_smem() {
