@@ -13,6 +13,8 @@
  *                                                      (trainers/base.py:1171-1187)  -> sbi_b200_nsf_vjp
  *   sbi/neural_nets/estimators/nflows_flow.py:111-128 NFlowsFlow.sample     -> sbi_b200_nsf_inverse
  *   sbi/neural_nets/estimators/nflows_flow.py:42-75   inverse_transform     -> sbi_b200_nsf_logprob (z_out)
+ *   sbi/neural_nets/ratio_estimators.py:132-154      RatioEstimator.forward -> sbi_b200_ratio_forward (resnet),
+ *                                                      sbi_b200_ratio_mlp_forward (mlp, linear)
  *   sbi/inference/trainers/base.py:1181-1187          clip_grad_norm_ + Adam.step -> sbi_b200_reduce_partials,
  *                                                                                  sbi_b200_adam_clip_step
  */
@@ -298,6 +300,38 @@ int sbi_b200_ratio_forward(const sbi_ratio_model* m, const sbi_pairs* pairs, flo
 int sbi_b200_ratio_vjp_parts(int64_t R);
 int sbi_b200_ratio_vjp(const sbi_ratio_model* m, const sbi_pairs* pairs, const float* d_gout,
                        float* d_logits, float* d_gpart, float* d_gtheta, void* stream);
+
+/* ---- ratio estimator: NRE `classifier_nn("mlp")` and `classifier_nn("linear")` (reference builders
+ * sbi/neural_nets/net_builders/classifier.py:49-169):
+ *   mlp:    logit = Linear(H,1)(relu(N(Linear(H,H)(relu(N(Linear(Dt+Dx,H)(u)))))))
+ *   linear: logit = Linear(Dt+Dx,1)(u)
+ * with u = cat(standardize(theta), standardize(x)) and N = nn.LayerNorm(H) (biased variance over the
+ * H features of a row, eps `ln_eps`, affine) or nn.Identity.  NL = number of hidden layers (2 or 0). */
+enum {
+  SBI_RM_W0 = 0, SBI_RM_B0 = 1,    /* hidden layer l at 4l: Linear [Hp][Kp] (Kp = Dtp+Dxp for l = 0, Hp after; */
+  SBI_RM_G0 = 2, SBI_RM_BE0 = 3,   /*   columns of layer 0 = [theta | pad | x | pad]), LayerNorm gamma, beta [Hp] */
+  SBI_RM_WF = 8, SBI_RM_BF = 9     /* output layer [4][Hp], or [4][Dtp+Dxp] when NL = 0 (row 0 is the logit) */
+};
+enum { SBI_RM_NORM_NONE = 0, SBI_RM_NORM_LAYER = 1 };
+typedef struct {
+  int32_t Dt, Dx, H, NL;
+  int32_t Dtp, Dxp, Hp;
+  int32_t norm;                   /* SBI_RM_NORM_* */
+  float ln_eps;
+  int32_t rpc0, rpc1;             /* weight rows per ring chunk: layer 0 / later layers */
+  int32_t wcap, nbuf, n_params;
+  const float* d_params;
+  const int32_t* d_tab;           /* SBI_RM_* offsets */
+  const float* d_stats;           /* as sbi_ratio_model */
+} sbi_ratio_mlp_model;
+
+/* same contracts as sbi_b200_ratio_forward / _vjp_parts / _vjp.  A shape whose tile does not fit the
+ * 227 KB of shared memory of one CTA returns SBI_ESMEM. */
+int sbi_b200_ratio_mlp_forward(const sbi_ratio_mlp_model* m, const sbi_pairs* pairs, float* d_logits,
+                               void* stream);
+int sbi_b200_ratio_mlp_vjp_parts(int64_t R);
+int sbi_b200_ratio_mlp_vjp(const sbi_ratio_mlp_model* m, const sbi_pairs* pairs, const float* d_gout,
+                           float* d_logits, float* d_gpart, float* d_gtheta, void* stream);
 
 /* tensor-core bulk evaluation of the classifier (same operand format and `sbi_nsf_tc` descriptor as
  * the NSF path: d_tab holds ONE stage list: initial layer, per block (W1, W2), final layer as an

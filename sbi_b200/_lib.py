@@ -89,6 +89,21 @@ class Pairs(C.Structure):
 R_W0, R_B0, R_WF, R_BF, R_BLK0 = 0, 1, 2, 3, 4
 
 
+class RatioMlpModel(C.Structure):
+    _fields_ = [
+        ("Dt", C.c_int32), ("Dx", C.c_int32), ("H", C.c_int32), ("NL", C.c_int32),
+        ("Dtp", C.c_int32), ("Dxp", C.c_int32), ("Hp", C.c_int32),
+        ("norm", C.c_int32), ("ln_eps", C.c_float),
+        ("rpc0", C.c_int32), ("rpc1", C.c_int32),
+        ("wcap", C.c_int32), ("nbuf", C.c_int32), ("n_params", C.c_int32),
+        ("d_params", C.c_void_p), ("d_tab", C.c_void_p), ("d_stats", C.c_void_p),
+    ]
+
+
+RM_W0, RM_B0, RM_G0, RM_BE0, RM_WF, RM_BF = 0, 1, 2, 3, 8, 9
+RM_NORM_NONE, RM_NORM_LAYER = 0, 1
+
+
 class FmModel(C.Structure):
     _fields_ = [
         ("D", C.c_int32), ("C", C.c_int32), ("H", C.c_int32), ("NL", C.c_int32), ("TE", C.c_int32),
@@ -174,6 +189,10 @@ _EXPORTS = {
     "sbi_b200_ratio_vjp_parts": (C.c_int, [C.c_int64]),
     "sbi_b200_ratio_vjp": (C.c_int, [C.POINTER(RatioModel), C.POINTER(Pairs), C.c_void_p, C.c_void_p,
                                      C.c_void_p, C.c_void_p, C.c_void_p]),
+    "sbi_b200_ratio_mlp_forward": (C.c_int, [C.POINTER(RatioMlpModel), C.POINTER(Pairs), C.c_void_p, C.c_void_p]),
+    "sbi_b200_ratio_mlp_vjp_parts": (C.c_int, [C.c_int64]),
+    "sbi_b200_ratio_mlp_vjp": (C.c_int, [C.POINTER(RatioMlpModel), C.POINTER(Pairs), C.c_void_p, C.c_void_p,
+                                         C.c_void_p, C.c_void_p, C.c_void_p]),
     "sbi_b200_fm_net_vjp": (C.c_int, [C.POINTER(FmModel), C.POINTER(Rows), C.c_void_p, C.c_void_p, C.c_void_p,
                                       C.c_void_p]),
     "sbi_b200_fm_plan": (C.c_int, [C.POINTER(FmModel), C.c_int32, C.POINTER(C.c_int32)]),

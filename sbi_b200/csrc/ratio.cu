@@ -50,29 +50,7 @@ __host__ __device__ inline RatioSmem ratio_smem_layout(const sbi_ratio_model& m,
 template <int TM>
 __device__ __forceinline__ void ratio_load(const sbi_ratio_model& m, const sbi_pairs& pr, int64_t row0,
                                            float* U) {
-  constexpr int LD = Tile<TM>::LD;
-  const float* __restrict__ st = m.d_stats;
-  const int Dt = m.Dt, Dx = m.Dx, Dtp = m.Dtp, Dxp = m.Dxp;
-  for (int e = threadIdx.x; e < TM * Dtp; e += kConsumerThreads) {
-    const int r = e / Dtp, d = e % Dtp;
-    const int64_t gr = row0 + r;
-    float val = 0.f;
-    if (d < Dt && gr < pr.R) {
-      const int64_t src = pr.d_theta_index ? __ldg(pr.d_theta_index + gr) : gr;
-      val = (__ldg(pr.d_theta + src * Dt + d) - __ldg(st + d)) / __ldg(st + Dtp + d);
-    }
-    U[d * LD + r] = val;
-  }
-  for (int e = threadIdx.x; e < TM * Dxp; e += kConsumerThreads) {
-    const int r = e / Dxp, d = e % Dxp;
-    const int64_t gr = row0 + r;
-    float val = 0.f;
-    if (d < Dx && gr < pr.R) {
-      const int64_t src = pr.x_shared ? 0 : (pr.d_x_index ? __ldg(pr.d_x_index + gr) : gr);
-      val = (__ldg(pr.d_x + src * Dx + d) - __ldg(st + 2 * Dtp + d)) / __ldg(st + 2 * Dtp + Dxp + d);
-    }
-    U[(Dtp + d) * LD + r] = val;
-  }
+  pairs_load<TM>(m.Dt, m.Dx, m.Dtp, m.Dxp, m.d_stats, pr, row0, U);
   consumer_sync();
 }
 

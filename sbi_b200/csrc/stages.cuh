@@ -116,6 +116,35 @@ __device__ __forceinline__ void load_rows(int D, int Dp, int C, int Cp, const fl
   }
 }
 
+// classifier input U = [theta | pad | x | pad] (Dtp + Dxp feature rows) of the pairs row0 .. row0+TM-1,
+// standardised by stats = [theta_mean(Dtp) | theta_std(Dtp) | x_mean(Dxp) | x_std(Dxp)] (include/sbi_b200.h
+// sbi_pairs); pad rows / rows beyond R are zero.  No barrier inside.
+template <int TM>
+__device__ __forceinline__ void pairs_load(int Dt, int Dx, int Dtp, int Dxp, const float* __restrict__ st,
+                                           const sbi_pairs& pr, int64_t row0, float* U) {
+  constexpr int LD = Tile<TM>::LD;
+  for (int e = threadIdx.x; e < TM * Dtp; e += kConsumerThreads) {
+    const int r = e / Dtp, d = e % Dtp;
+    const int64_t gr = row0 + r;
+    float val = 0.f;
+    if (d < Dt && gr < pr.R) {
+      const int64_t src = pr.d_theta_index ? __ldg(pr.d_theta_index + gr) : gr;
+      val = (__ldg(pr.d_theta + src * Dt + d) - __ldg(st + d)) / __ldg(st + Dtp + d);
+    }
+    U[d * LD + r] = val;
+  }
+  for (int e = threadIdx.x; e < TM * Dxp; e += kConsumerThreads) {
+    const int r = e / Dxp, d = e % Dxp;
+    const int64_t gr = row0 + r;
+    float val = 0.f;
+    if (d < Dx && gr < pr.R) {
+      const int64_t src = pr.x_shared ? 0 : (pr.d_x_index ? __ldg(pr.d_x_index + gr) : gr);
+      val = (__ldg(pr.d_x + src * Dx + d) - __ldg(st + 2 * Dtp + d)) / __ldg(st + 2 * Dtp + Dxp + d);
+    }
+    U[(Dtp + d) * LD + r] = val;
+  }
+}
+
 // carve the weight ring + its mbarriers out of shared memory (all threads call this)
 __device__ __forceinline__ WPipe make_pipe(int nbuf, int wcap, float* sm, int ring_off, int bar_bytes) {
   WPipe p;

@@ -13,7 +13,7 @@ from __future__ import annotations
 
 import math
 from dataclasses import dataclass, field
-from typing import Dict, List
+from typing import Dict, List, Optional
 
 import numpy as np
 import torch
@@ -910,6 +910,78 @@ class RatioLayout(_LayoutOps):
 
 
 RatioLayout.family = "ratio"
+
+
+@dataclass
+class MlpRatioLayout(_LayoutOps):
+    """Packed layout of the NRE `mlp` (NL = 2 hidden layers) and `linear` (NL = 0) classifiers
+    (include/sbi_b200.h `sbi_ratio_mlp_model`), keys as in the reference's nn.Sequential
+    (sbi/neural_nets/net_builders/classifier.py:49-169): `net.0/3/6.*` linears and
+    `net.1/4.*` LayerNorms (absent with `norm=None`, i.e. nn.Identity), or `net.weight/bias`."""
+    Dt: int
+    Dx: int
+    H: int = 50
+    NL: int = 2
+    norm: Optional[str] = "layer"
+    eps: float = 1e-5
+    wcap_target: int = 4096
+    n_params: int = 0
+    index: Dict[str, np.ndarray] = field(default_factory=dict, repr=False)
+
+    def __post_init__(self):
+        Dt, Dx, H, NL = self.Dt, self.Dx, self.H, self.NL
+        if NL not in (0, 2) or self.norm not in ("layer", None):
+            raise ValueError(f"MlpRatioLayout: NL must be 0 or 2 and norm 'layer' or None, got {NL}, {self.norm!r}")
+        self.Dtp, self.Dxp, self.Hp = round4(Dt), round4(Dx), round4(H)
+        K0p, Hp = self.Dtp + self.Dxp, self.Hp
+        KFp = Hp if NL else K0p
+        cap = max(self.wcap_target, 4 * K0p, 4 * Hp)
+        self.rpc0 = max(4, min(Hp, (cap // K0p) & ~3))
+        self.rpc1 = max(4, min(Hp, (cap // Hp) & ~3))
+        self.wcap = (max(self.rpc0 * K0p, self.rpc1 * Hp, 4 * KFp) + 31) & ~31
+        off = 0
+
+        def take(n):
+            nonlocal off
+            o = off
+            off += round4(n)
+            return o
+
+        tab = np.zeros(10, np.int32)
+        idx: Dict[str, np.ndarray] = {}
+        cols0 = np.concatenate([np.arange(Dt), self.Dtp + np.arange(Dx)])   # [theta | pad | x | pad]
+        for l in range(NL):
+            Kp, cols = (K0p, cols0) if l == 0 else (Hp, np.arange(H))
+            o = tab[4 * l + L.RM_W0] = take(Hp * Kp)
+            idx[f"net.{3 * l}.weight"] = o + np.arange(H)[:, None] * Kp + cols[None, :]
+            o = tab[4 * l + L.RM_B0] = take(Hp)
+            idx[f"net.{3 * l}.bias"] = o + np.arange(H)
+            if self.norm == "layer":
+                o = tab[4 * l + L.RM_G0] = take(Hp)
+                idx[f"net.{3 * l + 1}.weight"] = o + np.arange(H)
+                o = tab[4 * l + L.RM_BE0] = take(Hp)
+                idx[f"net.{3 * l + 1}.bias"] = o + np.arange(H)
+        pre = "net.6." if NL else "net."
+        o = tab[L.RM_WF] = take(4 * KFp)
+        idx[pre + "weight"] = o + (np.arange(H) if NL else cols0)[None, :]
+        o = tab[L.RM_BF] = take(4)
+        idx[pre + "bias"] = o + np.arange(1)
+        self.n_params = off
+        self.index = idx
+        self.tab = tab
+        self.buffers = {}
+
+    def fill_struct(self, s: "L.RatioMlpModel", nbuf: int):
+        s.Dt, s.Dx, s.H, s.NL = self.Dt, self.Dx, self.H, self.NL
+        s.Dtp, s.Dxp, s.Hp = self.Dtp, self.Dxp, self.Hp
+        s.norm = L.RM_NORM_LAYER if self.norm == "layer" else L.RM_NORM_NONE
+        s.ln_eps = self.eps
+        s.rpc0, s.rpc1 = self.rpc0, self.rpc1
+        s.wcap, s.nbuf, s.n_params = self.wcap, nbuf, self.n_params
+        return s
+
+
+MlpRatioLayout.family = "ratio_mlp"
 
 
 @dataclass

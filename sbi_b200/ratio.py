@@ -1,16 +1,19 @@
 """Ratio estimator (NRE) at sbi's estimator boundary, backed by the sm_90a kernels.
 
 `RatioEstimator` mirrors /root/reference/sbi/neural_nets/ratio_estimators.py:11-157 for the
-`resnet` classifier of /root/reference/sbi/neural_nets/net_builders/classifier.py:172-235:
+`linear`, `mlp` and `resnet` classifiers of /root/reference/sbi/neural_nets/net_builders/classifier.py:
 `forward(theta, x)` / `unnormalized_log_ratio` return logits of shape `(*batch_shape)` for
 equally-prefixed `theta` and `x` (no broadcasting, same error), `state_dict()` uses the
-reference's keys.  `classifier_nn` / `build_resnet_classifier` mirror factory.py:174-241.
+reference's keys.  `classifier_nn` / `build_*_classifier` mirror factory.py:174-241.  The layout
+selects the kernels: `RatioLayout` (resnet) csrc/ratio.cu and csrc/ratio_tc.cu, `MlpRatioLayout`
+(mlp, linear) csrc/ratio_mlp.cu.
 """
 from __future__ import annotations
 
 import ctypes as C
 import os
-from typing import Any, Callable, Optional
+import warnings
+from typing import Any, Callable, Optional, Union
 
 import torch
 from torch import Tensor, nn
@@ -19,13 +22,15 @@ from torch.nn import init
 from . import _lib as L
 from .estimators import Standardize
 from .neural_nets import _linear_init, check_data_device, standardizing_stats, z_score_parser
-from .pack import RatioLayout
+from .pack import MlpRatioLayout, RatioLayout
+
+_STRUCTS = {"ratio": L.RatioModel, "ratio_mlp": L.RatioMlpModel}
 
 
 class _RatioNet(nn.Module):
     """Sits at `estimator.net` (the reference's ResidualNet); owns the flat parameter buffer."""
 
-    def __init__(self, layout: RatioLayout):
+    def __init__(self, layout: Union[RatioLayout, MlpRatioLayout]):
         super().__init__()
         self.layout = layout
         self.flat = nn.Parameter(torch.zeros(layout.n_params, dtype=torch.float32))
@@ -59,7 +64,7 @@ class _RatioNet(nn.Module):
 class RatioEstimator(nn.Module):
     r"""log r(theta, x) = classifier logit; trained by NRE (ratio_estimators.py:11-157)."""
 
-    def __init__(self, layout: RatioLayout, theta_shape, x_shape, theta_stats, x_stats,
+    def __init__(self, layout: Union[RatioLayout, MlpRatioLayout], theta_shape, x_shape, theta_stats, x_stats,
                  embedding_net_theta: nn.Module = None, embedding_net_x: nn.Module = None):
         super().__init__()
         self._input_shape = torch.Size(theta_shape)
@@ -118,16 +123,28 @@ class RatioEstimator(nn.Module):
         self._cache["stats"] = (key, st)
         return st
 
-    def _model(self, nbuf: int) -> L.RatioModel:
+    def _model(self, nbuf: int):
         L.require_cuda(self.net.flat, "estimator parameters")
         st = self._stats()
-        s = L.RatioModel()
+        s = _STRUCTS[self.layout.family]()
         self.layout.fill_struct(s, nbuf)
         s.d_params = self.net.flat.data_ptr()
         s.d_tab = self.net._tab.data_ptr()
         s.d_stats = st.data_ptr()
         s._keep = (st,)
         return s
+
+    def _entry(self, name: str):
+        """The layout's C entry point `sbi_b200_<family>_<name>`."""
+        return getattr(L.load(), f"sbi_b200_{self.layout.family}_{name}")
+
+    def _check_rc(self, rc: int, what: str):
+        if rc == -2:
+            lay = self.layout
+            raise L.SbiB200Error(
+                f"{what}: a row tile of this classifier (Dt={lay.Dt}, Dx={lay.Dx}, H={lay.H}) needs more than "
+                "the 227 KB of shared memory one CTA can use on sm_90a (SBI_ESMEM)")
+        L.check(rc, what)
 
     def _gpart(self, n_part: int) -> Tensor:
         buf = self._cache.get("gpart")
@@ -179,7 +196,8 @@ class RatioEstimator(nn.Module):
             L.check(lib.sbi_b200_ratio_forward_tc(C.byref(m), C.byref(tc), C.byref(pr), L.ptr(out),
                                                   L.stream_ptr()), "ratio_forward_tc")
             return out
-        L.check(lib.sbi_b200_ratio_forward(C.byref(m), C.byref(pr), L.ptr(out), L.stream_ptr()), "ratio_forward")
+        self._check_rc(self._entry("forward")(C.byref(m), C.byref(pr), L.ptr(out), L.stream_ptr()),
+                    f"{self.layout.family}_forward")
         return out
 
     #: pairs from which the logits go through the wgmma kernel (csrc/ratio_tc.cu); the crossover against
@@ -189,7 +207,7 @@ class RatioEstimator(nn.Module):
     def _tc_state(self, m):
         """`NsfTc` descriptor with freshly packed operands, or None if the model is outside what
         the tensor-core kernel instantiates (see FlowEstimator._tc_state)."""
-        if os.environ.get("SBI_B200_TC", "") == "0":
+        if os.environ.get("SBI_B200_TC", "") == "0" or not hasattr(self.layout, "tc_plan"):
             return None
         flat = self.net.flat
         st = self._cache.get("tc")
@@ -226,7 +244,7 @@ class _RatioFn(torch.autograd.Function):
         est = ctx.est
         lib = L.load()
         R = g.shape[0]
-        n_part = lib.sbi_b200_ratio_vjp_parts(R)
+        n_part = est._entry("vjp_parts")(R)
         gpart = est._gpart(n_part)
         need_flat, need_th = ctx.needs_input_grad[0], ctx.needs_input_grad[1]
         gth = torch.empty(R, est.layout.Dt, dtype=torch.float32, device=theta.device) if need_th else None
@@ -234,8 +252,8 @@ class _RatioFn(torch.autograd.Function):
         pr = L.Pairs(theta.data_ptr(), x.data_ptr(), None if ctx.ti is None else ctx.ti.data_ptr(),
                      None if ctx.xi is None else ctx.xi.data_ptr(), R, 1 if ctx.x_shared else 0)
         g = g.contiguous().float()
-        L.check(lib.sbi_b200_ratio_vjp(C.byref(m), C.byref(pr), L.ptr(g), None, L.ptr(gpart), L.ptr(gth),
-                                       L.stream_ptr()), "ratio_vjp")
+        est._check_rc(est._entry("vjp")(C.byref(m), C.byref(pr), L.ptr(g), None, L.ptr(gpart), L.ptr(gth),
+                                     L.stream_ptr()), f"{est.layout.family}_vjp")
         gflat = None
         if need_flat:
             gflat = torch.empty(est.layout.n_params, dtype=torch.float32, device=theta.device)
@@ -282,21 +300,110 @@ def build_resnet_classifier(
     return est
 
 
+def _input_stats(batch_x: Tensor, batch_y: Tensor, z_score_x, z_score_y):
+    zx, sx = z_score_parser(z_score_x)
+    zy, sy = z_score_parser(z_score_y)
+    return (standardizing_stats(batch_x, sx) if zx else None), (standardizing_stats(batch_y, sy) if zy else None)
+
+
+def _norm_params(mod: nn.Module, H: int):
+    """(kind, eps, {weight, bias}) of a module built by `norm_layer(H)`; the kernels implement
+    nn.LayerNorm(H) with affine parameters (row-local) and nn.Identity."""
+    if type(mod) is nn.Identity:
+        return None, None, {}
+    if (type(mod) is nn.LayerNorm and tuple(mod.normalized_shape) == (H,) and mod.elementwise_affine
+            and mod.bias is not None):
+        return "layer", float(mod.eps), {"weight": mod.weight.detach(), "bias": mod.bias.detach()}
+    raise NotImplementedError(
+        f"the sm_90a mlp classifier kernels implement norm_layer=nn.LayerNorm (affine) or nn.Identity; got {mod!r}")
+
+
+def build_linear_classifier(
+    batch_x: Tensor, batch_y: Tensor, z_score_x: Optional[str] = "independent",
+    z_score_y: Optional[str] = "independent", embedding_net_x: nn.Module = nn.Identity(),
+    embedding_net_y: nn.Module = nn.Identity(), **kwargs,
+) -> RatioEstimator:
+    """classifier.py:49-104: logit = Linear(Dt + Dx, 1)(u); one nn.Linear draw from the global RNG.
+    Like the reference, other keyword arguments are ignored."""
+    check_data_device(batch_x, batch_y)
+    if z_score_x == "transform_to_unconstrained":
+        raise ValueError("Ratio-based classifiers (NRE) do not implement `transform_to_unconstrained`.")
+    Dt, Dx = batch_x[0].numel(), batch_y[0].numel()
+    lay = MlpRatioLayout(Dt=Dt, Dx=Dx, NL=0, norm=None)
+    state = {}
+    state["net.weight"], state["net.bias"] = _linear_init(1, Dt + Dx)
+    t_stats, x_stats = _input_stats(batch_x, batch_y, z_score_x, z_score_y)
+    est = RatioEstimator(lay, batch_x[0].shape, batch_y[0].shape, t_stats, x_stats,
+                         embedding_net_x, embedding_net_y)
+    with torch.no_grad():
+        lay.pack(state, out=est.net.flat.data)
+    return est
+
+
+def build_mlp_classifier(
+    batch_x: Tensor, batch_y: Tensor, z_score_x: Optional[str] = "independent",
+    z_score_y: Optional[str] = "independent", hidden_features: int = 50,
+    embedding_net_x: nn.Module = nn.Identity(), embedding_net_y: nn.Module = nn.Identity(),
+    norm_layer: Callable[[int], nn.Module] = nn.LayerNorm,
+) -> RatioEstimator:
+    """classifier.py:107-169: Sequential(Linear(Dt+Dx, H), norm_layer(H), ReLU, Linear(H, H),
+    norm_layer(H), ReLU, Linear(H, 1)).  Modules are constructed in that order, so a seed reproduces
+    the reference's initial weights; the norm layers' own parameters are taken as built."""
+    check_data_device(batch_x, batch_y)
+    if z_score_x == "transform_to_unconstrained":
+        raise ValueError("Ratio-based classifiers (NRE) do not implement `transform_to_unconstrained`.")
+    Dt, Dx, H = batch_x[0].numel(), batch_y[0].numel(), hidden_features
+    state, norms = {}, []
+    for l, fan_in in enumerate((Dt + Dx, H)):
+        state[f"net.{3 * l}.weight"], state[f"net.{3 * l}.bias"] = _linear_init(H, fan_in)
+        kind, eps, p = _norm_params(norm_layer(H), H)
+        norms.append((kind, eps))
+        state.update({f"net.{3 * l + 1}.{k}": v for k, v in p.items()})
+    if norms[0] != norms[1]:
+        raise NotImplementedError("the sm_90a mlp classifier kernels need both norm layers of the same kind and eps")
+    state["net.6.weight"], state["net.6.bias"] = _linear_init(1, H)
+    kind, eps = norms[0]
+    lay = MlpRatioLayout(Dt=Dt, Dx=Dx, H=H, NL=2, norm=kind, eps=eps if eps is not None else 1e-5)
+    t_stats, x_stats = _input_stats(batch_x, batch_y, z_score_x, z_score_y)
+    est = RatioEstimator(lay, batch_x[0].shape, batch_y[0].shape, t_stats, x_stats,
+                         embedding_net_x, embedding_net_y)
+    with torch.no_grad():
+        lay.pack(state, out=est.net.flat.data)
+    return est
+
+
+_BUILDERS = {"linear": build_linear_classifier, "mlp": build_mlp_classifier, "resnet": build_resnet_classifier}
+#: the model-specific arguments of estimator_configs.py:1375-1419 (`hidden_features` is a factory argument)
+_MODEL_ARGS = {"linear": set(), "mlp": {"hidden_features", "norm_layer"},
+               "resnet": {"hidden_features", "num_blocks", "dropout_probability", "use_batch_norm"}}
+
+
 def classifier_nn(
     model: str, z_score_theta: Optional[str] = "independent", z_score_x: Optional[str] = "independent",
     hidden_features: int = 50, embedding_net_theta: nn.Module = nn.Identity(),
     embedding_net_x: nn.Module = nn.Identity(), **kwargs: Any,
 ) -> Callable:
-    """factory.py:174-241: build function for the NRE classifier."""
-    if model != "resnet":
-        raise NotImplementedError(f"sbi_b200 implements the 'resnet' classifier on sm_90a; got {model!r}.")
+    """factory.py:174-241: build function for the NRE classifier `linear`, `mlp` or `resnet`.  An
+    argument that belongs to another model (or a non-default `hidden_features` for `linear`) raises
+    ValueError, as in the reference."""
+    if model not in _BUILDERS:
+        raise ValueError(f"Unknown classifier model {model!r}. Must be one of {sorted(_BUILDERS)}.")
+    given = set(kwargs) | ({"hidden_features"} if hidden_features != 50 else set())
+    unused = sorted((given & set().union(*_MODEL_ARGS.values())) - _MODEL_ARGS[model])
+    if unused:
+        raise ValueError(f"Argument(s) {unused} are not used by model={model!r} and would be silently ignored.")
+    unknown = sorted(set(kwargs) - set().union(*_MODEL_ARGS.values()))
+    if unknown:
+        warnings.warn(f"Unknown kwargs passed to the {model!r} classifier: {unknown}. These will be forwarded "
+                      "to the underlying builder. If this is unintentional, check for typos.", stacklevel=2)
+    if model != "linear":
+        kwargs["hidden_features"] = hidden_features
 
     def build_fn(batch_theta, batch_x):
         from ._refabc import register_with_reference
         register_with_reference()
-        return build_resnet_classifier(
+        return _BUILDERS[model](
             batch_x=batch_theta, batch_y=batch_x, z_score_x=z_score_theta, z_score_y=z_score_x,
-            hidden_features=hidden_features, embedding_net_x=embedding_net_theta,
-            embedding_net_y=embedding_net_x, **kwargs)
+            embedding_net_x=embedding_net_theta, embedding_net_y=embedding_net_x, **kwargs)
 
     return build_fn
