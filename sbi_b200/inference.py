@@ -15,6 +15,9 @@ What is different is where the work happens: the (theta, x) set lives in HBM, an
 CUDA-graph launch (steps_per_epoch x [fused fwd+bwd kernel -> partial-gradient reduce ->
 clip+Adam kernel] + the validation pass), and the host reads three scalars per epoch instead
 of syncing twice per step.
+
+Every trainer runs the same loop (`_Trainer._run`), the same device optimizer step (`_DeviceAdam`) and the
+same graph capture (`_capture`); a trainer supplies the body of one epoch.
 """
 from __future__ import annotations
 
@@ -47,22 +50,113 @@ def _process_device(device: str) -> str:
     return str(device)
 
 
-class _FlowTrainer:
-    """Shared first-round trainer for density estimators (NPE: q(theta|x); NLE: q(x|theta))."""
+class _DeviceAdam:
+    """Clip + Adam (`clip_grad_norm_` + `Adam.step`, trainers/base.py:1181-1187) on a network's flat
+    parameters, in the kernels of csrc/optim.cu.  With several ranks the gradient is first summed over
+    them: through our NVLink peer-memory kernel on one node (graph-capturable), else with an NCCL
+    all-reduce (eager launches).  The clip norm is always taken on the summed gradient."""
 
-    _swap = False   # NLE: estimator input = x, condition = theta
+    def __init__(self, net, state: Tensor, step: Tensor, lr: float, clip_max_norm: Optional[float], world: int):
+        self.lib = L.load()
+        self.flat, self.mask = net.flat, net.net._mask
+        self.P = net.layout.n_params
+        self.state, self.count = state, step
+        self.lr = lr
+        self.max_norm = float(clip_max_norm) if clip_max_norm is not None else 0.0
+        self.world = world
+        self.peer = None
+        if world > 1:
+            from .parallel import make_gradient_exchange
+            self.peer = make_gradient_exchange(self.P)      # None -> NCCL all-reduce
+        dev = state.device
+        self.grad = torch.zeros(self.P, dtype=torch.float32, device=dev)
+        # the peer exchange reads this rank's gradient from a buffer of its own
+        self.grad_local = torch.zeros(self.P, dtype=torch.float32, device=dev) if self.peer is not None else self.grad
+        n_sumsq = self.peer.n_sumsq if self.peer is not None else self.lib.sbi_b200_sumsq_blocks(self.P)
+        self.sumsq = torch.zeros(n_sumsq, dtype=torch.float32, device=dev)
 
-    def __init__(self, prior=None, density_estimator: Union[str, Callable] = "nsf",
-                 device: str = "cuda", logging_level: Union[int, str] = "WARNING",
-                 summary_writer=None, tracker=None, show_progress_bars: bool = False):
+    @property
+    def capturable(self) -> bool:
+        """Whether a step can be captured in a CUDA graph (not with the NCCL all-reduce)."""
+        return self.world == 1 or self.peer is not None
+
+    def step(self, grad: Tensor):
+        """One update from a gradient that is complete on this rank (autograd)."""
+        if self.peer is not None:     # summed over NVLink peer memory, with the sum(g^2) partials
+            self.peer.sum(grad, self.grad, self.mask, self.sumsq)
+            self._adam(self.grad, self.peer.n_sumsq)
+            return
+        if self.world > 1:
+            torch.distributed.all_reduce(grad)
+        self._adam(grad, 0)
+
+    def step_partials(self, gpart: Tensor, n_part: int):
+        """One update from the `n_part` per-CTA partial gradients of a fused loss kernel."""
+        if self.world == 1:           # the reduction kernel also emits the sum(g^2) partials
+            L.check(self.lib.sbi_b200_reduce_partials_norm(L.ptr(gpart), n_part, self.P, L.ptr(self.grad),
+                                                           L.ptr(self.mask), L.ptr(self.sumsq), L.stream_ptr()),
+                    "reduce_partials")
+            self._adam(self.grad, self.sumsq.shape[0])
+            return
+        L.check(self.lib.sbi_b200_reduce_partials(L.ptr(gpart), n_part, self.P, L.ptr(self.grad_local),
+                                                  L.stream_ptr()), "reduce_partials")
+        self.step(self.grad_local)
+
+    def _adam(self, grad: Tensor, n_sumsq: int):
+        """n_sumsq > 0: `sumsq` already holds that many sum(g^2) partials of `grad`."""
+        if n_sumsq:
+            L.check(self.lib.sbi_b200_adam_clip_step_norm(
+                L.ptr(self.flat.data), L.ptr(grad), L.ptr(self.state), L.ptr(self.count), L.ptr(self.mask), self.P,
+                self.lr, 0.9, 0.999, 1e-8, self.max_norm, 1.0, L.ptr(self.sumsq), n_sumsq, L.stream_ptr()),
+                "adam_clip_step")
+        else:
+            L.check(self.lib.sbi_b200_adam_clip_step(
+                L.ptr(self.flat.data), L.ptr(grad), L.ptr(self.state), L.ptr(self.count), L.ptr(self.mask), self.P,
+                self.lr, 0.9, 0.999, 1e-8, self.max_norm, 1.0, L.stream_ptr()), "adam_clip_step")
+
+    def snapshot(self):
+        return self.flat.data.clone(), self.state.clone(), self.count.clone()
+
+    def restore(self, snap):
+        for t, s in zip((self.flat.data, self.state, self.count), snap):
+            t.copy_(s)
+
+    def close(self):
+        if self.peer is not None:
+            timed_out = self.peer.error()
+            self.peer.close()
+            if timed_out:
+                raise RuntimeError("peer-memory gradient exchange timed out (a rank fell behind or died)")
+
+
+def _capture(opt: _DeviceAdam, warmup: Callable, *fns: Callable) -> list:
+    """One CUDA graph per function of `fns`.  `warmup()` runs first on a side stream (allocations, kernel
+    attributes); the parameters and the optimizer state are rewound after it and after the capture, so
+    neither changes the run."""
+    snap = opt.snapshot()
+    side = torch.cuda.Stream()
+    side.wait_stream(torch.cuda.current_stream())
+    with torch.cuda.stream(side):
+        warmup()
+    torch.cuda.current_stream().wait_stream(side)
+    opt.restore(snap)
+    graphs = []
+    for fn in fns:
+        graphs.append(torch.cuda.CUDAGraph())
+        with torch.cuda.graph(graphs[-1]):
+            fn()
+    opt.restore(snap)
+    return graphs
+
+
+class _Trainer:
+    """State and training loop shared by all trainers (trainers/base.py:1060-1284)."""
+
+    def __init__(self, prior, build_neural_net: Callable, device: str, show_progress_bars: bool = False):
         self._prior = prior
         self._device = _process_device(device)
-        if isinstance(density_estimator, str):
-            factory = likelihood_nn if self._swap else posterior_nn
-            self._build_neural_net = factory(model=density_estimator)
-        else:
-            self._build_neural_net = density_estimator
-        self._neural_net: Optional[NSFEstimator] = None
+        self._build_neural_net = build_neural_net
+        self._neural_net = None
         self._theta: Optional[Tensor] = None
         self._x: Optional[Tensor] = None
         self._show_progress_bars = show_progress_bars
@@ -72,12 +166,15 @@ class _FlowTrainer:
         self._summary: Dict[str, list] = dict(
             epochs_trained=[], best_validation_loss=[], validation_loss=[], training_loss=[],
             epoch_durations_sec=[])
-        self._graphs = {}
         self._dist = None   # (rank, world) when data-parallel
+        self._partition = "global"
+        self.train_indices = self.val_indices = None
+        self._opt_state = self._opt_step = None
         # multi-round bookkeeping (npe_base.py:188-299): round of every appended block and its proposal
         self._data_round_index: list = []
         self._proposal_roundwise: list = []
         self._round_rows: list = []          # rows of every appended block
+        self._mr_opt = self._mr_split_n = None
 
     # ------------------------------------------------------------------ data
     def data_parallel(self, partition: str = "global"):
@@ -102,8 +199,9 @@ class _FlowTrainer:
 
     # ---- data-parallel helpers (no-ops on one process) ---------------------------------------------
     def _dp(self):
-        rank, world = self._dist if getattr(self, "_dist", None) is not None else (0, 1)
-        return rank, world, (getattr(self, "_partition", "global") if world > 1 else "local")
+        """(rank, world size, whether the ranks share one global batch: partition='global')."""
+        rank, world = self._dist if self._dist is not None else (0, 1)
+        return rank, world, world > 1 and self._partition == "global"
 
     def _dp_agree(self, value: int, what: str):
         """All ranks must see the same `value` (step counts, set sizes): a mismatch would leave a
@@ -120,8 +218,7 @@ class _FlowTrainer:
     def _dp_split(self, N: int, n_train: int):
         """90/10 split indices (base.py:525-539); with partition='global' rank 0's split is used."""
         perm = torch.randperm(N)
-        rank, world, part = self._dp()
-        if world > 1 and part == "global":
+        if self._dp()[2]:
             p = perm.to(self._device)
             torch.distributed.broadcast(p, 0)
             perm = p.cpu()
@@ -148,8 +245,6 @@ class _FlowTrainer:
                            exclude_invalid_x: Optional[bool] = None, data_device: Optional[str] = None):
         """Store simulations (npe_base.py:188-299): float32 only, rows with NaN/Inf in x are
         dropped (user_input_checks.py:708-765, sbiutils.py:491-525)."""
-        if not hasattr(self, "_data_round_index"):      # trainers with their own __init__ (NRE, FMPE)
-            self._data_round_index, self._proposal_roundwise, self._round_rows = [], [], []
         # round of this block (npe_base.py:224-241): prior samples are round 0, anything else opens a new round
         if proposal is None or proposal is self._prior:
             current_round = 0
@@ -200,6 +295,174 @@ class _FlowTrainer:
         return self._theta, self._x
 
     # ------------------------------------------------------------------ training
+    def _prepare(self, validation_fraction: float, training_batch_size: int, resume_training: bool,
+                 retrain_from_scratch: bool = False):
+        """Set-up of a first-round run (base.py:499-563, npe_base.py:674-708): the 90/10 split on the CPU
+        global generator, the network built from the CPU training split, rank 0's replica on every rank.
+        Returns (network, B, Bv, steps, vsteps): training / validation batch rows and steps per epoch."""
+        if self._theta is None:
+            raise RuntimeError("call append_simulations() first")
+        dev = self._device
+        N = self._theta.shape[0]
+        if self._dp()[2]:
+            self._dp_agree(N, "number of simulations")
+        n_train = int((1 - validation_fraction) * N)
+        n_val = N - n_train
+        if not resume_training or self.train_indices is None:
+            self.train_indices, self.val_indices = self._dp_split(N, n_train)
+        if self._neural_net is None or retrain_from_scratch:
+            tr = self.train_indices.to(dev)
+            self._neural_net = self._build_neural_net(self._theta[tr].cpu(), self._x[tr].cpu())
+        net = self._neural_net.to(dev)
+        self._neural_net = net
+        if not resume_training:
+            self._dp_sync_net(net)
+        B, Bv = min(training_batch_size, n_train), min(training_batch_size, n_val)
+        steps, vsteps = n_train // B, (n_val // Bv if Bv > 0 else 0)
+        self._dp_agree(steps, "number of steps per epoch")
+        return net, B, Bv, steps, vsteps
+
+    def _reset_epochs(self):
+        self.epoch, self._val_loss = 0, float("Inf")
+        self._best_val_loss, self._best_flat, self._epochs_since_last_improvement = float("Inf"), None, 0
+
+    def _optimizer(self, net, learning_rate: float, clip_max_norm: Optional[float],
+                   resume_training: bool) -> _DeviceAdam:
+        """The device optimizer of this run; its Adam state and the epoch count carry over with `resume_training`."""
+        if not resume_training or self._opt_state is None:
+            P = net.layout.n_params
+            self._opt_state = torch.zeros(2 * P, dtype=torch.float32, device=self._device)
+            self._opt_step = torch.zeros(2, dtype=torch.int32, device=self._device)
+            self._reset_epochs()
+        return _DeviceAdam(net, self._opt_state, self._opt_step, learning_rate, clip_max_norm, self._dp()[1])
+
+    def _step_epochs(self, opt: _DeviceAdam, B: int, Bv: int, steps: int, vsteps: int,
+                     train_step: Callable, val_step: Callable, graphs: bool) -> Callable:
+        """Epochs of per-step launches (NRE, NPSE).  `train_step(idx)` / `val_step(idx)` read the batch rows
+        from a static index buffer, filled before each step, so that with `graphs` one CUDA graph per
+        optimisation step and one per validation step are captured and replayed: a step is many small
+        launches that the host cannot issue as fast as the GPU runs them at small batches.  Random draws
+        inside a graph use torch's graph-safe Philox offsets.  Returns the function that runs one epoch."""
+        dev = self._device
+        train_idx, val_idx = self.train_indices.to(dev), self.val_indices.to(dev)
+        idx_buf = torch.zeros(B, dtype=torch.int64, device=dev)
+        vidx_buf = torch.zeros(max(Bv, 1), dtype=torch.int64, device=dev)
+        run_train, run_val = (lambda: train_step(idx_buf)), (lambda: val_step(vidx_buf))
+        if graphs and steps > 0 and opt.capturable:
+            idx_buf.copy_(train_idx[:B])
+            if vsteps > 0:
+                vidx_buf.copy_(val_idx[:Bv])
+
+            def warmup():
+                for _ in range(3):
+                    run_train()
+                if vsteps > 0:
+                    run_val()
+            captured = _capture(opt, warmup, run_train, *([run_val] if vsteps > 0 else []))
+            run_train = captured[0].replay
+            if vsteps > 0:
+                run_val = captured[1].replay
+
+        def epoch():
+            perm = train_idx[torch.randperm(train_idx.shape[0], device=dev)]
+            vperm = val_idx[torch.randperm(val_idx.shape[0], device=dev)] if vsteps > 0 else None
+            if self._dp()[2]:      # one epoch order for all ranks: rank 0's
+                torch.distributed.broadcast(perm, 0)
+                if vperm is not None:
+                    torch.distributed.broadcast(vperm, 0)
+            for buf, order, n, run in ((idx_buf, perm, steps, run_train), (vidx_buf, vperm, vsteps, run_val)):
+                b = buf.shape[0]
+                for s in range(n):
+                    buf.copy_(order[s * b:(s + 1) * b])
+                    run()
+        return epoch
+
+    def _epoch_losses(self, stats: Tensor):
+        """The epoch's one host sync: (training, validation) loss sums from the accumulators [train sum,
+        train non-finite count, validation sum, validation non-finite count], summed over the ranks."""
+        tl, tb, vl, vb = self._dp_sum(stats.tolist())
+        if tb > 0 or vb > 0:
+            raise AssertionError(self._nan_message)
+        return tl, vl
+
+    def _converged(self, net, stop_after_epochs: int) -> bool:
+        """base.py:1254-1284."""
+        if self.epoch == 0 or self._val_loss < self._best_val_loss:
+            self._best_val_loss, self._epochs_since_last_improvement = self._val_loss, 0
+            self._best_flat = net.flat.data.clone()
+        else:
+            self._epochs_since_last_improvement += 1
+        if self._epochs_since_last_improvement > stop_after_epochs - 1:
+            net.flat.data.copy_(self._best_flat)
+            return True
+        return False
+
+    def _record_epoch(self, train_loss: float, val_loss: float):
+        self._val_loss = val_loss
+        self._summary["training_loss"].append(train_loss)
+        self._summary["validation_loss"].append(val_loss)
+
+    def _run(self, net, epoch: Callable, max_num_epochs: int, stop_after_epochs: int,
+             opt: Optional[_DeviceAdam] = None):
+        """The training loop (base.py:1060-1138).  `epoch()` trains and validates one epoch and returns
+        (training loss, validation loss) after the epoch's one host sync."""
+        while self.epoch <= max_num_epochs and not self._converged(net, stop_after_epochs):
+            t0 = time.time()
+            self._record_epoch(*epoch())
+            self._summary["epoch_durations_sec"].append(time.time() - t0)
+            self.epoch += 1
+        if self.epoch > max_num_epochs:   # base.py:1122-1129
+            if self._val_loss < self._best_val_loss:
+                self._best_val_loss, self._best_flat = self._val_loss, net.flat.data.clone()
+            elif self._best_flat is not None:
+                net.flat.data.copy_(self._best_flat)
+            warnings.warn(f"Maximum number of epochs `max_num_epochs={max_num_epochs}` reached, "
+                          "but network has not yet fully converged.", stacklevel=3)
+        self._summary["epochs_trained"].append(self.epoch)
+        self._summary["best_validation_loss"].append(self._best_val_loss)
+        net.zero_grad(set_to_none=True)
+        if opt is not None:
+            opt.close()
+
+    @property
+    def summary(self):
+        return self._summary
+
+
+class _PotentialPosterior:
+    """`build_posterior` of the trainers whose estimator gives a potential (NLE: likelihood, NRE: ratio)."""
+
+    def build_posterior(self, density_estimator=None, prior=None, sample_with: str = "mcmc",
+                        mcmc_method: str = "slice_np_vectorized", mcmc_parameters: Optional[dict] = None,
+                        rejection_sampling_parameters: Optional[dict] = None, **kwargs):
+        """nle_base.py:274-378, nre_base.py:311-394 (`sample_with` in {"mcmc", "rejection"})."""
+        from .posteriors import MCMCPosterior, RejectionPosterior
+        est = deepcopy(density_estimator if density_estimator is not None else self._neural_net)
+        prior = prior if prior is not None else self._prior
+        potential_fn, theta_transform = self._potential(est, prior)
+        if sample_with == "mcmc":
+            return MCMCPosterior(potential_fn, proposal=prior, theta_transform=theta_transform, method=mcmc_method,
+                                 device=self._device, **(mcmc_parameters or {}))
+        if sample_with == "rejection":
+            return RejectionPosterior(potential_fn, proposal=prior, device=self._device,
+                                      **(rejection_sampling_parameters or {}))
+        raise NotImplementedError(sample_with)
+
+
+class _FlowTrainer(_Trainer):
+    """Shared first-round trainer for density estimators (NPE: q(theta|x); NLE: q(x|theta))."""
+
+    _swap = False   # NLE: estimator input = x, condition = theta
+    _nan_message = "NaN/Inf present in NPE loss."
+
+    def __init__(self, prior=None, density_estimator: Union[str, Callable] = "nsf",
+                 device: str = "cuda", logging_level: Union[int, str] = "WARNING",
+                 summary_writer=None, tracker=None, show_progress_bars: bool = False):
+        if isinstance(density_estimator, str):
+            factory = likelihood_nn if self._swap else posterior_nn
+            density_estimator = factory(model=density_estimator)
+        super().__init__(prior, density_estimator, device, show_progress_bars)
+
     def _inp_cond(self):
         """(estimator input set, condition set) as (N, .) device tensors."""
         th, xx = self._theta, self._x.reshape(self._x.shape[0], -1)
@@ -214,9 +477,7 @@ class _FlowTrainer:
               dataloader_kwargs: Optional[dict] = None) -> NSFEstimator:
         if calibration_kernel is not None and self._swap:
             raise ValueError("calibration_kernel is an argument of the posterior-estimator trainers (NPE)")
-        if self._theta is None:
-            raise RuntimeError("call append_simulations() first")
-        self._round = max(self._data_round_index) if getattr(self, "_data_round_index", None) else 0
+        self._round = max(self._data_round_index) if self._data_round_index else 0
         if self._round > 0 and not self._swap and not force_first_round_loss:
             # later rounds of NPE: atomic proposal correction (npe_c.py), eager steps
             return self._train_multiround(
@@ -230,88 +491,47 @@ class _FlowTrainer:
                                       "(append only the rounds to train on)")
         lib = L.load()
         dev = self._device
-        N = self._theta.shape[0]
-        rank, world, part = self._dp()
-        glob = world > 1 and part == "global"
-        self._dp_agree(N, "number of simulations") if glob else None
-        # --- split (base.py:525-539): CPU global generator, like the reference
-        n_train = int((1 - validation_fraction) * N)
-        n_val = N - n_train
-        if not resume_training or not hasattr(self, "train_indices"):
-            self.train_indices, self.val_indices = self._dp_split(N, n_train)
-        # --- network (npe_base.py:674-708): built from the CPU training split
-        if self._neural_net is None or retrain_from_scratch:
-            th_cpu = self._theta[self.train_indices.to(dev)].cpu()
-            x_cpu = self._x[self.train_indices.to(dev)].cpu()
-            self._neural_net = self._build_neural_net(th_cpu, x_cpu)
-            del th_cpu, x_cpu
-        net = self._neural_net.to(dev)
-        self._neural_net = net
-        if not resume_training:
-            self._dp_sync_net(net)
+        rank, world, glob = self._dp()
+        net, B, Bv, steps, vsteps = self._prepare(validation_fraction, training_batch_size, resume_training,
+                                                  retrain_from_scratch)
         if not isinstance(net, FlowEstimator):
             raise TypeError(f"{type(self).__name__} needs an sbi_b200 flow estimator, "
                             f"got {type(net).__name__}")
-        lay = net.layout
         if not net._embed_identity:
             raise NotImplementedError(
                 "the fused trainer supports nn.Identity() embedding nets; train estimators with "
                 "torch embedding nets through estimator.loss(...).backward()")
-        P = lay.n_params
-        B = min(training_batch_size, n_train)        # rows of one optimisation step (global batch if `glob`)
-        Bv = min(training_batch_size, n_val)
-        steps = n_train // B
-        vsteps = n_val // Bv if Bv > 0 else 0
         if glob and B % world:
             raise ValueError(f"partition='global' needs training_batch_size ({B}) divisible by the "
                              f"number of ranks ({world})")
         Bl = B // world if glob else B                 # rows this rank differentiates per step
         Btot = B if glob else B * world                # rows behind one update
-        self._dp_agree(steps, "number of steps per epoch")
         # validation rows: every rank evaluates its contiguous share of the epoch's validation order
         from .parallel import shard_range
         v_lo, v_hi = shard_range(vsteps * Bv, rank, world) if glob else (0, vsteps * Bv)
-
-        if not resume_training or not hasattr(self, "_opt_state"):
-            self._opt_state = torch.zeros(2 * P, dtype=torch.float32, device=dev)
-            self._opt_step = torch.zeros(2, dtype=torch.int32, device=dev)
-            self.epoch, self._val_loss = 0, float("Inf")
-            self._best_val_loss = float("Inf")
-            self._best_flat = None
-            self._epochs_since_last_improvement = 0
+        opt = self._optimizer(net, learning_rate, clip_max_norm, resume_training)
 
         inp_all, cond_all = self._inp_cond()
         if hasattr(net, "with_dummy"):     # `made`: the network's dummy first feature (nn_utils.py:166-167)
             inp_all = net.with_dummy(inp_all).contiguous()
         train_idx = self.train_indices.to(dev)
         val_idx = self.val_indices.to(dev)
+        n_train, n_val = train_idx.shape[0], val_idx.shape[0]
         # static buffers the epoch graph reads
         perm_buf = torch.empty(steps * B, dtype=torch.int64, device=dev)
         vperm_buf = torch.empty(max(vsteps * Bv, 1), dtype=torch.int64, device=dev)
-        grad = torch.zeros(P, dtype=torch.float32, device=dev)
-        sumsq = torch.zeros(lib.sbi_b200_sumsq_blocks(P), dtype=torch.float32, device=dev)
         n_part = net.vjp_parts(Bl)
         gpart = net._gpart(n_part)
         loss_acc = torch.zeros(2, dtype=torch.float32, device=dev)
         val_lp = torch.empty(max(vsteps * Bv, 1), dtype=torch.float32, device=dev)
         stats = torch.zeros(4, dtype=torch.float32, device=dev)   # train nll sum, bad, val nll sum, val bad
-        mask = net.net._mask
-        max_norm = float(clip_max_norm) if clip_max_norm is not None else 0.0
-        # data-parallel on one node: sum the gradients with our peer-memory kernel (graph-capturable);
-        # SBI_B200_NCCL=1 keeps the NCCL all-reduce (eager launches)
-        peer, grad_local = None, grad
-        if world > 1:
-            from .parallel import make_gradient_exchange
-            peer = make_gradient_exchange(P)      # None -> NCCL all-reduce, eager launches
-            if peer is not None:
-                grad_local = torch.zeros(P, dtype=torch.float32, device=dev)
 
         # calibration kernel (npe_base.py:373-378, :563-575): loss_r = K(x_r) * (-log q_r); the weights of
         # all simulations are evaluated once, a step's upstream gradient is -K(x_r) / B per row
         w_all = None
         if calibration_kernel is not None:
             w_all = torch.as_tensor(calibration_kernel(self._x), dtype=torch.float32).reshape(-1).to(dev).contiguous()
-            if w_all.shape[0] != N:
+            if w_all.shape[0] != self._theta.shape[0]:
                 raise ValueError("calibration_kernel(x) must return one weight per simulation")
             g_rows = torch.empty(Bl, dtype=torch.float32, device=dev)
             lp_rows = torch.empty(Bl, dtype=torch.float32, device=dev)
@@ -333,29 +553,7 @@ class _FlowTrainer:
                     fin = torch.isfinite(lp_rows)
                     loss_acc[0] -= (torch.where(fin, lp_rows, torch.zeros_like(lp_rows)) * w).sum()
                     loss_acc[1] += (~fin).sum()
-                if peer is not None:   # gradients summed over NVLink peer memory (csrc/peer.cu)
-                    L.check(lib.sbi_b200_reduce_partials(L.ptr(gpart), n_part, P, L.ptr(grad_local),
-                                                         L.stream_ptr()), "reduce_partials")
-                    peer.sum(grad_local, grad, mask, sumsq)
-                    L.check(lib.sbi_b200_adam_clip_step_norm(
-                        L.ptr(net.flat.data), L.ptr(grad), L.ptr(self._opt_state), L.ptr(self._opt_step),
-                        L.ptr(mask), P, learning_rate, 0.9, 0.999, 1e-8, max_norm, 1.0, L.ptr(sumsq),
-                        peer.n_sumsq, L.stream_ptr()), "adam_clip_step")
-                elif world > 1:   # the clip norm must be taken on the all-reduced gradient
-                    L.check(lib.sbi_b200_reduce_partials(L.ptr(gpart), n_part, P, L.ptr(grad),
-                                                         L.stream_ptr()), "reduce_partials")
-                    torch.distributed.all_reduce(grad)
-                    L.check(lib.sbi_b200_adam_clip_step(
-                        L.ptr(net.flat.data), L.ptr(grad), L.ptr(self._opt_state), L.ptr(self._opt_step),
-                        L.ptr(mask), P, learning_rate, 0.9, 0.999, 1e-8, max_norm, 1.0,
-                        L.stream_ptr()), "adam_clip_step")
-                else:           # single GPU: the reduction kernel also emits sum(g^2) partials
-                    L.check(lib.sbi_b200_reduce_partials_norm(L.ptr(gpart), n_part, P, L.ptr(grad), L.ptr(mask),
-                                                              L.ptr(sumsq), L.stream_ptr()), "reduce_partials")
-                    L.check(lib.sbi_b200_adam_clip_step_norm(
-                        L.ptr(net.flat.data), L.ptr(grad), L.ptr(self._opt_state), L.ptr(self._opt_step),
-                        L.ptr(mask), P, learning_rate, 0.9, 0.999, 1e-8, max_norm, 1.0, L.ptr(sumsq),
-                        sumsq.shape[0], L.stream_ptr()), "adam_clip_step")
+                opt.step_partials(gpart, n_part)
             stats[0:2].copy_(loss_acc)
             stats[2:4].zero_()
             if v_hi > v_lo:
@@ -391,69 +589,20 @@ class _FlowTrainer:
                     torch.distributed.broadcast(vperm_buf, 0)
 
         # warm-up (also sets kernel attributes) on a throw-away copy of the state, then capture
-        graph = None
-        if world == 1 or peer is not None:
-            snap = (net.flat.data.clone(), self._opt_state.clone(), self._opt_step.clone())
+        run = run_epoch
+        if opt.capturable:
             rng = torch.cuda.get_rng_state(dev)      # the warm-up's permutation draw leaves no trace:
             fill_perms()                             # a seed gives the same run with and without graphs
             torch.cuda.set_rng_state(rng, dev)
-            side = torch.cuda.Stream()
-            side.wait_stream(torch.cuda.current_stream())
-            with torch.cuda.stream(side):
-                run_epoch()
-            torch.cuda.current_stream().wait_stream(side)
-            net.flat.data.copy_(snap[0]); self._opt_state.copy_(snap[1]); self._opt_step.copy_(snap[2])
-            graph = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(graph):
-                run_epoch()
-            net.flat.data.copy_(snap[0]); self._opt_state.copy_(snap[1]); self._opt_step.copy_(snap[2])
+            run = _capture(opt, run_epoch, run_epoch)[0].replay
 
-        def converged() -> bool:
-            """base.py:1254-1284."""
-            if self.epoch == 0 or self._val_loss < self._best_val_loss:
-                self._best_val_loss = self._val_loss
-                self._epochs_since_last_improvement = 0
-                self._best_flat = net.flat.data.clone()
-            else:
-                self._epochs_since_last_improvement += 1
-            if self._epochs_since_last_improvement > stop_after_epochs - 1:
-                net.flat.data.copy_(self._best_flat)
-                return True
-            return False
-
-        while self.epoch <= max_num_epochs and not converged():
-            t0 = time.time()
+        def epoch():
             fill_perms()
-            if graph is not None:
-                graph.replay()
-            else:
-                run_epoch()
-            s = self._dp_sum(stats.tolist())   # the one host sync of the epoch (+ one tiny all-reduce)
-            if s[1] > 0 or s[3] > 0:
-                raise AssertionError("NaN/Inf present in NPE loss.")
-            train_loss = s[0] / (steps * Btot)
-            self._val_loss = s[2] / (vsteps * Bv * (1 if glob else world)) if vsteps > 0 else float("nan")
-            self._summary["training_loss"].append(train_loss)
-            self._summary["validation_loss"].append(self._val_loss)
-            self._summary["epoch_durations_sec"].append(time.time() - t0)
-            self.epoch += 1
+            run()
+            tl, vl = self._epoch_losses(stats)
+            return tl / (steps * Btot), (vl / (vsteps * Bv * (1 if glob else world)) if vsteps > 0 else float("nan"))
 
-        if self.epoch > max_num_epochs:   # base.py:1122-1129
-            if self._val_loss < self._best_val_loss:
-                self._best_val_loss = self._val_loss
-                self._best_flat = net.flat.data.clone()
-            elif self._best_flat is not None:
-                net.flat.data.copy_(self._best_flat)
-            warnings.warn(f"Maximum number of epochs `max_num_epochs={max_num_epochs}` reached, "
-                          "but network has not yet fully converged.", stacklevel=2)
-        self._summary["epochs_trained"].append(self.epoch)
-        self._summary["best_validation_loss"].append(self._best_val_loss)
-        net.zero_grad(set_to_none=True)
-        if peer is not None:
-            timed_out = peer.error()
-            peer.close()
-            if timed_out:
-                raise RuntimeError("peer-memory gradient exchange timed out (a rank fell behind or died)")
+        self._run(net, epoch, max_num_epochs, stop_after_epochs, opt)
         return deepcopy(net)
 
     def _train_multiround(self, training_batch_size, learning_rate, validation_fraction, stop_after_epochs,
@@ -466,11 +615,11 @@ class _FlowTrainer:
         operation sequence; the B x num_atoms evaluations per step are what the kernels are for."""
         from .multiround import atomic_log_prob_proposal_posterior, clamp_num_atoms
         from .posteriors import prior_to_device
-        if getattr(self, "_dist", None) is not None and self._dp()[1] > 1:
+        if self._dp()[1] > 1:
             raise NotImplementedError("multi-round training is single-process")
         dev = self._device
-        num_atoms = int(getattr(self, "_num_atoms", 10))
-        combined = bool(getattr(self, "_use_combined_loss", False))
+        num_atoms = int(self._num_atoms)
+        combined = bool(self._use_combined_loss)
         start_round = int(bool(discard_prior_samples) and self._round > 0)        # base.py _get_start_index
         rounds = torch.repeat_interleave(torch.as_tensor(self._data_round_index),
                                          torch.as_tensor(self._round_rows)).to(dev)
@@ -480,7 +629,7 @@ class _FlowTrainer:
         N = theta_all.shape[0]
         n_train = int((1 - validation_fraction) * N)
         n_val = N - n_train
-        if not resume_training or getattr(self, "_mr_split_n", None) != N:
+        if not resume_training or self._mr_split_n != N:
             perm = torch.randperm(N)
             self.train_indices, self.val_indices = perm[:n_train], perm[n_train:]
             self._mr_split_n = N
@@ -492,10 +641,9 @@ class _FlowTrainer:
         prior = prior_to_device(self._prior, dev)
         B, Bv = min(training_batch_size, n_train), min(training_batch_size, n_val)
         steps, vsteps = n_train // B, (n_val // Bv if Bv > 0 else 0)
-        if not resume_training or not hasattr(self, "_mr_opt"):
+        if not resume_training or self._mr_opt is None:
             self._mr_opt = torch.optim.Adam(list(net.parameters()), lr=learning_rate)
-            self.epoch, self._val_loss = 0, float("Inf")
-            self._best_val_loss, self._best_flat, self._epochs_since_last_improvement = float("Inf"), None, 0
+            self._reset_epochs()
         opt = self._mr_opt
         train_idx, val_idx = self.train_indices.to(dev), self.val_indices.to(dev)
         w_all = None
@@ -506,25 +654,12 @@ class _FlowTrainer:
             th, xx, mk = theta_all[idx], x_all[idx], masks_all[idx]
             lp = atomic_log_prob_proposal_posterior(net, prior, th, xx, mk, num_atoms, combined)
             if not bool(torch.isfinite(lp).all()):
-                raise AssertionError("NaN/Inf present in NPE loss.")
+                raise AssertionError(self._nan_message)
             return -lp if w_all is None else -lp * w_all[idx]
 
-        def converged() -> bool:
-            if self.epoch == 0 or self._val_loss < self._best_val_loss:
-                self._best_val_loss, self._epochs_since_last_improvement = self._val_loss, 0
-                self._best_flat = net.flat.data.clone()
-            else:
-                self._epochs_since_last_improvement += 1
-            if self._epochs_since_last_improvement > stop_after_epochs - 1:
-                net.flat.data.copy_(self._best_flat)
-                return True
-            return False
-
-        clamp_num_atoms(num_atoms, min(B, Bv) if vsteps > 0 else B)      # warn once, like the reference does per call
-        with warnings.catch_warnings():
-            warnings.filterwarnings("ignore", message="num_atoms=")
-            while self.epoch <= max_num_epochs and not converged():
-                t0 = time.time()
+        def epoch():
+            with warnings.catch_warnings():
+                warnings.filterwarnings("ignore", message="num_atoms=")
                 net.train()
                 perm = train_idx[torch.randperm(n_train, device=dev)]
                 tsum = torch.zeros((), device=dev)
@@ -542,27 +677,13 @@ class _FlowTrainer:
                     vperm = val_idx[torch.randperm(n_val, device=dev)] if vsteps > 0 else None
                     for s_ in range(vsteps):
                         vsum += losses_of(vperm[s_ * Bv:(s_ + 1) * Bv]).sum()
-                self._summary["training_loss"].append(float(tsum.item()) / (steps * B))
-                self._val_loss = float(vsum.item()) / (vsteps * Bv) if vsteps > 0 else float("nan")
-                self._summary["validation_loss"].append(self._val_loss)
-                self._summary["epoch_durations_sec"].append(time.time() - t0)
-                self.epoch += 1
-        if self.epoch > max_num_epochs:
-            if self._val_loss < self._best_val_loss:
-                self._best_val_loss, self._best_flat = self._val_loss, net.flat.data.clone()
-            elif self._best_flat is not None:
-                net.flat.data.copy_(self._best_flat)
-            warnings.warn(f"Maximum number of epochs `max_num_epochs={max_num_epochs}` reached, "
-                          "but network has not yet fully converged.", stacklevel=3)
-        self._summary["epochs_trained"].append(self.epoch)
-        self._summary["best_validation_loss"].append(self._best_val_loss)
-        net.zero_grad(set_to_none=True)
+            val_loss = float(vsum.item()) / (vsteps * Bv) if vsteps > 0 else float("nan")
+            return float(tsum.item()) / (steps * B), val_loss
+
+        clamp_num_atoms(num_atoms, min(B, Bv) if vsteps > 0 else B)      # warn once, like the reference does per call
+        self._run(net, epoch, max_num_epochs, stop_after_epochs)
         net._cache.clear()
         return deepcopy(net)
-
-    @property
-    def summary(self):
-        return self._summary
 
 
 class NPE(_FlowTrainer):
@@ -602,9 +723,14 @@ NPE_C = NPE
 SNPE = NPE
 
 
-class NLE(_FlowTrainer):
+class NLE(_PotentialPosterior, _FlowTrainer):
     """Neural likelihood estimation (reference: NLE_A, nle_base.py:190-272, _loss :380-392)."""
     _swap = True
+
+    @staticmethod
+    def _potential(est, prior):
+        from .potentials import likelihood_estimator_based_potential
+        return likelihood_estimator_based_potential(est, prior, x_o=None)
 
 
 NLE_A = NLE
@@ -612,47 +738,26 @@ SNLE = NLE
 
 
 # =================================================================================================
-def _nle_build_posterior(self, density_estimator=None, prior=None, sample_with: str = "mcmc",
-                         mcmc_method: str = "slice_np_vectorized", mcmc_parameters: Optional[dict] = None,
-                         rejection_sampling_parameters: Optional[dict] = None, **kwargs):
-    """nle_base.py:274-378 (`sample_with` in {"mcmc", "rejection"})."""
-    from .posteriors import MCMCPosterior, RejectionPosterior
-    from .potentials import likelihood_estimator_based_potential
-    est = deepcopy(density_estimator if density_estimator is not None else self._neural_net)
-    prior = prior if prior is not None else self._prior
-    potential_fn, theta_transform = likelihood_estimator_based_potential(est, prior, x_o=None)
-    if sample_with == "mcmc":
-        return MCMCPosterior(potential_fn, proposal=prior, theta_transform=theta_transform, method=mcmc_method,
-                             device=self._device, **(mcmc_parameters or {}))
-    if sample_with == "rejection":
-        return RejectionPosterior(potential_fn, proposal=prior, device=self._device,
-                                  **(rejection_sampling_parameters or {}))
-    raise NotImplementedError(sample_with)
-
-
-NLE.build_posterior = _nle_build_posterior
-
-
-class NRE_B(_FlowTrainer):
+class NRE_B(_PotentialPosterior, _Trainer):
     """Neural ratio estimation, NRE-B / SRE (reference: trainers/nre/nre_base.py:184-309 train,
     :396-415 `_classifier_logits`; trainers/nre/nre_b.py:157-182 `_loss`): 1-out-of-`num_atoms`
     classification of the jointly drawn (theta, x) pair against `num_atoms - 1` contrastive thetas
     from the same batch.  The classifier forward / backward run in the ratio kernels; the contrastive
     index draw and the softmax head are a handful of torch device ops."""
 
+    _nan_message = "NaN/Inf present in NRE-B loss."
+
     def __init__(self, prior=None, classifier: Union[str, Callable] = "resnet", device: str = "cuda",
                  logging_level: Union[int, str] = "warning", summary_writer=None, tracker=None,
                  show_progress_bars: bool = False):
         from .ratio import classifier_nn
-        self._prior = prior
-        self._device = _process_device(device)
-        self._build_neural_net = classifier_nn(classifier) if isinstance(classifier, str) else classifier
-        self._neural_net = None
-        self._theta = self._x = None
-        self.epoch, self._val_loss = 0, float("Inf")
-        self._summary = dict(epochs_trained=[], best_validation_loss=[], validation_loss=[],
-                             training_loss=[], epoch_durations_sec=[])
-        self._dist = None
+        super().__init__(prior, classifier_nn(classifier) if isinstance(classifier, str) else classifier, device,
+                         show_progress_bars)
+
+    @staticmethod
+    def _potential(est, prior):
+        from .potentials import ratio_estimator_based_potential
+        return ratio_estimator_based_potential(est, prior, x_o=None)
 
     @staticmethod
     def _contrastive_choices(B: int, k: int, device, rows: Optional[tuple] = None) -> Tensor:
@@ -704,40 +809,12 @@ class NRE_B(_FlowTrainer):
               clip_max_norm: Optional[float] = 5.0, resume_training: bool = False,
               discard_prior_samples: bool = False, retrain_from_scratch: bool = False,
               show_train_summary: bool = False, dataloader_kwargs: Optional[dict] = None):
-        if self._theta is None:
-            raise RuntimeError("call append_simulations() first")
-        lib = L.load()
         dev = self._device
-        N = self._theta.shape[0]
-        self._x2d = self._x.reshape(N, -1).contiguous()
-        rank, world, part = self._dp()
-        glob = world > 1 and part == "global"
-        if glob:
-            self._dp_agree(N, "number of simulations")
-        n_train = int((1 - validation_fraction) * N)
-        n_val = N - n_train
-        if not resume_training or not hasattr(self, "train_indices"):
-            self.train_indices, self.val_indices = self._dp_split(N, n_train)
-        B = min(training_batch_size, n_train)
-        Bv = min(training_batch_size, n_val)
-        clipped = min(B, Bv)
-        num_atoms = int(min(max(num_atoms, 2), clipped))     # nre_base.py:236-238 (clamp to batch size)
-        if self._neural_net is None or retrain_from_scratch:
-            tr = self.train_indices.to(dev)
-            self._neural_net = self._build_neural_net(self._theta[tr].cpu(), self._x[tr].cpu())
-        net = self._neural_net.to(dev)
-        self._neural_net = net
-        if not resume_training:
-            self._dp_sync_net(net)
-        P = net.layout.n_params
-        if not resume_training or not hasattr(self, "_opt_state"):
-            self._opt_state = torch.zeros(2 * P, dtype=torch.float32, device=dev)
-            self._opt_step = torch.zeros(2, dtype=torch.int32, device=dev)
-            self.epoch, self._val_loss = 0, float("Inf")
-            self._best_val_loss, self._best_flat, self._epochs_since_last_improvement = float("Inf"), None, 0
-        train_idx, val_idx = self.train_indices.to(dev), self.val_indices.to(dev)
-        steps, vsteps = n_train // B, (n_val // Bv if Bv > 0 else 0)
-        self._dp_agree(steps, "number of steps per epoch")
+        rank, world, glob = self._dp()
+        net, B, Bv, steps, vsteps = self._prepare(validation_fraction, training_batch_size, resume_training,
+                                                  retrain_from_scratch)
+        self._x2d = self._x.reshape(self._x.shape[0], -1).contiguous()
+        num_atoms = int(min(max(num_atoms, 2), min(B, Bv)))     # nre_base.py:236-238 (clamp to batch size)
         self._dp_agree(vsteps, "number of validation steps per epoch")
         if glob and (B % world or Bv % world):
             raise ValueError(f"partition='global' needs the batch sizes ({B}, {Bv}) divisible by the "
@@ -745,147 +822,37 @@ class NRE_B(_FlowTrainer):
         # rows of each (global) batch whose loss this rank differentiates / evaluates
         t_rows = (rank * (B // world), (rank + 1) * (B // world)) if glob else (0, B)
         v_rows = (rank * (Bv // world), (rank + 1) * (Bv // world)) if glob else (0, Bv)
-        max_norm = float(clip_max_norm) if clip_max_norm is not None else 0.0
-        peer = None
-        if world > 1:
-            from .parallel import make_gradient_exchange
-            peer = make_gradient_exchange(P)          # None -> NCCL all-reduce, eager launches
-        grad_sum = torch.zeros(P, dtype=torch.float32, device=dev) if peer is not None else None
-        sumsq = torch.zeros(peer.n_sumsq, dtype=torch.float32, device=dev) if peer is not None else None
-
-        def converged() -> bool:
-            if self.epoch == 0 or self._val_loss < self._best_val_loss:
-                self._best_val_loss, self._epochs_since_last_improvement = self._val_loss, 0
-                self._best_flat = net.flat.data.clone()
-            else:
-                self._epochs_since_last_improvement += 1
-            if self._epochs_since_last_improvement > stop_after_epochs - 1:
-                net.flat.data.copy_(self._best_flat)
-                return True
-            return False
-
-        # One CUDA graph per optimisation step and one per validation step: a step is ~15 small
-        # launches (contrastive draws, index gathers, logits kernel, logsumexp, VJP kernel, reduce,
-        # clip+Adam) that the host cannot issue as fast as the GPU runs them at the default batch
-        # of 200.  The batch indices come from a static buffer filled before each replay; random
-        # draws inside the graph use torch's graph-safe Philox offsets.
-        idx_buf = torch.zeros(B, dtype=torch.int64, device=dev)
-        vidx_buf = torch.zeros(max(Bv, 1), dtype=torch.int64, device=dev)
+        opt = self._optimizer(net, learning_rate, clip_max_norm, resume_training)
         train_sum = torch.zeros((), device=dev)
         val_sum = torch.zeros((), device=dev)
 
-        def train_step():
+        def train_step(idx):
             net.net.flat.grad = None
             # every rank's rows weigh 1/world of the update's batch mean; gradients are summed
-            loss = self._loss_on(net, idx_buf, num_atoms, rows=t_rows) / world
+            loss = self._loss_on(net, idx, num_atoms, rows=t_rows) / world
             loss.backward()
             train_sum.add_(loss.detach())
-            if peer is not None:       # gradient sum over NVLink peer memory + sum(g^2) partials
-                peer.sum(net.flat.grad, grad_sum, net.net._mask, sumsq)
-                L.check(lib.sbi_b200_adam_clip_step_norm(
-                    L.ptr(net.flat.data), L.ptr(grad_sum), L.ptr(self._opt_state), L.ptr(self._opt_step),
-                    L.ptr(net.net._mask), P, learning_rate, 0.9, 0.999, 1e-8, max_norm, 1.0, L.ptr(sumsq),
-                    peer.n_sumsq, L.stream_ptr()), "adam_clip_step")
-                return
-            if world > 1:
-                torch.distributed.all_reduce(net.flat.grad)
-            L.check(lib.sbi_b200_adam_clip_step(
-                L.ptr(net.flat.data), L.ptr(net.flat.grad), L.ptr(self._opt_state), L.ptr(self._opt_step),
-                L.ptr(net.net._mask), P, learning_rate, 0.9, 0.999, 1e-8, max_norm, 1.0, L.stream_ptr()),
-                "adam_clip_step")
+            opt.step(net.flat.grad)
 
-        def val_step():
+        def val_step(idx):
             with torch.no_grad():
-                val_sum.add_(self._loss_on(net, vidx_buf, num_atoms, rows=v_rows) / world)
+                val_sum.add_(self._loss_on(net, idx, num_atoms, rows=v_rows) / world)
 
-        g_train = g_val = None
-        if (os.environ.get("SBI_B200_NRE_GRAPH", "1") != "0" and B - 1 <= 4096 and steps > 0
-                and (world == 1 or peer is not None)):
-            snap = (net.flat.data.clone(), self._opt_state.clone(), self._opt_step.clone())
-            idx_buf.copy_(train_idx[:B])
-            if vsteps > 0:
-                vidx_buf.copy_(val_idx[:Bv])
-            side = torch.cuda.Stream()
-            side.wait_stream(torch.cuda.current_stream())
-            with torch.cuda.stream(side):          # warm-up outside capture (allocations, kernel attributes)
-                for _ in range(3):
-                    train_step()
-                if vsteps > 0:
-                    val_step()
-            torch.cuda.current_stream().wait_stream(side)
-            g_train = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(g_train):
-                train_step()
-            if vsteps > 0:
-                g_val = torch.cuda.CUDAGraph()
-                with torch.cuda.graph(g_val):
-                    val_step()
-            net.flat.data.copy_(snap[0]); self._opt_state.copy_(snap[1]); self._opt_step.copy_(snap[2])
+        graphs = os.environ.get("SBI_B200_NRE_GRAPH", "1") != "0" and B - 1 <= 4096
+        run_steps = self._step_epochs(opt, B, Bv, steps, vsteps, train_step, val_step, graphs)
 
-        while self.epoch <= max_num_epochs and not converged():
-            t0 = time.time()
-            perm = train_idx[torch.randperm(n_train, device=dev)]
-            vperm = val_idx[torch.randperm(n_val, device=dev)] if vsteps > 0 else None
-            if glob:      # one epoch order for all ranks: rank 0's
-                torch.distributed.broadcast(perm, 0)
-                if vperm is not None:
-                    torch.distributed.broadcast(vperm, 0)
+        def epoch():
             train_sum.zero_()
-            for s in range(steps):
-                idx_buf.copy_(perm[s * B:(s + 1) * B])
-                if g_train is not None:
-                    g_train.replay()
-                else:
-                    train_step()
             val_sum.zero_()
-            for s in range(vsteps):
-                vidx_buf.copy_(vperm[s * Bv:(s + 1) * Bv])
-                if g_val is not None:
-                    g_val.replay()
-                else:
-                    val_step()
+            run_steps()
             tl, vl = self._dp_sum([float(train_sum.item()), float(val_sum.item())])
             if not (math.isfinite(tl) and math.isfinite(vl)):
-                raise AssertionError("NaN/Inf present in NRE-B loss.")
+                raise AssertionError(self._nan_message)
             # the reference divides the sum of per-batch MEAN losses by steps * batch_size (SURVEY a15 quirk)
-            self._summary["training_loss"].append(tl / (steps * B))
-            self._val_loss = vl / (vsteps * Bv) if vsteps > 0 else float("nan")
-            self._summary["validation_loss"].append(self._val_loss)
-            self._summary["epoch_durations_sec"].append(time.time() - t0)
-            self.epoch += 1
-        if self.epoch > max_num_epochs:
-            if self._val_loss < self._best_val_loss:
-                self._best_val_loss, self._best_flat = self._val_loss, net.flat.data.clone()
-            elif self._best_flat is not None:
-                net.flat.data.copy_(self._best_flat)
-            warnings.warn(f"Maximum number of epochs `max_num_epochs={max_num_epochs}` reached, "
-                          "but network has not yet fully converged.", stacklevel=2)
-        self._summary["epochs_trained"].append(self.epoch)
-        self._summary["best_validation_loss"].append(self._best_val_loss)
-        net.zero_grad(set_to_none=True)
-        if peer is not None:
-            timed_out = peer.error()
-            peer.close()
-            if timed_out:
-                raise RuntimeError("peer-memory gradient exchange timed out (a rank fell behind or died)")
-        return deepcopy(net)
+            return tl / (steps * B), (vl / (vsteps * Bv) if vsteps > 0 else float("nan"))
 
-    def build_posterior(self, density_estimator=None, prior=None, sample_with: str = "mcmc",
-                        mcmc_method: str = "slice_np_vectorized", mcmc_parameters: Optional[dict] = None,
-                        rejection_sampling_parameters: Optional[dict] = None, **kwargs):
-        """nre_base.py:311-394."""
-        from .posteriors import MCMCPosterior, RejectionPosterior
-        from .potentials import ratio_estimator_based_potential
-        est = deepcopy(density_estimator if density_estimator is not None else self._neural_net)
-        prior = prior if prior is not None else self._prior
-        potential_fn, theta_transform = ratio_estimator_based_potential(est, prior, x_o=None)
-        if sample_with == "mcmc":
-            return MCMCPosterior(potential_fn, proposal=prior, theta_transform=theta_transform, method=mcmc_method,
-                                 device=self._device, **(mcmc_parameters or {}))
-        if sample_with == "rejection":
-            return RejectionPosterior(potential_fn, proposal=prior, device=self._device,
-                                      **(rejection_sampling_parameters or {}))
-        raise NotImplementedError(sample_with)
+        self._run(net, epoch, max_num_epochs, stop_after_epochs, opt)
+        return deepcopy(net)
 
 
 SNRE_B = NRE_B
@@ -922,7 +889,7 @@ class BNRE(NRE_A):
 
     def train(self, regularization_strength: float = 100.0, training_batch_size: int = 200, **kwargs):
         self._regularization_strength = float(regularization_strength)
-        if getattr(self, "_dist", None) is not None and self._dp()[1] > 1:
+        if self._dp()[1] > 1:
             raise NotImplementedError("the balancing regulariser is a function of the batch mean: BNRE trains "
                                       "on one process")
         return NRE_A.train(self, training_batch_size=training_batch_size, **kwargs)
@@ -956,56 +923,31 @@ SNRE_C = NRE_C
 
 
 # =================================================================================================
-class FMPE(_FlowTrainer):
+class FMPE(_Trainer):
     """Flow-matching posterior estimation (reference: trainers/vfpe/fmpe.py, base_vf_inference.py:
     train :206-350, validation at fixed times :524-543, EMA-smoothed summaries :589-636, z-score of
     the loss as stopping rule :352-420)."""
+
+    _nan_message = "NaN/Inf present in FMPE loss."
 
     def __init__(self, prior=None, density_estimator: Union[str, Callable] = "mlp", device: str = "cuda",
                  logging_level: Union[int, str] = "WARNING", summary_writer=None, tracker=None,
                  show_progress_bars: bool = False):
         from .flowmatching import posterior_flow_nn
-        self._prior = prior
-        self._device = _process_device(device)
-        self._build_neural_net = (posterior_flow_nn(model=density_estimator)
-                                  if isinstance(density_estimator, str) else density_estimator)
-        self._neural_net = None
-        self._theta = self._x = None
-        self.epoch, self._val_loss = 0, float("Inf")
-        self._summary = dict(epochs_trained=[], best_validation_loss=[], validation_loss=[], training_loss=[],
-                             epoch_durations_sec=[])
-        self._dist = None
+        if isinstance(density_estimator, str):
+            density_estimator = posterior_flow_nn(model=density_estimator)
+        super().__init__(prior, density_estimator, device, show_progress_bars)
 
     def train(self, training_batch_size: int = 200, learning_rate: float = 5e-4, validation_fraction: float = 0.1,
               stop_after_epochs: int = 20, max_num_epochs: int = 2 ** 31 - 1, clip_max_norm: Optional[float] = 5.0,
               calibration_kernel=None, ema_loss_decay: float = 0.1, validation_times: Union[Tensor, int] = 10,
               validation_times_nugget: float = 0.05, resume_training: bool = False, **kwargs):
-        if self._theta is None:
-            raise RuntimeError("call append_simulations() first")
         self._vf_check_rounds(kwargs)
-        lib = L.load()
         dev = self._device
-        N = self._theta.shape[0]
-        x2d = self._x.reshape(N, -1).contiguous()
-        rank, world, part = self._dp()
-        glob = world > 1 and part == "global"
-        if glob:
-            self._dp_agree(N, "number of simulations")
-        n_train = int((1 - validation_fraction) * N)
-        n_val = N - n_train
-        if not resume_training or not hasattr(self, "train_indices"):
-            self.train_indices, self.val_indices = self._dp_split(N, n_train)
-        if self._neural_net is None:
-            tr = self.train_indices.to(dev)
-            self._neural_net = self._build_neural_net(self._theta[tr].cpu(), self._x[tr].cpu())
-        net = self._neural_net.to(dev)
-        self._neural_net = net
-        if not resume_training:
-            self._dp_sync_net(net)
-        P, D = net.layout.n_params, net.layout.D
-        B, Bv = min(training_batch_size, n_train), min(training_batch_size, n_val)
-        steps, vsteps = n_train // B, (n_val // Bv if Bv > 0 else 0)
-        self._dp_agree(steps, "number of steps per epoch")
+        rank, world, glob = self._dp()
+        net, B, Bv, steps, vsteps = self._prepare(validation_fraction, training_batch_size, resume_training)
+        x2d = self._x.reshape(self._x.shape[0], -1).contiguous()
+        D = net.layout.D
         self._dp_agree(vsteps, "number of validation steps per epoch")
         if glob and (B % world or Bv % world):
             raise ValueError(f"partition='global' needs the batch sizes ({B}, {Bv}) divisible by the "
@@ -1013,32 +955,15 @@ class FMPE(_FlowTrainer):
         Bl, Bvl = (B // world, Bv // world) if glob else (B, Bv)    # rows of a batch this rank handles
         o_t, o_v = (rank * Bl, rank * Bvl) if glob else (0, 0)
         Btot = B if glob else B * world                              # rows behind one update
-        if isinstance(validation_times, int):
-            validation_times = torch.linspace(net.t_min + validation_times_nugget,
-                                              net.t_max - validation_times_nugget, validation_times)
-        vt = validation_times.to(dev).float()
-        if not resume_training or not hasattr(self, "_opt_state"):
-            self._opt_state = torch.zeros(2 * P, dtype=torch.float32, device=dev)
-            self._opt_step = torch.zeros(2, dtype=torch.int32, device=dev)
-            self.epoch, self._val_loss = 0, float("Inf")
+        vt = self._validation_times(net, validation_times, validation_times_nugget)
+        opt = self._optimizer(net, learning_rate, clip_max_norm, resume_training)
+        self._ema_loss_decay = ema_loss_decay
         train_idx, val_idx = self.train_indices.to(dev), self.val_indices.to(dev)
-        grad = torch.zeros(P, dtype=torch.float32, device=dev)
+        n_train, n_val = train_idx.shape[0], val_idx.shape[0]
         loss_acc = torch.zeros(2, dtype=torch.float32, device=dev)
-        max_norm = float(clip_max_norm) if clip_max_norm is not None else 0.0
-        # data-parallel on one node: the gradient sum is our peer-memory kernel inside the epoch graph
-        peer, grad_local = None, grad
-        sumsq = None
-        if world > 1:
-            from .parallel import make_gradient_exchange
-            peer = make_gradient_exchange(P)      # None -> NCCL all-reduce, eager launches
-            if peer is not None:
-                grad_local = torch.zeros(P, dtype=torch.float32, device=dev)
-                sumsq = torch.zeros(peer.n_sumsq, dtype=torch.float32, device=dev)
 
-        converged = lambda: self._vf_converged(net, stop_after_epochs)
-
-        # One CUDA graph per epoch (single GPU): every step is [t ~ U, theta_1 ~ N draws, fused loss
-        # fwd+bwd kernel, reduce, clip+Adam]; the epoch's row permutations live in static buffers.
+        # One CUDA graph per epoch: every step is [t ~ U, theta_1 ~ N draws, fused loss fwd+bwd kernel,
+        # reduce, clip+Adam]; the epoch's row permutations live in static buffers.
         perm_buf = torch.zeros(max(steps * B, 1), dtype=torch.int64, device=dev)
         vperm_buf = torch.zeros(max(vsteps * Bv, 1), dtype=torch.int64, device=dev)
         stats = torch.zeros(4, dtype=torch.float32, device=dev)     # train loss sum, bad, val loss sum, bad
@@ -1051,20 +976,7 @@ class FMPE(_FlowTrainer):
                 eps = torch.randn(Bl, D, device=dev)
                 _, gpart, n_part = net.loss_raw(self._theta, x2d, tms, eps, index=idx, g_const=1.0 / Btot,
                                                 loss_acc=loss_acc, want_loss=False)
-                L.check(lib.sbi_b200_reduce_partials(L.ptr(gpart), n_part, P, L.ptr(grad_local), L.stream_ptr()),
-                        "reduce")
-                if peer is not None:
-                    peer.sum(grad_local, grad, net.net._mask, sumsq)
-                    L.check(lib.sbi_b200_adam_clip_step_norm(
-                        L.ptr(net.flat.data), L.ptr(grad), L.ptr(self._opt_state), L.ptr(self._opt_step),
-                        L.ptr(net.net._mask), P, learning_rate, 0.9, 0.999, 1e-8, max_norm, 1.0, L.ptr(sumsq),
-                        peer.n_sumsq, L.stream_ptr()), "adam")
-                    continue
-                if world > 1:
-                    torch.distributed.all_reduce(grad)
-                L.check(lib.sbi_b200_adam_clip_step(L.ptr(net.flat.data), L.ptr(grad), L.ptr(self._opt_state),
-                                                    L.ptr(self._opt_step), L.ptr(net.net._mask), P, learning_rate,
-                                                    0.9, 0.999, 1e-8, max_norm, 1.0, L.stream_ptr()), "adam")
+                opt.step_partials(gpart, n_part)
             stats[0:2].copy_(loss_acc)
             # validation: every batch evaluated at all validation times (:524-543); g = 0 -> loss only
             loss_acc.zero_()
@@ -1085,43 +997,28 @@ class FMPE(_FlowTrainer):
                 torch.distributed.broadcast(perm_buf, 0)
                 torch.distributed.broadcast(vperm_buf, 0)
 
-        graph = None
-        if (world == 1 or peer is not None) and os.environ.get("SBI_B200_FMPE_GRAPH", "1") != "0" and steps > 0:
-            snap = (net.flat.data.clone(), self._opt_state.clone(), self._opt_step.clone())
+        run = run_epoch
+        if opt.capturable and os.environ.get("SBI_B200_FMPE_GRAPH", "1") != "0" and steps > 0:
             fill_perms()
-            side = torch.cuda.Stream()
-            side.wait_stream(torch.cuda.current_stream())
-            with torch.cuda.stream(side):
-                run_epoch()
-            torch.cuda.current_stream().wait_stream(side)
-            net.flat.data.copy_(snap[0]); self._opt_state.copy_(snap[1]); self._opt_step.copy_(snap[2])
-            graph = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(graph):
-                run_epoch()
-            net.flat.data.copy_(snap[0]); self._opt_state.copy_(snap[1]); self._opt_step.copy_(snap[2])
+            run = _capture(opt, run_epoch, run_epoch)[0].replay
 
-        while self.epoch <= max_num_epochs and not converged():
-            t0 = time.time()
+        def epoch():
             fill_perms()
-            if graph is not None:
-                graph.replay()
-            else:
-                run_epoch()
-            tl, tb, vl, vb = self._dp_sum(stats.tolist())      # the one host sync of the epoch
-            if tb > 0 or vb > 0:
-                raise AssertionError("NaN/Inf present in FMPE loss.")
-            train_loss = tl / (steps * Btot)
+            run()
+            tl, vl = self._epoch_losses(stats)
             val_loss = vl / (vsteps * Bv * (1 if glob else world) * vt.shape[0]) if vsteps > 0 else float("nan")
             # the reference normalises by len(loader) * loader.batch_size, i.e. WITHOUT the repeat over times
             val_loss *= vt.shape[0] if vsteps > 0 else 1.0
-            self._vf_record_epoch(train_loss, val_loss, ema_loss_decay, t0)
-        self._vf_finish(net, max_num_epochs)
-        if peer is not None:
-            timed_out = peer.error()
-            peer.close()
-            if timed_out:
-                raise RuntimeError("peer-memory gradient exchange timed out (a rank fell behind or died)")
+            return tl / (steps * Btot), val_loss
+
+        self._run(net, epoch, max_num_epochs, stop_after_epochs, opt)
         return deepcopy(net)
+
+    def _validation_times(self, net, validation_times: Union[Tensor, int], nugget: float) -> Tensor:
+        """The fixed times every validation batch is evaluated at (base_vf_inference.py:524-543)."""
+        if isinstance(validation_times, int):
+            validation_times = torch.linspace(net.t_min + nugget, net.t_max - nugget, validation_times)
+        return validation_times.to(self._device).float()
 
     def _vf_check_rounds(self, kwargs):
         """base_vf_inference.py:451-496: only the first-round loss exists for vector-field trainers."""
@@ -1130,7 +1027,7 @@ class FMPE(_FlowTrainer):
             raise NotImplementedError(
                 f"Multi-round {self.__class__.__name__} with arbitrary proposals is not implemented")
 
-    def _vf_converged(self, net, stop_after_epochs: int) -> bool:
+    def _converged(self, net, stop_after_epochs: int) -> bool:
         """base_vf_inference.py:352-420: an epoch counts as "no improvement" only if the validation loss sits more
         than two standard deviations (of the recent EMA-smoothed losses) above the best one."""
         if self.epoch == 0:
@@ -1151,27 +1048,17 @@ class FMPE(_FlowTrainer):
             return True
         return False
 
-    def _vf_record_epoch(self, train_loss: float, val_loss: float, ema_loss_decay: float, t0: float):
+    def _record_epoch(self, train_loss: float, val_loss: float):
         # base.py:1110 keeps the RAW validation loss in self._val_loss (what _converged compares
         # with the best loss); only the summaries hold the exponential moving averages
         # (base_vf_inference.py:589-636), whose spread normalises the stopping rule
         self._val_loss = val_loss
         if self._summary["training_loss"]:
-            train_loss = (1 - ema_loss_decay) * self._summary["training_loss"][-1] + ema_loss_decay * train_loss
-            val_loss = (1 - ema_loss_decay) * self._summary["validation_loss"][-1] + ema_loss_decay * val_loss
+            decay = self._ema_loss_decay
+            train_loss = (1 - decay) * self._summary["training_loss"][-1] + decay * train_loss
+            val_loss = (1 - decay) * self._summary["validation_loss"][-1] + decay * val_loss
         self._summary["training_loss"].append(train_loss)
         self._summary["validation_loss"].append(val_loss)
-        self._summary["epoch_durations_sec"].append(time.time() - t0)
-        self.epoch += 1
-
-    def _vf_finish(self, net, max_num_epochs: int):
-        if self.epoch > max_num_epochs:
-            if self._val_loss < self._best_val_loss:
-                self._best_val_loss, self._best_flat = self._val_loss, net.flat.data.clone()
-            elif self._best_flat is not None:
-                net.flat.data.copy_(self._best_flat)
-        self._summary["epochs_trained"].append(self.epoch)
-        self._summary["best_validation_loss"].append(self._best_val_loss)
 
     def build_posterior(self, density_estimator=None, prior=None, sample_with: str = "ode", **kwargs):
         from .posteriors import VectorFieldPosterior
@@ -1192,6 +1079,8 @@ class NPSE(FMPE):
     parameter-gradient kernel, clip + Adam kernel], captured once as a CUDA graph and replayed per batch; the
     validation step (all validation times at once, base_vf_inference.py:524-543) is a second graph."""
 
+    _nan_message = "NaN/Inf present in NPSE loss."
+
     def __init__(self, prior=None, vf_estimator: Union[str, Callable, None] = None,
                  score_estimator: Union[str, Callable, None] = None, density_estimator: Optional[Callable] = None,
                  sde_type: Optional[str] = None, device: str = "cuda", logging_level: Union[int, str] = "WARNING",
@@ -1201,121 +1090,61 @@ class NPSE(FMPE):
         if len(given) > 1:
             raise ValueError("pass only one of vf_estimator / score_estimator / density_estimator")
         est = given[0] if given else "mlp"
-        super().__init__(prior=prior, density_estimator=(lambda *a: None), device=device)
         if isinstance(est, str):
-            self._build_neural_net = posterior_score_nn(model=est, sde_type=sde_type or "ve")
-        else:
-            if sde_type is not None:
-                warnings.warn("sde_type is ignored when a build function is passed", stacklevel=2)
-            self._build_neural_net = est
+            est = posterior_score_nn(model=est, sde_type=sde_type or "ve")
+        elif sde_type is not None:
+            warnings.warn("sde_type is ignored when a build function is passed", stacklevel=2)
+        _Trainer.__init__(self, prior, est, device, show_progress_bars)
 
     def train(self, training_batch_size: int = 200, learning_rate: float = 5e-4, validation_fraction: float = 0.1,
               stop_after_epochs: int = 20, max_num_epochs: int = 2 ** 31 - 1, clip_max_norm: Optional[float] = 5.0,
               calibration_kernel=None, ema_loss_decay: float = 0.1, validation_times: Union[Tensor, int] = 10,
               validation_times_nugget: float = 0.05, resume_training: bool = False, **kwargs):
-        if self._theta is None:
-            raise RuntimeError("call append_simulations() first")
         self._vf_check_rounds(kwargs)
         if self._dp()[1] > 1:
             raise NotImplementedError("NPSE training is single-process")
-        lib = L.load()
         dev = self._device
-        N = self._theta.shape[0]
-        x2d = self._x.reshape(N, -1).contiguous()
-        n_train = int((1 - validation_fraction) * N)
-        n_val = N - n_train
-        if not resume_training or not hasattr(self, "train_indices"):
-            self.train_indices, self.val_indices = self._dp_split(N, n_train)
-        if self._neural_net is None:
-            tr = self.train_indices.to(dev)
-            self._neural_net = self._build_neural_net(self._theta[tr].cpu(), self._x[tr].cpu())
-        net = self._neural_net.to(dev)
-        self._neural_net = net
-        P = net.layout.n_params
-        B, Bv = min(training_batch_size, n_train), min(training_batch_size, n_val)
-        steps, vsteps = n_train // B, (n_val // Bv if Bv > 0 else 0)
-        if isinstance(validation_times, int):
-            validation_times = torch.linspace(net.t_min + validation_times_nugget,
-                                              net.t_max - validation_times_nugget, validation_times)
-        vt = validation_times.to(dev).float()
+        net, B, Bv, steps, vsteps = self._prepare(validation_fraction, training_batch_size, resume_training)
+        x2d = self._x.reshape(self._x.shape[0], -1).contiguous()
+        vt = self._validation_times(net, validation_times, validation_times_nugget)
         nt = vt.shape[0]
-        if not resume_training or not hasattr(self, "_opt_state"):
-            self._opt_state = torch.zeros(2 * P, dtype=torch.float32, device=dev)
-            self._opt_step = torch.zeros(2, dtype=torch.int32, device=dev)
-            self.epoch, self._val_loss = 0, float("Inf")
-        train_idx, val_idx = self.train_indices.to(dev), self.val_indices.to(dev)
-        max_norm = float(clip_max_norm) if clip_max_norm is not None else 0.0
+        opt = self._optimizer(net, learning_rate, clip_max_norm, resume_training)
+        self._ema_loss_decay = ema_loss_decay
         w_all = None
         if calibration_kernel is not None:
             w_all = torch.as_tensor(calibration_kernel(self._x), dtype=torch.float32).reshape(-1).to(dev)
-        idx_buf = torch.zeros(B, dtype=torch.int64, device=dev)
-        vidx_buf = torch.zeros(max(Bv, 1), dtype=torch.int64, device=dev)
         stats = torch.zeros(4, dtype=torch.float32, device=dev)     # train loss sum, bad, val loss sum, bad
 
         def losses_on(idx, times):
             losses = net.loss(self._theta[idx], x2d[idx], times=times)
             return losses if w_all is None else w_all[idx] * losses
 
-        def train_step():
+        def train_step(idx):
             net.net.flat.grad = None
-            losses = losses_on(idx_buf, None)
+            losses = losses_on(idx, None)
             losses.mean().backward()
             ld = losses.detach()
             stats[0] += ld.sum()
             stats[1] += (~torch.isfinite(ld)).sum()
-            L.check(lib.sbi_b200_adam_clip_step(
-                L.ptr(net.flat.data), L.ptr(net.flat.grad), L.ptr(self._opt_state), L.ptr(self._opt_step),
-                L.ptr(net.net._mask), P, learning_rate, 0.9, 0.999, 1e-8, max_norm, 1.0, L.stream_ptr()),
-                "adam_clip_step")
+            opt.step(net.flat.grad)
 
-        def val_step():      # the batch repeated over all validation times (base_vf_inference.py:524-543)
+        def val_step(idx):      # the batch repeated over all validation times (base_vf_inference.py:524-543)
             with torch.no_grad():
-                ld = losses_on(vidx_buf.repeat(nt), vt.repeat_interleave(Bv))
+                ld = losses_on(idx.repeat(nt), vt.repeat_interleave(Bv))
                 stats[2] += ld.sum()
                 stats[3] += (~torch.isfinite(ld)).sum()
 
-        g_train = g_val = None
-        if os.environ.get("SBI_B200_NPSE_GRAPH", "1") != "0" and steps > 0:
-            snap = (net.flat.data.clone(), self._opt_state.clone(), self._opt_step.clone())
-            idx_buf.copy_(train_idx[:B])
-            if vsteps > 0:
-                vidx_buf.copy_(val_idx[:Bv])
-            side = torch.cuda.Stream()
-            side.wait_stream(torch.cuda.current_stream())
-            with torch.cuda.stream(side):          # warm-up outside capture (allocations, kernel attributes)
-                for _ in range(3):
-                    train_step()
-                if vsteps > 0:
-                    val_step()
-            torch.cuda.current_stream().wait_stream(side)
-            g_train = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(g_train):
-                train_step()
-            if vsteps > 0:
-                g_val = torch.cuda.CUDAGraph()
-                with torch.cuda.graph(g_val):
-                    val_step()
-            net.flat.data.copy_(snap[0]); self._opt_state.copy_(snap[1]); self._opt_step.copy_(snap[2])
+        graphs = os.environ.get("SBI_B200_NPSE_GRAPH", "1") != "0"
+        run_steps = self._step_epochs(opt, B, Bv, steps, vsteps, train_step, val_step, graphs)
 
-        while self.epoch <= max_num_epochs and not self._vf_converged(net, stop_after_epochs):
-            t0 = time.time()
-            perm = train_idx[torch.randperm(n_train, device=dev)]
-            vperm = val_idx[torch.randperm(n_val, device=dev)] if vsteps > 0 else None
+        def epoch():
             stats.zero_()
-            for s_ in range(steps):
-                idx_buf.copy_(perm[s_ * B:(s_ + 1) * B])
-                g_train.replay() if g_train is not None else train_step()
-            for s_ in range(vsteps):
-                vidx_buf.copy_(vperm[s_ * Bv:(s_ + 1) * Bv])
-                g_val.replay() if g_val is not None else val_step()
-            tl, tb, vl, vb = stats.tolist()                    # the one host sync of the epoch
-            if tb > 0 or vb > 0:
-                raise AssertionError("NaN/Inf present in NPSE loss.")
+            run_steps()
+            tl, vl = self._epoch_losses(stats)
             # the reference normalises the validation sum by len(loader) * batch_size, i.e. WITHOUT the repeat over times
-            self._vf_record_epoch(tl / (steps * B), vl / (vsteps * Bv) if vsteps > 0 else float("nan"),
-                                  ema_loss_decay, t0)
-        self._vf_finish(net, max_num_epochs)
-        net.zero_grad(set_to_none=True)
+            return tl / (steps * B), (vl / (vsteps * Bv) if vsteps > 0 else float("nan"))
+
+        self._run(net, epoch, max_num_epochs, stop_after_epochs, opt)
         net._cache.clear()
         return deepcopy(net)
 

@@ -159,9 +159,9 @@ def test_data_parallel_training_two_gpus(cuda_lib):
         assert all(v == v for v in vl) and vl[-1] < vl[0], vl
 
 
-def _run2(target, timeout=600, world=2):
-    if torch.cuda.device_count() < world:
-        pytest.skip(f"needs {world} GPUs on one node")
+def _run2(target, timeout=600, world=2, gpus=2):
+    if torch.cuda.device_count() < gpus:
+        pytest.skip(f"needs {gpus} GPUs on one node")
     import torch.multiprocessing as mp
     ctx = mp.get_context("spawn")
     q = ctx.Queue()
@@ -176,11 +176,16 @@ def _run2(target, timeout=600, world=2):
     return sorted(res)
 
 
-def _init(rank, world, port):
+def _init(rank, world, port, backend="nccl"):
+    """backend="gloo": every rank on cuda:0, gradients all-reduced through gloo (the NCCL-path code)."""
     import torch.distributed as dist
     os.environ.update(MASTER_ADDR="127.0.0.1", MASTER_PORT=str(port))
-    torch.cuda.set_device(rank)
-    dist.init_process_group("nccl", rank=rank, world_size=world, device_id=torch.device("cuda", rank))
+    if backend == "nccl":
+        torch.cuda.set_device(rank)
+        dist.init_process_group("nccl", rank=rank, world_size=world, device_id=torch.device("cuda", rank))
+    else:
+        os.environ["SBI_B200_NCCL"] = "1"
+        dist.init_process_group("gloo", rank=rank, world_size=world)
     return dist
 
 
@@ -194,6 +199,8 @@ def _lg(n, D, seed):
 
 
 def _identical(dist, flat, world):
+    if dist.get_backend() != "nccl":
+        flat = flat.cpu()
     both = [torch.zeros_like(flat) for _ in range(world)]
     dist.all_gather(both, flat)
     return all(torch.equal(both[0], b) for b in both)
@@ -234,16 +241,17 @@ def test_peer_exchange_epochs_of_one_to_three_steps(cuda_lib):
                                     f"({100 * frac_off:.2f}% of the weights by > 5e-5, max {dmax:.3e})"
 
 
-def _global_worker(rank, world, port, q):
+def _global_worker(rank, world, port, q, backend="nccl"):
     """partition='global' (SURVEY 8e): same data on every rank, rank 0's split and epoch orders, rank r
     takes rows [r*B/G, (r+1)*B/G) of each global batch: the run equals the single-GPU run up to the
     summation order of the gradient partials."""
     from sbi_b200.inference import FMPE, NPE, NRE_B
-    dist = _init(rank, world, port)
+    dist = _init(rank, world, port, backend)
+    dev = f"cuda:{rank}" if backend == "nccl" else "cuda:0"
     prior, theta, x = _lg(4000, 3, 5)                   # identical data on every rank
     res = {}
     torch.manual_seed(0)
-    inf = NPE(prior, density_estimator="nsf", device=f"cuda:{rank}").data_parallel("global")
+    inf = NPE(prior, density_estimator="nsf", device=dev).data_parallel("global")
     est = inf.append_simulations(theta, x).train(training_batch_size=400, max_num_epochs=3)
     res["npe_same"] = _identical(dist, est.flat.data, world)
     res["npe_val"] = list(inf.summary["validation_loss"])
@@ -256,17 +264,17 @@ def _global_worker(rank, world, port, q):
         res["solo_train"] = list(solo.summary["training_loss"])
     dist.barrier()
     torch.manual_seed(1)
-    fm = FMPE(prior, device=f"cuda:{rank}").data_parallel("global")
+    fm = FMPE(prior, device=dev).data_parallel("global")
     e2 = fm.append_simulations(theta, x).train(training_batch_size=400, max_num_epochs=4)
     res["fm_same"] = _identical(dist, e2.flat.data, world)
     res["fm_train"] = list(fm.summary["training_loss"])
     torch.manual_seed(2)
-    nre = NRE_B(prior, device=f"cuda:{rank}").data_parallel("global")
+    nre = NRE_B(prior, device=dev).data_parallel("global")
     e3 = nre.append_simulations(theta, x).train(training_batch_size=400, max_num_epochs=4)
     res["nre_same"] = _identical(dist, e3.flat.data, world)
     res["nre_val"] = list(nre.summary["validation_loss"])
     torch.manual_seed(3 + rank)                         # weak mode for the other two trainers
-    fm = FMPE(prior, device=f"cuda:{rank}").data_parallel("local")
+    fm = FMPE(prior, device=dev).data_parallel("local")
     e4 = fm.append_simulations(theta, x).train(training_batch_size=400, max_num_epochs=3)
     res["fm_local_same"] = _identical(dist, e4.flat.data, world)
     q.put((rank, res))
@@ -274,8 +282,7 @@ def _global_worker(rank, world, port, q):
     dist.destroy_process_group()
 
 
-def test_global_batch_data_parallel_all_trainers(cuda_lib):
-    out = dict(_run2(_global_worker, timeout=900))
+def _check_global(out):
     for rank, res in out.items():
         for k in ("npe_same", "fm_same", "nre_same", "fm_local_same"):
             assert res[k], f"rank {rank}: {k} failed (replicas diverged)"
@@ -285,3 +292,14 @@ def test_global_batch_data_parallel_all_trainers(cuda_lib):
     # same batches, same updates: the loss curves of the 2-GPU and the 1-GPU run agree
     for a, b in zip(r0["npe_train"] + r0["npe_val"], r0["solo_train"] + r0["solo_val"]):
         assert abs(a - b) < 2e-3 * max(1.0, abs(b)), (r0["npe_train"], r0["solo_train"], r0["npe_val"], r0["solo_val"])
+
+
+def test_global_batch_data_parallel_all_trainers(cuda_lib):
+    _check_global(dict(_run2(_global_worker, timeout=900)))
+
+
+def test_global_batch_data_parallel_all_reduce_one_gpu(cuda_lib):
+    """The same runs as two gloo processes sharing cuda:0 with SBI_B200_NCCL=1: every trainer's all-reduce
+    path (eager launches, no peer memory)."""
+    import functools
+    _check_global(dict(_run2(functools.partial(_global_worker, backend="gloo"), timeout=900, gpus=1)))

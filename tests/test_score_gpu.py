@@ -127,7 +127,8 @@ def test_npse_fits_linear_gaussian(cuda_lib, sde_type):
     x = theta + sig * torch.randn_like(theta)
     inf = NPSE(prior, sde_type=sde_type, device="cuda")
     inf.append_simulations(theta, x)
-    est = inf.train(training_batch_size=500, learning_rate=2e-3, max_num_epochs=150, stop_after_epochs=150)
+    with pytest.warns(UserWarning, match="Maximum number of epochs"):
+        est = inf.train(training_batch_size=500, learning_rate=2e-3, max_num_epochs=150, stop_after_epochs=150)
     assert inf.summary["epochs_trained"][-1] >= 100
     tl = inf.summary["training_loss"]
     assert all(math.isfinite(v) for v in tl) and tl[-1] < tl[0]
