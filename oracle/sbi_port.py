@@ -273,22 +273,39 @@ def build_maf(
     **kwargs,
 ) -> NFlowsFlow:
     """sbi/neural_nets/net_builders/flow.py:115-209."""
+    return _build_made_flow(batch_x, batch_y, z_score_x, z_score_y, embedding_net, num_transforms, partial(
+        transforms.MaskedAffineAutoregressiveTransform, hidden_features=hidden_features, num_blocks=num_blocks,
+        use_residual_blocks=False, random_mask=False, activation=torch.tanh,
+        dropout_probability=dropout_probability, use_batch_norm=use_batch_norm))
+
+
+def build_maf_rqs(
+    batch_x: Tensor, batch_y: Tensor, z_score_x="independent", z_score_y="independent",
+    hidden_features: int = 50, num_transforms: int = 5, embedding_net: nn.Module = None,
+    num_blocks: int = 2, num_bins: int = 10, tail_bound: float = 3.0, dropout_probability: float = 0.0,
+    use_batch_norm: bool = False, **kwargs,
+) -> NFlowsFlow:
+    """sbi/neural_nets/net_builders/flow.py:212-330 (tails="linear", the reference default)."""
+    return _build_made_flow(batch_x, batch_y, z_score_x, z_score_y, embedding_net, num_transforms, partial(
+        transforms.MaskedPiecewiseRationalQuadraticAutoregressiveTransform, hidden_features=hidden_features,
+        num_bins=num_bins, tails="linear", tail_bound=tail_bound, num_blocks=num_blocks,
+        use_residual_blocks=False, random_mask=False, activation=torch.tanh,
+        dropout_probability=dropout_probability, use_batch_norm=use_batch_norm))
+
+
+def _build_made_flow(batch_x, batch_y, z_score_x, z_score_y, embedding_net, num_transforms, made_transform):
+    """The flow both MAF builders assemble: per transform a MADE transform and a RandomPermutation."""
     embedding_net = embedding_net if embedding_net is not None else nn.Identity()
     x_numel = batch_x[0].numel()
     y_numel = embedding_net(batch_y[:1]).numel()
     if x_numel == 1:
         import warnings
         warnings.warn("In one-dimensional output space, this flow is limited to Gaussians",
-                      stacklevel=2)
+                      stacklevel=3)
     transform_list = []
     for _ in range(num_transforms):
         block = [
-            transforms.MaskedAffineAutoregressiveTransform(
-                features=x_numel, hidden_features=hidden_features, context_features=y_numel,
-                num_blocks=num_blocks, use_residual_blocks=False, random_mask=False,
-                activation=torch.tanh, dropout_probability=dropout_probability,
-                use_batch_norm=use_batch_norm,
-            ),
+            made_transform(features=x_numel, context_features=y_numel),
             transforms.RandomPermutation(features=x_numel),
         ]
         transform_list += block

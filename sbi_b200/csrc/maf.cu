@@ -579,6 +579,11 @@ static int maf_launch_rows(KF kernel, const sbi_maf_model* m, const sbi_rows* ro
   return (int)cudaGetLastError();
 }
 
+// large batches take 64-row tiles when the model's 64-row layout fits, else stay on 32-row tiles
+static bool maf_big_tile(const sbi_maf_model* m, const sbi_rows* rows) {
+  return rows->R >= (int64_t)64 * sbi::dev_num_sms() * 2 && maf_smem_layout(*m, 64, false).total_bytes <= 227 * 1024;
+}
+
 extern "C" int sbi_b200_maf_logprob(const sbi_maf_model* m, const sbi_rows* rows, float* d_logp,
                                     float* d_noise, void* stream) {
   sbi::DeviceGuard dev_guard_(m ? m->d_params : nullptr);
@@ -586,7 +591,7 @@ extern "C" int sbi_b200_maf_logprob(const sbi_maf_model* m, const sbi_rows* rows
   if (rc) return rc;
   if (!rows || !rows->d_input || !rows->d_cond || rows->R < 0 || !d_logp) return SBI_EINVAL;
   if (rows->R == 0) return 0;
-  if (rows->R >= (int64_t)64 * sbi::dev_num_sms() * 2)
+  if (maf_big_tile(m, rows))
     return maf_launch_rows<0, 64, 4>(maf_logprob_kernel<64, 4>, m, rows, d_logp, d_noise, (cudaStream_t)stream);
   return maf_launch_rows<1, 32, 2>(maf_logprob_kernel<32, 2>, m, rows, d_logp, d_noise, (cudaStream_t)stream);
 }
@@ -598,7 +603,7 @@ extern "C" int sbi_b200_maf_inverse(const sbi_maf_model* m, const sbi_rows* rows
   if (rc) return rc;
   if (!rows || !rows->d_input || !rows->d_cond || rows->R < 0 || !d_out) return SBI_EINVAL;
   if (rows->R == 0) return 0;
-  if (rows->R >= (int64_t)64 * sbi::dev_num_sms() * 2)
+  if (maf_big_tile(m, rows))
     return maf_launch_rows<2, 64, 4>(maf_inverse_kernel<64, 4>, m, rows, d_out, d_logabsdet, (cudaStream_t)stream);
   return maf_launch_rows<3, 32, 2>(maf_inverse_kernel<32, 2>, m, rows, d_out, d_logabsdet, (cudaStream_t)stream);
 }

@@ -652,7 +652,11 @@ extern "C" int sbi_b200_device_ok(void) {
   return (p.major == 9 && p.minor == 0) ? 1 : 0;
 }
 
-static bool use_big_tile(int64_t R) { return R >= (int64_t)64 * sbi::dev_num_sms() * 2; }
+// Large batches take TM-row tiles (TM = 64, or 128 on request) when the model's TM-row layout fits; a
+// model that only fits a 32-row tile evaluates every batch on 32-row tiles.
+static bool use_big_tile(const sbi_nsf_model& m, int64_t R, int TM) {
+  return R >= (int64_t)64 * sbi::dev_num_sms() * 2 && nsf_smem_layout(m, TM, false).total_bytes <= 227 * 1024;
+}
 
 extern "C" int sbi_b200_nsf_logprob(const sbi_nsf_model* m, const sbi_rows* rows, float* d_logp,
                                     float* d_noise, void* stream) {
@@ -663,7 +667,7 @@ extern "C" int sbi_b200_nsf_logprob(const sbi_nsf_model* m, const sbi_rows* rows
   if (rows->R == 0) return 0;
   cudaStream_t s = (cudaStream_t)stream;
   static const int tm_env = getenv("SBI_B200_LOGPROB_TM") ? atoi(getenv("SBI_B200_LOGPROB_TM")) : 0;
-  if (tm_env == 128 && use_big_tile(rows->R)) {
+  if (tm_env == 128 && use_big_tile(*m, rows->R, 128)) {
     constexpr int TM = 128;
     const NsfSmem L = nsf_smem_layout(*m, TM, false);
     auto k = nsf_logprob_kernel<TM, 4>;
@@ -673,7 +677,7 @@ extern "C" int sbi_b200_nsf_logprob(const sbi_nsf_model* m, const sbi_rows* rows
     k<<<grid, kThreads, L.total_bytes, s>>>(*m, *rows, d_logp, d_noise);
     return (int)cudaGetLastError();
   }
-  if (use_big_tile(rows->R) && tm_env != 32) {
+  if (tm_env != 32 && use_big_tile(*m, rows->R, 64)) {
     constexpr int TM = 64;
     const NsfSmem L = nsf_smem_layout(*m, TM, false);
     auto k = nsf_logprob_kernel<TM, 4>;
@@ -722,7 +726,7 @@ extern "C" int sbi_b200_nsf_inverse(const sbi_nsf_model* m, const sbi_rows* rows
   if (!rows || !rows->d_input || !rows->d_cond || rows->R < 0 || !d_out) return SBI_EINVAL;
   if (rows->R == 0) return 0;
   cudaStream_t s = (cudaStream_t)stream;
-  if (use_big_tile(rows->R)) {
+  if (use_big_tile(*m, rows->R, 64)) {
     constexpr int TM = 64;
     const NsfSmem L = nsf_smem_layout(*m, TM, false);
     auto k = nsf_inverse_kernel<TM, 4>;

@@ -305,7 +305,8 @@ extern "C" int sbi_b200_ratio_forward(const sbi_ratio_model* m, const sbi_pairs*
   if (!pairs || !pairs->d_theta || !pairs->d_x || pairs->R < 0 || !d_logits) return SBI_EINVAL;
   if (pairs->R == 0) return 0;
   cudaStream_t s = (cudaStream_t)stream;
-  if (pairs->R >= (int64_t)64 * sbi::dev_num_sms() * 2) {
+  // large batches take 64-row tiles when the model's 64-row layout fits, else stay on 32-row tiles
+  if (pairs->R >= (int64_t)64 * sbi::dev_num_sms() * 2 && ratio_smem_layout(*m, 64, false).total_bytes <= 227 * 1024) {
     constexpr int TM = 64;
     const RatioSmem L = ratio_smem_layout(*m, TM, false);
     auto k = ratio_forward_kernel<TM, 4>;

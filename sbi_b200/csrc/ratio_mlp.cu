@@ -357,7 +357,8 @@ extern "C" int sbi_b200_ratio_mlp_forward(const sbi_ratio_mlp_model* m, const sb
   if (pairs->R == 0) return 0;
   cudaStream_t s = (cudaStream_t)stream;
   const int sms = sbi::dev_num_sms();
-  if (pairs->R >= (int64_t)64 * sms * 2) {
+  // large batches take 64-row tiles when the model's 64-row layout fits, else stay on 32-row tiles
+  if (pairs->R >= (int64_t)64 * sms * 2 && mlp_smem_layout(*m, 64, false).total_bytes <= 227 * 1024) {
     constexpr int TM = 64;
     const MlpSmem L = mlp_smem_layout(*m, TM, false);
     auto k = ratio_mlp_forward_kernel<TM, 4>;

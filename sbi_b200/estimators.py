@@ -220,6 +220,14 @@ class FlowEstimator(nn.Module):
         s._keep = (st,)
         return s
 
+    def _check_rc(self, rc: int, what: str):
+        if rc == -2:
+            lay = self.layout
+            raise L.SbiB200Error(
+                f"{what}: a row tile of this flow (D={lay.D}, C={lay.C}, H={lay.H}, num_blocks={lay.NB}) needs "
+                "more than the 227 KB of shared memory one CTA can use on sm_90a (SBI_ESMEM)")
+        L.check(rc, what)
+
     def _embed(self, condition: Tensor) -> Tensor:
         """Context fed to the kernels.  Identity embedding: raw condition (standardised
         in-kernel); otherwise the torch embedding net runs first."""
@@ -376,8 +384,8 @@ class FlowEstimator(nn.Module):
                 L.check(L.load().sbi_b200_nsf_inverse_tc(C.byref(m), C.byref(tc), C.byref(rows), L.ptr(out),
                                                          L.ptr(lad), L.stream_ptr()), "nsf_inverse_tc")
                 return out, lad
-        L.check(self.fam.fn("inverse")(C.byref(m), C.byref(rows), L.ptr(out), L.ptr(lad),
-                                       L.stream_ptr()), f"{self.fam.name}_inverse")
+        self._check_rc(self.fam.fn("inverse")(C.byref(m), C.byref(rows), L.ptr(out), L.ptr(lad),
+                                              L.stream_ptr()), f"{self.fam.name}_inverse")
         return out, lad
 
     # ---- tensor-core bulk path (nsf only) --------------------------------------------------------
@@ -491,9 +499,9 @@ class FlowEstimator(nn.Module):
                                                 g_const, L.ptr(logp), L.ptr(gpart), L.ptr(loss_acc), L.ptr(save),
                                                 save.numel() * 4, L.stream_ptr()), "nsf_vjp_tc")
                 return
-        L.check(self.fam.fn("vjp")(C.byref(m), C.byref(rows), L.ptr(gout), g_const, L.ptr(logp), L.ptr(gpart),
-                                   L.ptr(ginput), L.ptr(gcond), L.ptr(loss_acc), L.stream_ptr()),
-                f"{self.fam.name}_vjp")
+        self._check_rc(self.fam.fn("vjp")(C.byref(m), C.byref(rows), L.ptr(gout), g_const, L.ptr(logp),
+                                          L.ptr(gpart), L.ptr(ginput), L.ptr(gcond), L.ptr(loss_acc),
+                                          L.stream_ptr()), f"{self.fam.name}_vjp")
 
     # ---- raw kernel entry (no autograd) --------------------------------------------------------------
     def _logprob_raw(self, inp: Tensor, ctx: Tensor, shared: bool, want_noise=False,
@@ -515,8 +523,8 @@ class FlowEstimator(nn.Module):
                 L.check(lib.sbi_b200_nsf_logprob_tc(C.byref(m), C.byref(tc), C.byref(rows), L.ptr(lp),
                                                     L.ptr(noise), L.stream_ptr()), "nsf_logprob_tc")
                 return lp, noise
-        L.check(self.fam.fn("logprob")(C.byref(m), C.byref(rows), L.ptr(lp), L.ptr(noise),
-                                       L.stream_ptr()), f"{self.fam.name}_logprob")
+        self._check_rc(self.fam.fn("logprob")(C.byref(m), C.byref(rows), L.ptr(lp), L.ptr(noise),
+                                              L.stream_ptr()), f"{self.fam.name}_logprob")
         return lp, noise
 
 

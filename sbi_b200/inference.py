@@ -568,8 +568,8 @@ class _FlowTrainer(_Trainer):
                     L.check(lib.sbi_b200_nsf_logprob_tc(C.byref(m_ev), C.byref(tc_ev), C.byref(rows),
                                                         L.ptr(vlp), None, L.stream_ptr()), "nsf_logprob_tc")
                 else:
-                    L.check(net.fam.fn("logprob")(C.byref(m_ev), C.byref(rows), L.ptr(vlp), None,
-                                                  L.stream_ptr()), "flow_logprob")
+                    net._check_rc(net.fam.fn("logprob")(C.byref(m_ev), C.byref(rows), L.ptr(vlp), None,
+                                                        L.stream_ptr()), "flow_logprob")
                 if w_all is None:
                     # -sum of the finite log-probs and the count of non-finite ones, one fused launch
                     L.check(lib.sbi_b200_nll_stats(L.ptr(vlp), v_hi - v_lo, L.ptr(stats[2:]), L.stream_ptr()),

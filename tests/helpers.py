@@ -26,23 +26,27 @@ def b200_from_oracle(flow, theta, x, device="cuda", **kw):
     return est.to(device)
 
 
-def oracle_maf(D=3, C=2, n=2000, seed=0, perturb=0.1, scale_fn="softplus", **kw):
+def oracle_maf(D=3, C=2, n=2000, seed=0, perturb=0.1, scale_fn="softplus", rqs=False, **kw):
+    """Oracle MAF, or with `rqs` MAF-RQS (spline element-wise maps), with perturbed weights."""
     from oracle.nflows_port.transforms import autoregressive as _ar
     _ar.MAF_SCALE_FN = scale_fn
     g = torch.Generator().manual_seed(seed)
     theta = 0.7 * torch.randn(n, D, generator=g) + 0.3
     x = 1.3 * torch.randn(n, C, generator=g) - 0.2
     torch.manual_seed(seed)
-    flow = sbi_port.build_maf(theta, x, **kw)
+    flow = (sbi_port.build_maf_rqs if rqs else sbi_port.build_maf)(theta, x, **kw)
     with torch.no_grad():
         for name, p in flow.named_parameters():
             p.add_(perturb * torch.randn(p.shape, generator=g))
     return flow, theta, x
 
 
-def b200_maf_from_oracle(flow, theta, x, device="cuda", scale_fn="softplus", **kw):
-    from sbi_b200.neural_nets import build_maf
-    est = build_maf(theta, x, maf_scale_softplus=(scale_fn == "softplus"), **kw)
+def b200_maf_from_oracle(flow, theta, x, device="cuda", scale_fn="softplus", rqs=False, **kw):
+    from sbi_b200.neural_nets import build_maf, build_maf_rqs
+    if rqs:
+        est = build_maf_rqs(theta, x, **kw)
+    else:
+        est = build_maf(theta, x, maf_scale_softplus=(scale_fn == "softplus"), **kw)
     est.load_state_dict(flow.state_dict())
     return est.to(device)
 
