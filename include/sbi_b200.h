@@ -215,6 +215,16 @@ int64_t sbi_b200_nsf_vjp_tc_save_bytes(const sbi_nsf_model* m, int64_t R);
 int sbi_b200_nsf_vjp_tc(const sbi_nsf_model* m, const sbi_nsf_tc* tc_fwd, const sbi_nsf_tc* tc_bwd,
                         const sbi_rows* rows, const float* d_gout, float g_const, float* d_logp,
                         float* d_gpart, float* d_loss_acc, float* d_save, int64_t save_bytes, void* stream);
+/* The same step plus the condition gradient d_gcond (R, C) of sum_r g_r log q_r in raw condition space (the
+ * context columns of every layer's initial linear and the GLU context linear of every residual block, accumulated
+ * per row over the layers; one writer per entry, repeated calls are bit-identical).  The parameter partials are
+ * those of sbi_b200_nsf_vjp_tc.  The instantiation adds no shared memory, so _cond_supported applies the same layout
+ * check as sbi_b200_nsf_vjp_tc_supported; models it declines run sbi_b200_nsf_vjp with d_gcond. */
+int sbi_b200_nsf_vjp_tc_cond_supported(const sbi_nsf_model* m, const sbi_nsf_tc* tc_fwd, const sbi_nsf_tc* tc_bwd);
+int sbi_b200_nsf_vjp_tc_cond(const sbi_nsf_model* m, const sbi_nsf_tc* tc_fwd, const sbi_nsf_tc* tc_bwd,
+                             const sbi_rows* rows, const float* d_gout, float g_const, float* d_logp,
+                             float* d_gpart, float* d_loss_acc, float* d_gcond, float* d_save, int64_t save_bytes,
+                             void* stream);
 
 /* ---- masked autoregressive flow (sbi `posterior_nn("maf")`, reference builder
  * sbi/neural_nets/net_builders/flow.py:115-209: T x [MaskedAffineAutoregressiveTransform(MADE,
@@ -415,6 +425,13 @@ int sbi_b200_fm_vjp_parts(int64_t R);
 int sbi_b200_fm_loss_vjp(const sbi_fm_model* m, const sbi_rows* rows, const float* d_time,
                          const float* d_eps, const float* d_gout, float g_const, float* d_loss,
                          float* d_gpart, float* d_loss_acc, void* stream);
+/* the same, plus the gradient of sum_r g_r * loss_r with respect to the condition rows as given in d_cond:
+ * d_gcond (R, C), through condition_layer and the in-kernel z-score (an embedding net's output when the caller
+ * embeds the condition itself with identity statistics).  One writer per entry: repeated calls are bit-identical.
+ * sbi_b200_fm_loss_vjp is this call with d_gcond == NULL. */
+int sbi_b200_fm_loss_vjp_cond(const sbi_fm_model* m, const sbi_rows* rows, const float* d_time,
+                              const float* d_eps, const float* d_gout, float g_const, float* d_loss,
+                              float* d_gpart, float* d_loss_acc, float* d_gcond, void* stream);
 
 /* Introspection, no device work: the weight-pipeline plan (ring depth, chunk rows, shared memory) that a launch of
  * kernel 0 (sbi_b200_fm_forward), 1 (sbi_b200_fm_loss_vjp / sbi_b200_fm_net_vjp) or 2 (sbi_b200_fm_forward_div)

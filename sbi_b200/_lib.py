@@ -173,6 +173,10 @@ _EXPORTS = {
     "sbi_b200_nsf_vjp_tc": (C.c_int, [C.POINTER(NsfModel), C.POINTER(NsfTc), C.POINTER(NsfTc), C.POINTER(Rows),
                                       C.c_void_p, C.c_float, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                       C.c_int64, C.c_void_p]),
+    "sbi_b200_nsf_vjp_tc_cond_supported": (C.c_int, [C.POINTER(NsfModel), C.POINTER(NsfTc), C.POINTER(NsfTc)]),
+    "sbi_b200_nsf_vjp_tc_cond": (C.c_int, [C.POINTER(NsfModel), C.POINTER(NsfTc), C.POINTER(NsfTc), C.POINTER(Rows),
+                                           C.c_void_p, C.c_float, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                           C.c_void_p, C.c_int64, C.c_void_p]),
     "sbi_b200_maf_logprob": (C.c_int, [C.POINTER(MafModel), C.POINTER(Rows), C.c_void_p,
                                        C.c_void_p, C.c_void_p]),
     "sbi_b200_maf_vjp_parts": (C.c_int, [C.c_int64]),
@@ -215,6 +219,9 @@ _EXPORTS = {
     "sbi_b200_fm_vjp_parts": (C.c_int, [C.c_int64]),
     "sbi_b200_fm_loss_vjp": (C.c_int, [C.POINTER(FmModel), C.POINTER(Rows), C.c_void_p, C.c_void_p, C.c_void_p,
                                        C.c_float, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "sbi_b200_fm_loss_vjp_cond": (C.c_int, [C.POINTER(FmModel), C.POINTER(Rows), C.c_void_p, C.c_void_p,
+                                            C.c_void_p, C.c_float, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                            C.c_void_p]),
     "sbi_b200_slice_init": (C.c_int, [C.POINTER(SliceChains), C.c_void_p, C.c_void_p]),
     "sbi_b200_slice_step": (C.c_int, [C.POINTER(SliceChains), C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "sbi_b200_reduce_partials": (C.c_int, [C.c_void_p, C.c_int, C.c_int64, C.c_void_p,

@@ -462,7 +462,7 @@ __global__ void __launch_bounds__(kThreads, 1)
 fm_vjp_kernel(const __grid_constant__ sbi_fm_model m, const __grid_constant__ sbi_rows rows,
               const float* __restrict__ time, const float* __restrict__ eps, const float* __restrict__ gout,
               float g_const, float* __restrict__ loss, float* __restrict__ gpart, float* __restrict__ loss_acc,
-              const float* __restrict__ dout) {
+              const float* __restrict__ dout, float* __restrict__ dcond) {
   constexpr int LD = Tile<TM>::LD;
   constexpr int PARTS = kConsumerThreads / TM;
   extern __shared__ __align__(128) float sm[];
@@ -648,6 +648,19 @@ fm_vjp_kernel(const __grid_constant__ sbi_fm_model m, const __grid_constant__ sb
     consumer_sync();
     gemm_dw<TM>(dAB, H, sm + L.TN, m.D, m.Dp, gp + __ldg(T + SBI_F_WI), gp + __ldg(T + SBI_F_BI), accum);
     gemm_dw<TM>(dAB + Hp * LD, H, sm + L.CTX, m.C, m.Cp, gp + __ldg(T + SBI_F_WC), gp + __ldg(T + SBI_F_BC), accum);
+    if (dcond != nullptr) {
+      // condition gradient of the row: W_c^T dc through the in-kernel z-score, one thread per (row, feature)
+      const float* wc = P + __ldg(T + SBI_F_WC);
+      const float* csd = m.d_stats + 2 * m.Dp + m.Cp;
+      const float* dC = dAB + Hp * LD;
+      for (int e = threadIdx.x; e < TM * m.C; e += kConsumerThreads) {
+        const int r = e / m.C, c = e % m.C;
+        if (row0 + r >= rows.R) continue;
+        float a = 0.f;
+        for (int n = 0; n < H; ++n) a = fmaf(dC[n * LD + r], __ldg(wc + n * m.Cp + c), a);
+        dcond[(row0 + r) * m.C + c] = a / __ldg(csd + c);
+      }
+    }
     consumer_sync();
   }
 }
@@ -797,10 +810,22 @@ extern "C" int sbi_b200_fm_vjp_parts(int64_t R) {
 extern "C" int sbi_b200_fm_loss_vjp(const sbi_fm_model* m, const sbi_rows* rows, const float* d_time,
                                     const float* d_eps, const float* d_gout, float g_const, float* d_loss,
                                     float* d_gpart, float* d_loss_acc, void* stream) {
+  return sbi_b200_fm_loss_vjp_cond(m, rows, d_time, d_eps, d_gout, g_const, d_loss, d_gpart, d_loss_acc, nullptr,
+                                   stream);
+}
+
+extern "C" int sbi_b200_fm_loss_vjp_cond(const sbi_fm_model* m, const sbi_rows* rows, const float* d_time,
+                                         const float* d_eps, const float* d_gout, float g_const, float* d_loss,
+                                         float* d_gpart, float* d_loss_acc, float* d_gcond, void* stream) {
   sbi::DeviceGuard dev_guard_(m ? m->d_params : nullptr);
   int rc = fm_check(m);
   if (rc) return rc;
   if (!rows || !rows->d_input || !rows->d_cond || rows->R < 1 || !d_time || !d_eps || !d_gpart) return SBI_EINVAL;
+  if (d_gcond != nullptr && d_gout == nullptr && g_const == 0.f) {
+    // no upstream gradient: the kernel skips the backward sweep, so the condition gradient is zero
+    cudaError_t e = cudaMemsetAsync(d_gcond, 0, (size_t)rows->R * m->C * sizeof(float), (cudaStream_t)stream);
+    if (e != cudaSuccess) return (int)e;
+  }
   constexpr int TM = 16;
   const sbi_fm_model md = fm_tune(*m, TM, kFmTrain);
   const FmSmem L = fm_smem_layout(md, TM, kFmTrain);
@@ -808,7 +833,7 @@ extern "C" int sbi_b200_fm_loss_vjp(const sbi_fm_model* m, const sbi_rows* rows,
   if ((rc = fm_set_smem<1>(k, L.total_bytes))) return rc;
   const int grid = sbi_b200_fm_vjp_parts(rows->R);
   k<<<grid, kThreads, L.total_bytes, (cudaStream_t)stream>>>(md, *rows, d_time, d_eps, d_gout, g_const, d_loss,
-                                                           d_gpart, d_loss_acc, nullptr);
+                                                           d_gpart, d_loss_acc, nullptr, d_gcond);
   return (int)cudaGetLastError();
 }
 
@@ -826,6 +851,6 @@ extern "C" int sbi_b200_fm_net_vjp(const sbi_fm_model* m, const sbi_rows* rows, 
   if ((rc = fm_set_smem<1>(k, L.total_bytes))) return rc;
   const int grid = sbi_b200_fm_vjp_parts(rows->R);
   k<<<grid, kThreads, L.total_bytes, (cudaStream_t)stream>>>(md, *rows, d_time, nullptr, nullptr, 0.f, nullptr, d_gpart,
-                                                           nullptr, d_dout);
+                                                           nullptr, d_dout, nullptr);
   return (int)cudaGetLastError();
 }

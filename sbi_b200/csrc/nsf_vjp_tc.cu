@@ -17,6 +17,13 @@
 //     pre-transposed operand blocks (pack.NsfLayout.tc_bwd_plan) through a 2-slot ring; relu / GLU
 //     masks, the spline backward (rqs.cuh) and the LULinear backward are per-thread code on the
 //     thread's own row between the MMAs;
+//   * COND instantiation only: the condition gradient d(sum g log q)/d ctx in raw condition space, accumulated
+//     per row over the T layers from the context columns of the initial layer (dh W0[:, :C]) and the GLU
+//     context layer of every residual block (dG Wc).  dh / dG of the whole row sit in the staged weight-gradient
+//     operand (A') once it is handed over, so each of the row's two threads takes half of the C features over
+//     all H columns, on the CUDA cores from the fp32 parameters (C is small next to H), and accumulates them in
+//     place in d_gcond: every entry has one owner thread and a fixed summation order.  No shared memory is
+//     added, so the parameter-only layout and plan serve both instantiations;
 //   * weight gradients  dW = dY^T X  (K = the 128 rows of the tile) on the same tensor core with BOTH
 //     operands from shared memory: the row threads write dY^T and X^T into K-major staging buffers
 //     ([row/4][feature][row%4], one padding row per slab so that the 32 rows of a warp hit 32 banks),
@@ -115,12 +122,13 @@ __device__ __noinline__ void dw_read_fn(uint32_t row, uint32_t col, const DwGeo 
   }
 }
 
-template <int H, int KB>
+template <int H, int KB, bool COND>
 __global__ void __launch_bounds__(kThreads, 1)
 nsf_vjp_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_constant__ sbi_nsf_tc tcb,
                   const __grid_constant__ sbi_rows rows, const float* __restrict__ gout, float g_const,
                   float* __restrict__ gpart, float* __restrict__ loss_acc,
-                  const float* __restrict__ save, int accum_first, const StoreArgs sa) {
+                  const float* __restrict__ save, int accum_first, const StoreArgs sa,
+                  float* __restrict__ dcond) {
   constexpr int HP8 = (H + 7) & ~7;
   constexpr int NCH = HP8 / 8;
   constexpr int NC = HP8 / 2;
@@ -151,6 +159,19 @@ nsf_vjp_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_constant
   RqsConst rc = rqs_const(m);
   rc.K = KB;
   float* gp = gpart + (size_t)blockIdx.x * m.n_params;
+  // condition gradient: features [c_lo, c_hi) of this thread's row; dY = the handed-over A' operand
+  const int c_half = (C + 1) >> 1;
+  const int c_lo = half * c_half, c_hi = min(C, c_lo + c_half);
+  auto dctx_add = [&](const float* As, const float* W, int ldw, int64_t row0) {
+    if (row0 + row >= rows.R) return;
+    const float* csd = m.d_stats + 2 * m.Dp + Cp;
+    float* out = dcond + (row0 + row) * C;
+    for (int c = c_lo; c < c_hi; ++c) {
+      float a = 0.f;
+      for (int n = 0; n < H; ++n) a = fmaf(As[((row >> 2) * kStLd + n) * 4 + (row & 3)], __ldg(W + n * ldw + c), a);
+      out[c] += a / __ldg(csd + c);
+    }
+  };
 
   uint32_t dwn = 0u;           // weight-gradient MMAs issued so far (slot = dwn & 1, issuing warp = dwn & 7)
   bool pend0 = false, pend1 = false;
@@ -277,6 +298,8 @@ nsf_vjp_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_constant
           dzs[(4 * i + 3) * kRows + row] = live ? -g * t.w : 0.f;
         }
       }
+      if (COND && live)
+        for (int c = c_lo; c < c_hi; ++c) dcond[(row0 + row) * C + c] = 0.f;
       prep_lu(m, m.T - 1, sm + L.lum);
       group_sync();
     }
@@ -508,7 +531,7 @@ nsf_vjp_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_constant
         float dT[NC], a1[NC];
         tc_load_cols<NC>(svl + SV.a1(b), row, half, a1);
         {
-          // ---- dWc = dG^T ctx  (GLU gate; no input gradient wanted for the context)
+          // ---- dWc = dG^T ctx  (GLU gate; the COND instantiation also takes dctx += dG Wc)
           const int slot = (int)(dwn & 1u);
           dw_free(slot);
           float* As = stg + (2 * slot) * kStFloats;
@@ -524,6 +547,7 @@ nsf_vjp_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_constant
             st_put(Bs, n, n < C ? ctx_s[n * kRows + row] : (n == Cp ? 1.f : 0.f));
           fence_async_smem();
           group_sync();
+          if (COND) dctx_add(As, P + __ldg(BT + 4), Cp, row0);     // dG Wc
           DwGeo g;
           g.oW = __ldg(BT + 4); g.ldw = Cp; g.oB = __ldg(BT + 5); g.nX = Cp; g.ones = Cp; g.Mv = Hp; g.N = Nc;
           dw_issue(slot, g);
@@ -628,6 +652,7 @@ nsf_vjp_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_constant
         }
         write_a(dh, 0);
         hand_over();
+        if (COND) dctx_add(As, P + __ldg(v.LT + SBI_L_W0), K0p, row0);     // the context columns of dh W0
         {
           uint32_t acc = 0u;
           iss.begin(__ldg(tab + 5 + 4 * stage));
@@ -689,6 +714,12 @@ extern "C" int sbi_b200_nsf_vjp_tc_supported(const sbi_nsf_model* m, const sbi_n
   return vjp_tc_ok(m, tc_fwd, tc_bwd);
 }
 
+extern "C" int sbi_b200_nsf_vjp_tc_cond_supported(const sbi_nsf_model* m, const sbi_nsf_tc* tc_fwd,
+                                                  const sbi_nsf_tc* tc_bwd) {
+  if (!m || !tc_fwd || !tc_bwd) return 0;
+  return vjp_tc_ok(m, tc_fwd, tc_bwd);
+}
+
 // rows of one forward + backward launch pair (one tile per CTA, every SM busy once)
 static int64_t vjp_tc_chunk_rows() { return (int64_t)tc::kRows * sbi::dev_num_sms(); }
 
@@ -703,20 +734,20 @@ extern "C" int64_t sbi_b200_nsf_vjp_tc_save_bytes(const sbi_nsf_model* m, int64_
   return (int64_t)sizeof(float) * SV.tile_stride * sbi_b200_nsf_vjp_tc_parts(R);
 }
 
-extern "C" int sbi_b200_nsf_vjp_tc(const sbi_nsf_model* m, const sbi_nsf_tc* tc_fwd, const sbi_nsf_tc* tc_bwd,
-                                   const sbi_rows* rows, const float* d_gout, float g_const, float* d_logp,
-                                   float* d_gpart, float* d_loss_acc, float* d_save, int64_t save_bytes,
-                                   void* stream) {
+template <bool COND>
+static int vjp_tc_launch(const sbi_nsf_model* m, const sbi_nsf_tc* tc_fwd, const sbi_nsf_tc* tc_bwd,
+                         const sbi_rows* rows, const float* d_gout, float g_const, float* d_logp, float* d_gpart,
+                         float* d_loss_acc, float* d_gcond, float* d_save, int64_t save_bytes, void* stream) {
   sbi::DeviceGuard dev_guard_(m ? m->d_params : nullptr);
   if (!m || !tc_fwd || !tc_bwd || !rows || !rows->d_input || !rows->d_cond || rows->R < 1 || !d_gpart ||
-      !d_save)
+      !d_save || (COND && !d_gcond))
     return SBI_EINVAL;
   if (!vjp_tc_ok(m, tc_fwd, tc_bwd)) return SBI_ESMEM;
   if (save_bytes < sbi_b200_nsf_vjp_tc_save_bytes(m, rows->R)) return SBI_EINVAL;
   cudaStream_t s = (cudaStream_t)stream;
   const tc::BwdSmem Lb = tc::bwd_smem_layout(tc_bwd->stage_cap, tc::bwd_ldmax(*m));
-  auto kb = tc::nsf_vjp_tc_kernel<50, 10>;
-  if (int e = sbi::set_smem<0>(kb, Lb.total_bytes)) return e;
+  auto kb = tc::nsf_vjp_tc_kernel<50, 10, COND>;
+  if (int e = sbi::set_smem<COND ? 1 : 0>(kb, Lb.total_bytes)) return e;
   // chunks of one tile per SM: forward sweep (saves activations) then backward sweep of the same rows;
   // later chunks accumulate into the partial-gradient slabs
   tc::StoreArgs sa;
@@ -734,9 +765,26 @@ extern "C" int sbi_b200_nsf_vjp_tc(const sbi_nsf_model* m, const sbi_nsf_tc* tc_
     const int rc = tc::launch_forward_save(m, tc_fwd, &rr, d_logp ? d_logp + r0 : nullptr, d_save, s);
     if (rc) return rc;
     kb<<<grid, tc::kThreads, Lb.total_bytes, s>>>(*m, *tc_bwd, rr, d_gout ? d_gout + r0 : nullptr, g_const,
-                                                  d_gpart, d_loss_acc, d_save, r0 > 0 ? 1 : 0, sa);
+                                                  d_gpart, d_loss_acc, d_save, r0 > 0 ? 1 : 0, sa,
+                                                  COND ? d_gcond + r0 * m->C : nullptr);
   }
   return (int)cudaGetLastError();
+}
+
+extern "C" int sbi_b200_nsf_vjp_tc(const sbi_nsf_model* m, const sbi_nsf_tc* tc_fwd, const sbi_nsf_tc* tc_bwd,
+                                   const sbi_rows* rows, const float* d_gout, float g_const, float* d_logp,
+                                   float* d_gpart, float* d_loss_acc, float* d_save, int64_t save_bytes,
+                                   void* stream) {
+  return vjp_tc_launch<false>(m, tc_fwd, tc_bwd, rows, d_gout, g_const, d_logp, d_gpart, d_loss_acc, nullptr, d_save,
+                              save_bytes, stream);
+}
+
+extern "C" int sbi_b200_nsf_vjp_tc_cond(const sbi_nsf_model* m, const sbi_nsf_tc* tc_fwd, const sbi_nsf_tc* tc_bwd,
+                                        const sbi_rows* rows, const float* d_gout, float g_const, float* d_logp,
+                                        float* d_gpart, float* d_loss_acc, float* d_gcond, float* d_save,
+                                        int64_t save_bytes, void* stream) {
+  return vjp_tc_launch<true>(m, tc_fwd, tc_bwd, rows, d_gout, g_const, d_logp, d_gpart, d_loss_acc, d_gcond, d_save,
+                             save_bytes, stream);
 }
 
 #ifdef SBI_TC_TIMELINE

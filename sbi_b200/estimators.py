@@ -481,13 +481,25 @@ class FlowEstimator(nn.Module):
             return bool(st["ok"])
         return self._tc_train_state(self._model(nbuf=3)) is not None
 
-    def vjp(self, m, rows, R: int, gout, g_const: float, logp, gpart, ginput=None, gcond=None, loss_acc=None):
+    def vjp_cond_uses_tc(self, R: int) -> bool:
+        """Whether the trainer's step with a condition gradient (embedding net) runs on the tensor cores
+        (`sbi_b200_nsf_vjp_tc_cond`): same row threshold and switches as the parameter-only step, and the model
+        must fit that instantiation's shared-memory layout.  `log_prob().backward()` does not use this path."""
+        if not self._vjp_uses_tc(R, True):
+            return False
+        tcs = self._tc_train_state(self._model(nbuf=3), pack=False)
+        return tcs is not None and bool(L.load().sbi_b200_nsf_vjp_tc_cond_supported(
+            C.byref(self._model(nbuf=3)), C.byref(tcs[0]), C.byref(tcs[1])))
+
+    def vjp(self, m, rows, R: int, gout, g_const: float, logp, gpart, ginput=None, gcond=None, loss_acc=None,
+            cond_tc: bool = False):
         """One launch (pair) of the fused forward+backward of `R` rows: partial parameter gradients of
         sum_r g_r log q_r into `gpart` ((vjp_parts(R, ...), n_params)), optionally the gradients
         w.r.t. the inputs / conditions, the log-probs and the loss statistics.  Tensor-core kernels when
-        only parameter gradients are wanted (the trainer's case), else the SIMT kernel."""
+        only parameter gradients are wanted, or with `cond_tc` (the trainer's step with an embedding net, after
+        `vjp_cond_uses_tc(R)`) parameter and condition gradients; else the SIMT kernel."""
         lib = L.load()
-        if ginput is None and gcond is None and self._vjp_uses_tc(R, True):
+        if ginput is None and (gcond is None or cond_tc) and self._vjp_uses_tc(R, True):
             tcs = self._tc_train_state(m)
             if tcs is not None:
                 nbytes = int(lib.sbi_b200_nsf_vjp_tc_save_bytes(C.byref(m), R))
@@ -495,6 +507,12 @@ class FlowEstimator(nn.Module):
                 if save is None or save.numel() * 4 < nbytes or save.device != self.net.flat.device:
                     save = torch.empty((nbytes + 3) // 4, dtype=torch.float32, device=self.net.flat.device)
                     self._cache["vjp_save"] = save
+                if gcond is not None:
+                    L.check(lib.sbi_b200_nsf_vjp_tc_cond(
+                        C.byref(m), C.byref(tcs[0]), C.byref(tcs[1]), C.byref(rows), L.ptr(gout), g_const, L.ptr(logp),
+                        L.ptr(gpart), L.ptr(loss_acc), L.ptr(gcond), L.ptr(save), save.numel() * 4, L.stream_ptr()),
+                        "nsf_vjp_tc_cond")
+                    return
                 L.check(lib.sbi_b200_nsf_vjp_tc(C.byref(m), C.byref(tcs[0]), C.byref(tcs[1]), C.byref(rows), L.ptr(gout),
                                                 g_const, L.ptr(logp), L.ptr(gpart), L.ptr(loss_acc), L.ptr(save),
                                                 save.numel() * 4, L.stream_ptr()), "nsf_vjp_tc")

@@ -75,8 +75,9 @@ class FlowMatchingEstimator(nn.Module):
         super().__init__()
         self._input_shape, self._condition_shape = torch.Size(input_shape), torch.Size(condition_shape)
         user = embedding_net if embedding_net is not None else nn.Identity()
-        if not isinstance(user, nn.Identity):
-            raise NotImplementedError("the sm_90a flow-matching kernels take nn.Identity() embedding nets")
+        # identity embedding: the kernels z-score the raw condition themselves; otherwise the embedding net
+        # (behind the condition z-score) runs in torch and the kernels see its output with identity statistics
+        self._embed_identity = isinstance(user, nn.Identity)
         self._embedding_net = nn.Sequential(Standardize(*cond_stats), user) if cond_stats else user
         self.noise_scale = noise_scale
         self.register_buffer("mean_0", torch.as_tensor(mean_0, dtype=torch.float32).expand(input_shape).clone())
@@ -114,7 +115,8 @@ class FlowMatchingEstimator(nn.Module):
         lay = self.layout
         emb = self._embedding_net
         srcs = [self.mean_0, self.std_0, self.net._div_term]
-        if isinstance(emb, nn.Sequential):
+        kernel_zscore = isinstance(emb, nn.Sequential) and self._embed_identity
+        if kernel_zscore:
             srcs += [emb[0]._mean, emb[0]._std]
         key = tuple((t.data_ptr(), t._version) for t in srcs) + (str(self.net.flat.device),)
         hit = self._cache.get("stats")
@@ -126,7 +128,7 @@ class FlowMatchingEstimator(nn.Module):
         st[2 * lay.Dp + lay.Cp:2 * lay.Dp + 2 * lay.Cp] = 1.0
         st[:lay.D] = self.mean_0.reshape(-1)
         st[lay.Dp:lay.Dp + lay.D] = self.std_0.reshape(-1)
-        if isinstance(emb, nn.Sequential):
+        if kernel_zscore:
             st[2 * lay.Dp:2 * lay.Dp + lay.C] = emb[0]._mean.reshape(-1).expand(lay.C)
             st[2 * lay.Dp + lay.Cp:2 * lay.Dp + lay.Cp + lay.C] = emb[0]._std.reshape(-1).expand(lay.C)
         o = 2 * lay.Dp + 2 * lay.Cp
@@ -153,9 +155,18 @@ class FlowMatchingEstimator(nn.Module):
             self._cache["gpart"] = buf
         return buf
 
+    def _embed(self, condition: Tensor) -> Tensor:
+        """(n, *condition_shape) -> (n, C): the context the kernels read.  Identity embedding: the raw condition
+        (z-scored in-kernel); otherwise the embedding net runs in torch, with autograd when enabled."""
+        n = condition.shape[0]
+        if self._embed_identity:
+            return condition.reshape(n, self.layout.C).float()
+        return self._embedding_net(condition).reshape(n, -1).float()
+
     # ---- reference API -------------------------------------------------------------------------
     def forward(self, input: Tensor, condition: Tensor, time: Tensor) -> Tensor:
-        """Velocity in ORIGINAL space (flowmatching_estimator.py:205-268); batch shapes broadcast."""
+        """Velocity in ORIGINAL space (flowmatching_estimator.py:205-268); batch shapes broadcast.  The condition
+        is embedded once per distinct condition row, before broadcasting."""
         lib = L.load()
         L.require_cuda(input, "input")
         bs_in = input.shape[:-len(self.input_shape)]
@@ -164,9 +175,10 @@ class FlowMatchingEstimator(nn.Module):
         inp = torch.broadcast_to(input, bshape + self.input_shape).reshape(-1, self.layout.D).contiguous().float()
         R = inp.shape[0]
         shared = int(torch.Size(bs_c).numel()) == 1
-        cond = condition.reshape(-1, self.layout.C) if shared else torch.broadcast_to(
-            condition, bshape + self.condition_shape).reshape(-1, self.layout.C)
-        cond = cond.contiguous().float()
+        ctx = self._embed(condition.reshape(-1, *self.condition_shape))
+        cond = ctx if shared else torch.broadcast_to(ctx.reshape(*bs_c, self.layout.C),
+                                                     bshape + (self.layout.C,)).reshape(-1, self.layout.C)
+        cond = cond.contiguous()
         time = torch.as_tensor(time, dtype=torch.float32, device=inp.device)
         t_shared = time.numel() == 1
         tt = time.reshape(1) if t_shared else torch.broadcast_to(time, bshape).reshape(-1)
@@ -181,12 +193,12 @@ class FlowMatchingEstimator(nn.Module):
     def forward_and_divergence(self, input: Tensor, condition: Tensor, time: Tensor):
         """(v, sum_i dv_i/dtheta_i): the velocity in ORIGINAL space and its exact divergence w.r.t. the
         input, one kernel (csrc/fm.cu `fm_trace_kernel`: forward + D forward-mode tangents).  input (R, D),
-        condition (R, C) or (1, C), time scalar or (R,)."""
+        condition (R, *condition_shape) or (1, *condition_shape) (embedded here), time scalar or (R,)."""
         lib = L.load()
         L.require_cuda(input, "input")
         inp = input.reshape(-1, self.layout.D).contiguous().float()
         R = inp.shape[0]
-        cond = condition.reshape(-1, self.layout.C).contiguous().float()
+        cond = self._embed(condition.reshape(-1, *self.condition_shape)).contiguous()
         shared = cond.shape[0] == 1
         time = torch.as_tensor(time, dtype=torch.float32, device=inp.device)
         t_shared = time.numel() == 1
@@ -244,18 +256,20 @@ class FlowMatchingEstimator(nn.Module):
 
     def loss(self, input: Tensor, condition: Tensor, times: Optional[Tensor] = None, **kwargs) -> Tensor:
         """(batch,) flow-matching losses; flowmatching_estimator.py:270-347.  t ~ U(0,1) and
-        theta_1 ~ N(0, I) are drawn with torch on the device in the reference's order."""
+        theta_1 ~ N(0, I) are drawn with torch on the device in the reference's order; the embedding net's
+        gradient flows through the kernel's condition gradient."""
         if times is None:
             times = torch.rand(input.shape[:-1], device=input.device, dtype=input.dtype)
         theta_1 = torch.randn_like(input)
-        return _FmLoss.apply(self.net.flat, input.reshape(-1, self.layout.D).contiguous().float(),
-                             condition.reshape(-1, self.layout.C).contiguous().float(),
+        ctx = self._embed(condition.reshape(-1, *self.condition_shape))
+        return _FmLoss.apply(self.net.flat, input.reshape(-1, self.layout.D).contiguous().float(), ctx.contiguous(),
                              times.reshape(-1).contiguous().float(), theta_1.reshape(-1, self.layout.D).contiguous(),
                              self).reshape(input.shape[:-1])
 
     def loss_raw(self, inp, cond, times, eps, index=None, R=None, g_const=0.0, gpart=None, loss_acc=None,
-                 want_loss=True):
-        """Fused loss forward+backward on (optionally index-gathered) rows; returns the per-row loss."""
+                 want_loss=True, gcond=None):
+        """Fused loss forward+backward on (optionally index-gathered) rows; returns the per-row loss.  `gcond`
+        (R, C): receives the gradient with respect to the condition rows."""
         lib = L.load()
         R = (index.shape[0] if index is not None else inp.shape[0]) if R is None else R
         loss = torch.empty(R, dtype=torch.float32, device=inp.device) if want_loss else None
@@ -263,8 +277,9 @@ class FlowMatchingEstimator(nn.Module):
         gpart = self._gpart(n_part) if gpart is None else gpart
         m = self._model(nbuf=2)
         rows = L.Rows(inp.data_ptr(), cond.data_ptr(), None if index is None else index.data_ptr(), R, 0)
-        L.check(lib.sbi_b200_fm_loss_vjp(C.byref(m), C.byref(rows), L.ptr(times), L.ptr(eps), None, g_const,
-                                         L.ptr(loss), L.ptr(gpart), L.ptr(loss_acc), L.stream_ptr()), "fm_loss_vjp")
+        L.check(lib.sbi_b200_fm_loss_vjp_cond(C.byref(m), C.byref(rows), L.ptr(times), L.ptr(eps), None, g_const,
+                                              L.ptr(loss), L.ptr(gpart), L.ptr(loss_acc), L.ptr(gcond),
+                                              L.stream_ptr()), "fm_loss_vjp")
         return loss, gpart, n_part
 
 
@@ -296,12 +311,15 @@ class _FmLoss(torch.autograd.Function):
         m = est._model(nbuf=2)
         rows = L.Rows(inp.data_ptr(), cond.data_ptr(), None, R, 0)
         g = g.contiguous().float()
-        L.check(lib.sbi_b200_fm_loss_vjp(C.byref(m), C.byref(rows), L.ptr(times), L.ptr(eps), L.ptr(g), 0.0, None,
-                                         L.ptr(gpart), None, L.stream_ptr()), "fm_loss_vjp")
-        gflat = torch.empty(est.layout.n_params, dtype=torch.float32, device=inp.device)
-        L.check(lib.sbi_b200_reduce_partials(L.ptr(gpart), n_part, est.layout.n_params, L.ptr(gflat), L.stream_ptr()),
-                "reduce_partials")
-        return gflat, None, None, None, None, None
+        gcond = torch.empty_like(cond) if ctx.needs_input_grad[2] else None
+        L.check(lib.sbi_b200_fm_loss_vjp_cond(C.byref(m), C.byref(rows), L.ptr(times), L.ptr(eps), L.ptr(g), 0.0,
+                                              None, L.ptr(gpart), None, L.ptr(gcond), L.stream_ptr()), "fm_loss_vjp")
+        gflat = None
+        if ctx.needs_input_grad[0]:
+            gflat = torch.empty(est.layout.n_params, dtype=torch.float32, device=inp.device)
+            L.check(lib.sbi_b200_reduce_partials(L.ptr(gpart), n_part, est.layout.n_params, L.ptr(gflat),
+                                                 L.stream_ptr()), "reduce_partials")
+        return gflat, None, gcond, None, None, None
 
 
 def build_vector_field_estimator(
@@ -318,7 +336,10 @@ def build_vector_field_estimator(
     if estimator_type != "flow" or net != "mlp" or gaussian_baseline or compose_standardization:
         raise NotImplementedError("sbi_b200 implements estimator_type='flow', net='mlp' without gaussian "
                                   "baseline / composed standardization")
-    D, Cn, H = batch_x[0].numel(), batch_y[0].numel(), int(hidden_features)
+    # the network's condition width is the embedded size (get_numel on the raw batch_y, like the reference)
+    with torch.no_grad():
+        Cn = embedding_net(batch_y[:1]).numel()
+    D, H = batch_x[0].numel(), int(hidden_features)
     lay = FmLayout(D=D, C=Cn, H=H, NL=num_layers, TE=time_embedding_dim)
     st = {}
     st["net.input_layer.weight"], st["net.input_layer.bias"] = _linear_init(H, D)
@@ -528,11 +549,13 @@ def _generic_rhs(est, cond: Tensor, R: int, with_div: bool, solver: "DeviceDopri
 
 
 def _make_solver(est, cond, R, n, dev, with_div, atol, rtol):
+    """`cond`: the raw condition (1, C).  The flow-matching kernels read the embedded condition, computed once here."""
     if getattr(est, "IS_SCORE", False):
         solver = DeviceDopri5(n, dev, None, atol=atol, rtol=rtol)
-        solver.rhs = _generic_rhs(est, cond, R, with_div, solver)
+        solver.rhs = _generic_rhs(est, cond.reshape(1, -1).contiguous(), R, with_div, solver)
         return solver
-    return DeviceDopri5(n, dev, _fm_rhs(est, cond, R, with_div), atol=atol, rtol=rtol)
+    ctx = est._embed(cond.reshape(1, *est.condition_shape)).contiguous()
+    return DeviceDopri5(n, dev, _fm_rhs(est, ctx, R, with_div), atol=atol, rtol=rtol)
 
 
 @torch.no_grad()
@@ -542,7 +565,7 @@ def sample_ode(est: FlowMatchingEstimator, num_samples: int, condition: Tensor, 
     (VectorFieldPosterior.sample_via_ode, vector_field_posterior.py:436-465).  `device_control=False` keeps
     the host-side loop (`odeint_dopri5`) for comparison."""
     dev = est.net.flat.device
-    cond = condition.reshape(1, *est.condition_shape).to(dev).float().reshape(1, -1).contiguous()
+    cond = condition.reshape(1, *est.condition_shape).to(dev).float()
     D = est.layout.D
     y0 = est._mean_base.to(dev) + est._std_base.to(dev) * torch.randn(num_samples, D, device=dev)
     if not device_control:
@@ -566,7 +589,7 @@ def log_prob_ode(est: FlowMatchingEstimator, theta: Tensor, condition: Tensor, a
     D = est.layout.D
     th = theta.reshape(-1, D).to(dev).float().contiguous()
     R = th.shape[0]
-    cond = condition.reshape(1, *est.condition_shape).to(dev).float().reshape(1, -1).contiguous()
+    cond = condition.reshape(1, *est.condition_shape).to(dev).float()
     y0 = torch.cat([th.reshape(-1), torch.zeros(R, device=dev)])
     solver = _make_solver(est, cond, R, R * D + R, dev, True, atol, rtol)
     y, nfe, _, _ = solver.solve(y0, est.t_min, est.t_max)
@@ -608,7 +631,7 @@ def sample_sde(est: FlowMatchingEstimator, num_samples: int, condition: Tensor, 
     generic path: the same torch arithmetic as the reference around the network kernel."""
     assert eta > 0, "eta must be positive."
     dev = est.net.flat.device
-    cond = condition.to(dev).float().reshape(-1, est.layout.C).contiguous()
+    cond = condition.to(dev).float().reshape(-1, *est.condition_shape)
     n_iid = cond.shape[0]
     if n_iid > 1 and iid_method != "fnpe":
         raise NotImplementedError(f"{n_iid} iid observations need iid_method='fnpe' (the factorised score, "
@@ -669,6 +692,7 @@ def sample_sde(est: FlowMatchingEstimator, num_samples: int, condition: Tensor, 
     z = torch.empty_like(theta)
     ctrl = torch.stack([ts[0], torch.ones((), device=dev)]).contiguous()       # [t_cur, next grid index]
     m = est._model(nbuf=2)
+    cond = est._embed(cond).contiguous()          # x_o embedded once for all steps
     rows = L.Rows(theta.data_ptr(), cond.data_ptr(), None, num_samples, 1)
 
     def step():

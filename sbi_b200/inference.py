@@ -33,7 +33,7 @@ import torch
 from torch import Tensor, nn
 
 from . import _lib as L
-from .estimators import FlowEstimator, NSFEstimator
+from .estimators import FlowEstimator, NSFEstimator, Standardize
 from .neural_nets import likelihood_nn, posterior_nn
 
 
@@ -50,17 +50,47 @@ def _process_device(device: str) -> str:
     return str(device)
 
 
+def _embedding_params(net) -> list:
+    """The trainable parameters of an estimator's torch embedding net ([] for an identity embedding)."""
+    if getattr(net, "_embed_identity", True):
+        return []
+    return [p for p in net.embedding_net.parameters() if p.requires_grad]
+
+
+def _embedding_buffers(emb: nn.Module) -> list:
+    """The embedding net's buffers that training can change (e.g. BatchNorm statistics).  The condition z-score
+    (`Standardize`) is fixed at build time and is left alone: writing it would invalidate the kernel statistics
+    that captured graphs read."""
+    return [b for m in emb.modules() if not isinstance(m, Standardize) for b in m.buffers(recurse=False)]
+
+
+def _weights(net) -> list:
+    """The tensors a best-epoch snapshot covers: the kernel parameters and the embedding net's parameters and
+    buffers (the reference deep-copies the whole state_dict, trainers/base.py:1127, :1275)."""
+    emb = getattr(net, "embedding_net", None)
+    extra = [] if emb is None else [p.data for p in emb.parameters()] + _embedding_buffers(emb)
+    return [net.flat.data] + extra
+
+
 class _DeviceAdam:
     """Clip + Adam (`clip_grad_norm_` + `Adam.step`, trainers/base.py:1181-1187) on a network's flat
     parameters, in the kernels of csrc/optim.cu.  With several ranks the gradient is first summed over
     them: through our NVLink peer-memory kernel on one node (graph-capturable), else with an NCCL
-    all-reduce (eager launches).  The clip norm is always taken on the summed gradient."""
+    all-reduce (eager launches).  The clip norm is always taken on the summed gradient.
+
+    A torch embedding net's parameters join the same update (one clip norm, one step count, one Adam state,
+    like `Adam(neural_net.parameters())` in the reference): the flat kernel parameters and the embedding
+    parameters become views of one vector `[flat | embedding]`, and each embedding parameter's `.grad` a view
+    of the matching gradient slice, which autograd accumulates into in place."""
 
     def __init__(self, net, state: Tensor, step: Tensor, lr: float, clip_max_norm: Optional[float], world: int):
         self.lib = L.load()
         self.flat, self.mask = net.flat, net.net._mask
         self.P = net.layout.n_params
         self.state, self.count = state, step
+        self.emb = _embedding_params(net)
+        self.emb_buffers = _embedding_buffers(net.embedding_net) if self.emb else []
+        self.n = self.P + sum(p.numel() for p in self.emb)
         self.lr = lr
         self.max_norm = float(clip_max_norm) if clip_max_norm is not None else 0.0
         self.world = world
@@ -74,6 +104,27 @@ class _DeviceAdam:
         self.grad_local = torch.zeros(self.P, dtype=torch.float32, device=dev) if self.peer is not None else self.grad
         n_sumsq = self.peer.n_sumsq if self.peer is not None else self.lib.sbi_b200_sumsq_blocks(self.P)
         self.sumsq = torch.zeros(n_sumsq, dtype=torch.float32, device=dev)
+        self.params = None           # the joint parameter vector, with an embedding net
+        if self.emb:
+            if world > 1:
+                raise NotImplementedError("data-parallel training with an embedding net is not implemented")
+            if any(p.dtype != torch.float32 for p in self.emb):
+                raise TypeError("the fused trainers train float32 embedding nets (the optimizer state is float32)")
+            self.params = torch.cat([self.flat.data.reshape(-1)] + [p.data.reshape(-1).float() for p in self.emb])
+            self.grad = torch.zeros(self.n, dtype=torch.float32, device=dev)
+            self.mask = torch.cat([self.mask, torch.ones(self.n - self.P, dtype=self.mask.dtype, device=dev)])
+            self.flat.data = self.params[:self.P]
+            o = self.P
+            for p in self.emb:
+                k = p.numel()
+                p.data = self.params[o:o + k].view_as(p)
+                p.grad = self.grad[o:o + k].view_as(p)
+                o += k
+
+    def zero_grad(self):
+        """Clear the embedding gradients before the next backward accumulates into them."""
+        if self.emb:
+            self.grad[self.P:].zero_()
 
     @property
     def capturable(self) -> bool:
@@ -91,7 +142,13 @@ class _DeviceAdam:
         self._adam(grad, 0)
 
     def step_partials(self, gpart: Tensor, n_part: int):
-        """One update from the `n_part` per-CTA partial gradients of a fused loss kernel."""
+        """One update from the `n_part` per-CTA partial gradients of a fused loss kernel (and, with an
+        embedding net, the embedding gradients autograd accumulated since `zero_grad`)."""
+        if self.emb:                  # the clip+Adam kernel takes the norm over [flat | embedding] itself
+            L.check(self.lib.sbi_b200_reduce_partials(L.ptr(gpart), n_part, self.P, L.ptr(self.grad),
+                                                      L.stream_ptr()), "reduce_partials")
+            self._adam(self.grad, 0)
+            return
         if self.world == 1:           # the reduction kernel also emits the sum(g^2) partials
             L.check(self.lib.sbi_b200_reduce_partials_norm(L.ptr(gpart), n_part, self.P, L.ptr(self.grad),
                                                            L.ptr(self.mask), L.ptr(self.sumsq), L.stream_ptr()),
@@ -104,6 +161,11 @@ class _DeviceAdam:
 
     def _adam(self, grad: Tensor, n_sumsq: int):
         """n_sumsq > 0: `sumsq` already holds that many sum(g^2) partials of `grad`."""
+        if self.emb:
+            L.check(self.lib.sbi_b200_adam_clip_step(
+                L.ptr(self.params), L.ptr(grad), L.ptr(self.state), L.ptr(self.count), L.ptr(self.mask), self.n,
+                self.lr, 0.9, 0.999, 1e-8, self.max_norm, 1.0, L.stream_ptr()), "adam_clip_step")
+            return
         if n_sumsq:
             L.check(self.lib.sbi_b200_adam_clip_step_norm(
                 L.ptr(self.flat.data), L.ptr(grad), L.ptr(self.state), L.ptr(self.count), L.ptr(self.mask), self.P,
@@ -114,14 +176,23 @@ class _DeviceAdam:
                 L.ptr(self.flat.data), L.ptr(grad), L.ptr(self.state), L.ptr(self.count), L.ptr(self.mask), self.P,
                 self.lr, 0.9, 0.999, 1e-8, self.max_norm, 1.0, L.stream_ptr()), "adam_clip_step")
 
+    def _tensors(self):
+        params = self.flat.data if self.params is None else self.params
+        return [params, self.state, self.count] + self.emb_buffers
+
     def snapshot(self):
-        return self.flat.data.clone(), self.state.clone(), self.count.clone()
+        return [t.clone() for t in self._tensors()]
 
     def restore(self, snap):
-        for t, s in zip((self.flat.data, self.state, self.count), snap):
+        for t, s in zip(self._tensors(), snap):
             t.copy_(s)
 
     def close(self):
+        if self.emb:      # after training the parameters own their storage again; gradients are released
+            self.flat.data = self.flat.data.clone()
+            for p in self.emb:
+                p.data = p.data.clone()
+                p.grad = None
         if self.peer is not None:
             timed_out = self.peer.error()
             self.peer.close()
@@ -330,7 +401,7 @@ class _Trainer:
                    resume_training: bool) -> _DeviceAdam:
         """The device optimizer of this run; its Adam state and the epoch count carry over with `resume_training`."""
         if not resume_training or self._opt_state is None:
-            P = net.layout.n_params
+            P = net.layout.n_params + sum(p.numel() for p in _embedding_params(net))
             self._opt_state = torch.zeros(2 * P, dtype=torch.float32, device=self._device)
             self._opt_step = torch.zeros(2, dtype=torch.int32, device=self._device)
             self._reset_epochs()
@@ -389,13 +460,20 @@ class _Trainer:
         """base.py:1254-1284."""
         if self.epoch == 0 or self._val_loss < self._best_val_loss:
             self._best_val_loss, self._epochs_since_last_improvement = self._val_loss, 0
-            self._best_flat = net.flat.data.clone()
+            self._save_best(net)
         else:
             self._epochs_since_last_improvement += 1
         if self._epochs_since_last_improvement > stop_after_epochs - 1:
-            net.flat.data.copy_(self._best_flat)
+            self._load_best(net)
             return True
         return False
+
+    def _save_best(self, net):
+        self._best_flat = [t.clone() for t in _weights(net)]
+
+    def _load_best(self, net):
+        for t, s in zip(_weights(net), self._best_flat):
+            t.copy_(s)
 
     def _record_epoch(self, train_loss: float, val_loss: float):
         self._val_loss = val_loss
@@ -413,9 +491,10 @@ class _Trainer:
             self.epoch += 1
         if self.epoch > max_num_epochs:   # base.py:1122-1129
             if self._val_loss < self._best_val_loss:
-                self._best_val_loss, self._best_flat = self._val_loss, net.flat.data.clone()
+                self._best_val_loss = self._val_loss
+                self._save_best(net)
             elif self._best_flat is not None:
-                net.flat.data.copy_(self._best_flat)
+                self._load_best(net)
             warnings.warn(f"Maximum number of epochs `max_num_epochs={max_num_epochs}` reached, "
                           "but network has not yet fully converged.", stacklevel=3)
         self._summary["epochs_trained"].append(self.epoch)
@@ -497,10 +576,11 @@ class _FlowTrainer(_Trainer):
         if not isinstance(net, FlowEstimator):
             raise TypeError(f"{type(self).__name__} needs an sbi_b200 flow estimator, "
                             f"got {type(net).__name__}")
-        if not net._embed_identity:
-            raise NotImplementedError(
-                "the fused trainer supports nn.Identity() embedding nets; train estimators with "
-                "torch embedding nets through estimator.loss(...).backward()")
+        embed = not net._embed_identity
+        if embed and self._dist is not None:
+            raise NotImplementedError("data-parallel training with an embedding net is not implemented")
+        # a parameter-free or frozen embedding only transforms the condition: no condition gradient is needed
+        train_emb = bool(_embedding_params(net))
         if glob and B % world:
             raise ValueError(f"partition='global' needs training_batch_size ({B}) divisible by the "
                              f"number of ranks ({world})")
@@ -514,14 +594,20 @@ class _FlowTrainer(_Trainer):
         inp_all, cond_all = self._inp_cond()
         if hasattr(net, "with_dummy"):     # `made`: the network's dummy first feature (nn_utils.py:166-167)
             inp_all = net.with_dummy(inp_all).contiguous()
+        # embedding net: the condition rows in their event shape (e.g. (N, 1, 50) for a Conv1d) go through
+        # Standardize + the user's module in torch; the VJP kernel returns the gradient of the embedded context
+        cond_raw = (self._theta if self._swap else self._x) if embed else None
+        emb = net.embedding_net
         train_idx = self.train_indices.to(dev)
         val_idx = self.val_indices.to(dev)
         n_train, n_val = train_idx.shape[0], val_idx.shape[0]
         # static buffers the epoch graph reads
         perm_buf = torch.empty(steps * B, dtype=torch.int64, device=dev)
         vperm_buf = torch.empty(max(vsteps * Bv, 1), dtype=torch.int64, device=dev)
-        n_part = net.vjp_parts(Bl)
+        cond_tc = train_emb and net.vjp_cond_uses_tc(Bl)
+        n_part = lib.sbi_b200_nsf_vjp_tc_parts(Bl) if cond_tc else net.vjp_parts(Bl, param_grads_only=not train_emb)
         gpart = net._gpart(n_part)
+        gcond = torch.empty(Bl, net.layout.C, dtype=torch.float32, device=dev) if train_emb else None
         loss_acc = torch.zeros(2, dtype=torch.float32, device=dev)
         val_lp = torch.empty(max(vsteps * Bv, 1), dtype=torch.float32, device=dev)
         stats = torch.zeros(4, dtype=torch.float32, device=dev)   # train nll sum, bad, val nll sum, val bad
@@ -540,19 +626,30 @@ class _FlowTrainer(_Trainer):
             """All kernels of one epoch on the current stream (graph-capturable)."""
             m_tr = net._model(nbuf=3)
             loss_acc.zero_()
+            if embed:
+                emb.train()
             for s in range(steps):
                 o = s * B + (rank * Bl if glob else 0)
                 idx = perm_buf[o:o + Bl]
-                rows = L.Rows(inp_all.data_ptr(), cond_all.data_ptr(), idx.data_ptr(), Bl, 0)
+                if embed:
+                    opt.zero_grad()
+                    with torch.set_grad_enabled(train_emb):
+                        ctx = net._embed(cond_raw[idx]).contiguous()
+                    inp_b = inp_all[idx]
+                    rows = L.Rows(inp_b.data_ptr(), ctx.data_ptr(), None, Bl, 0)
+                else:
+                    rows = L.Rows(inp_all.data_ptr(), cond_all.data_ptr(), idx.data_ptr(), Bl, 0)
                 if w_all is None:
-                    net.vjp(m_tr, rows, Bl, None, -1.0 / Btot, None, gpart, None, None, loss_acc)
+                    net.vjp(m_tr, rows, Bl, None, -1.0 / Btot, None, gpart, None, gcond, loss_acc, cond_tc=cond_tc)
                 else:
                     w = w_all[idx]
                     torch.mul(w, -1.0 / Btot, out=g_rows)
-                    net.vjp(m_tr, rows, Bl, g_rows, 0.0, lp_rows, gpart, None, None, None)
+                    net.vjp(m_tr, rows, Bl, g_rows, 0.0, lp_rows, gpart, None, gcond, None, cond_tc=cond_tc)
                     fin = torch.isfinite(lp_rows)
                     loss_acc[0] -= (torch.where(fin, lp_rows, torch.zeros_like(lp_rows)) * w).sum()
                     loss_acc[1] += (~fin).sum()
+                if train_emb:
+                    ctx.backward(gcond)
                 opt.step_partials(gpart, n_part)
             stats[0:2].copy_(loss_acc)
             stats[2:4].zero_()
@@ -560,7 +657,14 @@ class _FlowTrainer(_Trainer):
                 m_ev = net._model(nbuf=2)
                 vrows = vperm_buf[v_lo:v_hi]
                 vlp = val_lp[:v_hi - v_lo]
-                rows = L.Rows(inp_all.data_ptr(), cond_all.data_ptr(), vrows.data_ptr(), v_hi - v_lo, 0)
+                if embed:
+                    emb.eval()
+                    with torch.no_grad():
+                        vctx = net._embed(cond_raw[vrows]).contiguous()
+                    vinp = inp_all[vrows]
+                    rows = L.Rows(vinp.data_ptr(), vctx.data_ptr(), None, v_hi - v_lo, 0)
+                else:
+                    rows = L.Rows(inp_all.data_ptr(), cond_all.data_ptr(), vrows.data_ptr(), v_hi - v_lo, 0)
                 # validation rows go through the tensor-core kernel when the model fits it (its
                 # operands are re-packed from the just-updated parameters inside _tc_state)
                 tc_ev = net._tc_state(m_ev) if v_hi - v_lo >= net.TC_MIN_ROWS else None
@@ -948,6 +1052,11 @@ class FMPE(_Trainer):
         net, B, Bv, steps, vsteps = self._prepare(validation_fraction, training_batch_size, resume_training)
         x2d = self._x.reshape(self._x.shape[0], -1).contiguous()
         D = net.layout.D
+        embed = not net._embed_identity
+        if embed and self._dist is not None:
+            raise NotImplementedError("data-parallel training with an embedding net is not implemented")
+        train_emb = bool(_embedding_params(net))      # False: a parameter-free or frozen embedding
+        emb = net.embedding_net
         self._dp_agree(vsteps, "number of validation steps per epoch")
         if glob and (B % world or Bv % world):
             raise ValueError(f"partition='global' needs the batch sizes ({B}, {Bv}) divisible by the "
@@ -968,25 +1077,50 @@ class FMPE(_Trainer):
         vperm_buf = torch.zeros(max(vsteps * Bv, 1), dtype=torch.int64, device=dev)
         stats = torch.zeros(4, dtype=torch.float32, device=dev)     # train loss sum, bad, val loss sum, bad
 
+        # embedding net: the batch's x rows (event shape) go through Standardize + the user's module in torch; the
+        # loss kernel returns the gradient of the embedded condition, which autograd takes back through the module
+        gcond = torch.empty(Bl, net.layout.C, dtype=torch.float32, device=dev) if train_emb else None
+
         def run_epoch():
             loss_acc.zero_()
+            if embed:
+                emb.train()
             for s in range(steps):
                 idx = perm_buf[s * B + o_t:s * B + o_t + Bl]
                 tms = torch.rand(Bl, device=dev)
                 eps = torch.randn(Bl, D, device=dev)
-                _, gpart, n_part = net.loss_raw(self._theta, x2d, tms, eps, index=idx, g_const=1.0 / Btot,
-                                                loss_acc=loss_acc, want_loss=False)
+                if embed:
+                    opt.zero_grad()
+                    with torch.set_grad_enabled(train_emb):
+                        ctx = net._embed(self._x[idx]).contiguous()
+                    _, gpart, n_part = net.loss_raw(self._theta[idx], ctx, tms, eps, g_const=1.0 / Btot,
+                                                    loss_acc=loss_acc, want_loss=False, gcond=gcond)
+                    if train_emb:
+                        ctx.backward(gcond)
+                else:
+                    _, gpart, n_part = net.loss_raw(self._theta, x2d, tms, eps, index=idx, g_const=1.0 / Btot,
+                                                    loss_acc=loss_acc, want_loss=False)
                 opt.step_partials(gpart, n_part)
             stats[0:2].copy_(loss_acc)
             # validation: every batch evaluated at all validation times (:524-543); g = 0 -> loss only
             loss_acc.zero_()
             if vsteps > 0:
                 nt = vt.shape[0]
+                if embed:
+                    emb.eval()
                 for s in range(vsteps):
-                    idx = vperm_buf[s * Bv + o_v:s * Bv + o_v + Bvl].repeat(nt).contiguous()
+                    vi = vperm_buf[s * Bv + o_v:s * Bv + o_v + Bvl]
+                    idx = vi.repeat(nt).contiguous()
                     tms = vt.repeat_interleave(Bvl).contiguous()
                     eps = torch.randn(Bvl * nt, D, device=dev)
-                    net.loss_raw(self._theta, x2d, tms, eps, index=idx, g_const=0.0, loss_acc=loss_acc, want_loss=False)
+                    if embed:
+                        with torch.no_grad():
+                            vctx = net._embed(self._x[vi]).repeat(nt, 1).contiguous()
+                        net.loss_raw(self._theta[idx], vctx, tms, eps, g_const=0.0, loss_acc=loss_acc,
+                                     want_loss=False)
+                    else:
+                        net.loss_raw(self._theta, x2d, tms, eps, index=idx, g_const=0.0, loss_acc=loss_acc,
+                                     want_loss=False)
             stats[2:4].copy_(loss_acc)
 
         def fill_perms():
@@ -1034,7 +1168,7 @@ class FMPE(_Trainer):
             self._best_val_loss, self._epochs_since_last_improvement, self._best_flat = float("inf"), 0, None
         if self._val_loss < self._best_val_loss:
             self._best_val_loss, self._epochs_since_last_improvement = self._val_loss, 0
-            self._best_flat = net.flat.data.clone()
+            self._save_best(net)
         else:
             if len(self._summary["validation_loss"]) >= stop_after_epochs:
                 recent = torch.tensor(self._summary["validation_loss"][-stop_after_epochs * 2:])
@@ -1044,7 +1178,7 @@ class FMPE(_Trainer):
                 return False
         if self._epochs_since_last_improvement > stop_after_epochs - 1:
             if self._best_flat is not None:
-                net.flat.data.copy_(self._best_flat)
+                self._load_best(net)
             return True
         return False
 

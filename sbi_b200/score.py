@@ -69,6 +69,8 @@ class ConditionalScoreEstimator(FlowMatchingEstimator):
                  embedding_net: Optional[nn.Module] = None, weight_fn: Union[str, Callable] = "max_likelihood",
                  beta_min: float = 0.01, beta_max: float = 10.0, t_min: float = 1e-3, t_max: float = 1.0):
         super().__init__(layout, input_shape, condition_shape, mean_0, std_0, cond_stats, div_term, embedding_net)
+        if not self._embed_identity:
+            raise NotImplementedError("the sm_90a score estimators take nn.Identity() embedding nets")
         self.t_min, self.t_max = t_min, t_max
         self.beta_min, self.beta_max = beta_min, beta_max
         self._set_weight_fn(weight_fn)
