@@ -1,7 +1,7 @@
 """Coverage diagnostics that hammer `posterior.sample` (SURVEY 8f-4): simulation-based calibration and TARP with
 the reference's signatures and return values (/root/reference/sbi/diagnostics/sbc.py:23-188,
 /root/reference/sbi/diagnostics/tarp.py:27-195).  The posterior draws for ALL observations come from one
-batched sampling call (`DirectPosterior.sample_batched`: one sampling-kernel launch per rejection round), and the
+batched sampling call (`sample_batched` of the direct, MCMC and vector-field posteriors), and the
 rank statistics are single device reductions instead of the reference's Python loop with a host read per
 (observation, dimension).  The downstream checks (`check_sbc`, `check_tarp`: KS / c2st tests on the returned
 tensors) are the reference's own, unchanged."""
@@ -23,10 +23,11 @@ def _clean(thetas: Tensor, xs: Tensor) -> Tuple[Tensor, Tensor]:
     return thetas[ok], xs[ok]
 
 
-def _posterior_samples(xs: Tensor, posterior, num_posterior_samples: int, show_progress_bar: bool) -> Tensor:
-    """(num_posterior_samples, num_xs, dim): batched sampling when the posterior has it, else one call per x
-    (utils/diagnostics_utils.py:19-98)."""
-    if hasattr(posterior, "sample_batched"):
+def _posterior_samples(xs: Tensor, posterior, num_posterior_samples: int, show_progress_bar: bool,
+                       use_batched_sampling: bool = True) -> Tensor:
+    """(num_posterior_samples, num_xs, dim): batched sampling when asked for and the posterior has it, else one
+    call per x (utils/diagnostics_utils.py:19-98)."""
+    if use_batched_sampling and hasattr(posterior, "sample_batched"):
         try:
             return posterior.sample_batched((num_posterior_samples,), x=xs, show_progress_bars=show_progress_bar)
         except (NotImplementedError, AssertionError):
@@ -66,7 +67,7 @@ def run_sbc(thetas: Tensor, xs: Tensor, posterior, num_posterior_samples: int = 
                       "results.", stacklevel=2)
     if thetas.shape[0] != xs.shape[0]:
         raise ValueError("Unequal number of parameters and observations.")
-    samples = _posterior_samples(xs, posterior, num_posterior_samples, show_progress_bar)
+    samples = _posterior_samples(xs, posterior, num_posterior_samples, show_progress_bar, use_batched_sampling)
     dap_samples = samples[0, :, :]
     assert dap_samples.shape == (n, thetas.shape[1]), "Wrong DAP shape."
     return sbc_ranks(thetas, xs, samples, reduce_fns), dap_samples
@@ -121,7 +122,7 @@ def run_tarp(thetas: Tensor, xs: Tensor, posterior, references: Optional[Tensor]
     n, d = thetas.shape
     if n < 100:
         warnings.warn("Number of TARP samples should be on the order of 100s to give reliable results.", stacklevel=2)
-    samples = _posterior_samples(xs, posterior, num_posterior_samples, show_progress_bar)
+    samples = _posterior_samples(xs, posterior, num_posterior_samples, show_progress_bar, use_batched_sampling)
     assert samples.shape == (num_posterior_samples, n, d), f"Wrong posterior samples shape for TARP: {samples.shape}"
     if references is None:
         references = get_tarp_references(thetas)

@@ -512,14 +512,16 @@ class DeviceDopri5:
 
 
 def _fm_rhs(est: FlowMatchingEstimator, cond: Tensor, R: int, with_div: bool):
-    """Right-hand side launcher for DeviceDopri5: state = theta (R, D) [| log|det| (R)]."""
+    """Right-hand side launcher for DeviceDopri5: state = theta (R, D) [| log|det| (R)]; `cond` is the embedded
+    condition, one row shared by all R rows or one row per state row."""
     lib = L.load()
     D = est.layout.D
     m = est._model(nbuf=2)
     keep = (m, cond)
+    shared = 1 if cond.shape[0] == 1 else 0
 
     def rhs(y: Tensor, t_ptr: int, out: Tensor):
-        rows = L.Rows(y.data_ptr(), keep[1].data_ptr(), None, R, 1)
+        rows = L.Rows(y.data_ptr(), keep[1].data_ptr(), None, R, shared)
         if with_div:
             L.check(lib.sbi_b200_fm_forward_div(C.byref(keep[0]), C.byref(rows), t_ptr, 1, out.data_ptr(),
                                                 out.data_ptr() + 4 * R * D, L.stream_ptr()), "fm_forward_div")
@@ -549,32 +551,44 @@ def _generic_rhs(est, cond: Tensor, R: int, with_div: bool, solver: "DeviceDopri
 
 
 def _make_solver(est, cond, R, n, dev, with_div, atol, rtol):
-    """`cond`: the raw condition (1, C).  The flow-matching kernels read the embedded condition, computed once here."""
+    """`cond`: the raw condition, (1, *condition_shape) shared by all R rows, or (B, *condition_shape) with state
+    row r belonging to observation r % B.  The flow-matching kernels read the embedded condition, computed once
+    per observation here and expanded to one row per state row."""
+    B = cond.shape[0]
     if getattr(est, "IS_SCORE", False):
         solver = DeviceDopri5(n, dev, None, atol=atol, rtol=rtol)
-        solver.rhs = _generic_rhs(est, cond.reshape(1, -1).contiguous(), R, with_div, solver)
+        c = cond.reshape(B, -1)
+        solver.rhs = _generic_rhs(est, (c if B == 1 else c.repeat(R // B, 1)).contiguous(), R, with_div, solver)
         return solver
-    ctx = est._embed(cond.reshape(1, *est.condition_shape)).contiguous()
+    ctx = est._embed(cond.reshape(B, *est.condition_shape))
+    ctx = (ctx if B == 1 else ctx.repeat(R // B, 1)).contiguous()
     return DeviceDopri5(n, dev, _fm_rhs(est, ctx, R, with_div), atol=atol, rtol=rtol)
 
 
 @torch.no_grad()
 def sample_ode(est: FlowMatchingEstimator, num_samples: int, condition: Tensor, atol: float = 1e-6,
-               rtol: float = 1e-5, return_nfe: bool = False, device_control: bool = True):
+               rtol: float = 1e-5, return_nfe: bool = False, device_control: bool = True, batched: bool = False):
     """Draw theta ~ q(theta | x): base N(mean_base, std_base) at t = t_max, integrate to t = t_min
     (VectorFieldPosterior.sample_via_ode, vector_field_posterior.py:436-465).  `device_control=False` keeps
-    the host-side loop (`odeint_dopri5`) for comparison."""
+    the host-side loop (`odeint_dopri5`) for comparison.  `batched=True`: `condition` holds B observations
+    (B, *condition_shape) and the result is (num_samples, B, D), from ONE solve over all num_samples·B states with
+    one step size for the whole state, as zuko's `odeint` takes it on a batched tensor."""
     dev = est.net.flat.device
-    cond = condition.reshape(1, *est.condition_shape).to(dev).float()
+    cond = condition.reshape(-1 if batched else 1, *est.condition_shape).to(dev).float()
+    B = cond.shape[0]
+    R = num_samples * B
     D = est.layout.D
-    y0 = est._mean_base.to(dev) + est._std_base.to(dev) * torch.randn(num_samples, D, device=dev)
+    y0 = est._mean_base.to(dev) + est._std_base.to(dev) * torch.randn(R, D, device=dev)
     if not device_control:
-        y, nfe = odeint_dopri5(lambda y, t: est.ode_fn(y, cond, torch.tensor(t, device=dev)), y0, est.t_max, est.t_min,
+        rows = cond if B == 1 else cond.repeat(num_samples, *([1] * len(est.condition_shape)))
+        y, nfe = odeint_dopri5(lambda y, t: est.ode_fn(y, rows, torch.tensor(t, device=dev)), y0, est.t_max, est.t_min,
                                atol=atol, rtol=rtol)
-        return (y, nfe) if return_nfe else y
-    solver = _make_solver(est, cond, num_samples, num_samples * D, dev, False, atol, rtol)
-    y, nfe, _, _ = solver.solve(y0, est.t_max, est.t_min)
-    y = y.reshape(num_samples, D).clone()
+    else:
+        solver = _make_solver(est, cond, R, R * D, dev, False, atol, rtol)
+        y, nfe, _, _ = solver.solve(y0, est.t_max, est.t_min)
+        y = y.reshape(R, D).clone()
+    if batched:
+        y = y.reshape(num_samples, B, D)
     return (y, nfe) if return_nfe else y
 
 
@@ -619,7 +633,7 @@ def factorised_iid_score(est, prior, theta: Tensor, cond: Tensor, t: Tensor, pri
 def sample_sde(est: FlowMatchingEstimator, num_samples: int, condition: Tensor, steps: int = 500,
                ts: Optional[Tensor] = None, eta: float = 1.0, fused: bool = True, corrector: Optional[str] = None,
                corrector_params: Optional[dict] = None, iid_method: Optional[str] = None, prior=None,
-               iid_params: Optional[dict] = None) -> Tensor:
+               iid_params: Optional[dict] = None, batched: bool = False) -> Tensor:
     """Draw theta ~ q(theta | x) with the reverse SDE, Euler-Maruyama predictor, no corrector
     (Diffuser.run, samplers/score/diffuser.py:124-180; EulerMaruyama.predict,
     samplers/score/predictors.py:112-120; driver VectorFieldPosterior._sample_via_diffusion,
@@ -628,11 +642,15 @@ def sample_sde(est: FlowMatchingEstimator, num_samples: int, condition: Tensor, 
     `fused=False` keeps the step arithmetic in torch ops in the reference's order (for comparison).
     `corrector` in {None, "langevin", "gibbs"} (samplers/score/correctors.py) and several iid observations
     (`condition` of N rows, `iid_method="fnpe"`, inference/potentials/vector_field_adaptor.py:725-813) take the
-    generic path: the same torch arithmetic as the reference around the network kernel."""
+    generic path: the same torch arithmetic as the reference around the network kernel.
+    `batched=True`: `condition` holds B observations (B, *condition_shape), not iid trials; all num_samples·B
+    particles (row n·B + b belongs to observation b) run in every step, and the result is (num_samples, B, D)."""
     assert eta > 0, "eta must be positive."
     dev = est.net.flat.device
     cond = condition.to(dev).float().reshape(-1, *est.condition_shape)
-    n_iid = cond.shape[0]
+    B = cond.shape[0] if batched else 1
+    n_iid = 1 if batched else cond.shape[0]
+    R = num_samples * B
     if n_iid > 1 and iid_method != "fnpe":
         raise NotImplementedError(f"{n_iid} iid observations need iid_method='fnpe' (the factorised score, "
                                   "vector_field_adaptor.py:725-813); 'gauss' / 'auto_gauss' / 'jac_gauss' are not built")
@@ -644,8 +662,10 @@ def sample_sde(est: FlowMatchingEstimator, num_samples: int, condition: Tensor, 
     std0 = est._std_base.to(dev).reshape(1, D)
     if iid_method == "fnpe":        # Diffuser.initialize (diffuser.py:104-121) narrows the base for this method
         std0 = math.sqrt(1 / n_iid) * std0
-    theta = est._mean_base.to(dev).reshape(1, D) + std0 * torch.randn(num_samples, D, device=dev)
+    theta = est._mean_base.to(dev).reshape(1, D) + std0 * torch.randn(R, D, device=dev)
     score_of = lambda th, t: est.score(th, cond, t)
+    if B > 1:       # (num_samples, B, D) against (1, B, C): each observation's condition is embedded once
+        score_of = lambda th, t: est.score(th.reshape(num_samples, B, D), cond.unsqueeze(0), t).reshape(R, D)
     if n_iid > 1:
         w_fn = (iid_params or {}).get("prior_score_weight")
         score_of = lambda th, t: factorised_iid_score(est, prior, th, cond, t, w_fn)
@@ -684,7 +704,7 @@ def sample_sde(est: FlowMatchingEstimator, num_samples: int, condition: Tensor, 
             theta = predict(theta, t1, t0)
             if corrector is not None:
                 theta = correct(theta, t0, t1)
-        return theta
+        return theta.reshape(num_samples, B, D) if batched else theta
     lib = L.load()
     theta = theta.contiguous()
     n = theta.numel()
@@ -692,8 +712,9 @@ def sample_sde(est: FlowMatchingEstimator, num_samples: int, condition: Tensor, 
     z = torch.empty_like(theta)
     ctrl = torch.stack([ts[0], torch.ones((), device=dev)]).contiguous()       # [t_cur, next grid index]
     m = est._model(nbuf=2)
-    cond = est._embed(cond).contiguous()          # x_o embedded once for all steps
-    rows = L.Rows(theta.data_ptr(), cond.data_ptr(), None, num_samples, 1)
+    cond = est._embed(cond)                       # x_o embedded once for all steps
+    cond = (cond if B == 1 else cond.repeat(num_samples, 1)).contiguous()
+    rows = L.Rows(theta.data_ptr(), cond.data_ptr(), None, R, 1 if B == 1 else 0)
 
     def step():
         L.check(lib.sbi_b200_fm_forward(C.byref(m), C.byref(rows), ctrl.data_ptr(), 1, v.data_ptr(), L.stream_ptr()),
@@ -704,8 +725,9 @@ def sample_sde(est: FlowMatchingEstimator, num_samples: int, condition: Tensor, 
                 "sde_em_step")
 
     nsteps = ts.numel() - 1
+    out = theta.reshape(num_samples, B, D) if batched else theta
     if nsteps < 1:
-        return theta
+        return out
     step()                                        # first step eagerly (kernel attributes), the rest replayed
     if nsteps > 1:
         graph = torch.cuda.CUDAGraph()
@@ -721,4 +743,4 @@ def sample_sde(est: FlowMatchingEstimator, num_samples: int, condition: Tensor, 
         theta.copy_(snap[0]); ctrl.copy_(snap[1])
         for _ in range(nsteps - 1):
             graph.replay()
-    return theta
+    return out

@@ -153,6 +153,46 @@ def accept_reject_sample(
     return samples, acceptance_rate.to(samples.device)
 
 
+@torch.no_grad()
+def accept_reject_batched(propose: Callable[[int], Tensor], prior, num_samples: int, B: int, D: int,
+                          max_sampling_batch_size: int, max_sampling_time: Optional[float] = None,
+                          return_partial_on_timeout: bool = False, device: str = "cuda") -> Tuple[Tensor, Tensor]:
+    """`accept_reject_sample` with `num_xos = B`, resolved on the device: `propose(n)` returns (n, B, D) draws for
+    all observations from one sampling launch; the accepted draws of each observation are placed by a cumulative
+    count, so a round costs one host sync whatever B is.  Returns ((num_samples, B, D) samples, acceptance rate per
+    observation); after a timeout with `return_partial_on_timeout`, the first rows every observation has filled."""
+    out = torch.empty(num_samples, B, D, dtype=torch.float32, device=device)
+    filled = torch.zeros(B, dtype=torch.int64, device=device)
+    drawn, accepted_total = 0, torch.zeros(B, dtype=torch.int64, device=device)
+    batch = min(num_samples, max_sampling_batch_size)
+    start = time.time()
+    while True:
+        cand = propose(batch)
+        ok = within_support(prior, cand.reshape(-1, D)).reshape(batch, B)
+        pos = torch.cumsum(ok.long(), dim=0) - 1 + filled.unsqueeze(0)            # slot of every accepted draw
+        valid = ok & (pos < num_samples)
+        sel = torch.nonzero(valid)                                                # the round's one host sync
+        out[pos[sel[:, 0], sel[:, 1]], sel[:, 1]] = cand[sel[:, 0], sel[:, 1]]
+        acc = ok.sum(0)
+        accepted_total += acc
+        drawn += batch
+        filled = torch.minimum(filled + acc, torch.full_like(filled, num_samples))
+        remaining = int((num_samples - filled).max().item())
+        if remaining <= 0:
+            break
+        if max_sampling_time is not None and (time.time() - start) > max_sampling_time:
+            n_ok = int(filled.min().item())
+            if return_partial_on_timeout and n_ok > 0:
+                warnings.warn(f"Timeout exceeded after collecting {n_ok}/{num_samples} samples. "
+                              "Returning partial results.", stacklevel=3)
+                return out[:n_ok], accepted_total.float() / drawn
+            raise RuntimeError("Sampling aborted early because rejection sampling exceeded max_sampling_time. "
+                               "This is likely due to extremely low acceptance.")
+        rate = float((accepted_total.float() / drawn).min().item())
+        batch = min(max_sampling_batch_size, max(int(1.5 * remaining / max(rate, 1e-12)), 100))
+    return out, accepted_total.float() / drawn
+
+
 class DirectPosterior:
     """p(theta | x) represented by the trained estimator itself (NPE)."""
 
@@ -251,37 +291,12 @@ class DirectPosterior:
             max_sampling_batch_size = max(1, 4_000_000 // B)
         if not (reject_outside_prior and self.prior is not None):
             return est.sample(torch.Size([num_samples]), condition=x).reshape(*torch.Size(sample_shape), B, *est.input_shape)
-        out = torch.empty(num_samples, B, D, dtype=torch.float32, device=self._device)
-        filled = torch.zeros(B, dtype=torch.int64, device=self._device)
-        drawn, accepted_total = 0, torch.zeros(B, dtype=torch.int64, device=self._device)
-        batch = min(num_samples, max_sampling_batch_size)
-        start = time.time()
-        bidx = torch.arange(B, device=self._device)
-        while True:
-            cand = est.sample(torch.Size([batch]), condition=x).reshape(batch, B, D)
-            ok = within_support(self.prior, cand.reshape(-1, D)).reshape(batch, B)
-            pos = torch.cumsum(ok.long(), dim=0) - 1 + filled.unsqueeze(0)            # slot of every accepted draw
-            valid = ok & (pos < num_samples)
-            sel = torch.nonzero(valid)                                                # the round's one host sync
-            out[pos[sel[:, 0], sel[:, 1]], sel[:, 1]] = cand[sel[:, 0], sel[:, 1]]
-            acc = ok.sum(0)
-            accepted_total += acc
-            drawn += batch
-            filled = torch.minimum(filled + acc, torch.full_like(filled, num_samples))
-            remaining = int((num_samples - filled).max().item())
-            if remaining <= 0:
-                break
-            if max_sampling_time is not None and (time.time() - start) > max_sampling_time:
-                n_ok = int(filled.min().item())
-                if return_partial_on_timeout and n_ok > 0:
-                    warnings.warn(f"Timeout exceeded after collecting {n_ok}/{num_samples} samples. "
-                                  "Returning partial results.", stacklevel=2)
-                    return out[:n_ok]
-                raise RuntimeError("Sampling aborted early because rejection sampling exceeded max_sampling_time. "
-                                   "This is likely due to extremely low acceptance.")
-            rate = float((accepted_total.float() / drawn).min().item())
-            batch = min(max_sampling_batch_size, max(int(1.5 * remaining / max(rate, 1e-12)), 100))
-        self._last_acceptance_rate = accepted_total.float() / drawn
+        propose = lambda n: est.sample(torch.Size([n]), condition=x).reshape(n, B, D)   # noqa: E731
+        out, self._last_acceptance_rate = accept_reject_batched(
+            propose, self.prior, num_samples, B, D, max_sampling_batch_size, max_sampling_time,
+            return_partial_on_timeout, self._device)
+        if out.shape[0] < num_samples:          # partial result after a timeout
+            return out
         return out.reshape(*torch.Size(sample_shape), B, *est.input_shape)
 
     def log_prob_batched(self, theta: Tensor, x: Tensor, norm_posterior: bool = True, track_gradients: bool = False,
@@ -440,6 +455,71 @@ class MCMCPosterior:
         samples = self.theta_transform.inv(samples)
         return samples.reshape((*torch.Size(sample_shape), -1))
 
+    @torch.no_grad()
+    def sample_batched(self, sample_shape, x: Tensor, method: Optional[str] = None, thin: Optional[int] = None,
+                       warmup_steps: Optional[int] = None, num_chains: Optional[int] = None,
+                       init_strategy: Optional[str] = None, init_strategy_parameters: Optional[dict] = None,
+                       num_workers: Optional[int] = None, mp_context: Optional[str] = None,
+                       show_progress_bars: bool = True) -> Tensor:
+        """Samples from p(theta | x_1), ..., p(theta | x_B): (*sample_shape, B, *input_shape)
+        (mcmc_posterior.py:369-515).  `num_chains` chains per observation, observation-major, all B·C of them in
+        ONE vectorized slice sampler: every lock-step is one potential launch over B·C (theta_c, x_{c // C}) rows
+        (`x_is_iid=False`)."""
+        from math import ceil
+        from .potentials import transformed_potential
+        from .samplers import SliceSamplerVectorized, init_batched
+        method = self.method if method is None else method
+        thin = self.thin if thin is None else thin
+        warmup_steps = self.warmup_steps if warmup_steps is None else warmup_steps
+        num_chains = self.num_chains if num_chains is None else num_chains
+        init_strategy = self.init_strategy if init_strategy is None else init_strategy
+        init_strategy_parameters = dict(self.init_strategy_parameters if init_strategy_parameters is None
+                                        else init_strategy_parameters)
+        assert method == "slice_np_vectorized", "Batched sampling only supported for vectorized samplers!"
+        num_requested = torch.Size(sample_shape).numel()
+        if num_chains > num_requested:
+            warnings.warn("The passed number of MCMC chains is larger than the number of requested samples: "
+                          f"{num_chains} > {num_requested}, resetting it to {num_requested}.", stacklevel=2)
+            num_chains = num_requested
+        x = torch.as_tensor(x, dtype=torch.float32).to(self._device)
+        if x.dim() == 1:
+            x = x.unsqueeze(0)
+        B = x.shape[0]
+        chains = B * num_chains
+        if chains > 100:
+            warnings.warn("Note that for batched sampling, we use num_chains many chains for each x in the batch. "
+                          f"With the given settings, this results in a large number of chains ({chains}), which can "
+                          "be slow and memory-intensive for vectorized MCMC. Consider reducing the number of chains "
+                          "or batch size.", stacklevel=2)
+        init_strategy_parameters.pop("num_return_samples", None)
+        if init_strategy == "latest_sample":
+            if self._mcmc_init_params is None or self._mcmc_init_params.shape[0] != chains:
+                raise ValueError(f"init_strategy='latest_sample' needs {chains} stored chain states (num_chains per "
+                                 "observation, observation-major) from an earlier call")
+            initial_params = self._mcmc_init_params
+        else:
+            initial_params = init_batched(self.proposal, self.potential_fn, self.theta_transform, x, num_chains,
+                                          init_strategy, **init_strategy_parameters)
+        self.potential_fn.set_x(x.repeat_interleave(num_chains, dim=0), x_is_iid=False)
+        dim = initial_params.shape[1]
+
+        def log_prob_fn(params):
+            return transformed_potential(params, self.potential_fn, self.theta_transform, self._device,
+                                         track_gradients=False).flatten()
+
+        sampler = SliceSamplerVectorized(log_prob_fn=log_prob_fn, init_params=initial_params.double().cpu().numpy(),
+                                         num_chains=chains, thin=thin, verbose=show_progress_bars,
+                                         device=self._device, graph=True)
+        num_samples_ = ceil((num_requested * B * thin) / chains)
+        samples = sampler.run(warmup_steps * thin + num_samples_)        # (B·C, n, dim), already thinned
+        samples = torch.from_numpy(samples[:, warmup_steps:, :])
+        self._posterior_sampler = sampler
+        self._mcmc_init_params = samples[:, -1, :].reshape(chains, dim).float().to(self._device)
+        samples = self.theta_transform.inv(samples.type(torch.float32).to(self._device))
+        # chain c belongs to observation c // num_chains: (B, C·n, dim) -> (C·n, B, dim), chain-major per observation
+        samples = samples.reshape(B, -1, dim).permute(1, 0, 2)[:num_requested]
+        return samples.reshape(*torch.Size(sample_shape), B, dim)
+
     def log_prob(self, theta: Tensor, x: Optional[Tensor] = None, track_gradients: bool = False) -> Tensor:
         """Unnormalised potential (mcmc_posterior.py:205-235)."""
         x = x if x is not None else self.default_x
@@ -486,6 +566,15 @@ class RejectionPosterior:
             max_sampling_time=max_sampling_time, return_partial_on_timeout=return_partial_on_timeout,
             device=self._device)
         return samples.reshape((*torch.Size(sample_shape), -1))
+
+    def sample_batched(self, sample_shape, x: Tensor, max_sampling_batch_size: int = 10_000,
+                       show_progress_bars: bool = True) -> Tensor:
+        """rejection_posterior.py:228-239: not implemented, so batched callers fall back to one `sample` per x."""
+        raise NotImplementedError(
+            "Batched sampling is not implemented for RejectionPosterior. "
+            "Alternatively you can use `sample` in a loop "
+            "[posterior.sample(theta, x_o) for x_o in x]."
+        )
 
     def log_prob(self, theta: Tensor, x: Optional[Tensor] = None, track_gradients: bool = False) -> Tensor:
         x = x if x is not None else self.default_x
@@ -559,6 +648,61 @@ class VectorFieldPosterior:
         else:
             samples = proposal((num_samples,))[:, 0]
         return samples.reshape(*torch.Size(sample_shape), -1)
+
+    @torch.no_grad()
+    def sample_batched(self, sample_shape, x: Tensor, predictor: str = "euler_maruyama", corrector: Optional[str] = None,
+                       predictor_params: Optional[dict] = None, corrector_params: Optional[dict] = None,
+                       steps: int = 500, ts: Optional[Tensor] = None, max_sampling_batch_size: int = 10_000,
+                       show_progress_bars: bool = True, reject_outside_prior: bool = True,
+                       max_sampling_time: Optional[float] = None, return_partial_on_timeout: bool = False) -> Tensor:
+        """Samples from p(theta | x_1), ..., p(theta | x_B): (*sample_shape, B, *input_shape)
+        (vector_field_posterior.py:507-640).  Each round is ONE ODE solve or ONE SDE run over draws x B particles
+        with one condition row per particle (each observation embedded once); draws outside the prior support
+        are rejected per observation with a cumulative count, one host sync per round."""
+        from .flowmatching import sample_ode, sample_sde
+        est = self.vector_field_estimator
+        if est.compose_enabled:
+            raise NotImplementedError("compose_standardization does not yet support sample_batched (batched / "
+                                      "multi-observation sampling). Use a single observation via sample(), or "
+                                      "disable compose_standardization.")
+        if predictor != "euler_maruyama":
+            raise NotImplementedError("predictor: only 'euler_maruyama' (the reference's only predictor)")
+        cs = est.condition_shape
+        x = torch.as_tensor(x, dtype=torch.float32).to(self._device)
+        if x.dim() == len(cs):
+            x = x.unsqueeze(0)
+        if x.dim() != len(cs) + 1 or x.shape[1:] != cs:
+            raise NotImplementedError("Batched sampling for multiple `x` is not supported for iid conditions: "
+                                      f"expected x of shape (B, *{tuple(cs)}), got {tuple(x.shape)}.")
+        B = x.shape[0]
+        D = int(torch.Size(est.input_shape).numel())
+        num_samples = torch.Size(sample_shape).numel()
+        if max_sampling_batch_size is None:
+            max_sampling_batch_size = self.max_sampling_batch_size
+        if max_sampling_batch_size * B > 100_000:
+            capped = max(1, 100_000 // B)
+            warnings.warn(f"Capping max_sampling_batch_size from {max_sampling_batch_size} to {capped} to avoid "
+                          "excessive memory usage.", stacklevel=2)
+            max_sampling_batch_size = capped
+        eta = (predictor_params or {}).get("eta", 1.0)
+
+        def propose(n: int) -> Tensor:
+            if self.sample_with == "sde":
+                s = sample_sde(est, n, x, steps=steps, ts=ts, eta=eta, corrector=corrector,
+                               corrector_params=corrector_params, batched=True)
+                self.num_function_evaluations += (steps if ts is None else ts.numel()) - 1
+            else:
+                s, nfe = sample_ode(est, n, x, return_nfe=True, batched=True)
+                self.num_function_evaluations += nfe
+            return s
+
+        if not (reject_outside_prior and self.prior is not None):
+            return propose(num_samples).reshape(*torch.Size(sample_shape), B, *est.input_shape)
+        samples, _ = accept_reject_batched(propose, self.prior, num_samples, B, D, max_sampling_batch_size,
+                                           max_sampling_time, return_partial_on_timeout, self._device)
+        if samples.shape[0] < num_samples:          # partial result after a timeout
+            return samples
+        return samples.reshape(*torch.Size(sample_shape), B, *est.input_shape)
 
     @torch.no_grad()
     def log_prob(self, theta: Tensor, x: Optional[Tensor] = None, track_gradients: bool = False,

@@ -122,8 +122,16 @@ class PosteriorBasedPotential(BasePotential):
             return torch.where(inside, lp, torch.full_like(lp, float("-inf")))    # (no host scalar: graph-capturable)
 
 
+def _check_pairs(theta: Tensor, x: Tensor):
+    """x_is_iid=False: row r of theta pairs with row r of x_o (likelihood_based_potential.py:117-124)."""
+    if theta.shape[0] != x.shape[0]:
+        raise AssertionError(f"Batch size mismatch: {theta.shape[0]} and {x.shape[0]}. When performing batched "
+                             "sampling for multiple `x`, the batch size of `theta` must match the batch size of `x`.")
+
+
 class LikelihoodBasedPotential(BasePotential):
-    """likelihood_based_potential.py:59-130: sum_trials log q(x_o,i | theta) + log p(theta)."""
+    """likelihood_based_potential.py:59-130: sum_trials log q(x_o,i | theta) + log p(theta); with
+    `x_is_iid=False`, log q(x_o,r | theta_r) + log p(theta_r) per row."""
 
     def __init__(self, likelihood_estimator, prior, x_o=None, device="cuda"):
         super().__init__(prior, x_o, device)
@@ -135,7 +143,11 @@ class LikelihoodBasedPotential(BasePotential):
         if theta.dim() == 1:
             theta = theta.unsqueeze(0)
         est = self.likelihood_estimator
-        x = self.x_o.reshape(-1, *est.input_shape)          # (n_iid, Dx)
+        x = self.x_o.reshape(-1, *est.input_shape)          # (n_iid, Dx), or (R, Dx) paired with theta
+        if not self._x_is_iid:
+            _check_pairs(theta, x)
+            with torch.set_grad_enabled(track_gradients):     # one launch, input and condition per row
+                return est.log_prob(x.unsqueeze(0), condition=theta)[0] + self.prior.log_prob(theta)
         with torch.set_grad_enabled(track_gradients):
             # _log_likelihoods_over_trials (:186-239): x (n_iid, 1, Dx) broadcast against theta (R, D)
             ll = est.log_prob(x.unsqueeze(1).expand(-1, theta.shape[0], *est.input_shape), condition=theta).sum(0)
@@ -143,7 +155,8 @@ class LikelihoodBasedPotential(BasePotential):
 
 
 class RatioBasedPotential(BasePotential):
-    """ratio_based_potential.py:49-119: sum_trials log r(theta, x_o,i) + log p(theta)."""
+    """ratio_based_potential.py:49-119: sum_trials log r(theta, x_o,i) + log p(theta); with `x_is_iid=False`,
+    log r(theta_r, x_o,r) + log p(theta_r) per row."""
 
     def __init__(self, ratio_estimator, prior, x_o=None, device="cuda"):
         super().__init__(prior, x_o, device)
@@ -159,7 +172,10 @@ class RatioBasedPotential(BasePotential):
         x = self.x_o.reshape(-1, est.layout.Dx).contiguous()       # (n_iid, Dx)
         th = theta.reshape(-1, est.layout.Dt).contiguous()
         with torch.set_grad_enabled(track_gradients):
-            if x.shape[0] == 1:   # one observation: x is shared by every pair, never repeated
+            if not self._x_is_iid:   # one pairs launch over the R (theta_r, x_r) rows
+                _check_pairs(th, x)
+                lr = _RatioFn.apply(est.net.flat, th, x, est, None, None, False)
+            elif x.shape[0] == 1:   # one observation: x is shared by every pair, never repeated
                 lr = _RatioFn.apply(est.net.flat, th, x, est, None, None, True)
             else:                 # _log_ratios_over_trials (:122-160)
                 n = x.shape[0]

@@ -325,3 +325,43 @@ def sir_init(proposal: Any, potential_fn: Callable, transform: torch_tf.Transfor
             idx = torch.multinomial(probs, 1, replacement=False)
             outs.append(transform(cands[idx, :]))
         return torch.cat(outs)
+
+
+def init_batched(proposal: Any, potential_fn: Any, transform: torch_tf.Transform, x: Tensor, num_chains: int,
+                 init_strategy: str, num_candidate_samples: int = 10_000, num_batches: int = 1,
+                 max_rows: int = 4_000_000, **kwargs: Any) -> Tensor:
+    """Initial states of `num_chains` chains for every observation in `x` (B, *event_shape), observation-major
+    (chain c belongs to observation c // num_chains), as `_get_initial_params_batched` (mcmc_posterior.py:661-735)
+    with `proposal`, `resample` or `sir` (init_strategy.py:37-114).  Like the reference, every (observation,
+    chain) group draws its own candidates; unlike its loop over observations, the potential runs with
+    `x_is_iid=False` over the candidates of many groups at once, in chunks of at most `max_rows` rows, and the
+    categorical draw is one `torch.multinomial` over the chunk's groups.  Leaves `potential_fn` set to the last
+    chunk's rows."""
+    B = x.shape[0]
+    G = B * num_chains
+    if init_strategy == "proposal":
+        return transform(proposal.sample((G,)))
+    if init_strategy not in ("resample", "sir"):
+        raise NotImplementedError(init_strategy)
+    K = num_candidate_samples * (num_batches if init_strategy == "resample" else 1)
+    per_chunk = max(1, max_rows // K)
+    outs = []
+    with torch.set_grad_enabled(False):
+        for g0 in range(0, G, per_chunk):
+            g = min(per_chunk, G - g0)
+            obs = torch.arange(g0, g0 + g, device=x.device) // num_chains
+            cands = proposal.sample((g * K,)).detach()
+            potential_fn.set_x(x[obs].repeat_interleave(K, dim=0), x_is_iid=False)
+            logw = potential_fn(cands).detach().reshape(g, K)
+            if init_strategy == "resample":
+                probs = torch.exp(logw - torch.logsumexp(logw, dim=1, keepdim=True))
+                probs[torch.isnan(probs)] = 0.0
+                probs[torch.isinf(probs)] = 0.0
+                probs /= probs.sum(dim=1, keepdim=True)
+            else:
+                logw = logw - proposal.log_prob(cands).reshape(g, K)
+                probs = torch.softmax(logw, dim=1)
+                probs[torch.isnan(probs)] = 0.0
+            idx = torch.multinomial(probs, 1, replacement=False).reshape(-1)
+            outs.append(transform(cands.reshape(g, K, -1)[torch.arange(g, device=idx.device), idx]))
+    return torch.cat(outs)
