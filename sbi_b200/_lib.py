@@ -335,3 +335,10 @@ def require_cuda(t: torch.Tensor, name: str):
 
 def ptr(t):
     return None if t is None else C.c_void_p(t.data_ptr())
+
+
+def reduce_partials(gpart: torch.Tensor, n_part: int, n_params: int) -> torch.Tensor:
+    """The sum of the first `n_part` partial-gradient slabs of `gpart`, as a fresh (n_params,) tensor."""
+    g = torch.empty(n_params, dtype=torch.float32, device=gpart.device)
+    check(load().sbi_b200_reduce_partials(ptr(gpart), n_part, n_params, ptr(g), stream_ptr()), "reduce_partials")
+    return g

@@ -8,36 +8,40 @@ same method names, argument meaning, output shapes and error behaviour, and a
 All parameters live in ONE flat `nn.Parameter` (the packed layout of `pack.NsfLayout`);
 `log_prob` is a `torch.autograd.Function` whose forward is the fused log-prob kernel and
 whose backward is the fused forward+backward (VJP) kernel.  No CPU path exists.
+`PackedNet` (the flat buffer and its `state_dict` mapping) and `_PackedEstimator` (statistics vector, model
+struct, C entry points, scratch) are shared with the ratio and vector-field estimators.
 """
 from __future__ import annotations
 
 import ctypes as C
 import os
-from typing import Optional, Tuple
+from typing import Dict, NamedTuple, Optional, Sequence, Tuple
 
 import torch
 from torch import Tensor, nn
 
 from . import _lib as L
-from .pack import MafLayout, NsfLayout
 
 
-class _Family:
-    """C-ABI entry points + model struct of one flow family (include/sbi_b200.h)."""
-
-    def __init__(self, name, struct, tab_fields, c_prefix=None):
-        self.name, self.struct, self.tab_fields = name, struct, tab_fields
-        self.c_prefix = c_prefix or name
-
-    def fn(self, what):
-        return getattr(L.load(), f"sbi_b200_{self.c_prefix}_{what}")
+class _Family(NamedTuple):
+    """How the host hands one layout family to the library (include/sbi_b200.h)."""
+    struct: type                    # the model struct of the C entry points
+    tab_fields: Tuple[str, ...]     # its table pointers, in the order of `layout.tables()`
+    prefix: str                     # C entry points `sbi_b200_<prefix>_<name>`
+    tc: Optional[str]               # prefix of the wgmma evaluation entry points (`<tc>_tc_pack`), if any
+    what: str                       # the model in error messages, formatted with the layout's fields
 
 
-FAMILIES = {
-    "nsf": _Family("nsf", L.NsfModel, ("d_layer_tab", "d_feat_tab")),
-    "maf": _Family("maf", L.MafModel, ("d_layer_tab", "d_perm_tab")),
+_FLOW = "flow (D={D}, C={C}, H={H}, num_blocks={NB})"
+_CLASSIFIER = "classifier (Dt={Dt}, Dx={Dx}, H={H})"
+_FAMILIES = {
+    "nsf": _Family(L.NsfModel, ("d_layer_tab", "d_feat_tab"), "nsf", "nsf", _FLOW),
     # `made`: the masked residual conditioner + mixture head run on the NSF kernels (head = SBI_NSF_MOG)
-    "made": _Family("made", L.NsfModel, ("d_layer_tab", "d_feat_tab"), c_prefix="nsf"),
+    "made": _Family(L.NsfModel, ("d_layer_tab", "d_feat_tab"), "nsf", None, _FLOW),
+    "maf": _Family(L.MafModel, ("d_layer_tab", "d_perm_tab"), "maf", None, _FLOW),
+    "ratio": _Family(L.RatioModel, ("d_tab",), "ratio", "ratio", _CLASSIFIER),
+    "ratio_mlp": _Family(L.RatioMlpModel, ("d_tab",), "ratio_mlp", None, _CLASSIFIER),
+    "fm": _Family(L.FmModel, ("d_tab",), "fm", None, "vector field (D={D}, C={C}, H={H}, num_layers={NL})"),
 }
 
 
@@ -54,76 +58,224 @@ class Standardize(nn.Module):
         return (tensor - self._mean) / self._std
 
 
-class _FlowNet(nn.Module):
-    """Plays the role of the nflows `Flow` object that sits at `estimator.net`."""
+def _zscore_of(emb: nn.Module) -> Optional[Tuple[Tensor, Tensor]]:
+    """(mean, std) of the `Standardize` in front of an embedding net, or None."""
+    if isinstance(emb, nn.Sequential) and isinstance(emb[0], Standardize):
+        return emb[0]._mean, emb[0]._std
+    return None
 
-    def __init__(self, layout, shift: Tensor, scale: Tensor, embedding_net: nn.Module):
+
+class PackedNet(nn.Module):
+    """Sits at `estimator.net`, where the reference keeps its network.  Owns the ONE flat fp32 parameter buffer in
+    the packed layout of `layout`, the trainable mask and the layout's index tables, and maps them to and from the
+    reference's `state_dict` keys (the layout's `net.` names without that prefix, then its structural `buffers`).
+
+    buffers: {name: tensor} kept as non-persistent buffers of the net (the flows' input z-score, FM's `div_term`);
+    head / tail: (reference key, buffer name) pairs saved before / after the layout's tensors and loaded back."""
+
+    def __init__(self, layout, buffers: Optional[Dict[str, Tensor]] = None,
+                 head: Sequence[Tuple[str, str]] = (), tail: Sequence[Tuple[str, str]] = ()):
         super().__init__()
         self.layout = layout
         self.flat = nn.Parameter(torch.zeros(layout.n_params, dtype=torch.float32))
-        self.register_buffer("_shift", shift.clone().float(), persistent=False)
-        self.register_buffer("_scale", scale.clone().float(), persistent=False)
-        tab_a, tab_b = layout.tables()
-        self.register_buffer("_layer_tab", torch.from_numpy(tab_a.copy()), persistent=False)
-        self.register_buffer("_feat_tab", torch.from_numpy(tab_b.copy()), persistent=False)
+        for name, t in (buffers or {}).items():
+            self.register_buffer(name, t.clone().float(), persistent=False)
+        self._n_tabs = 0
+        for t in layout.tables():
+            self.register_buffer(f"_tab{self._n_tabs}", torch.from_numpy(t.copy()), persistent=False)
+            self._n_tabs += 1
         self.register_buffer("_mask", layout.trainable_mask(), persistent=False)
         # masked-out raw MADE weights, kept only so that state_dict() round-trips exactly
         self.register_buffer("_raw", torch.zeros(layout.n_params if layout._wm() else 1), persistent=False)
-        self._embedding_net = embedding_net
+        self._head, self._tail = tuple(head), tuple(tail)
 
-    # -- reference-compatible (de)serialisation ---------------------------------------------
+    def tables(self):
+        """The layout's index tables on the parameter device, in `layout.tables()` order."""
+        return [getattr(self, f"_tab{i}") for i in range(self._n_tabs)]
+
+    def _raw_or_none(self):
+        return self._raw if self.layout._wm() else None
+
     def _save_to_state_dict(self, destination, prefix, keep_vars):
         lay = self.layout
-        if lay.zscore_input:
-            destination[prefix + "_transform._transforms.0._shift"] = self._shift.detach().clone()
-            destination[prefix + "_transform._transforms.0._scale"] = self._scale.detach().clone()
-        for k, t in lay.unpack(self.flat, self._raw if lay._wm() else None).items():
+        for key, name in self._head:
+            destination[prefix + key] = getattr(self, name).detach().clone()
+        for k, t in lay.unpack(self.flat, self._raw_or_none()).items():
             destination[prefix + k[len("net."):]] = t
         for k, t in lay.buffers.items():
             destination[prefix + k[len("net."):]] = t.to(self.flat.device)
+        for key, name in self._tail:
+            destination[prefix + key] = getattr(self, name).detach().clone()
 
     def _load_from_state_dict(self, state_dict, prefix, local_metadata, strict, missing_keys,
                               unexpected_keys, error_msgs):
         lay = self.layout
-        if prefix + "flat" in state_dict:   # native format
-            with torch.no_grad():
-                self.flat.copy_(state_dict.pop(prefix + "flat"))
-        else:
-            src = {}
-            for k in lay.index:
-                kk = prefix + k[len("net."):]
-                if kk in state_dict:
-                    src[k] = state_dict.pop(kk)
-                elif strict:
-                    missing_keys.append(kk)
-            if len(src) == len(lay.index):
-                with torch.no_grad():
-                    lay.pack(src, out=self.flat.data, raw_out=self._raw if lay._wm() else None)
-        for name, buf in (("_shift", self._shift), ("_scale", self._scale)):
-            kk = prefix + "_transform._transforms.0." + name
-            if kk in state_dict:
-                with torch.no_grad():
-                    buf.copy_(state_dict.pop(kk))
-        incoming = {}
-        for k in lay.buffers:
+        src = {}
+        for k in lay.index:
             kk = prefix + k[len("net."):]
             if kk in state_dict:
-                incoming[k] = state_dict.pop(kk)
-        if incoming and hasattr(lay, "load_buffers"):
+                src[k] = state_dict.pop(kk)
+            elif strict:
+                missing_keys.append(kk)
+        with torch.no_grad():
+            if len(src) == len(lay.index):
+                lay.pack(src, out=self.flat.data, raw_out=self._raw_or_none())
+            for key, name in self._head + self._tail:
+                if prefix + key in state_dict:
+                    getattr(self, name).copy_(state_dict.pop(prefix + key))
+            incoming = {k: state_dict.pop(prefix + k[len("net."):]) for k in list(lay.buffers)
+                        if prefix + k[len("net."):] in state_dict}
             # structural buffers that are data (MAF permutations): adopt them
-            new_tab_b = lay.load_buffers(incoming)
-            if new_tab_b is not None:
-                with torch.no_grad():
-                    self._feat_tab.copy_(torch.from_numpy(new_tab_b).to(self._feat_tab.device))
+            if incoming and hasattr(lay, "load_buffers") and lay.load_buffers(incoming) is not None:
+                for buf, t in zip(self.tables(), lay.tables()):
+                    buf.copy_(torch.from_numpy(t))
 
 
-def _is_identity(m: nn.Module) -> bool:
-    return isinstance(m, nn.Identity)
+class _PackedEstimator(nn.Module):
+    """What the flow, ratio and vector-field estimators share: the `PackedNet` at `self.net`, the derived kernel
+    inputs in `_cache` (never copied or pickled), the z-score statistics vector, the model struct of the layout's
+    family, partial-gradient scratch and the wgmma operand plan.  Subclasses set `net`, `_input_shape`,
+    `_condition_shape` and `_cache`, and name the sources of the statistics vector (`_stat_sources`)."""
+
+    #: input features in front of the z-scored ones (kept at shift 0, scale 1): `made`'s dummy feature
+    _STATS_OFFSET = 0
+    #: whether `_stats` returns ld_zscore = sum log|input scale| (the flows' log-determinant of the z-score)
+    _LD_ZSCORE = False
+
+    input_shape = property(lambda self: self._input_shape)
+    condition_shape = property(lambda self: self._condition_shape)
+    layout = property(lambda self: self.net.layout)
+    flat = property(lambda self: self.net.flat)
+    _family = property(lambda self: _FAMILIES[self.net.layout.family])
+
+    def __deepcopy__(self, memo):
+        import copy
+        new = self.__class__.__new__(self.__class__)
+        memo[id(self)] = new
+        for k, v in self.__dict__.items():
+            new.__dict__[k] = {} if k == "_cache" else copy.deepcopy(v, memo)
+        return new
+
+    def __getstate__(self):
+        d = dict(self.__dict__)
+        d["_cache"] = {}
+        return d
+
+    # ---- the statistics vector ------------------------------------------------------------------
+    def _stat_widths(self) -> Tuple[int, int, int, int, int]:
+        """(padded, real input width, padded, real condition width, trailing block length) of `_stats`."""
+        lay = self.layout
+        return lay.Dp, lay.D, lay.Cp, lay.C, 0
+
+    def _stat_sources(self, raw_condition: bool):
+        """((input shift, input scale) or None, (condition mean, condition std) or None, trailing block or None)."""
+        raise NotImplementedError
+
+    def _stats(self, raw_condition: bool = False) -> Tuple[Tensor, float]:
+        """The kernels' statistics vector on the parameter device, `[input shift (Dp) | input scale (Dp) |
+        condition mean (Cp) | condition std (Cp) | trailing block]` (include/sbi_b200.h `d_stats`; padding and
+        absent statistics are 0 / 1), and ld_zscore (0 unless `_LD_ZSCORE`).  Rebuilt when a source tensor's data
+        pointer or version, or the device, changes.  raw_condition: identity condition statistics, cached apart
+        (see FlowEstimator.inverse_transform)."""
+        inp, cond, tail = self._stat_sources(raw_condition)
+        srcs = [t for t in (*(inp or ()), *(cond or ()), tail) if t is not None]
+        dev = self.net.flat.device
+        key = tuple((t.data_ptr(), t._version) for t in srcs) + (str(dev),)
+        ck = "stats_raw" if raw_condition else "stats"
+        hit = self._cache.get(ck)
+        if hit is not None and hit[0] == key:
+            return hit[1], hit[2]
+        Dp, D, Cp, C, n_tail = self._stat_widths()
+        o = self._STATS_OFFSET
+        st = torch.zeros(2 * Dp + 2 * Cp + n_tail, dtype=torch.float32, device=dev)
+        st[Dp:2 * Dp] = 1.0
+        st[2 * Dp + Cp:2 * Dp + 2 * Cp] = 1.0
+        ld = 0.0
+        if inp is not None:
+            st[o:D] = inp[0].reshape(-1).expand(D - o)
+            st[Dp + o:Dp + D] = inp[1].reshape(-1).expand(D - o)
+            if self._LD_ZSCORE:
+                ld = float(torch.log(torch.abs(inp[1].double())).reshape(-1).expand(D - o).sum())
+        if cond is not None:
+            st[2 * Dp:2 * Dp + C] = cond[0].reshape(-1).expand(C)
+            st[2 * Dp + Cp:2 * Dp + Cp + C] = cond[1].reshape(-1).expand(C)
+        if tail is not None:
+            st[2 * Dp + 2 * Cp:2 * Dp + 2 * Cp + tail.numel()] = tail
+        self._cache[ck] = (key, st, ld)
+        return st, ld
+
+    # ---- the C entry points -----------------------------------------------------------------------
+    def _model(self, nbuf: int, raw_condition: bool = False):
+        """The family's model struct for the current parameters (pointers into `net` and the stats vector)."""
+        net, fam = self.net, self._family
+        L.require_cuda(net.flat, "estimator parameters")
+        st, ld = self._stats(raw_condition)
+        s = fam.struct()
+        self.layout.fill_struct(s, nbuf)
+        s.d_params = net.flat.data_ptr()
+        for field, tab in zip(fam.tab_fields, net.tables()):
+            setattr(s, field, tab.data_ptr())
+        s.d_stats = st.data_ptr()
+        s._keep = (st,)
+        self._fill_model(s, ld)
+        return s
+
+    def _fill_model(self, s, ld: float):
+        """Family-specific scalars of the model struct."""
+
+    def _entry(self, name: str):
+        """The layout's C entry point `sbi_b200_<prefix>_<name>`."""
+        return getattr(L.load(), f"sbi_b200_{self._family.prefix}_{name}")
+
+    def _check_rc(self, rc: int, what: str):
+        if rc == -2:
+            raise L.SbiB200Error(
+                f"{what}: a row tile of this {self._family.what.format(**vars(self.layout))} needs more than "
+                "the 227 KB of shared memory one CTA can use on sm_90a (SBI_ESMEM)")
+        L.check(rc, what)
+
+    def _gpart(self, n_part: int) -> Tensor:
+        """Partial-gradient scratch, (>= n_part, n_params), zeroed when (re)allocated."""
+        buf = self._cache.get("gpart")
+        dev = self.net.flat.device
+        if buf is None or buf.shape[0] < n_part or buf.device != dev:
+            buf = torch.zeros(max(n_part, 1), self.layout.n_params, dtype=torch.float32, device=dev)
+            self._cache["gpart"] = buf
+        return buf
+
+    def _tc_state(self, m):
+        """`NsfTc` descriptor of the family's wgmma evaluation kernel for the current parameters, or None if the
+        family has none, SBI_B200_TC=0, or the model is outside what the kernel instantiates.  The operands are
+        re-packed from the flat parameter buffer on every call (a ~1 MB elementwise kernel): the optimizer
+        kernels update the parameters through raw pointers, so no version counter could be trusted."""
+        tc = self._family.tc
+        if tc is None or os.environ.get("SBI_B200_TC", "") == "0":
+            return None
+        dev = self.net.flat.device
+        st = self._cache.get("tc")
+        if st is None or st["dev"] != dev:
+            plan = self.layout.tc_plan()
+            st = {"dev": dev, "plan": plan}
+            if plan is not None:
+                st.update(src=torch.as_tensor(plan["src"], device=dev), tab=torch.as_tensor(plan["tab"], device=dev),
+                          tcw=torch.empty(plan["n_words"], dtype=torch.float32, device=dev))
+            self._cache["tc"] = st
+        if st["plan"] is None:
+            return None
+        desc = L.NsfTc(st["plan"]["n_words"], st["plan"]["stage_cap"], st["src"].data_ptr(),
+                       st["tab"].data_ptr(), st["tcw"].data_ptr())
+        lib = L.load()
+        if not getattr(lib, f"sbi_b200_{tc}_tc_supported")(C.byref(m), C.byref(desc)):
+            return None
+        L.check(getattr(lib, f"sbi_b200_{tc}_tc_pack")(C.byref(m), C.byref(desc), L.stream_ptr()), f"{tc}_tc_pack")
+        return desc
 
 
-class FlowEstimator(nn.Module):
+class FlowEstimator(_PackedEstimator):
     r"""Normalizing flow q(input | condition) evaluated by hand-written sm_90a kernels
     (families: neural spline flow `nsf`, masked autoregressive flow `maf`)."""
+
+    _LD_ZSCORE = True
 
     def __init__(self, layout, input_shape, condition_shape, shift: Tensor,
                  scale: Tensor, cond_mean: Optional[Tensor], cond_std: Optional[Tensor],
@@ -132,101 +284,29 @@ class FlowEstimator(nn.Module):
         self._input_shape = torch.Size(input_shape)
         self._condition_shape = torch.Size(condition_shape)
         user_net = embedding_net if embedding_net is not None else nn.Identity()
-        self._embed_identity = _is_identity(user_net)
+        self._embed_identity = isinstance(user_net, nn.Identity)
         if cond_mean is not None:
             emb = nn.Sequential(Standardize(cond_mean, cond_std), user_net)
         else:
             emb = user_net
-        self.net = _FlowNet(layout, shift, scale, emb)
+        zscore = [("_transform._transforms.0._shift", "_shift"), ("_transform._transforms.0._scale", "_scale")]
+        # plays the role of the nflows `Flow` object that sits at `estimator.net`
+        self.net = PackedNet(layout, dict(_shift=shift, _scale=scale), head=zscore if layout.zscore_input else ())
+        self.net._embedding_net = emb
         self._cache = {}
-        self.fam = FAMILIES[layout.family]
-
-    # ---- properties of the reference interface ---------------------------------------------
-    @property
-    def layout(self):
-        return self.net.layout
-
-    @property
-    def input_shape(self) -> torch.Size:
-        return self._input_shape
-
-    @property
-    def condition_shape(self) -> torch.Size:
-        return self._condition_shape
 
     @property
     def embedding_net(self) -> nn.Module:
         return self.net._embedding_net
 
-    @property
-    def flat(self) -> nn.Parameter:
-        return self.net.flat
-
-    def __deepcopy__(self, memo):
-        import copy
-        cls = self.__class__
-        new = cls.__new__(cls)
-        memo[id(self)] = new
-        for k, v in self.__dict__.items():
-            if k == "_cache":
-                new.__dict__[k] = {}
-            else:
-                new.__dict__[k] = copy.deepcopy(v, memo)
-        return new
-
-    def __getstate__(self):
-        d = dict(self.__dict__)
-        d["_cache"] = {}
-        return d
-
     # ---- kernel-side views --------------------------------------------------------------------
-    def _kernel_stats(self, raw_condition: bool = False) -> Tuple[Tensor, float]:
-        """[shift(Dp) | scale(Dp) | ctx_mean(Cp) | ctx_std(Cp)] on the parameter device.
-        raw_condition: identity statistics for the condition (see inverse_transform)."""
-        lay = self.layout
+    def _stat_sources(self, raw_condition: bool):
         net = self.net
-        emb = net._embedding_net
-        std_mod = emb[0] if isinstance(emb, nn.Sequential) and isinstance(emb[0], Standardize) else None
-        srcs = [net._shift, net._scale] + ([std_mod._mean, std_mod._std] if std_mod is not None else [])
-        key = tuple((t.data_ptr(), t._version) for t in srcs) + (str(net.flat.device), raw_condition)
-        ck = "stats_raw" if raw_condition else "stats"
-        hit = self._cache.get(ck)
-        if hit is not None and hit[0] == key:
-            return hit[1], hit[2]
-        dev = net.flat.device
-        st = torch.zeros(2 * lay.Dp + 2 * lay.Cp, dtype=torch.float32, device=dev)
-        st[lay.Dp:2 * lay.Dp] = 1.0
-        st[2 * lay.Dp + lay.Cp:] = 1.0
-        st[:lay.D] = net._shift.expand(lay.D)
-        st[lay.Dp:lay.Dp + lay.D] = net._scale.expand(lay.D)
-        if std_mod is not None and self._embed_identity and not raw_condition:
-            st[2 * lay.Dp:2 * lay.Dp + lay.C] = std_mod._mean.reshape(-1).expand(lay.C)
-            st[2 * lay.Dp + lay.Cp:2 * lay.Dp + lay.Cp + lay.C] = std_mod._std.reshape(-1).expand(lay.C)
-        ld = float(torch.log(torch.abs(net._scale.double())).expand(lay.D).sum())
-        self._cache[ck] = (key, st, ld)
-        return st, ld
+        cond = None if raw_condition or not self._embed_identity else _zscore_of(net._embedding_net)
+        return (net._shift, net._scale), cond, None
 
-    def _model(self, nbuf: int, raw_condition: bool = False):
-        net = self.net
-        L.require_cuda(net.flat, "estimator parameters")
-        st, ld = self._kernel_stats(raw_condition)
-        s = self.fam.struct()
-        self.layout.fill_struct(s, nbuf)
+    def _fill_model(self, s, ld: float):
         s.ld_zscore = ld
-        s.d_params = net.flat.data_ptr()
-        setattr(s, self.fam.tab_fields[0], net._layer_tab.data_ptr())
-        setattr(s, self.fam.tab_fields[1], net._feat_tab.data_ptr())
-        s.d_stats = st.data_ptr()
-        s._keep = (st,)
-        return s
-
-    def _check_rc(self, rc: int, what: str):
-        if rc == -2:
-            lay = self.layout
-            raise L.SbiB200Error(
-                f"{what}: a row tile of this flow (D={lay.D}, C={lay.C}, H={lay.H}, num_blocks={lay.NB}) needs "
-                "more than the 227 KB of shared memory one CTA can use on sm_90a (SBI_ESMEM)")
-        L.check(rc, what)
 
     def _embed(self, condition: Tensor) -> Tensor:
         """Context fed to the kernels.  Identity embedding: raw condition (standardised
@@ -234,14 +314,6 @@ class FlowEstimator(nn.Module):
         if self._embed_identity:
             return condition.reshape(condition.shape[0], -1)
         return self.net._embedding_net(condition).reshape(condition.shape[0], -1)
-
-    def _gpart(self, n_part: int) -> Tensor:
-        buf = self._cache.get("gpart")
-        n = self.layout.n_params
-        if buf is None or buf.shape[0] < n_part or buf.device != self.net.flat.device:
-            buf = torch.zeros(max(n_part, 1), n, dtype=torch.float32, device=self.net.flat.device)
-            self._cache["gpart"] = buf
-        return buf
 
     # ---- shape handling: base.py:84-198 --------------------------------------------------------
     def _check_condition_shape(self, condition: Tensor):
@@ -377,53 +449,22 @@ class FlowEstimator(nn.Module):
         lad = torch.empty(R, dtype=torch.float32, device=noise.device)
         m = self._model(nbuf=2)
         rows = L.Rows(noise.data_ptr(), ctx.data_ptr(), None, R, 1 if shared else 0)
-        force = os.environ.get("SBI_B200_TC", "") == "1"
-        if self.fam.name == "nsf" and (R >= self.TC_MIN_ROWS or force):
+        if R >= self.TC_MIN_ROWS or os.environ.get("SBI_B200_TC", "") == "1":
             tc = self._tc_state(m)
             if tc is not None:
-                L.check(L.load().sbi_b200_nsf_inverse_tc(C.byref(m), C.byref(tc), C.byref(rows), L.ptr(out),
-                                                         L.ptr(lad), L.stream_ptr()), "nsf_inverse_tc")
+                L.check(lib.sbi_b200_nsf_inverse_tc(C.byref(m), C.byref(tc), C.byref(rows), L.ptr(out),
+                                                L.ptr(lad), L.stream_ptr()), "nsf_inverse_tc")
                 return out, lad
-        self._check_rc(self.fam.fn("inverse")(C.byref(m), C.byref(rows), L.ptr(out), L.ptr(lad),
-                                              L.stream_ptr()), f"{self.fam.name}_inverse")
+        self._check_rc(self._entry("inverse")(C.byref(m), C.byref(rows), L.ptr(out), L.ptr(lad), L.stream_ptr()),
+                       f"{self.layout.family}_inverse")
         return out, lad
 
     # ---- tensor-core bulk path (nsf only) --------------------------------------------------------
     #: rows from which log_prob / sampling go through the wgmma kernel (csrc/nsf_tc.cu).  The
     #: crossover against the SIMT kernel has not been measured for the wgmma kernel (profiles/tc_cross.py
     #: measures it); 1024 is carried over from the earlier tensor-core design.
-    #: SBI_B200_TC=0 disables, =1 forces.
+    #: SBI_B200_TC=0 disables, =1 forces (`_PackedEstimator._tc_state`).
     TC_MIN_ROWS = int(os.environ.get("SBI_B200_TC_MIN_ROWS", 1024))
-
-    def _tc_state(self, m):
-        """NsfTc struct for the current parameters, or None if the model is outside what the
-        tensor-core kernel instantiates.  The operands are re-packed from the flat parameter
-        buffer on every call (a ~1 MB elementwise kernel): the optimizer kernels update the
-        parameters through raw pointers, so no version counter could be trusted."""
-        if self.fam.name != "nsf" or os.environ.get("SBI_B200_TC", "") == "0":
-            return None
-        flat = self.net.flat
-        st = self._cache.get("tc")
-        if st is None or st["dev"] != flat.device:
-            plan = self.layout.tc_plan()
-            if plan is None:
-                self._cache["tc"] = {"dev": flat.device, "plan": None}
-                return None
-            dev = flat.device
-            st = {"dev": dev, "plan": plan,
-                  "src": torch.as_tensor(plan["src"], device=dev),
-                  "tab": torch.as_tensor(plan["tab"], device=dev),
-                  "tcw": torch.empty(plan["n_words"], dtype=torch.float32, device=dev)}
-            self._cache["tc"] = st
-        if st["plan"] is None:
-            return None
-        tc = L.NsfTc(st["plan"]["n_words"], st["plan"]["stage_cap"], st["src"].data_ptr(),
-                     st["tab"].data_ptr(), st["tcw"].data_ptr())
-        lib = L.load()
-        if not lib.sbi_b200_nsf_tc_supported(C.byref(m), C.byref(tc)):
-            return None
-        L.check(lib.sbi_b200_nsf_tc_pack(C.byref(m), C.byref(tc), L.stream_ptr()), "nsf_tc_pack")
-        return tc
 
     # ---- fused forward+backward of a batch (parameter / input / condition gradients) --------------
     #: rows from which the training VJP runs on the tensor cores (csrc/nsf_vjp_tc.cu) when only parameter
@@ -434,7 +475,7 @@ class FlowEstimator(nn.Module):
     def _tc_train_state(self, m, pack: bool = True):
         """(tc_fwd, tc_bwd, tc_both) operand descriptors for the tensor-core training step, freshly
         packed from the current parameters by ONE pack launch over both plans (`tc_both`), or None."""
-        if self.fam.name != "nsf" or os.environ.get("SBI_B200_VJP_TC", "") == "0":
+        if self.layout.family != "nsf" or os.environ.get("SBI_B200_VJP_TC", "") == "0":
             return None
         flat = self.net.flat
         st = self._cache.get("tc_train")
@@ -468,11 +509,11 @@ class FlowEstimator(nn.Module):
         """Number of partial-gradient slabs `vjp` writes for R rows."""
         if self._vjp_uses_tc(R, param_grads_only):
             return L.load().sbi_b200_nsf_vjp_tc_parts(R)
-        return self.fam.fn("vjp_parts")(R)
+        return self._entry("vjp_parts")(R)
 
     def _vjp_uses_tc(self, R: int, param_grads_only: bool) -> bool:
         env = os.environ.get("SBI_B200_VJP_TC", "")
-        if self.fam.name != "nsf" or env == "0" or not param_grads_only:
+        if self.layout.family != "nsf" or env == "0" or not param_grads_only:
             return False
         if R < self.VJP_TC_MIN_ROWS and env != "1":
             return False
@@ -517,32 +558,34 @@ class FlowEstimator(nn.Module):
                                                 g_const, L.ptr(logp), L.ptr(gpart), L.ptr(loss_acc), L.ptr(save),
                                                 save.numel() * 4, L.stream_ptr()), "nsf_vjp_tc")
                 return
-        self._check_rc(self.fam.fn("vjp")(C.byref(m), C.byref(rows), L.ptr(gout), g_const, L.ptr(logp),
+        self._check_rc(self._entry("vjp")(C.byref(m), C.byref(rows), L.ptr(gout), g_const, L.ptr(logp),
                                           L.ptr(gpart), L.ptr(ginput), L.ptr(gcond), L.ptr(loss_acc),
-                                          L.stream_ptr()), f"{self.fam.name}_vjp")
+                                          L.stream_ptr()), f"{self.layout.family}_vjp")
 
     # ---- raw kernel entry (no autograd) --------------------------------------------------------------
     def _logprob_raw(self, inp: Tensor, ctx: Tensor, shared: bool, want_noise=False,
                      index: Optional[Tensor] = None, n_rows: Optional[int] = None,
-                     raw_condition: bool = False):
+                     raw_condition: bool = False, out: Optional[Tensor] = None):
+        """Log-probs (and with `want_noise` the base-space noise) of R rows, R = n_rows or len(inp), with the
+        condition of row r at ctx[r] (ctx[0] when `shared`) and optional row `index`; written into `out` (R,) if
+        given.  wgmma kernel from TC_MIN_ROWS rows when the model fits it, else the SIMT kernel."""
         lib = L.load()
         L.require_cuda(inp, "input")
         L.require_cuda(ctx, "condition")
         R = inp.shape[0] if n_rows is None else n_rows
-        lp = torch.empty(R, dtype=torch.float32, device=inp.device)
+        lp = torch.empty(R, dtype=torch.float32, device=inp.device) if out is None else out
         noise = torch.empty(R, self.layout.D, dtype=torch.float32, device=inp.device) if want_noise else None
         m = self._model(nbuf=2, raw_condition=raw_condition)
         rows = L.Rows(inp.data_ptr(), ctx.data_ptr(),
                       None if index is None else index.data_ptr(), R, 1 if shared else 0)
-        force = os.environ.get("SBI_B200_TC", "") == "1"
-        if self.fam.name == "nsf" and (R >= self.TC_MIN_ROWS or force):
+        if R >= self.TC_MIN_ROWS or os.environ.get("SBI_B200_TC", "") == "1":
             tc = self._tc_state(m)
             if tc is not None:
                 L.check(lib.sbi_b200_nsf_logprob_tc(C.byref(m), C.byref(tc), C.byref(rows), L.ptr(lp),
                                                     L.ptr(noise), L.stream_ptr()), "nsf_logprob_tc")
                 return lp, noise
-        self._check_rc(self.fam.fn("logprob")(C.byref(m), C.byref(rows), L.ptr(lp), L.ptr(noise),
-                                              L.stream_ptr()), f"{self.fam.name}_logprob")
+        self._check_rc(self._entry("logprob")(C.byref(m), C.byref(rows), L.ptr(lp), L.ptr(noise), L.stream_ptr()),
+                       f"{self.layout.family}_logprob")
         return lp, noise
 
 
@@ -558,7 +601,6 @@ class _NsfLogProb(torch.autograd.Function):
     def backward(ctx, g):
         inp, cond = ctx.saved_tensors
         est, shared = ctx.est, ctx.shared
-        lib = L.load()
         need_flat, need_inp, need_cond = ctx.needs_input_grad[0], ctx.needs_input_grad[1], ctx.needs_input_grad[2]
         R = inp.shape[0]
         n_part = est.vjp_parts(R, not (need_inp or need_cond))
@@ -569,11 +611,7 @@ class _NsfLogProb(torch.autograd.Function):
         rows = L.Rows(inp.data_ptr(), cond.data_ptr(), None, R, 1 if shared else 0)
         g = g.contiguous().float()
         est.vjp(m, rows, R, g, 0.0, None, gpart, ginp, gcond, None)
-        gflat = None
-        if need_flat:
-            gflat = torch.empty(est.layout.n_params, dtype=torch.float32, device=inp.device)
-            L.check(lib.sbi_b200_reduce_partials(L.ptr(gpart), n_part, est.layout.n_params,
-                                                 L.ptr(gflat), L.stream_ptr()), "reduce_partials")
+        gflat = L.reduce_partials(gpart, n_part, est.layout.n_params) if need_flat else None
         if need_cond and shared:
             gcond = gcond.sum(0, keepdim=True)
         return gflat, ginp, gcond, None, None
@@ -590,29 +628,7 @@ class MadeEstimator(FlowEstimator):
     kernels see `input dim + 1` features, feature 0 is fed 0 by `log_prob` and -- like the reference's
     `_sample` -- drawn from its own mixture in `sample` and dropped from the result."""
 
-    def _kernel_stats(self, raw_condition: bool = False):
-        lay, net = self.layout, self.net
-        emb = net._embedding_net
-        std_mod = emb[0] if isinstance(emb, nn.Sequential) and isinstance(emb[0], Standardize) else None
-        srcs = [net._shift, net._scale] + ([std_mod._mean, std_mod._std] if std_mod is not None else [])
-        key = tuple((t.data_ptr(), t._version) for t in srcs) + (str(net.flat.device), raw_condition)
-        ck = "stats_raw" if raw_condition else "stats"
-        hit = self._cache.get(ck)
-        if hit is not None and hit[0] == key:
-            return hit[1], hit[2]
-        dev = net.flat.device
-        Din = lay.D - 1
-        st = torch.zeros(2 * lay.Dp + 2 * lay.Cp, dtype=torch.float32, device=dev)
-        st[lay.Dp:2 * lay.Dp] = 1.0
-        st[2 * lay.Dp + lay.Cp:] = 1.0
-        st[1:lay.D] = net._shift.expand(Din)                      # feature 0 (dummy): shift 0, scale 1
-        st[lay.Dp + 1:lay.Dp + lay.D] = net._scale.expand(Din)
-        if std_mod is not None and self._embed_identity and not raw_condition:
-            st[2 * lay.Dp:2 * lay.Dp + lay.C] = std_mod._mean.reshape(-1).expand(lay.C)
-            st[2 * lay.Dp + lay.Cp:2 * lay.Dp + lay.Cp + lay.C] = std_mod._std.reshape(-1).expand(lay.C)
-        ld = float(torch.log(torch.abs(net._scale.double())).expand(Din).sum())
-        self._cache[ck] = (key, st, ld)
-        return st, ld
+    _STATS_OFFSET = 1        # feature 0 (dummy): shift 0, scale 1
 
     @staticmethod
     def with_dummy(inp: Tensor) -> Tensor:

@@ -21,50 +21,13 @@ import torch
 from torch import Tensor, nn
 
 from . import _lib as L
-from .estimators import Standardize
+from .estimators import PackedNet, Standardize, _PackedEstimator, _zscore_of
 from .neural_nets import (_linear_init, check_data_device, standardizing_stats, z_score_parser,
                           z_standardization)
 from .pack import FmLayout
 
 
-class _FmNet(nn.Module):
-    def __init__(self, layout: FmLayout, div_term: Tensor):
-        super().__init__()
-        self.layout = layout
-        self.flat = nn.Parameter(torch.zeros(layout.n_params, dtype=torch.float32))
-        self.register_buffer("_tab", torch.from_numpy(layout.tab.copy()), persistent=False)
-        self.register_buffer("_mask", layout.trainable_mask(), persistent=False)
-        self.register_buffer("_div_term", div_term.float(), persistent=False)
-
-    def _save_to_state_dict(self, destination, prefix, keep_vars):
-        for k, t in self.layout.unpack(self.flat).items():
-            destination[prefix + k[len("net."):]] = t
-        destination[prefix + "time_emb.div_term"] = self._div_term.detach().clone()
-
-    def _load_from_state_dict(self, state_dict, prefix, local_metadata, strict, missing_keys,
-                              unexpected_keys, error_msgs):
-        lay = self.layout
-        if prefix + "flat" in state_dict:
-            with torch.no_grad():
-                self.flat.copy_(state_dict.pop(prefix + "flat"))
-            return
-        src = {}
-        for k in lay.index:
-            kk = prefix + k[len("net."):]
-            if kk in state_dict:
-                src[k] = state_dict.pop(kk)
-            elif strict:
-                missing_keys.append(kk)
-        if len(src) == len(lay.index):
-            with torch.no_grad():
-                lay.pack(src, out=self.flat.data)
-        kk = prefix + "time_emb.div_term"
-        if kk in state_dict:
-            with torch.no_grad():
-                self._div_term.copy_(state_dict.pop(kk))
-
-
-class FlowMatchingEstimator(nn.Module):
+class FlowMatchingEstimator(_PackedEstimator):
     """Rectified-flow vector field v(theta_t, t; x); t=0 is data, t=1 is noise."""
 
     SCORE_DEFINED, SDE_DEFINED, MARGINALS_DEFINED = True, True, True
@@ -89,71 +52,22 @@ class FlowMatchingEstimator(nn.Module):
         self.register_buffer("_theta_shift", torch.zeros(1, *self._input_shape, dtype=torch.float32))
         self.register_buffer("_theta_scale", torch.ones(1, *self._input_shape, dtype=torch.float32))
         self.register_buffer("_compose_standardization", torch.tensor(False), persistent=True)
-        self.net = _FmNet(layout, div_term)
+        self.net = PackedNet(layout, dict(_div_term=div_term), tail=[("time_emb.div_term", "_div_term")])
         self._cache = {}
 
-    input_shape = property(lambda self: self._input_shape)
-    condition_shape = property(lambda self: self._condition_shape)
     embedding_net = property(lambda self: self._embedding_net)
-    layout = property(lambda self: self.net.layout)
-    flat = property(lambda self: self.net.flat)
 
-    def __deepcopy__(self, memo):
-        import copy
-        new = self.__class__.__new__(self.__class__)
-        memo[id(self)] = new
-        for k, v in self.__dict__.items():
-            new.__dict__[k] = {} if k == "_cache" else copy.deepcopy(v, memo)
-        return new
-
-    def __getstate__(self):
-        d = dict(self.__dict__)
-        d["_cache"] = {}
-        return d
-
-    def _stats(self) -> Tensor:
+    # ---- kernel views: [mean_0 (Dp) | std_0 (Dp) | ctx_mean (Cp) | ctx_std (Cp) | div_term (TEp/2) | 4 pad]
+    def _stat_widths(self):
         lay = self.layout
-        emb = self._embedding_net
-        srcs = [self.mean_0, self.std_0, self.net._div_term]
-        kernel_zscore = isinstance(emb, nn.Sequential) and self._embed_identity
-        if kernel_zscore:
-            srcs += [emb[0]._mean, emb[0]._std]
-        key = tuple((t.data_ptr(), t._version) for t in srcs) + (str(self.net.flat.device),)
-        hit = self._cache.get("stats")
-        if hit is not None and hit[0] == key:
-            return hit[1]
-        dev = self.net.flat.device
-        st = torch.zeros(2 * lay.Dp + 2 * lay.Cp + lay.TEp // 2 + 4, dtype=torch.float32, device=dev)
-        st[lay.Dp:2 * lay.Dp] = 1.0
-        st[2 * lay.Dp + lay.Cp:2 * lay.Dp + 2 * lay.Cp] = 1.0
-        st[:lay.D] = self.mean_0.reshape(-1)
-        st[lay.Dp:lay.Dp + lay.D] = self.std_0.reshape(-1)
-        if kernel_zscore:
-            st[2 * lay.Dp:2 * lay.Dp + lay.C] = emb[0]._mean.reshape(-1).expand(lay.C)
-            st[2 * lay.Dp + lay.Cp:2 * lay.Dp + lay.Cp + lay.C] = emb[0]._std.reshape(-1).expand(lay.C)
-        o = 2 * lay.Dp + 2 * lay.Cp
-        st[o:o + lay.TE // 2] = self.net._div_term
-        self._cache["stats"] = (key, st)
-        return st
+        return lay.Dp, lay.D, lay.Cp, lay.C, lay.TEp // 2 + 4
 
-    def _model(self, nbuf: int) -> L.FmModel:
-        L.require_cuda(self.net.flat, "estimator parameters")
-        st = self._stats()
-        s = L.FmModel()
-        self.layout.fill_struct(s, nbuf)
+    def _stat_sources(self, raw_condition: bool):
+        cond = _zscore_of(self._embedding_net) if self._embed_identity else None
+        return (self.mean_0, self.std_0), cond, self.net._div_term
+
+    def _fill_model(self, s, ld: float):
         s.noise_scale = self.noise_scale
-        s.d_params = self.net.flat.data_ptr()
-        s.d_tab = self.net._tab.data_ptr()
-        s.d_stats = st.data_ptr()
-        s._keep = (st,)
-        return s
-
-    def _gpart(self, n_part: int) -> Tensor:
-        buf = self._cache.get("gpart")
-        if buf is None or buf.shape[0] < n_part or buf.device != self.net.flat.device:
-            buf = torch.zeros(max(n_part, 1), self.layout.n_params, dtype=torch.float32, device=self.net.flat.device)
-            self._cache["gpart"] = buf
-        return buf
 
     def _embed(self, condition: Tensor) -> Tensor:
         """(n, *condition_shape) -> (n, C): the context the kernels read.  Identity embedding: the raw condition
@@ -314,11 +228,7 @@ class _FmLoss(torch.autograd.Function):
         gcond = torch.empty_like(cond) if ctx.needs_input_grad[2] else None
         L.check(lib.sbi_b200_fm_loss_vjp_cond(C.byref(m), C.byref(rows), L.ptr(times), L.ptr(eps), L.ptr(g), 0.0,
                                               None, L.ptr(gpart), None, L.ptr(gcond), L.stream_ptr()), "fm_loss_vjp")
-        gflat = None
-        if ctx.needs_input_grad[0]:
-            gflat = torch.empty(est.layout.n_params, dtype=torch.float32, device=inp.device)
-            L.check(lib.sbi_b200_reduce_partials(L.ptr(gpart), n_part, est.layout.n_params, L.ptr(gflat),
-                                                 L.stream_ptr()), "reduce_partials")
+        gflat = L.reduce_partials(gpart, n_part, est.layout.n_params) if ctx.needs_input_grad[0] else None
         return gflat, None, gcond, None, None, None
 
 

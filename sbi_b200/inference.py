@@ -21,7 +21,6 @@ same graph capture (`_capture`); a trainer supplies the body of one epoch.
 """
 from __future__ import annotations
 
-import ctypes as C
 import math
 import os
 import time
@@ -654,26 +653,17 @@ class _FlowTrainer(_Trainer):
             stats[0:2].copy_(loss_acc)
             stats[2:4].zero_()
             if v_hi > v_lo:
-                m_ev = net._model(nbuf=2)
                 vrows = vperm_buf[v_lo:v_hi]
                 vlp = val_lp[:v_hi - v_lo]
+                # the estimator's log-prob dispatch (wgmma kernel for bulk rows, its operands re-packed from the
+                # just-updated parameters), written into the static buffer the captured graph reads
                 if embed:
                     emb.eval()
                     with torch.no_grad():
                         vctx = net._embed(cond_raw[vrows]).contiguous()
-                    vinp = inp_all[vrows]
-                    rows = L.Rows(vinp.data_ptr(), vctx.data_ptr(), None, v_hi - v_lo, 0)
+                    net._logprob_raw(inp_all[vrows], vctx, False, out=vlp)
                 else:
-                    rows = L.Rows(inp_all.data_ptr(), cond_all.data_ptr(), vrows.data_ptr(), v_hi - v_lo, 0)
-                # validation rows go through the tensor-core kernel when the model fits it (its
-                # operands are re-packed from the just-updated parameters inside _tc_state)
-                tc_ev = net._tc_state(m_ev) if v_hi - v_lo >= net.TC_MIN_ROWS else None
-                if tc_ev is not None:
-                    L.check(lib.sbi_b200_nsf_logprob_tc(C.byref(m_ev), C.byref(tc_ev), C.byref(rows),
-                                                        L.ptr(vlp), None, L.stream_ptr()), "nsf_logprob_tc")
-                else:
-                    net._check_rc(net.fam.fn("logprob")(C.byref(m_ev), C.byref(rows), L.ptr(vlp), None,
-                                                        L.stream_ptr()), "flow_logprob")
+                    net._logprob_raw(inp_all, cond_all, False, index=vrows, n_rows=v_hi - v_lo, out=vlp)
                 if w_all is None:
                     # -sum of the finite log-probs and the count of non-finite ones, one fused launch
                     L.check(lib.sbi_b200_nll_stats(L.ptr(vlp), v_hi - v_lo, L.ptr(stats[2:]), L.stream_ptr()),

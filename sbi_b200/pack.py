@@ -71,6 +71,11 @@ class _LayoutOps:
     def num_real_params(self) -> int:
         return int(sum(v.size for v in self.index.values()))
 
+    def tables(self):
+        """The int32 index tables the model struct points to, in the order of its table fields (one `tab` here;
+        the flow layouts return their layer table and their feature / permutation table)."""
+        return (self.tab,)
+
 
 @dataclass
 class NsfLayout(_LayoutOps):

@@ -20,48 +20,12 @@ from torch import Tensor, nn
 from torch.nn import init
 
 from . import _lib as L
-from .estimators import Standardize
+from .estimators import PackedNet, Standardize, _PackedEstimator, _zscore_of
 from .neural_nets import _linear_init, check_data_device, standardizing_stats, z_score_parser
 from .pack import MlpRatioLayout, RatioLayout
 
-_STRUCTS = {"ratio": L.RatioModel, "ratio_mlp": L.RatioMlpModel}
 
-
-class _RatioNet(nn.Module):
-    """Sits at `estimator.net` (the reference's ResidualNet); owns the flat parameter buffer."""
-
-    def __init__(self, layout: Union[RatioLayout, MlpRatioLayout]):
-        super().__init__()
-        self.layout = layout
-        self.flat = nn.Parameter(torch.zeros(layout.n_params, dtype=torch.float32))
-        self.register_buffer("_tab", torch.from_numpy(layout.tab.copy()), persistent=False)
-        self.register_buffer("_mask", layout.trainable_mask(), persistent=False)
-        self.hidden_features = layout.H
-
-    def _save_to_state_dict(self, destination, prefix, keep_vars):
-        for k, t in self.layout.unpack(self.flat).items():
-            destination[prefix + k[len("net."):]] = t
-
-    def _load_from_state_dict(self, state_dict, prefix, local_metadata, strict, missing_keys,
-                              unexpected_keys, error_msgs):
-        lay = self.layout
-        if prefix + "flat" in state_dict:
-            with torch.no_grad():
-                self.flat.copy_(state_dict.pop(prefix + "flat"))
-            return
-        src = {}
-        for k in lay.index:
-            kk = prefix + k[len("net."):]
-            if kk in state_dict:
-                src[k] = state_dict.pop(kk)
-            elif strict:
-                missing_keys.append(kk)
-        if len(src) == len(lay.index):
-            with torch.no_grad():
-                lay.pack(src, out=self.flat.data)
-
-
-class RatioEstimator(nn.Module):
+class RatioEstimator(_PackedEstimator):
     r"""log r(theta, x) = classifier logit; trained by NRE (ratio_estimators.py:11-157)."""
 
     def __init__(self, layout: Union[RatioLayout, MlpRatioLayout], theta_shape, x_shape, theta_stats, x_stats,
@@ -76,83 +40,18 @@ class RatioEstimator(nn.Module):
             raise NotImplementedError("the sm_90a ratio kernels take nn.Identity() embedding nets")
         self.embedding_net_theta = nn.Sequential(Standardize(*theta_stats), et) if theta_stats else et
         self.embedding_net_x = nn.Sequential(Standardize(*x_stats), ex) if x_stats else ex
-        self.net = _RatioNet(layout)
+        # sits where the reference keeps its ResidualNet / nn.Sequential
+        self.net = PackedNet(layout)
+        self.net.hidden_features = layout.H
         self._cache = {}
 
-    input_shape = property(lambda self: self._input_shape)
-    condition_shape = property(lambda self: self._condition_shape)
-    layout = property(lambda self: self.net.layout)
-    flat = property(lambda self: self.net.flat)
-
-    def __deepcopy__(self, memo):
-        import copy
-        new = self.__class__.__new__(self.__class__)
-        memo[id(self)] = new
-        for k, v in self.__dict__.items():
-            new.__dict__[k] = {} if k == "_cache" else copy.deepcopy(v, memo)
-        return new
-
-    def __getstate__(self):
-        d = dict(self.__dict__)
-        d["_cache"] = {}
-        return d
-
-    # ---- kernel views
-    def _stats(self) -> Tensor:
+    # ---- kernel views: [theta mean (Dtp) | theta std (Dtp) | x mean (Dxp) | x std (Dxp)]
+    def _stat_widths(self):
         lay = self.layout
-        srcs = []
-        for emb in (self.embedding_net_theta, self.embedding_net_x):
-            if isinstance(emb, nn.Sequential) and isinstance(emb[0], Standardize):
-                srcs += [emb[0]._mean, emb[0]._std]
-        key = tuple((t.data_ptr(), t._version) for t in srcs) + (str(self.net.flat.device),)
-        hit = self._cache.get("stats")
-        if hit is not None and hit[0] == key:
-            return hit[1]
-        dev = self.net.flat.device
-        st = torch.zeros(2 * lay.Dtp + 2 * lay.Dxp, dtype=torch.float32, device=dev)
-        st[lay.Dtp:2 * lay.Dtp] = 1.0
-        st[2 * lay.Dtp + lay.Dxp:] = 1.0
-        emb = self.embedding_net_theta
-        if isinstance(emb, nn.Sequential):
-            st[:lay.Dt] = emb[0]._mean.reshape(-1).expand(lay.Dt)
-            st[lay.Dtp:lay.Dtp + lay.Dt] = emb[0]._std.reshape(-1).expand(lay.Dt)
-        emb = self.embedding_net_x
-        if isinstance(emb, nn.Sequential):
-            st[2 * lay.Dtp:2 * lay.Dtp + lay.Dx] = emb[0]._mean.reshape(-1).expand(lay.Dx)
-            st[2 * lay.Dtp + lay.Dxp:2 * lay.Dtp + lay.Dxp + lay.Dx] = emb[0]._std.reshape(-1).expand(lay.Dx)
-        self._cache["stats"] = (key, st)
-        return st
+        return lay.Dtp, lay.Dt, lay.Dxp, lay.Dx, 0
 
-    def _model(self, nbuf: int):
-        L.require_cuda(self.net.flat, "estimator parameters")
-        st = self._stats()
-        s = _STRUCTS[self.layout.family]()
-        self.layout.fill_struct(s, nbuf)
-        s.d_params = self.net.flat.data_ptr()
-        s.d_tab = self.net._tab.data_ptr()
-        s.d_stats = st.data_ptr()
-        s._keep = (st,)
-        return s
-
-    def _entry(self, name: str):
-        """The layout's C entry point `sbi_b200_<family>_<name>`."""
-        return getattr(L.load(), f"sbi_b200_{self.layout.family}_{name}")
-
-    def _check_rc(self, rc: int, what: str):
-        if rc == -2:
-            lay = self.layout
-            raise L.SbiB200Error(
-                f"{what}: a row tile of this classifier (Dt={lay.Dt}, Dx={lay.Dx}, H={lay.H}) needs more than "
-                "the 227 KB of shared memory one CTA can use on sm_90a (SBI_ESMEM)")
-        L.check(rc, what)
-
-    def _gpart(self, n_part: int) -> Tensor:
-        buf = self._cache.get("gpart")
-        if buf is None or buf.shape[0] < n_part or buf.device != self.net.flat.device:
-            buf = torch.zeros(max(n_part, 1), self.layout.n_params, dtype=torch.float32,
-                              device=self.net.flat.device)
-            self._cache["gpart"] = buf
-        return buf
+    def _stat_sources(self, raw_condition: bool):
+        return _zscore_of(self.embedding_net_theta), _zscore_of(self.embedding_net_x), None
 
     # ---- shape checks: ratio_estimators.py:53-112
     def _check(self, theta: Tensor, x: Tensor):
@@ -204,31 +103,6 @@ class RatioEstimator(nn.Module):
     #: the SIMT kernel has not been measured for the wgmma kernel (profiles/tc_ratio_time.py measures it)
     TC_MIN_ROWS = int(os.environ.get("SBI_B200_RATIO_TC_MIN_ROWS", 32768))
 
-    def _tc_state(self, m):
-        """`NsfTc` descriptor with freshly packed operands, or None if the model is outside what
-        the tensor-core kernel instantiates (see FlowEstimator._tc_state)."""
-        if os.environ.get("SBI_B200_TC", "") == "0" or not hasattr(self.layout, "tc_plan"):
-            return None
-        flat = self.net.flat
-        st = self._cache.get("tc")
-        if st is None or st["dev"] != flat.device:
-            plan = self.layout.tc_plan()
-            st = {"dev": flat.device, "plan": plan}
-            if plan is not None:
-                st.update(src=torch.as_tensor(plan["src"], device=flat.device),
-                          tab=torch.as_tensor(plan["tab"], device=flat.device),
-                          tcw=torch.empty(plan["n_words"], dtype=torch.float32, device=flat.device))
-            self._cache["tc"] = st
-        if st["plan"] is None:
-            return None
-        tc = L.NsfTc(st["plan"]["n_words"], st["plan"]["stage_cap"], st["src"].data_ptr(),
-                     st["tab"].data_ptr(), st["tcw"].data_ptr())
-        lib = L.load()
-        if not lib.sbi_b200_ratio_tc_supported(C.byref(m), C.byref(tc)):
-            return None
-        L.check(lib.sbi_b200_ratio_tc_pack(C.byref(m), C.byref(tc), L.stream_ptr()), "ratio_tc_pack")
-        return tc
-
 
 class _RatioFn(torch.autograd.Function):
     @staticmethod
@@ -242,7 +116,6 @@ class _RatioFn(torch.autograd.Function):
     def backward(ctx, g):
         theta, x = ctx.saved_tensors
         est = ctx.est
-        lib = L.load()
         R = g.shape[0]
         n_part = est._entry("vjp_parts")(R)
         gpart = est._gpart(n_part)
@@ -254,11 +127,7 @@ class _RatioFn(torch.autograd.Function):
         g = g.contiguous().float()
         est._check_rc(est._entry("vjp")(C.byref(m), C.byref(pr), L.ptr(g), None, L.ptr(gpart), L.ptr(gth),
                                      L.stream_ptr()), f"{est.layout.family}_vjp")
-        gflat = None
-        if need_flat:
-            gflat = torch.empty(est.layout.n_params, dtype=torch.float32, device=theta.device)
-            L.check(lib.sbi_b200_reduce_partials(L.ptr(gpart), n_part, est.layout.n_params, L.ptr(gflat),
-                                                 L.stream_ptr()), "reduce_partials")
+        gflat = L.reduce_partials(gpart, n_part, est.layout.n_params) if need_flat else None
         if need_th and ctx.ti is not None:
             raise NotImplementedError("theta gradients with an index gather are not needed by any caller")
         return gflat, gth, None, None, None, None, None

@@ -53,10 +53,7 @@ class _RawNet(torch.autograd.Function):
         g = g.contiguous().float()
         L.check(lib.sbi_b200_fm_net_vjp(C.byref(m), C.byref(rows), L.ptr(tenc), L.ptr(g), L.ptr(gpart),
                                         L.stream_ptr()), "fm_net_vjp")
-        gflat = torch.empty(est.layout.n_params, dtype=torch.float32, device=inp.device)
-        L.check(lib.sbi_b200_reduce_partials(L.ptr(gpart), n_part, est.layout.n_params, L.ptr(gflat), L.stream_ptr()),
-                "reduce_partials")
-        return gflat, None, None, None, None
+        return L.reduce_partials(gpart, n_part, est.layout.n_params), None, None, None, None
 
 
 class ConditionalScoreEstimator(FlowMatchingEstimator):
@@ -84,10 +81,9 @@ class ConditionalScoreEstimator(FlowMatchingEstimator):
         self._std_base = torch.broadcast_to(self.approx_marginal_std(t_tensor), (1, *self._input_shape)).clone()
 
     # ---- the bare network on the kernels ------------------------------------------------------------------
-    def _model(self, nbuf: int):
-        s = super()._model(nbuf)
+    def _fill_model(self, s, ld: float):
+        super()._fill_model(s, ld)
         s.raw = 1
-        return s
 
     def _raw_forward(self, inp: Tensor, cond: Tensor, tenc: Tensor) -> Tensor:
         lib = L.load()
