@@ -310,6 +310,17 @@ int sbi_b200_ratio_forward(const sbi_ratio_model* m, const sbi_pairs* pairs, flo
 int sbi_b200_ratio_vjp_parts(int64_t R);
 int sbi_b200_ratio_vjp(const sbi_ratio_model* m, const sbi_pairs* pairs, const float* d_gout,
                        float* d_logits, float* d_gpart, float* d_gtheta, void* stream);
+/* the same VJP with both input gradients: d_gtheta (R, Dt) and d_gx (R, Dx) per pair, each optional
+ * (NULL = not wanted), divided by the side's std (1 where an embedding net standardises in torch).
+ * d_gpart, d_logits and d_gtheta are bit-identical with and without d_gx. */
+int sbi_b200_ratio_vjp_inputs(const sbi_ratio_model* m, const sbi_pairs* pairs, const float* d_gout,
+                              float* d_logits, float* d_gpart, float* d_gtheta, float* d_gx, void* stream);
+/* per-row sums of per-pair rows (gradients of gathered rows): d_out (n_rows, width) with
+ * out[j] = sum_{k in [row_ptr[j], row_ptr[j+1])} gpair[order[k]], added in k order by one owner per
+ * entry (no atomics: repeat calls are bit-identical); d_order NULL = consecutive segments (order[k] = k).
+ * d_row_ptr (n_rows + 1,) int64, non-decreasing. */
+int sbi_b200_pair_rows_sum(const float* d_gpair, int32_t width, const int64_t* d_order,
+                           const int64_t* d_row_ptr, int64_t n_rows, float* d_out, void* stream);
 
 /* ---- ratio estimator: NRE `classifier_nn("mlp")` and `classifier_nn("linear")` (reference builders
  * sbi/neural_nets/net_builders/classifier.py:49-169):

@@ -193,6 +193,10 @@ _EXPORTS = {
     "sbi_b200_ratio_vjp_parts": (C.c_int, [C.c_int64]),
     "sbi_b200_ratio_vjp": (C.c_int, [C.POINTER(RatioModel), C.POINTER(Pairs), C.c_void_p, C.c_void_p,
                                      C.c_void_p, C.c_void_p, C.c_void_p]),
+    "sbi_b200_ratio_vjp_inputs": (C.c_int, [C.POINTER(RatioModel), C.POINTER(Pairs), C.c_void_p, C.c_void_p,
+                                            C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "sbi_b200_pair_rows_sum": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p,
+                                         C.c_void_p]),
     "sbi_b200_ratio_mlp_forward": (C.c_int, [C.POINTER(RatioMlpModel), C.POINTER(Pairs), C.c_void_p, C.c_void_p]),
     "sbi_b200_ratio_mlp_vjp_parts": (C.c_int, [C.c_int64]),
     "sbi_b200_ratio_mlp_vjp": (C.c_int, [C.POINTER(RatioMlpModel), C.POINTER(Pairs), C.c_void_p, C.c_void_p,

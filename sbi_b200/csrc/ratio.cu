@@ -151,7 +151,7 @@ template <int TM, int RN, int RK>
 __global__ void __launch_bounds__(kThreads, 1)
 ratio_vjp_kernel(const __grid_constant__ sbi_ratio_model m, const __grid_constant__ sbi_pairs pr,
                  const float* __restrict__ gout, float* __restrict__ logits, float* __restrict__ gpart,
-                 float* __restrict__ gtheta) {
+                 float* __restrict__ gtheta, float* __restrict__ gx) {
   constexpr int LD = Tile<TM>::LD;
   extern __shared__ __align__(128) float sm[];
   const RatioSmem L = ratio_smem_layout(m, TM, true);
@@ -160,7 +160,8 @@ ratio_vjp_kernel(const __grid_constant__ sbi_ratio_model m, const __grid_constan
   const float* __restrict__ P = m.d_params;
   const int* T = m.d_tab;
   const int Hp = m.Hp, K0p = m.Dtp + m.Dxp;
-  const bool need_dth = (gtheta != nullptr);
+  // the W0 dX stage yields dU for every input column; it runs when either side's gradient is wanted
+  const bool need_du = (gtheta != nullptr) || (gx != nullptr);
 
   if (threadIdx.x >= kConsumerThreads) {
     if (threadIdx.x == kConsumerThreads) {
@@ -173,7 +174,7 @@ ratio_vjp_kernel(const __grid_constant__ sbi_ratio_model m, const __grid_constan
           dx_stage<kProducer, TM, RK>(pipe, P + __ldg(BT + 2), Hp, Hp, m.rpc1, nullptr, Hp, noop);
           dx_stage<kProducer, TM, RK>(pipe, P + __ldg(BT + 0), Hp, Hp, m.rpc1, nullptr, Hp, noop);
         }
-        if (need_dth) dx_stage<kProducer, TM, RK>(pipe, P + __ldg(T + SBI_R_W0), Hp, K0p, m.rpc0, nullptr, K0p, noop);
+        if (need_du) dx_stage<kProducer, TM, RK>(pipe, P + __ldg(T + SBI_R_W0), Hp, K0p, m.rpc0, nullptr, K0p, noop);
       }
     }
     return;
@@ -246,7 +247,7 @@ ratio_vjp_kernel(const __grid_constant__ sbi_ratio_model m, const __grid_constan
                                   });
     }
     gemm_dw<TM>(dH, m.H, sm + L.U, K0p, K0p, gp + __ldg(T + SBI_R_W0), gp + __ldg(T + SBI_R_B0), accum);
-    if (need_dth) {
+    if (need_du) {
       dx_stage<kConsumer, TM, RK>(pipe, nullptr, Hp, K0p, m.rpc0, dH, K0p,
                                   [&](int k0, int r0, float(&acc)[RK][4], bool first) {
 #pragma unroll
@@ -261,13 +262,37 @@ ratio_vjp_kernel(const __grid_constant__ sbi_ratio_model m, const __grid_constan
                                       st4(p, o);
                                     }
                                   });
-      for (int e = threadIdx.x; e < TM * m.Dt; e += kConsumerThreads) {
-        const int r = e / m.Dt, d = e % m.Dt;
-        if (row0 + r < pr.R) gtheta[(row0 + r) * m.Dt + d] = dU[d * LD + r] / __ldg(st + m.Dtp + d);
-      }
+      if (gtheta != nullptr)
+        for (int e = threadIdx.x; e < TM * m.Dt; e += kConsumerThreads) {
+          const int r = e / m.Dt, d = e % m.Dt;
+          if (row0 + r < pr.R) gtheta[(row0 + r) * m.Dt + d] = dU[d * LD + r] / __ldg(st + m.Dtp + d);
+        }
+      if (gx != nullptr)
+        for (int e = threadIdx.x; e < TM * m.Dx; e += kConsumerThreads) {
+          const int r = e / m.Dx, d = e % m.Dx;
+          if (row0 + r < pr.R)
+            gx[(row0 + r) * m.Dx + d] = dU[(m.Dtp + d) * LD + r] / __ldg(st + 2 * m.Dtp + m.Dxp + d);
+        }
     }
     consumer_sync();
   }
+}
+
+// out[j] = sum_{k in [row_ptr[j], row_ptr[j+1])} gpair[order ? order[k] : k], summed in k order by the one
+// thread that owns out[j][c]: no atomics, so repeated calls are bit-identical.
+__global__ void pair_rows_sum_kernel(const float* __restrict__ gpair, int width, const int64_t* __restrict__ order,
+                                     const int64_t* __restrict__ row_ptr, int64_t n_rows, float* __restrict__ out) {
+  const int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (e >= n_rows * width) return;
+  const int64_t j = e / width;
+  const int c = (int)(e % width);
+  const int64_t k1 = __ldg(row_ptr + j + 1);
+  float acc = 0.f;
+  for (int64_t k = __ldg(row_ptr + j); k < k1; ++k) {
+    const int64_t src = order ? __ldg(order + k) : k;
+    acc += __ldg(gpair + src * width + c);
+  }
+  out[e] = acc;
 }
 
 }  // namespace sbi
@@ -331,8 +356,9 @@ extern "C" int sbi_b200_ratio_vjp_parts(int64_t R) {
   return (int)std::max<int64_t>(1, std::min<int64_t>(ntiles, ratio_num_sms()));
 }
 
-extern "C" int sbi_b200_ratio_vjp(const sbi_ratio_model* m, const sbi_pairs* pairs, const float* d_gout,
-                                  float* d_logits, float* d_gpart, float* d_gtheta, void* stream) {
+extern "C" int sbi_b200_ratio_vjp_inputs(const sbi_ratio_model* m, const sbi_pairs* pairs, const float* d_gout,
+                                         float* d_logits, float* d_gpart, float* d_gtheta, float* d_gx,
+                                         void* stream) {
   sbi::DeviceGuard dev_guard_(m ? m->d_params : nullptr);
   int rc = ratio_check(m);
   if (rc) return rc;
@@ -342,6 +368,22 @@ extern "C" int sbi_b200_ratio_vjp(const sbi_ratio_model* m, const sbi_pairs* pai
   auto k = ratio_vjp_kernel<TM, 2, 2>;
   if ((rc = ratio_set_smem<2>(k, L.total_bytes))) return rc;
   const int grid = sbi_b200_ratio_vjp_parts(pairs->R);
-  k<<<grid, kThreads, L.total_bytes, (cudaStream_t)stream>>>(*m, *pairs, d_gout, d_logits, d_gpart, d_gtheta);
+  k<<<grid, kThreads, L.total_bytes, (cudaStream_t)stream>>>(*m, *pairs, d_gout, d_logits, d_gpart, d_gtheta, d_gx);
+  return (int)cudaGetLastError();
+}
+
+extern "C" int sbi_b200_ratio_vjp(const sbi_ratio_model* m, const sbi_pairs* pairs, const float* d_gout,
+                                  float* d_logits, float* d_gpart, float* d_gtheta, void* stream) {
+  return sbi_b200_ratio_vjp_inputs(m, pairs, d_gout, d_logits, d_gpart, d_gtheta, nullptr, stream);
+}
+
+extern "C" int sbi_b200_pair_rows_sum(const float* d_gpair, int32_t width, const int64_t* d_order,
+                                      const int64_t* d_row_ptr, int64_t n_rows, float* d_out, void* stream) {
+  if (width < 1 || n_rows < 0 || !d_row_ptr || !d_out || (n_rows > 0 && !d_gpair)) return SBI_EINVAL;
+  if (n_rows == 0) return 0;
+  sbi::DeviceGuard dev_guard_(d_out);
+  const int64_t n = n_rows * width;
+  pair_rows_sum_kernel<<<(unsigned)((n + 255) / 256), 256, 0, (cudaStream_t)stream>>>(d_gpair, width, d_order,
+                                                                                   d_row_ptr, n_rows, d_out);
   return (int)cudaGetLastError();
 }

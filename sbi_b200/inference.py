@@ -49,26 +49,37 @@ def _process_device(device: str) -> str:
     return str(device)
 
 
+def _embedding_nets(net) -> list:
+    """The torch embedding nets an estimator runs ahead of its kernels: the flows' and vector fields' condition
+    embedding, the ratio estimator's theta and x embeddings ([] where every embedding is the identity)."""
+    if hasattr(net, "embedding_nets"):
+        return list(net.embedding_nets)
+    return [] if getattr(net, "_embed_identity", True) else [net.embedding_net]
+
+
 def _embedding_params(net) -> list:
-    """The trainable parameters of an estimator's torch embedding net ([] for an identity embedding)."""
-    if getattr(net, "_embed_identity", True):
-        return []
-    return [p for p in net.embedding_net.parameters() if p.requires_grad]
+    """The trainable parameters of an estimator's torch embedding nets ([] for identity embeddings)."""
+    seen, out = set(), []
+    for emb in _embedding_nets(net):
+        for p in emb.parameters():
+            if p.requires_grad and id(p) not in seen:
+                seen.add(id(p))
+                out.append(p)
+    return out
 
 
-def _embedding_buffers(emb: nn.Module) -> list:
-    """The embedding net's buffers that training can change (e.g. BatchNorm statistics).  The condition z-score
+def _embedding_buffers(embs: list) -> list:
+    """The embedding nets' buffers that training can change (e.g. BatchNorm statistics).  The z-score
     (`Standardize`) is fixed at build time and is left alone: writing it would invalidate the kernel statistics
     that captured graphs read."""
-    return [b for m in emb.modules() if not isinstance(m, Standardize) for b in m.buffers(recurse=False)]
+    return [b for emb in embs for m in emb.modules() if not isinstance(m, Standardize) for b in m.buffers(recurse=False)]
 
 
 def _weights(net) -> list:
-    """The tensors a best-epoch snapshot covers: the kernel parameters and the embedding net's parameters and
+    """The tensors a best-epoch snapshot covers: the kernel parameters and the embedding nets' parameters and
     buffers (the reference deep-copies the whole state_dict, trainers/base.py:1127, :1275)."""
-    emb = getattr(net, "embedding_net", None)
-    extra = [] if emb is None else [p.data for p in emb.parameters()] + _embedding_buffers(emb)
-    return [net.flat.data] + extra
+    embs = _embedding_nets(net)
+    return [net.flat.data] + [p.data for emb in embs for p in emb.parameters()] + _embedding_buffers(embs)
 
 
 class _DeviceAdam:
@@ -88,7 +99,7 @@ class _DeviceAdam:
         self.P = net.layout.n_params
         self.state, self.count = state, step
         self.emb = _embedding_params(net)
-        self.emb_buffers = _embedding_buffers(net.embedding_net) if self.emb else []
+        self.emb_buffers = _embedding_buffers(_embedding_nets(net)) if self.emb else []
         self.n = self.P + sum(p.numel() for p in self.emb)
         self.lr = lr
         self.max_norm = float(clip_max_norm) if clip_max_norm is not None else 0.0
@@ -131,7 +142,13 @@ class _DeviceAdam:
         return self.world == 1 or self.peer is not None
 
     def step(self, grad: Tensor):
-        """One update from a gradient that is complete on this rank (autograd)."""
+        """One update from a gradient that is complete on this rank (autograd).  With an embedding net, `grad` is
+        the flat parameters' gradient; the embedding gradients are the ones autograd accumulated since
+        `zero_grad`."""
+        if self.emb:
+            self.grad[:self.P].copy_(grad)
+            self._adam(self.grad, 0)
+            return
         if self.peer is not None:     # summed over NVLink peer memory, with the sum(g^2) partials
             self.peer.sum(grad, self.grad, self.mask, self.sumsq)
             self._adam(self.grad, self.peer.n_sumsq)
@@ -875,26 +892,46 @@ class NRE_B(_PotentialPosterior, _Trainer):
         own = torch.arange(lo, hi, device=device).unsqueeze(1)
         return draws + (draws >= own).long()
 
+    def _embed_batch(self, net, idx: Tensor):
+        """(theta rows, x rows) of the batch `idx` through the estimator's embedding nets, each embedded once (the
+        reference embeds its B x num_atoms repeated rows, nre_base.py:396-415): None for a side whose embedding
+        is the identity (its rows are gathered raw by the kernels), None altogether when both are."""
+        if net._embed_theta_identity and net._embed_x_identity:
+            return None
+        th = None if net._embed_theta_identity else net.embed_theta(self._theta[idx])
+        xx = None if net._embed_x_identity else net.embed_x(self._x[idx])
+        return th, xx
+
     def _logits_on(self, net, idx: Tensor, num_atoms: int, choices: Optional[Tensor] = None,
-                   rows: Optional[tuple] = None) -> Tensor:
+                   rows: Optional[tuple] = None, emb: Optional[tuple] = None) -> Tensor:
         """`_classifier_logits` (nre_base.py:396-415) of the batch rows [rows[0], rows[1]) (default: all)
         of the batch `idx`: (n, num_atoms) logits, column 0 the jointly drawn pair; the contrastive thetas
         of a row come from the WHOLE batch (SURVEY 8e: with the global batch on every rank the
-        data-parallel loss keeps the single-GPU semantics)."""
+        data-parallel loss keeps the single-GPU semantics).  `emb`: the batch's embedded rows
+        (`_embed_batch`); an embedded side is paired by its batch-local index."""
         from .ratio import _RatioFn
         B = idx.shape[0]
         lo, hi = rows if rows is not None else (0, B)
         if choices is None:
             choices = self._contrastive_choices(B, num_atoms - 1, idx.device, (lo, hi))
         local = torch.cat([torch.arange(lo, hi, device=idx.device).unsqueeze(1), choices], dim=1)   # (n, A)
-        ti = idx[local].reshape(-1).contiguous()
-        xi = idx[lo:hi].repeat_interleave(num_atoms).contiguous()
-        return _RatioFn.apply(net.net.flat, self._theta, self._x2d, net, ti, xi, False).reshape(hi - lo, num_atoms)
+        if emb is None:
+            ti = idx[local].reshape(-1).contiguous()
+            xi = idx[lo:hi].repeat_interleave(num_atoms).contiguous()
+            return _RatioFn.apply(net.net.flat, self._theta, self._x2d, net, ti, xi, False).reshape(hi - lo, num_atoms)
+        th_e, x_e = emb
+        th, ti = (self._theta, idx[local]) if th_e is None else (th_e, local)
+        if x_e is None:
+            xx, xi = self._x2d, idx[lo:hi].repeat_interleave(num_atoms)
+        else:
+            xx, xi = x_e, torch.arange(lo, hi, device=idx.device).repeat_interleave(num_atoms)
+        return _RatioFn.apply(net.net.flat, th, xx, net, ti.reshape(-1).contiguous(), xi.contiguous(), False,
+                              x_e is not None).reshape(hi - lo, num_atoms)
 
     def _loss_on(self, net, idx: Tensor, num_atoms: int, choices: Optional[Tensor] = None,
                  rows: Optional[tuple] = None) -> Tensor:
         """NRE-B loss (nre_b.py:157-182): 1-out-of-`num_atoms` cross-entropy."""
-        logits = self._logits_on(net, idx, num_atoms, choices, rows)
+        logits = self._logits_on(net, idx, num_atoms, choices, rows, self._embed_batch(net, idx))
         log_prob = logits[:, 0] - torch.logsumexp(logits, dim=-1)
         return -torch.mean(log_prob)
 
@@ -907,6 +944,9 @@ class NRE_B(_PotentialPosterior, _Trainer):
         rank, world, glob = self._dp()
         net, B, Bv, steps, vsteps = self._prepare(validation_fraction, training_batch_size, resume_training,
                                                   retrain_from_scratch)
+        embs = net.embedding_nets
+        if embs and self._dist is not None:
+            raise NotImplementedError("data-parallel training with an embedding net is not implemented")
         self._x2d = self._x.reshape(self._x.shape[0], -1).contiguous()
         num_atoms = int(min(max(num_atoms, 2), min(B, Bv)))     # nre_base.py:236-238 (clamp to batch size)
         self._dp_agree(vsteps, "number of validation steps per epoch")
@@ -922,6 +962,9 @@ class NRE_B(_PotentialPosterior, _Trainer):
 
         def train_step(idx):
             net.net.flat.grad = None
+            for e in embs:
+                e.train()
+            opt.zero_grad()
             # every rank's rows weigh 1/world of the update's batch mean; gradients are summed
             loss = self._loss_on(net, idx, num_atoms, rows=t_rows) / world
             loss.backward()
@@ -929,6 +972,8 @@ class NRE_B(_PotentialPosterior, _Trainer):
             opt.step(net.flat.grad)
 
         def val_step(idx):
+            for e in embs:
+                e.eval()
             with torch.no_grad():
                 val_sum.add_(self._loss_on(net, idx, num_atoms, rows=v_rows) / world)
 
@@ -970,7 +1015,7 @@ class NRE_A(NRE_B):
 
     def _loss_on(self, net, idx, num_atoms, choices=None, rows=None):
         from .multiround import nre_a_loss
-        return nre_a_loss(self._logits_on(net, idx, 2, choices, rows))
+        return nre_a_loss(self._logits_on(net, idx, 2, choices, rows, self._embed_batch(net, idx)))
 
 
 SNRE_A = NRE_A
@@ -990,7 +1035,8 @@ class BNRE(NRE_A):
 
     def _loss_on(self, net, idx, num_atoms, choices=None, rows=None):
         from .multiround import bnre_loss
-        return bnre_loss(self._logits_on(net, idx, 2, choices, rows), self._regularization_strength)
+        return bnre_loss(self._logits_on(net, idx, 2, choices, rows, self._embed_batch(net, idx)),
+                         self._regularization_strength)
 
 
 class NRE_C(NRE_B):
@@ -1008,8 +1054,9 @@ class NRE_C(NRE_B):
         if K < 1:
             raise AssertionError(f"num_classes = {K} must be greater than 1.")
         cm, cj = (choices if choices is not None else (None, None))
-        logits_marginal = self._logits_on(net, idx, K + 1, cm, rows)
-        logits_joint = self._logits_on(net, idx, K, cj, rows)
+        emb = self._embed_batch(net, idx)       # both draws pair the same embedded rows
+        logits_marginal = self._logits_on(net, idx, K + 1, cm, rows, emb)
+        logits_joint = self._logits_on(net, idx, K, cj, rows, emb)
         return nre_c_loss(logits_marginal, logits_joint, self._gamma)
 
 

@@ -156,12 +156,22 @@ class LikelihoodBasedPotential(BasePotential):
 
 class RatioBasedPotential(BasePotential):
     """ratio_based_potential.py:49-119: sum_trials log r(theta, x_o,i) + log p(theta); with `x_is_iid=False`,
-    log r(theta_r, x_o,r) + log p(theta_r) per row."""
+    log r(theta_r, x_o,r) + log p(theta_r) per row.  The rows of x_o go through the x embedding net once per
+    `set_x` (the reference re-embeds them on every call); iid trials are paired with theta by index in the
+    kernel, never materialised as n x R rows."""
 
     def __init__(self, ratio_estimator, prior, x_o=None, device="cuda"):
-        super().__init__(prior, x_o, device)
         self.ratio_estimator = ratio_estimator
         self.ratio_estimator.eval()
+        super().__init__(prior, x_o, device)
+
+    def set_x(self, x_o: Optional[Tensor], x_is_iid: Optional[bool] = True):
+        super().set_x(x_o, x_is_iid)
+        self._x_rows = None
+        if self._x_o is not None:
+            est = self.ratio_estimator
+            with torch.no_grad():
+                self._x_rows = est.embed_x(self._x_o.reshape(-1, *est.x_shape))     # (n_iid, Dx) kernel rows
 
     def __call__(self, theta: Tensor, track_gradients: bool = True) -> Tensor:
         from .ratio import _RatioFn
@@ -169,17 +179,20 @@ class RatioBasedPotential(BasePotential):
         if theta.dim() == 1:
             theta = theta.unsqueeze(0)
         est = self.ratio_estimator
-        x = self.x_o.reshape(-1, est.layout.Dx).contiguous()       # (n_iid, Dx)
-        th = theta.reshape(-1, est.layout.Dt).contiguous()
+        self.x_o      # raises without an observation
+        x = self._x_rows
         with torch.set_grad_enabled(track_gradients):
+            th = est.embed_theta(theta.reshape(-1, *est.theta_shape))
             if not self._x_is_iid:   # one pairs launch over the R (theta_r, x_r) rows
                 _check_pairs(th, x)
                 lr = _RatioFn.apply(est.net.flat, th, x, est, None, None, False)
             elif x.shape[0] == 1:   # one observation: x is shared by every pair, never repeated
                 lr = _RatioFn.apply(est.net.flat, th, x, est, None, None, True)
-            else:                 # _log_ratios_over_trials (:122-160)
-                n = x.shape[0]
-                lr = est(th.repeat(n, 1), x.repeat_interleave(th.shape[0], dim=0)).reshape(n, -1).sum(0)
+            else:                 # _log_ratios_over_trials (:122-160): pair k = (theta[k % R], x[k // R])
+                n, R = x.shape[0], th.shape[0]
+                ti = torch.arange(R, device=th.device).repeat(n)
+                xi = torch.arange(n, device=th.device).repeat_interleave(R)
+                lr = _RatioFn.apply(est.net.flat, th, x, est, ti, xi, False, True).reshape(n, -1).sum(0)
             return lr + self.prior.log_prob(theta)
 
 

@@ -26,7 +26,11 @@ from .pack import MlpRatioLayout, RatioLayout
 
 
 class RatioEstimator(_PackedEstimator):
-    r"""log r(theta, x) = classifier logit; trained by NRE (ratio_estimators.py:11-157)."""
+    r"""log r(theta, x) = classifier logit; trained by NRE (ratio_estimators.py:11-157).
+
+    Each side (theta, x) has its own embedding net.  An identity side hands its raw rows to the kernels, which
+    z-score them in-kernel; an embedded side runs `Standardize` + the user's module in torch and the kernels read
+    the embedded rows with identity statistics (`resnet` classifier only)."""
 
     def __init__(self, layout: Union[RatioLayout, MlpRatioLayout], theta_shape, x_shape, theta_stats, x_stats,
                  embedding_net_theta: nn.Module = None, embedding_net_x: nn.Module = None):
@@ -36,8 +40,11 @@ class RatioEstimator(_PackedEstimator):
         self.theta_shape, self.x_shape = self._input_shape, self._condition_shape
         et = embedding_net_theta if embedding_net_theta is not None else nn.Identity()
         ex = embedding_net_x if embedding_net_x is not None else nn.Identity()
-        if not isinstance(et, nn.Identity) or not isinstance(ex, nn.Identity):
-            raise NotImplementedError("the sm_90a ratio kernels take nn.Identity() embedding nets")
+        self._embed_theta_identity = isinstance(et, nn.Identity)
+        self._embed_x_identity = isinstance(ex, nn.Identity)
+        if not (self._embed_theta_identity and self._embed_x_identity) and not isinstance(layout, RatioLayout):
+            raise NotImplementedError("the sm_90a mlp / linear classifier kernels take nn.Identity() embedding nets "
+                                      "(embedding nets are implemented for the resnet classifier)")
         self.embedding_net_theta = nn.Sequential(Standardize(*theta_stats), et) if theta_stats else et
         self.embedding_net_x = nn.Sequential(Standardize(*x_stats), ex) if x_stats else ex
         # sits where the reference keeps its ResidualNet / nn.Sequential
@@ -45,13 +52,36 @@ class RatioEstimator(_PackedEstimator):
         self.net.hidden_features = layout.H
         self._cache = {}
 
+    @property
+    def embedding_nets(self) -> list:
+        """The embedding nets that run in torch ahead of the kernels (the non-identity sides)."""
+        return [e for e, ident in ((self.embedding_net_theta, self._embed_theta_identity),
+                                   (self.embedding_net_x, self._embed_x_identity)) if not ident]
+
     # ---- kernel views: [theta mean (Dtp) | theta std (Dtp) | x mean (Dxp) | x std (Dxp)]
     def _stat_widths(self):
         lay = self.layout
         return lay.Dtp, lay.Dt, lay.Dxp, lay.Dx, 0
 
     def _stat_sources(self, raw_condition: bool):
-        return _zscore_of(self.embedding_net_theta), _zscore_of(self.embedding_net_x), None
+        th = _zscore_of(self.embedding_net_theta) if self._embed_theta_identity else None
+        xx = _zscore_of(self.embedding_net_x) if self._embed_x_identity else None
+        return th, xx, None
+
+    def embed_theta(self, theta: Tensor) -> Tensor:
+        """(N, *theta_shape) -> the (N, Dt) rows the kernels read: raw (z-scored in-kernel) for an identity
+        embedding, else Standardize + the embedding net in torch."""
+        n = theta.shape[0]
+        if self._embed_theta_identity:
+            return theta.reshape(n, -1).contiguous().float()
+        return self.embedding_net_theta(theta).reshape(n, -1).contiguous().float()
+
+    def embed_x(self, x: Tensor) -> Tensor:
+        """(N, *x_shape) -> the (N, Dx) rows the kernels read (see `embed_theta`)."""
+        n = x.shape[0]
+        if self._embed_x_identity:
+            return x.reshape(n, -1).contiguous().float()
+        return self.embedding_net_x(x).reshape(n, -1).contiguous().float()
 
     # ---- shape checks: ratio_estimators.py:53-112
     def _check(self, theta: Tensor, x: Tensor):
@@ -69,8 +99,8 @@ class RatioEstimator(_PackedEstimator):
 
     def unnormalized_log_ratio(self, theta: Tensor, x: Tensor) -> Tensor:
         prefix = self._check(theta, x)
-        th = theta.reshape(-1, self.layout.Dt).contiguous().float()
-        xx = x.reshape(-1, self.layout.Dx).contiguous().float()
+        th = self.embed_theta(theta.reshape(-1, *self.theta_shape))
+        xx = self.embed_x(x.reshape(-1, *self.x_shape))
         return _RatioFn.apply(self.net.flat, th, xx, self, None, None, False).reshape(*prefix)
 
     def forward(self, *args, **kwargs) -> Tensor:
@@ -105,11 +135,16 @@ class RatioEstimator(_PackedEstimator):
 
 
 class _RatioFn(torch.autograd.Function):
+    """Logits of the pairs (theta[ti[r]], x[xi[r]]) (x[0] with `x_shared`) and their VJP.  The backward returns
+    the gradients of the flat parameters and of the `theta` and `x` rows, each when asked for: per-pair input
+    gradients from the VJP kernel, summed onto the gathered rows by `pair_rows_sum`.  `xi_sorted`: xi is
+    non-decreasing (the rows' pairs are consecutive), so the x side needs no sort."""
+
     @staticmethod
-    def forward(ctx, flat, theta, x, est: RatioEstimator, ti, xi, x_shared):
+    def forward(ctx, flat, theta, x, est: RatioEstimator, ti, xi, x_shared, xi_sorted=False):
         out = est.logits_raw(theta, x, ti, xi, x_shared)
         ctx.save_for_backward(theta, x)
-        ctx.est, ctx.ti, ctx.xi, ctx.x_shared = est, ti, xi, x_shared
+        ctx.est, ctx.ti, ctx.xi, ctx.x_shared, ctx.xi_sorted = est, ti, xi, x_shared, xi_sorted
         return out
 
     @staticmethod
@@ -119,18 +154,53 @@ class _RatioFn(torch.autograd.Function):
         R = g.shape[0]
         n_part = est._entry("vjp_parts")(R)
         gpart = est._gpart(n_part)
-        need_flat, need_th = ctx.needs_input_grad[0], ctx.needs_input_grad[1]
+        need_flat, need_th, need_x = ctx.needs_input_grad[0], ctx.needs_input_grad[1], ctx.needs_input_grad[2]
+        resnet = est.layout.family == "ratio"
+        need_x = need_x and resnet
         gth = torch.empty(R, est.layout.Dt, dtype=torch.float32, device=theta.device) if need_th else None
+        gx = torch.empty(R, est.layout.Dx, dtype=torch.float32, device=theta.device) if need_x else None
         m = est._model(nbuf=3)
         pr = L.Pairs(theta.data_ptr(), x.data_ptr(), None if ctx.ti is None else ctx.ti.data_ptr(),
                      None if ctx.xi is None else ctx.xi.data_ptr(), R, 1 if ctx.x_shared else 0)
         g = g.contiguous().float()
-        est._check_rc(est._entry("vjp")(C.byref(m), C.byref(pr), L.ptr(g), None, L.ptr(gpart), L.ptr(gth),
-                                     L.stream_ptr()), f"{est.layout.family}_vjp")
+        if resnet:
+            est._check_rc(L.load().sbi_b200_ratio_vjp_inputs(C.byref(m), C.byref(pr), L.ptr(g), None, L.ptr(gpart),
+                                                            L.ptr(gth), L.ptr(gx), L.stream_ptr()), "ratio_vjp")
+        else:
+            if need_th and ctx.ti is not None:
+                raise NotImplementedError("theta gradients with an index gather are not needed by any caller")
+            est._check_rc(est._entry("vjp")(C.byref(m), C.byref(pr), L.ptr(g), None, L.ptr(gpart), L.ptr(gth),
+                                            L.stream_ptr()), f"{est.layout.family}_vjp")
         gflat = L.reduce_partials(gpart, n_part, est.layout.n_params) if need_flat else None
         if need_th and ctx.ti is not None:
-            raise NotImplementedError("theta gradients with an index gather are not needed by any caller")
-        return gflat, gth, None, None, None, None, None
+            gth = pair_rows_sum(gth, ctx.ti, theta.shape[0])
+        if need_x:
+            if ctx.x_shared:
+                gx = pair_rows_sum(gx, None, 1, torch.arange(2, dtype=torch.int64, device=gx.device) * R)
+            elif ctx.xi is not None:
+                gx = pair_rows_sum(gx, ctx.xi, x.shape[0], sorted_index=ctx.xi_sorted)
+        return gflat, gth, gx, None, None, None, None, None
+
+
+def pair_rows_sum(gpair: Tensor, index: Optional[Tensor], n_rows: int, row_ptr: Optional[Tensor] = None,
+                  sorted_index: bool = False) -> Tensor:
+    """(n_rows, W) gradients of gathered rows from the (R, W) gradients of their pairs: row j receives the sum of
+    gpair[r] over the pairs r with index[r] == j (csrc/ratio.cu `pair_rows_sum_kernel`: one owner per entry, no
+    atomics).  The CSR of the index is built on the device (stable sort + searchsorted, graph-capturable); a
+    non-decreasing index (`sorted_index`) needs no sort.  `row_ptr` given: consecutive segments."""
+    dev = gpair.device
+    order = None
+    if row_ptr is None:
+        keys = index
+        if not sorted_index:
+            keys, order = torch.sort(index, stable=True)
+            order = order.contiguous()
+        row_ptr = torch.searchsorted(keys, torch.arange(n_rows + 1, dtype=keys.dtype, device=dev))
+    out = torch.empty(n_rows, gpair.shape[1], dtype=torch.float32, device=dev)
+    L.check(L.load().sbi_b200_pair_rows_sum(L.ptr(gpair.contiguous()), gpair.shape[1], L.ptr(order),
+                                            L.ptr(row_ptr.contiguous()), n_rows, L.ptr(out), L.stream_ptr()),
+            "pair_rows_sum")
+    return out
 
 
 def build_resnet_classifier(
@@ -141,13 +211,17 @@ def build_resnet_classifier(
 ) -> RatioEstimator:
     """classifier.py:172-235 (in the classifier's view x = theta, y = x).  Parameters are drawn in
     nflows' construction order (initial layer, per block two linears with the second re-drawn
-    U(-1e-3, 1e-3), final layer), so a seed reproduces the reference's initial weights."""
+    U(-1e-3, 1e-3), final layer), so a seed reproduces the reference's initial weights.  With embedding
+    nets the network is built on the embedded widths, each probed with one batch row like the reference."""
     check_data_device(batch_x, batch_y)
     if z_score_x == "transform_to_unconstrained":
         raise ValueError("Ratio-based classifiers (NRE) do not implement `transform_to_unconstrained`.")
     if dropout_probability != 0.0 or use_batch_norm:
         raise NotImplementedError("dropout / batch norm are not implemented in the sm_90a ratio kernels")
-    Dt, Dx, H = batch_x[0].numel(), batch_y[0].numel(), hidden_features
+    # get_numel (nn_utils.py:17-47): the widths the classifier sees are those of the embedded rows
+    Dt = embedding_net_x.to(batch_x.device)(batch_x[:1]).numel()
+    Dx = embedding_net_y.to(batch_y.device)(batch_y[:1]).numel()
+    H = hidden_features
     lay = RatioLayout(Dt=Dt, Dx=Dx, H=H, NB=num_blocks)
     state = {}
     state["net.initial_layer.weight"], state["net.initial_layer.bias"] = _linear_init(H, Dt + Dx)
