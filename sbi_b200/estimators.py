@@ -126,7 +126,7 @@ class PackedNet(nn.Module):
             incoming = {k: state_dict.pop(prefix + k[len("net."):]) for k in list(lay.buffers)
                         if prefix + k[len("net."):] in state_dict}
             # structural buffers that are data (MAF permutations): adopt them
-            if incoming and hasattr(lay, "load_buffers") and lay.load_buffers(incoming) is not None:
+            if incoming and lay.load_buffers(incoming) is not None:
                 for buf, t in zip(self.tables(), lay.tables()):
                     buf.copy_(torch.from_numpy(t))
 
@@ -480,7 +480,7 @@ class FlowEstimator(_PackedEstimator):
         flat = self.net.flat
         st = self._cache.get("tc_train")
         if st is None or st["dev"] != flat.device:
-            pf, pb = self.layout.tc_plan(), (self.layout.tc_bwd_plan() if hasattr(self.layout, "tc_bwd_plan") else None)
+            pf, pb = self.layout.tc_plan(), self.layout.tc_bwd_plan()
             st = {"dev": flat.device, "ok": pf is not None and pb is not None}
             if st["ok"]:
                 import numpy as np

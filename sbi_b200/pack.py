@@ -6,13 +6,13 @@ cp.async.bulk and float4 shared-memory reads) and the output dimension padded to
 of 4 with zero rows.  `NsfLayout` computes offsets, the per-layer descriptor table the
 kernels index (include/sbi_b200.h, SBI_L_*), and, for every tensor of the reference
 module (`net._transform._transforms.{i}...`, names as produced by the reference builder
-/root/reference/sbi/neural_nets/net_builders/flow.py:333-460 on nflows 0.14), an index map
+sbi/neural_nets/net_builders/flow.py:333-460 on nflows 0.14), an index map
 into the flat buffer, so a reference state_dict can be loaded / exported verbatim.
 """
 from __future__ import annotations
 
 import math
-from dataclasses import dataclass, field
+from dataclasses import dataclass
 from typing import Dict, List, Optional
 
 import numpy as np
@@ -25,20 +25,129 @@ def round4(x: int) -> int:
     return (x + 3) & ~3
 
 
-class _LayoutOps:
-    """pack / unpack between reference-named tensors and the flat kernel buffer.  `weight_masks`
-    holds, for masked (MADE) weights, the 0/1 mask: the flat buffer stores W*M, the masked-out raw
-    values are kept aside (`raw`) only so that state_dict() round-trips exactly."""
+def round32(x: int) -> int:
+    return (x + 31) & ~31
 
-    def _wm(self):
-        return getattr(self, "_weight_masks", None) or {}
+
+class _Alloc:
+    """The running offset into the flat buffer and the index map of the reference tensors placed so far."""
+
+    def __init__(self):
+        self.off = 0
+        self.index: Dict[str, np.ndarray] = {}
+
+    def take(self, n: int) -> int:
+        """Reserve n floats, rounded up to a multiple of 4; returns their offset."""
+        o = self.off
+        self.off += round4(n)
+        return o
+
+    def linear(self, name: str, tab: np.ndarray, slots, N: int, K: int, Kp: int, cols=None, rows=None):
+        """Reserve the torch Linear `name` (N outputs, K inputs): its weight in rows of Kp floats, then its bias, with
+        their offsets stored at tab[slots[0]] and tab[slots[1]].  Input k sits in column cols[k] (default k) and
+        output n in row rows[n] (default n); both blocks hold the rows up to the last used one, rounded up to 4."""
+        cols = np.arange(K) if cols is None else cols
+        rows = np.arange(N) if rows is None else rows
+        n_rows = round4(int(rows[-1]) + 1)
+        o = tab[slots[0]] = self.take(n_rows * Kp)
+        self.index[name + ".weight"] = o + rows[:, None] * Kp + cols[None, :]
+        o = tab[slots[1]] = self.take(n_rows)
+        self.index[name + ".bias"] = o + rows
+
+
+def _plan_ring(cap: int, mats, extra=()):
+    """Weight-ring chunking.  For each matrix (row length, row count): the rows per chunk, as many whole rows as fit
+    in `cap` floats, a multiple of 4, at least 4 and at most the row count.  Returns those and the ring slot size
+    wcap: the largest chunk or `extra` term in floats, rounded up to 32."""
+    rpc = [max(4, min(nmax, (cap // rowlen) & ~3)) for rowlen, nmax in mats]
+    used = max([r * rowlen for r, (rowlen, _) in zip(rpc, mats)] + list(extra))
+    return rpc, round32(used)
+
+
+def _made_masks(D: int, H: int, out_mult: int):
+    """nflows MADE with sequential degrees (transforms/made.py) on D inputs, H hidden units and out_mult outputs per
+    input: the input, hidden and output degrees and the (H, D) initial, (H, H) hidden and (out_mult*D, H) final
+    masks."""
+    in_deg = np.arange(1, D + 1)
+    max_, min_ = max(1, D - 1), min(1, D - 1)
+    hid_deg = np.arange(H) % max_ + min_
+    out_deg = np.repeat(in_deg, out_mult)
+    m_init = (hid_deg[:, None] >= in_deg[None, :]).astype(np.float32)
+    m_hid = (hid_deg[:, None] >= hid_deg[None, :]).astype(np.float32)
+    m_out = (out_deg[:, None] > hid_deg[None, :]).astype(np.float32)
+    return in_deg, hid_deg, out_deg, m_init, m_hid, m_out
+
+
+def _add_mask(lay, name: str, mask: np.ndarray, degrees: np.ndarray):
+    """MADE's masked linear `name`: the packed weight holds W * mask; the module's `mask` / `degrees` buffers."""
+    lay._weight_masks[name + ".weight"] = mask
+    lay.buffers[name + ".mask"] = torch.as_tensor(mask)
+    lay.buffers[name + ".degrees"] = torch.as_tensor(degrees)
+
+
+def _residual_blocks(a: _Alloc, lay, prefix: str, tab: np.ndarray, hidden_mask=None):
+    """The `{prefix}blocks.{b}` of an nflows ResidualNet with a context layer: linear_layers.0, linear_layers.1 and
+    context_layer at table fields L_BLK0 + 6b .. L_BLK0 + 6b + 5.  hidden_mask: (mask, degrees) of MADE's masked
+    linear_layers."""
+    for b in range(lay.NB):
+        pb = prefix + f"blocks.{b}."
+        t = L.L_BLK0 + 6 * b
+        for j in range(2):
+            a.linear(pb + f"linear_layers.{j}", tab, (t + 2 * j, t + 2 * j + 1), lay.H, lay.H, lay.Hp)
+            if hidden_mask is not None:
+                _add_mask(lay, pb + f"linear_layers.{j}", *hidden_mask)
+        a.linear(pb + "context_layer", tab, (t + 4, t + 5), lay.H, lay.C, lay.Cp)
+
+
+def _tc_block(N: int, K: int, fill):
+    """One K-major no-swizzle wgmma operand block [K/4 slabs][N rows][4 floats], flattened.
+    fill(n, k) -> the parameter index of element (n, k), or -1 for a zero."""
+    blk = np.full((K // 4, N, 4), -1, np.int64)
+    n = np.arange(N)[:, None] + 0 * np.arange(K)[None, :]
+    k = np.arange(K)[None, :] + 0 * np.arange(N)[:, None]
+    blk[k // 4, n, k % 4] = fill(n, k)
+    return blk.reshape(-1)
+
+
+def _tc_assemble(rows):
+    """Gather map and stage table of a wgmma operand plan (include/sbi_b200.h `sbi_nsf_tc`).  rows: per table row
+    (layer) its second header word and its stages (hi, N, aux), hi the gather map of the stage's hi half; word 0 is
+    the stage count.  A stage is its hi half, then its lo half (-2 - index where hi holds a parameter).
+    Returns dict(src=int32 (n_words,), tab=int32 (rows * STRIDE,), stage_cap=int, n_words=int)."""
+    tab = np.zeros((len(rows), L.SBI_NSF_TC_STRIDE), np.int32)
+    chunks, off, stage_cap = [], 0, 0
+    for r, (word1, stages) in enumerate(rows):
+        tab[r, 0], tab[r, 1] = len(stages), word1
+        for s, (hi, N, aux) in enumerate(stages):
+            nfl = 2 * hi.size
+            tab[r, 4 + 4 * s: 8 + 4 * s] = (off, nfl, N, aux)
+            chunks += [hi, np.where(hi >= 0, -2 - hi, -1)]
+            off += nfl
+            stage_cap = max(stage_cap, nfl)
+    return dict(src=np.concatenate(chunks).astype(np.int32), tab=tab.reshape(-1),
+                stage_cap=round32(stage_cap), n_words=off)
+
+
+class _LayoutOps:
+    """Base of the packed layouts: pack / unpack between reference-named tensors and the flat kernel buffer.
+    `_weight_masks` holds, for masked (MADE) weights, the 0/1 mask: the flat buffer stores W*M, the masked-out raw
+    values are kept aside (`raw`) only so that state_dict() round-trips exactly.  Subclasses set `n_params`, `index`
+    and `buffers`."""
+
+    family: str                  # the estimator family the layout belongs to
+    _tables = ("tab",)           # the attributes `tables()` returns
+    _weight_masks: Dict[str, np.ndarray] = {}      # shared empty default: masked layouts assign their own
+
+    def _wm(self) -> Dict[str, np.ndarray]:
+        """The weight masks, {reference weight name: 0/1 mask}; empty unless the layout has masked weights."""
+        return self._weight_masks
 
     def trainable_mask(self) -> torch.Tensor:
         m = torch.zeros(self.n_params, dtype=torch.uint8)
         for k, v in self.index.items():
             ix = torch.as_tensor(v.reshape(-1))
-            if k in self._wm():
-                m[ix] = torch.as_tensor(self._wm()[k].reshape(-1)).to(torch.uint8)
+            if k in self._weight_masks:
+                m[ix] = torch.as_tensor(self._weight_masks[k].reshape(-1)).to(torch.uint8)
             else:
                 m[ix] = 1
         return m
@@ -50,8 +159,8 @@ class _LayoutOps:
         for k, ix in self.index.items():
             src = state[k].detach().to(dtype=torch.float32, device=flat.device).reshape(-1)
             pos = torch.as_tensor(ix.reshape(-1), device=flat.device)
-            if k in self._wm():
-                mk = torch.as_tensor(self._wm()[k].reshape(-1), dtype=torch.float32, device=flat.device)
+            if k in self._weight_masks:
+                mk = torch.as_tensor(self._weight_masks[k].reshape(-1), dtype=torch.float32, device=flat.device)
                 if raw_out is not None:
                     raw_out[pos] = src * (1 - mk)
                 src = src * mk
@@ -63,7 +172,7 @@ class _LayoutOps:
         for k, ix in self.index.items():
             pos = torch.as_tensor(ix.reshape(-1), device=flat.device)
             t = flat.detach()[pos]
-            if raw is not None and k in self._wm():
+            if raw is not None and k in self._weight_masks:
                 t = t + raw[pos]
             out[k] = t.reshape(ix.shape).clone()
         return out
@@ -72,13 +181,50 @@ class _LayoutOps:
         return int(sum(v.size for v in self.index.values()))
 
     def tables(self):
-        """The int32 index tables the model struct points to, in the order of its table fields (one `tab` here;
-        the flow layouts return their layer table and their feature / permutation table)."""
-        return (self.tab,)
+        """The int32 index tables the model struct points to, in the order of its table fields."""
+        return tuple(getattr(self, name).reshape(-1).astype(np.int32) for name in self._tables)
+
+    def tc_plan(self):
+        """The operand plan of the family's wgmma evaluation kernel, or None if there is none for this model."""
+        return None
+
+    def tc_bwd_plan(self):
+        """The operand plan of the transposed linears for the wgmma training kernel, or None."""
+        return None
+
+    def load_buffers(self, incoming: Dict[str, torch.Tensor]):
+        """Adopt structural buffers of a loaded state_dict that are data rather than architecture.  Returns None when
+        the index tables did not change."""
+        return None
+
+
+class _NsfKernelLayout(_LayoutOps):
+    """The layouts that run on the NSF kernels (include/sbi_b200.h `sbi_nsf_model`): the weight ring and the
+    common struct fields.  Subclasses set the head fields of the struct."""
+
+    _tables = ("layer_tab", "feat_tab")
+
+    def _plan_nsf_ring(self):
+        """Ring chunks of the initial ([., K0p]), hidden ([., Hp]) and context-gated ([., Hp + Cp]) matrices, and of
+        the final layer: nf_chunk features of PR x Hp floats each."""
+        Hp, Cp, K0p, PR = self.Hp, self.Cp, self.K0p, self.PR
+        cap = max(self.wcap_target, 4 * K0p, 4 * (Hp + Cp), PR * Hp)
+        self.nf_chunk = max(1, min(self.TRmax, cap // (PR * Hp)))
+        (self.rpc0, self.rpc1, self.rpc2), self.wcap = _plan_ring(
+            cap, [(K0p, Hp), (Hp, Hp), (Hp + Cp, Hp)], [self.nf_chunk * PR * Hp])
+
+    def fill_struct(self, s: "L.NsfModel", nbuf: int):
+        s.D, s.C, s.H, s.NB, s.KB, s.T = self.D, self.C, self.H, self.NB, self.KB, self.T
+        s.Dp, s.Cp, s.IDp, s.Hp, s.PR = self.Dp, self.Cp, self.IDp, self.Hp, self.PR
+        s.TRmax, s.nf_chunk = self.TRmax, self.nf_chunk
+        s.rpc0, s.rpc1, s.rpc2 = self.rpc0, self.rpc1, self.rpc2
+        s.wcap, s.nbuf, s.n_params = self.wcap, nbuf, self.n_params
+        s.min_bw = s.min_bh = s.min_d = 1e-3
+        return s
 
 
 @dataclass
-class NsfLayout(_LayoutOps):
+class NsfLayout(_NsfKernelLayout):
     D: int
     C: int
     H: int = 50
@@ -91,9 +237,7 @@ class NsfLayout(_LayoutOps):
     embed_is_identity: bool = True
     wcap_target: int = int(__import__('os').environ.get('SBI_B200_WCAP', 4096))
 
-    # derived
-    n_params: int = 0
-    index: Dict[str, np.ndarray] = field(default_factory=dict, repr=False)
+    family = "nsf"
 
     def __post_init__(self):
         D, C, H, NB, KB, T = self.D, self.C, self.H, self.NB, self.KB, self.T
@@ -115,101 +259,48 @@ class NsfLayout(_LayoutOps):
         self.IDp = round4(max(len(f) for f in self.id_feats))
         self.TRmax = max(len(f) for f in self.tr_feats)
         self.K0p = self.Cp + self.IDp
+        self._plan_nsf_ring()
 
-        # weight-ring chunking
-        Hp, Cp = self.Hp, self.Cp
-        cap = max(self.wcap_target, 4 * self.K0p, 4 * (Hp + Cp), self.PR * Hp)
-
-        def rows(rowlen):
-            return max(4, min(Hp, (cap // rowlen) & ~3))
-
-        self.rpc0, self.rpc1, self.rpc2 = rows(self.K0p), rows(Hp), rows(Hp + Cp)
-        self.nf_chunk = max(1, min(self.TRmax, cap // (self.PR * Hp)))
-        used = max(self.rpc0 * self.K0p, self.rpc1 * Hp, self.rpc2 * (Hp + Cp),
-                   self.nf_chunk * self.PR * Hp)
-        self.wcap = (used + 31) & ~31
-
-        # ---- offsets -------------------------------------------------------------------
-        off = 0
-
-        def take(n):
-            nonlocal off
-            o = off
-            off += round4(n)
-            return o
-
+        a = _Alloc()
         tab = np.zeros((T, L.SBI_NSF_LAYER_STRIDE), np.int32)
         feat = []
         ntri = D * (D - 1) // 2
-        tri_lo = np.tril_indices(D, -1)
-        tri_up = np.triu_indices(D, 1)
         base = 1 if self.zscore_input else 0
-        idx: Dict[str, np.ndarray] = {}
         self.buffers: Dict[str, torch.Tensor] = {}
         for l in range(T):
             idf, trf = self.id_feats[l], self.tr_feats[l]
             n_id, n_tr = len(idf), len(trf)
-            ci, li = base + 2 * l, base + 2 * l + 1
-            pc = f"net._transform._transforms.{ci}."
-            pl = f"net._transform._transforms.{li}."
-            tab[l, L.L_NID], tab[l, L.L_NTR] = n_id, n_tr
-            tab[l, L.L_FEAT] = len(feat)
+            pc = f"net._transform._transforms.{base + 2 * l}."
+            pl = f"net._transform._transforms.{base + 2 * l + 1}."
+            t = tab[l]
+            t[L.L_NID], t[L.L_NTR], t[L.L_FEAT] = n_id, n_tr, len(feat)
             feat += list(idf) + list(trf)
             self.buffers[pc + "identity_features"] = torch.as_tensor(idf)
             self.buffers[pc + "transform_features"] = torch.as_tensor(trf)
             # initial layer: nflows columns [id | ctx] -> packed columns [ctx | pad | id | pad]
-            o = take(Hp * self.K0p)
-            tab[l, L.L_W0] = o
-            cols = np.concatenate([Cp + np.arange(n_id), np.arange(C)])
-            idx[pc + "transform_net.initial_layer.weight"] = (
-                o + np.arange(H)[:, None] * self.K0p + cols[None, :])
-            o = take(Hp)
-            tab[l, L.L_B0] = o
-            idx[pc + "transform_net.initial_layer.bias"] = o + np.arange(H)
-            for b in range(NB):
-                pb = pc + f"transform_net.blocks.{b}."
-                t = L.L_BLK0 + 6 * b
-                for slot, (name, K, Kp) in enumerate(
-                        [("linear_layers.0", H, Hp), ("linear_layers.1", H, Hp),
-                         ("context_layer", C, Cp)]):
-                    o = take(Hp * Kp)
-                    tab[l, t + 2 * slot] = o
-                    idx[pb + name + ".weight"] = o + np.arange(H)[:, None] * Kp + np.arange(K)[None, :]
-                    o = take(Hp)
-                    tab[l, t + 2 * slot + 1] = o
-                    idx[pb + name + ".bias"] = o + np.arange(H)
+            a.linear(pc + "transform_net.initial_layer", t, (L.L_W0, L.L_B0), H, n_id + C, self.K0p,
+                     cols=np.concatenate([self.Cp + np.arange(n_id), np.arange(C)]))
+            _residual_blocks(a, self, pc + "transform_net.", t)
             # final layer: feature f owns packed rows f*PR .. f*PR+NPAR-1
-            o = take(n_tr * self.PR * Hp)
-            tab[l, L.L_WF] = o
             prow = (np.arange(n_tr)[:, None] * self.PR + np.arange(self.NPAR)[None, :]).reshape(-1)
-            idx[pc + "transform_net.final_layer.weight"] = o + prow[:, None] * Hp + np.arange(H)[None, :]
-            o = take(n_tr * self.PR)
-            tab[l, L.L_BF] = o
-            idx[pc + "transform_net.final_layer.bias"] = o + prow
+            a.linear(pc + "transform_net.final_layer", t, (L.L_WF, L.L_BF), n_tr * self.NPAR, H, self.Hp, rows=prow)
             # LULinear
-            tab[l, L.L_HAS_LU] = 1
-            o = take(ntri)
-            tab[l, L.L_LU_LOWER] = o
-            idx[pl + "lower_entries"] = o + np.arange(ntri)
-            o = take(ntri)
-            tab[l, L.L_LU_UPPER] = o
-            idx[pl + "upper_entries"] = o + np.arange(ntri)
-            o = take(D)
-            tab[l, L.L_LU_DIAG] = o
-            idx[pl + "unconstrained_upper_diag"] = o + np.arange(D)
-            o = take(D)
-            tab[l, L.L_LU_BIAS] = o
-            idx[pl + "bias"] = o + np.arange(D)
-        del tri_lo, tri_up
-        self.n_params = off
-        self.index = idx
+            t[L.L_HAS_LU] = 1
+            for slot, name, n in ((L.L_LU_LOWER, "lower_entries", ntri), (L.L_LU_UPPER, "upper_entries", ntri),
+                                  (L.L_LU_DIAG, "unconstrained_upper_diag", D), (L.L_LU_BIAS, "bias", D)):
+                o = t[slot] = a.take(n)
+                a.index[pl + name] = o + np.arange(n)
+        self.n_params = a.off
+        self.index = a.index
         self.layer_tab = tab
         self.feat_tab = np.asarray(feat, np.int32)
         self.edge_raw = float(np.log(np.exp(1 - 1e-3) - 1))
 
-    # ------------------------------------------------------------------------------ helpers
-    def tables(self):
-        return self.layer_tab.reshape(-1).astype(np.int32), self.feat_tab.astype(np.int32)
+    def fill_struct(self, s: "L.NsfModel", nbuf: int):
+        super().fill_struct(s, nbuf)
+        s.tail_bound, s.inv_sqrt_h, s.edge_raw = self.tail_bound, 1.0 / math.sqrt(self.H), self.edge_raw
+        s.head, s.M, s.mog_eps, s.cond_mlp = 0, 0, 0.0, 0
+        return s
 
     # ------------------------------------------------------------- tensor-core operand plan
     def tc_plan(self):
@@ -230,26 +321,13 @@ class NsfLayout(_LayoutOps):
         HP8 = (H + 7) & ~7
         KC0 = H // 8
         nkc = (H + C + 7) // 8 - KC0
-        tab = np.zeros((T, L.SBI_NSF_TC_STRIDE), np.int32)
-        chunks = []          # per stage: int64 array of the hi half (param index or -1)
-        off = 0
-        stage_cap = 0
-
-        def block(N, K, fill):
-            """fill(n, k) -> param index or -1 ; returns the flattened [K/4][N][4] block"""
-            blk = np.full((K // 4, N, 4), -1, np.int64)
-            n = np.arange(N)[:, None]
-            k = np.arange(K)[None, :]
-            vals = fill(n + 0 * k, k + 0 * n)
-            blk[(k // 4) + 0 * n, n + 0 * k, (k % 4) + 0 * n] = vals
-            return blk.reshape(-1)
 
         def ctx_block(woff, rowlen):
             def fill(n, k):
                 c = 8 * KC0 + k - H
                 ok = (n < H) & (c >= 0) & (c < C)
                 return np.where(ok, woff + n * rowlen + np.clip(c, 0, max(C - 1, 0)), -1)
-            return block(64, 8 * nkc, fill)
+            return _tc_block(64, 8 * nkc, fill)
 
         def hidden_block(woff, N, rowmap):
             """rowmap(n) -> (valid, packed row index) of the [.,Hp] weight matrix"""
@@ -257,20 +335,20 @@ class NsfLayout(_LayoutOps):
                 valid, row = rowmap(n)
                 ok = valid & (k < H)
                 return np.where(ok, woff + row * Hp + np.minimum(k, H - 1), -1)
-            return block(N, HP8, fill)
+            return _tc_block(N, HP8, fill)
 
+        rows = []
         for l in range(T):
             lt = self.layer_tab[l]
             n_id, n_tr = int(lt[L.L_NID]), int(lt[L.L_NTR])
             kid8 = (n_id + 7) & ~7
-            stages = []      # (hi half, N, aux)
             w0 = int(lt[L.L_W0])
 
             def fill_id(n, k, w0=w0, n_id=n_id):
                 ok = (n < H) & (k < n_id)
                 return np.where(ok, w0 + n * K0p + Cp + np.minimum(k, max(n_id - 1, 0)), -1)
 
-            stages.append((np.concatenate([block(64, kid8, fill_id), ctx_block(w0, K0p)]), 64, 0))
+            stages = [(np.concatenate([_tc_block(64, kid8, fill_id), ctx_block(w0, K0p)]), 64, 0)]
             ident = lambda n: (n < H, np.minimum(n, H - 1))
             for b in range(NB):
                 t = L.L_BLK0 + 6 * b
@@ -292,18 +370,8 @@ class NsfLayout(_LayoutOps):
                 f0 += nf
             if len(stages) > L.SBI_NSF_TC_MAX_STAGES:
                 return None
-            tab[l, 0], tab[l, 1] = len(stages), kid8
-            for s, (hi, N, aux) in enumerate(stages):
-                nfl = 2 * hi.size
-                tab[l, 4 + 4 * s: 8 + 4 * s] = (off, nfl, N, aux)
-                chunks.append(hi)
-                chunks.append(np.where(hi >= 0, -2 - hi, -1))
-                off += nfl
-                stage_cap = max(stage_cap, nfl)
-        src = np.concatenate(chunks).astype(np.int32)
-        assert src.size == off
-        return dict(src=src, tab=tab.reshape(-1).astype(np.int32),
-                    stage_cap=int((stage_cap + 31) & ~31), n_words=int(off))
+            rows.append((kid8, stages))
+        return _tc_assemble(rows)
 
     def tc_bwd_plan(self):
         """Gather map + stage table of the TRANSPOSED linears for the wgmma training kernel's
@@ -315,22 +383,12 @@ class NsfLayout(_LayoutOps):
             initial layer, identity-feature columns only:  N = 16, K = 56
         Same return format as tc_plan (the context columns are not needed: training never asks for
         the condition's gradient on this path)."""
-        D, C, H, NB, T = self.D, self.C, self.H, self.NB, self.T
+        H, NB, T = self.H, self.NB, self.T
         if self.tc_plan() is None or self.IDp > 16:
             return None
         Hp, Cp, K0p, PR, NPAR = self.Hp, self.Cp, self.K0p, self.PR, self.NPAR
         HP8 = (H + 7) & ~7
-        tab = np.zeros((T, L.SBI_NSF_TC_STRIDE), np.int32)
-        chunks, off, stage_cap = [], 0, 0
-
-        def block(N, K, fill):
-            blk = np.full((K // 4, N, 4), -1, np.int64)
-            n = np.arange(N)[:, None]
-            k = np.arange(K)[None, :]
-            vals = fill(n + 0 * k, k + 0 * n)
-            blk[(k // 4) + 0 * n, n + 0 * k, (k % 4) + 0 * n] = vals
-            return blk.reshape(-1)
-
+        rows = []
         for l in range(T):
             lt = self.layer_tab[l]
             n_id, n_tr = int(lt[L.L_NID]), int(lt[L.L_NTR])
@@ -346,7 +404,7 @@ class NsfLayout(_LayoutOps):
                     return np.where(ok, wf + ((f0 + np.minimum(f, nf - 1)) * PR + np.minimum(i, NPAR - 1)) * Hp
                                     + np.minimum(n, H - 1), -1)
 
-                stages.append((block(64, 32 * nf, fill_f), 64, 4 * nf))
+                stages.append((_tc_block(64, 32 * nf, fill_f), 64, 4 * nf))
                 f0 += nf
             for b in range(NB - 1, -1, -1):
                 t = L.L_BLK0 + 6 * b
@@ -356,45 +414,20 @@ class NsfLayout(_LayoutOps):
                         ok = (n < H) & (k < H)
                         return np.where(ok, w + np.minimum(k, H - 1) * Hp + np.minimum(n, H - 1), -1)
 
-                    stages.append((block(64, HP8, fill_h), 64, HP8 // 8))
+                    stages.append((_tc_block(64, HP8, fill_h), 64, HP8 // 8))
             w0 = int(lt[L.L_W0])
 
             def fill_0(n, k, w0=w0, n_id=n_id):
                 ok = (n < n_id) & (k < H)
                 return np.where(ok, w0 + np.minimum(k, H - 1) * K0p + Cp + np.minimum(n, max(n_id - 1, 0)), -1)
 
-            stages.append((block(16, HP8, fill_0), 16, HP8 // 8))
-            tab[l, 0], tab[l, 1] = len(stages), (n_tr + 1) // 2
-            for s, (hi, N, aux) in enumerate(stages):
-                nfl = 2 * hi.size
-                tab[l, 4 + 4 * s: 8 + 4 * s] = (off, nfl, N, aux)
-                chunks.append(hi)
-                chunks.append(np.where(hi >= 0, -2 - hi, -1))
-                off += nfl
-                stage_cap = max(stage_cap, nfl)
-        src = np.concatenate(chunks).astype(np.int32)
-        return dict(src=src, tab=tab.reshape(-1).astype(np.int32),
-                    stage_cap=int((stage_cap + 31) & ~31), n_words=int(off))
-
-    def fill_struct(self, s: "L.NsfModel", nbuf: int):
-        s.D, s.C, s.H, s.NB, s.KB, s.T = self.D, self.C, self.H, self.NB, self.KB, self.T
-        s.Dp, s.Cp, s.IDp, s.Hp, s.PR = self.Dp, self.Cp, self.IDp, self.Hp, self.PR
-        s.TRmax, s.nf_chunk = self.TRmax, self.nf_chunk
-        s.rpc0, s.rpc1, s.rpc2 = self.rpc0, self.rpc1, self.rpc2
-        s.wcap, s.nbuf, s.n_params = self.wcap, nbuf, self.n_params
-        s.tail_bound = self.tail_bound
-        s.inv_sqrt_h = 1.0 / math.sqrt(self.H)
-        s.min_bw = s.min_bh = s.min_d = 1e-3
-        s.edge_raw = self.edge_raw
-        s.head, s.M, s.mog_eps, s.cond_mlp = 0, 0, 0.0, 0
-        return s
-
-
-NsfLayout.family = "nsf"
+            stages.append((_tc_block(16, HP8, fill_0), 16, HP8 // 8))
+            rows.append(((n_tr + 1) // 2, stages))
+        return _tc_assemble(rows)
 
 
 @dataclass
-class Nsf1dLayout(_LayoutOps):
+class Nsf1dLayout(_NsfKernelLayout):
     """Packed layout of the ONE-dimensional neural spline flow (flow.py:401-432 with x_numel == 1): T spline
     transforms of the single feature whose 3K-1 parameters come from a context-only MLP (`ContextSplineMap`,
     flow.py:1419-1478: Linear -> ReLU -> hidden_layers x [one shared Linear -> ReLU] -> Linear), no LULinear.
@@ -409,9 +442,9 @@ class Nsf1dLayout(_LayoutOps):
     zscore_cond: bool = True
     embed_is_identity: bool = True
     wcap_target: int = 4096
-    n_params: int = 0
-    index: Dict[str, np.ndarray] = field(default_factory=dict, repr=False)
     D: int = 1
+
+    family = "nsf"
 
     def __post_init__(self):
         C, H, NB, KB, T = self.C, self.H, self.NB, self.KB, self.T
@@ -423,86 +456,45 @@ class Nsf1dLayout(_LayoutOps):
         if self.PR > self.Hp:
             raise ValueError("hidden_features must be >= the padded spline parameter count")
         self.IDp, self.TRmax, self.K0p = 0, 1, self.Cp
-        Hp, Cp = self.Hp, self.Cp
-        cap = max(self.wcap_target, 4 * self.K0p, 4 * (Hp + Cp), self.PR * Hp)
-
-        def rows(rowlen):
-            return max(4, min(Hp, (cap // rowlen) & ~3))
-
-        self.rpc0, self.rpc1, self.rpc2 = rows(self.K0p), rows(Hp), rows(Hp + Cp)
-        self.nf_chunk = 1
-        used = max(self.rpc0 * self.K0p, self.rpc1 * Hp, self.rpc2 * (Hp + Cp), self.PR * Hp)
-        self.wcap = (used + 31) & ~31
-        off = 0
-
-        def take(n):
-            nonlocal off
-            o = off
-            off += round4(n)
-            return o
-
+        self._plan_nsf_ring()
+        Hp = self.Hp
+        a = _Alloc()
         tab = np.zeros((T, L.SBI_NSF_LAYER_STRIDE), np.int32)
-        idx: Dict[str, np.ndarray] = {}
         self.buffers: Dict[str, torch.Tensor] = {}
         base = 1 if self.zscore_input else 0
         for l in range(T):
             pc = f"net._transform._transforms.{base + l}."
             pn = pc + "transform_net.spline_predictor."
-            tab[l, L.L_NID], tab[l, L.L_NTR], tab[l, L.L_FEAT] = 0, 1, l
+            t = tab[l]
+            t[L.L_NID], t[L.L_NTR], t[L.L_FEAT] = 0, 1, l
             self.buffers[pc + "identity_features"] = torch.zeros(0, dtype=torch.int64)
             self.buffers[pc + "transform_features"] = torch.zeros(1, dtype=torch.int64)
-            o = take(Hp * Cp)
-            tab[l, L.L_W0] = o
-            idx[pn + "0.weight"] = o + np.arange(H)[:, None] * Cp + np.arange(C)[None, :]
-            o = take(Hp)
-            tab[l, L.L_B0] = o
-            idx[pn + "0.bias"] = o + np.arange(H)
-            ow, ob = take(Hp * Hp), take(Hp)
-            tab[l, L.L_BLK0], tab[l, L.L_BLK0 + 1] = ow, ob
+            a.linear(pn + "0", t, (L.L_W0, L.L_B0), H, C, self.Cp)
+            ow = t[L.L_BLK0] = a.take(Hp * Hp)
+            ob = t[L.L_BLK0 + 1] = a.take(Hp)
             for k in range(NB):      # nn.Sequential lists the shared module once per position
-                idx[pn + f"{2 + 2 * k}.weight"] = ow + np.arange(H)[:, None] * Hp + np.arange(H)[None, :]
-                idx[pn + f"{2 + 2 * k}.bias"] = ob + np.arange(H)
-            o = take(self.PR * Hp)
-            tab[l, L.L_WF] = o
-            idx[pn + f"{2 + 2 * NB}.weight"] = o + np.arange(self.NPAR)[:, None] * Hp + np.arange(H)[None, :]
-            o = take(self.PR)
-            tab[l, L.L_BF] = o
-            idx[pn + f"{2 + 2 * NB}.bias"] = o + np.arange(self.NPAR)
-            tab[l, L.L_HAS_LU] = 0
-        self.n_params = off
-        self.index = idx
+                a.index[pn + f"{2 + 2 * k}.weight"] = ow + np.arange(H)[:, None] * Hp + np.arange(H)[None, :]
+                a.index[pn + f"{2 + 2 * k}.bias"] = ob + np.arange(H)
+            a.linear(pn + f"{2 + 2 * NB}", t, (L.L_WF, L.L_BF), self.NPAR, H, Hp)
+            t[L.L_HAS_LU] = 0
+        self.n_params = a.off
+        self.index = a.index
         self.layer_tab = tab
         self.feat_tab = np.zeros(T, np.int32)            # layer l: no identity features, transformed feature 0
         self.edge_raw = float(np.log(np.exp(1 - 1e-3) - 1))
-
-    def tables(self):
-        return self.layer_tab.reshape(-1).astype(np.int32), self.feat_tab.astype(np.int32)
-
-    def tc_plan(self):
-        return None
 
     def num_real_params(self) -> int:
         return int(len({int(i) for v in self.index.values() for i in v.reshape(-1)}))
 
     def fill_struct(self, s: "L.NsfModel", nbuf: int):
-        s.D, s.C, s.H, s.NB, s.KB, s.T = 1, self.C, self.H, self.NB, self.KB, self.T
-        s.Dp, s.Cp, s.IDp, s.Hp, s.PR = self.Dp, self.Cp, 0, self.Hp, self.PR
-        s.TRmax, s.nf_chunk = 1, 1
-        s.rpc0, s.rpc1, s.rpc2 = self.rpc0, self.rpc1, self.rpc2
-        s.wcap, s.nbuf, s.n_params = self.wcap, nbuf, self.n_params
-        s.tail_bound = self.tail_bound
-        s.inv_sqrt_h = 1.0 / math.sqrt(self.H)
-        s.min_bw = s.min_bh = s.min_d = 1e-3
-        s.edge_raw = self.edge_raw
+        super().fill_struct(s, nbuf)
+        s.tail_bound, s.inv_sqrt_h, s.edge_raw = self.tail_bound, 1.0 / math.sqrt(self.H), self.edge_raw
         s.head, s.M, s.mog_eps, s.cond_mlp = 0, 0, 0.0, 1
         return s
 
 
-Nsf1dLayout.family = "nsf"
-
-
 @dataclass
-class MadeLayout(_LayoutOps):
+class MadeLayout(_NsfKernelLayout):
     """Packed layout of sbi's `made` density estimator (flow.py:37-112): ONE masked residual network
     (nflows MixtureOfGaussiansMADE behind sbi's MADEMoGWrapper, nn_utils.py:133-201: `features + 1`
     inputs with a dummy first feature) emitting, per feature, num_mixture_components x (logit, mean,
@@ -521,8 +513,8 @@ class MadeLayout(_LayoutOps):
     zscore_cond: bool = True
     embed_is_identity: bool = True
     wcap_target: int = 4096
-    n_params: int = 0
-    index: Dict[str, np.ndarray] = field(default_factory=dict, repr=False)
+
+    family = "made"
 
     def __post_init__(self):
         D, C, H, NB, M = self.D, self.C, self.H, self.NB, self.M
@@ -537,114 +529,49 @@ class MadeLayout(_LayoutOps):
         self.IDp = round4(D)
         self.TRmax = D
         self.K0p = self.Cp + self.IDp
-        Hp, Cp = self.Hp, self.Cp
-        cap = max(self.wcap_target, 4 * self.K0p, 4 * (Hp + Cp), self.PR * Hp)
+        self._plan_nsf_ring()
+        Hp, Cp, K0p = self.Hp, self.Cp, self.K0p
+        _, hid_deg, out_deg, m_init, m_hid, m_out = _made_masks(D, H, 3 * M)
 
-        def rows(rowlen):
-            return max(4, min(Hp, (cap // rowlen) & ~3))
-
-        self.rpc0, self.rpc1, self.rpc2 = rows(self.K0p), rows(Hp), rows(Hp + Cp)
-        self.nf_chunk = max(1, min(self.TRmax, cap // (self.PR * Hp)))
-        used = max(self.rpc0 * self.K0p, self.rpc1 * Hp, self.rpc2 * (Hp + Cp), self.nf_chunk * self.PR * Hp)
-        self.wcap = (used + 31) & ~31
-
-        # MADE degrees / masks (nflows transforms/made.py, sequential degrees; residual blocks)
-        in_deg = np.arange(1, D + 1)
-        max_, min_ = max(1, D - 1), min(1, D - 1)
-        hid_deg = np.arange(H) % max_ + min_
-        m_init = (hid_deg[:, None] >= in_deg[None, :]).astype(np.float32)      # (H, D)
-        m_hid = (hid_deg[:, None] >= hid_deg[None, :]).astype(np.float32)      # (H, H)
-        out_deg = np.repeat(in_deg, 3 * M)
-        m_out = (out_deg[:, None] > hid_deg[None, :]).astype(np.float32)       # (3M*D, H)
-
-        off = 0
-
-        def take(n):
-            nonlocal off
-            o = off
-            off += round4(n)
-            return o
-
+        a = _Alloc()
         tab = np.zeros((1, L.SBI_NSF_LAYER_STRIDE), np.int32)
-        idx: Dict[str, np.ndarray] = {}
-        wm: Dict[str, np.ndarray] = {}
+        t = tab[0]
+        self._weight_masks: Dict[str, np.ndarray] = {}
         self.buffers: Dict[str, torch.Tensor] = {}
         pm = "net._distribution._made."
-        feats = list(range(D))
-        tab[0, L.L_NID], tab[0, L.L_NTR], tab[0, L.L_FEAT] = D, D, 0
+        t[L.L_NID], t[L.L_NTR], t[L.L_FEAT] = D, D, 0
         # initial layer: packed columns [ctx | pad | inputs | pad]; MADE's context_layer supplies the ctx columns
-        o = take(Hp * self.K0p)
-        tab[0, L.L_W0] = o
-        idx[pm + "initial_layer.weight"] = o + np.arange(H)[:, None] * self.K0p + (Cp + np.arange(D))[None, :]
-        wm[pm + "initial_layer.weight"] = m_init
-        self.buffers[pm + "initial_layer.mask"] = torch.as_tensor(m_init)
-        self.buffers[pm + "initial_layer.degrees"] = torch.as_tensor(hid_deg)
-        idx[pm + "context_layer.weight"] = o + np.arange(H)[:, None] * self.K0p + np.arange(C)[None, :]
-        o = take(Hp)
-        tab[0, L.L_B0] = o
-        idx[pm + "initial_layer.bias"] = o + np.arange(H)
-        o = take(Hp)
-        tab[0, L.L_BC0] = o
-        idx[pm + "context_layer.bias"] = o + np.arange(H)
-        for b in range(NB):
-            pb = pm + f"blocks.{b}."
-            t = L.L_BLK0 + 6 * b
-            for slot, (name, K, Kp, masked) in enumerate(
-                    [("linear_layers.0", H, Hp, True), ("linear_layers.1", H, Hp, True),
-                     ("context_layer", C, Cp, False)]):
-                o = take(Hp * Kp)
-                tab[0, t + 2 * slot] = o
-                idx[pb + name + ".weight"] = o + np.arange(H)[:, None] * Kp + np.arange(K)[None, :]
-                if masked:
-                    wm[pb + name + ".weight"] = m_hid
-                    self.buffers[pb + name + ".mask"] = torch.as_tensor(m_hid)
-                    self.buffers[pb + name + ".degrees"] = torch.as_tensor(hid_deg)
-                o = take(Hp)
-                tab[0, t + 2 * slot + 1] = o
-                idx[pb + name + ".bias"] = o + np.arange(H)
+        o = t[L.L_W0] = a.take(Hp * K0p)
+        a.index[pm + "initial_layer.weight"] = o + np.arange(H)[:, None] * K0p + (Cp + np.arange(D))[None, :]
+        _add_mask(self, pm + "initial_layer", m_init, hid_deg)
+        a.index[pm + "context_layer.weight"] = o + np.arange(H)[:, None] * K0p + np.arange(C)[None, :]
+        o = t[L.L_B0] = a.take(Hp)
+        a.index[pm + "initial_layer.bias"] = o + np.arange(H)
+        o = t[L.L_BC0] = a.take(Hp)
+        a.index[pm + "context_layer.bias"] = o + np.arange(H)
+        _residual_blocks(a, self, pm, t, hidden_mask=(m_hid, hid_deg))
         # final layer: feature f owns packed rows f*PR .. f*PR + 3M - 1 (nflows row f*3M + 3m + k)
-        o = take(D * self.PR * Hp)
-        tab[0, L.L_WF] = o
         prow = (np.arange(D)[:, None] * self.PR + np.arange(self.NPAR)[None, :]).reshape(-1)
-        idx[pm + "final_layer.weight"] = o + prow[:, None] * Hp + np.arange(H)[None, :]
-        wm[pm + "final_layer.weight"] = m_out
-        self.buffers[pm + "final_layer.mask"] = torch.as_tensor(m_out)
-        self.buffers[pm + "final_layer.degrees"] = torch.as_tensor(out_deg)
-        o = take(D * self.PR)
-        tab[0, L.L_BF] = o
-        idx[pm + "final_layer.bias"] = o + prow
-        tab[0, L.L_HAS_LU] = 0
-        self.n_params = off
-        self.index = idx
-        self._weight_masks = wm
+        a.linear(pm + "final_layer", t, (L.L_WF, L.L_BF), D * self.NPAR, H, Hp, rows=prow)
+        _add_mask(self, pm + "final_layer", m_out, out_deg)
+        t[L.L_HAS_LU] = 0
+        self.n_params = a.off
+        self.index = a.index
         self.layer_tab = tab
-        self.feat_tab = np.asarray(feats + feats, np.int32)
-
-    def tables(self):
-        return self.layer_tab.reshape(-1).astype(np.int32), self.feat_tab.astype(np.int32)
-
-    def tc_plan(self):
-        return None
+        self.feat_tab = np.asarray(list(range(D)) * 2, np.int32)
 
     def fill_struct(self, s: "L.NsfModel", nbuf: int):
-        s.D, s.C, s.H, s.NB, s.KB, s.T = self.D, self.C, self.H, self.NB, 2, 1
-        s.Dp, s.Cp, s.IDp, s.Hp, s.PR = self.Dp, self.Cp, self.IDp, self.Hp, self.PR
-        s.TRmax, s.nf_chunk = self.TRmax, self.nf_chunk
-        s.rpc0, s.rpc1, s.rpc2 = self.rpc0, self.rpc1, self.rpc2
-        s.wcap, s.nbuf, s.n_params = self.wcap, nbuf, self.n_params
+        super().fill_struct(s, nbuf)
+        s.KB = 2
         s.tail_bound, s.inv_sqrt_h, s.edge_raw = 1.0, 1.0, 0.0
-        s.min_bw = s.min_bh = s.min_d = 1e-3
         s.head, s.M, s.mog_eps, s.cond_mlp = 1, self.M, self.epsilon, 0
         return s
-
-
-MadeLayout.family = "made"
 
 
 @dataclass
 class MafLayout(_LayoutOps):
     """Packed layout of the MAF kernels (include/sbi_b200.h `sbi_maf_model`), mapping the tensors of
-    the reference module built by /root/reference/sbi/neural_nets/net_builders/flow.py:115-209 on
+    the reference module built by sbi/neural_nets/net_builders/flow.py:115-209 on
     nflows 0.14 (MaskedAffineAutoregressiveTransform(MADE) + RandomPermutation per layer)."""
     D: int
     C: int
@@ -657,8 +584,6 @@ class MafLayout(_LayoutOps):
     embed_is_identity: bool = True
     scale_softplus: bool = True          # softplus(s)+1e-3 (see oracle/nflows_port/transforms/autoregressive.py)
     wcap_target: int = 4096
-    n_params: int = 0
-    index: Dict[str, np.ndarray] = field(default_factory=dict, repr=False)
     # element-wise transform: "affine" (maf) or "rqs" (maf_rqs, flow.py:212-330; linear tails)
     head: str = "affine"
     KB: int = 10
@@ -666,6 +591,9 @@ class MafLayout(_LayoutOps):
     min_bin_width: float = 1e-3
     min_bin_height: float = 1e-3
     min_derivative: float = 1e-3
+
+    family = "maf"
+    _tables = ("layer_tab", "perm_tab")
 
     def __post_init__(self):
         D, C, H, NB, T = self.D, self.C, self.H, self.NB, self.T
@@ -680,97 +608,45 @@ class MafLayout(_LayoutOps):
         self.OUTp = round4(self.OUTM * D)
         Hp, Dp, Cp = self.Hp, self.Dp, self.Cp
         cap = max(self.wcap_target, 4 * (Dp + Cp), 4 * Hp)
-
-        def rows(rowlen, nmax):
-            return max(4, min(nmax, (cap // rowlen) & ~3))
-
-        self.rpc0, self.rpc1, self.rpcf = rows(Dp + Cp, Hp), rows(Hp, Hp), rows(Hp, self.OUTp)
-        used = max(self.rpc0 * (Dp + Cp), self.rpc1 * Hp, self.rpcf * Hp, 4 * Cp, 4 * Dp)
-        self.wcap = (used + 31) & ~31
-
-        # MADE degrees / masks (nflows transforms/made.py, sequential degrees)
-        in_deg = np.arange(1, D + 1)
-        max_, min_ = max(1, D - 1), min(1, D - 1)
-        hid_deg = np.arange(H) % max_ + min_
-        m_init = (hid_deg[:, None] >= in_deg[None, :]).astype(np.float32)      # (H, D)
-        m_hid = (hid_deg[:, None] >= hid_deg[None, :]).astype(np.float32)      # (H, H)
-        out_deg = np.repeat(in_deg, self.OUTM)                                 # tile(.., OUTM)
-        m_out = (out_deg[:, None] > hid_deg[None, :]).astype(np.float32)       # (OUTM*D, H)
+        (self.rpc0, self.rpc1, self.rpcf), self.wcap = _plan_ring(
+            cap, [(Dp + Cp, Hp), (Hp, Hp), (Hp, self.OUTp)], [4 * Cp, 4 * Dp])
+        in_deg, hid_deg, out_deg, m_init, m_hid, m_out = _made_masks(D, H, self.OUTM)
         self.degrees = dict(input=in_deg, hidden=hid_deg, output=out_deg)
-
-        off = 0
-
-        def take(n):
-            nonlocal off
-            o = off
-            off += round4(n)
-            return o
 
         if self.perms is None:
             self.perms = [np.arange(D) for _ in range(T)]
+        a = _Alloc()
         tab = np.zeros((T, L.SBI_MAF_LAYER_STRIDE), np.int32)
-        ptab = []
-        idx: Dict[str, np.ndarray] = {}
-        wm: Dict[str, np.ndarray] = {}
+        self._weight_masks: Dict[str, np.ndarray] = {}
         self.buffers: Dict[str, torch.Tensor] = {}
         base = 1 if self.zscore_input else 0
         for l in range(T):
             pa = f"net._transform._transforms.{base + 2 * l}.autoregressive_net."
             pp = f"net._transform._transforms.{base + 2 * l + 1}."
-            perm = np.asarray(self.perms[l], np.int64)
-            tab[l, L.M_PERM] = len(ptab)
-            ptab += list(perm) + list(np.argsort(perm))
-            self.buffers[pp + "_permutation"] = torch.as_tensor(perm)
-            o = take(Hp * Dp)
-            tab[l, L.M_W0] = o
-            idx[pa + "initial_layer.weight"] = o + np.arange(H)[:, None] * Dp + np.arange(D)[None, :]
-            wm[pa + "initial_layer.weight"] = m_init
-            self.buffers[pa + "initial_layer.mask"] = torch.as_tensor(m_init)
-            self.buffers[pa + "initial_layer.degrees"] = torch.as_tensor(hid_deg)
-            o = take(Hp)
-            tab[l, L.M_B0] = o
-            idx[pa + "initial_layer.bias"] = o + np.arange(H)
-            o = take(Hp * Cp)
-            tab[l, L.M_WC] = o
-            idx[pa + "context_layer.weight"] = o + np.arange(H)[:, None] * Cp + np.arange(C)[None, :]
-            o = take(Hp)
-            tab[l, L.M_BC] = o
-            idx[pa + "context_layer.bias"] = o + np.arange(H)
+            t = tab[l]
+            t[L.M_PERM] = 2 * D * l                      # the perm table holds (perm, inverse) per layer
+            self.buffers[pp + "_permutation"] = torch.as_tensor(np.asarray(self.perms[l], np.int64))
+            a.linear(pa + "initial_layer", t, (L.M_W0, L.M_B0), H, D, Dp)
+            _add_mask(self, pa + "initial_layer", m_init, hid_deg)
+            a.linear(pa + "context_layer", t, (L.M_WC, L.M_BC), H, C, Cp)
             for b in range(NB):
-                pb = pa + f"blocks.{b}.linear."
-                o = take(Hp * Hp)
-                tab[l, L.M_BLK0 + 2 * b] = o
-                idx[pb + "weight"] = o + np.arange(H)[:, None] * Hp + np.arange(H)[None, :]
-                wm[pb + "weight"] = m_hid
-                self.buffers[pb + "mask"] = torch.as_tensor(m_hid)
-                self.buffers[pb + "degrees"] = torch.as_tensor(hid_deg)
-                o = take(Hp)
-                tab[l, L.M_BLK0 + 2 * b + 1] = o
-                idx[pb + "bias"] = o + np.arange(H)
-            o = take(self.OUTp * Hp)
-            tab[l, L.M_WF] = o
-            idx[pa + "final_layer.weight"] = o + np.arange(self.OUTM * D)[:, None] * Hp + np.arange(H)[None, :]
-            wm[pa + "final_layer.weight"] = m_out
-            self.buffers[pa + "final_layer.mask"] = torch.as_tensor(m_out)
-            self.buffers[pa + "final_layer.degrees"] = torch.as_tensor(out_deg)
-            o = take(self.OUTp)
-            tab[l, L.M_BF] = o
-            idx[pa + "final_layer.bias"] = o + np.arange(self.OUTM * D)
-        self.n_params = off
-        self.index = idx
-        self._weight_masks = wm
+                a.linear(pa + f"blocks.{b}.linear", t, (L.M_BLK0 + 2 * b, L.M_BLK0 + 2 * b + 1), H, H, Hp)
+                _add_mask(self, pa + f"blocks.{b}.linear", m_hid, hid_deg)
+            a.linear(pa + "final_layer", t, (L.M_WF, L.M_BF), self.OUTM * D, H, Hp)
+            _add_mask(self, pa + "final_layer", m_out, out_deg)
+        self.n_params = a.off
+        self.index = a.index
         self.layer_tab = tab
-        self.perm_tab = np.asarray(ptab, np.int32)
+        self.perm_tab = self._perm_table()
 
-    def tables(self):
-        return self.layer_tab.reshape(-1).astype(np.int32), self.perm_tab.astype(np.int32)
+    def _perm_table(self):
+        return np.asarray([i for p in self.perms for i in (*p, *np.argsort(p))], np.int32)
 
     def load_buffers(self, incoming: Dict[str, torch.Tensor]):
         """Adopt the permutations of a loaded reference state_dict (RandomPermutation buffers are
         drawn at construction, so they are data, not architecture).  Returns the new perm table."""
         base = 1 if self.zscore_input else 0
         changed = False
-        ptab = []
         for l in range(self.T):
             key = f"net._transform._transforms.{base + 2 * l + 1}._permutation"
             if key in incoming:
@@ -781,8 +657,7 @@ class MafLayout(_LayoutOps):
                     changed = True
                 self.perms[l] = perm
                 self.buffers[key] = torch.as_tensor(perm)
-            ptab += list(self.perms[l]) + list(np.argsort(self.perms[l]))
-        self.perm_tab = np.asarray(ptab, np.int32)
+        self.perm_tab = self._perm_table()
         return self.perm_tab if changed else None
 
     def fill_struct(self, s: "L.MafModel", nbuf: int):
@@ -798,63 +673,36 @@ class MafLayout(_LayoutOps):
         return s
 
 
-MafLayout.family = "maf"
-
-
 @dataclass
 class RatioLayout(_LayoutOps):
     """Packed layout of the NRE `resnet` classifier (include/sbi_b200.h `sbi_ratio_model`): nflows
     ResidualNet(in=Dt+Dx, out=1, hidden, context=None, num_blocks) as built by
-    /root/reference/sbi/neural_nets/net_builders/classifier.py:172-235."""
+    sbi/neural_nets/net_builders/classifier.py:172-235."""
     Dt: int
     Dx: int
     H: int = 50
     NB: int = 2
     wcap_target: int = 4096
-    n_params: int = 0
-    index: Dict[str, np.ndarray] = field(default_factory=dict, repr=False)
+
+    family = "ratio"
 
     def __post_init__(self):
         Dt, Dx, H, NB = self.Dt, self.Dx, self.H, self.NB
         self.Dtp, self.Dxp, self.Hp = round4(Dt), round4(Dx), round4(H)
         K0p, Hp = self.Dtp + self.Dxp, self.Hp
         cap = max(self.wcap_target, 4 * K0p, 4 * Hp)
-        self.rpc0 = max(4, min(Hp, (cap // K0p) & ~3))
-        self.rpc1 = max(4, min(Hp, (cap // Hp) & ~3))
-        self.wcap = (max(self.rpc0 * K0p, self.rpc1 * Hp, 4 * Hp) + 31) & ~31
-        off = 0
-
-        def take(n):
-            nonlocal off
-            o = off
-            off += round4(n)
-            return o
-
+        (self.rpc0, self.rpc1), self.wcap = _plan_ring(cap, [(K0p, Hp), (Hp, Hp)], [4 * Hp])
+        a = _Alloc()
         tab = np.zeros(4 + 4 * 8, np.int32)
-        idx: Dict[str, np.ndarray] = {}
-        o = take(Hp * K0p)
-        tab[L.R_W0] = o
-        cols = np.concatenate([np.arange(Dt), self.Dtp + np.arange(Dx)])   # [theta | pad | x | pad]
-        idx["net.initial_layer.weight"] = o + np.arange(H)[:, None] * K0p + cols[None, :]
-        o = take(Hp)
-        tab[L.R_B0] = o
-        idx["net.initial_layer.bias"] = o + np.arange(H)
+        a.linear("net.initial_layer", tab, (L.R_W0, L.R_B0), H, Dt + Dx, K0p,
+                 cols=np.concatenate([np.arange(Dt), self.Dtp + np.arange(Dx)]))   # [theta | pad | x | pad]
         for b in range(NB):
             for j in range(2):
-                o = take(Hp * Hp)
-                tab[L.R_BLK0 + 4 * b + 2 * j] = o
-                idx[f"net.blocks.{b}.linear_layers.{j}.weight"] = o + np.arange(H)[:, None] * Hp + np.arange(H)[None, :]
-                o = take(Hp)
-                tab[L.R_BLK0 + 4 * b + 2 * j + 1] = o
-                idx[f"net.blocks.{b}.linear_layers.{j}.bias"] = o + np.arange(H)
-        o = take(4 * Hp)
-        tab[L.R_WF] = o
-        idx["net.final_layer.weight"] = o + np.arange(H)[None, :]
-        o = take(4)
-        tab[L.R_BF] = o
-        idx["net.final_layer.bias"] = o + np.arange(1)
-        self.n_params = off
-        self.index = idx
+                t = L.R_BLK0 + 4 * b + 2 * j
+                a.linear(f"net.blocks.{b}.linear_layers.{j}", tab, (t, t + 1), H, H, Hp)
+        a.linear("net.final_layer", tab, (L.R_WF, L.R_BF), 1, H, Hp)
+        self.n_params = a.off
+        self.index = a.index
         self.tab = tab
         self.buffers = {}
 
@@ -867,15 +715,6 @@ class RatioLayout(_LayoutOps):
         HP8 = (H + 7) & ~7
         K0 = Dt + Dx
         k0p8 = (K0 + 7) & ~7
-        tab = np.zeros(L.SBI_NSF_TC_STRIDE, np.int32)
-
-        def block(N, K, fill):
-            blk = np.full((K // 4, N, 4), -1, np.int64)
-            n = np.arange(N)[:, None] + 0 * np.arange(K)[None, :]
-            k = np.arange(K)[None, :] + 0 * np.arange(N)[:, None]
-            blk[k // 4, n, k % 4] = fill(n, k)
-            return blk.reshape(-1)
-
         t = self.tab
         w0 = int(t[L.R_W0])
 
@@ -888,23 +727,14 @@ class RatioLayout(_LayoutOps):
             def fill(n, k):
                 ok = (n < rows_valid) & (k < H)
                 return np.where(ok, woff + np.minimum(n, rows_valid - 1) * Hp + np.minimum(k, H - 1), -1)
-            return block(N, HP8, fill)
+            return _tc_block(N, HP8, fill)
 
-        stages = [(block(64, k0p8, fill0), 64)]
+        stages = [(_tc_block(64, k0p8, fill0), 64, 0)]
         for b in range(NB):
-            stages.append((hidden(int(t[L.R_BLK0 + 4 * b + 0]), 64, H), 64))
-            stages.append((hidden(int(t[L.R_BLK0 + 4 * b + 2]), 64, H), 64))
-        stages.append((hidden(int(t[L.R_WF]), 16, 1), 16))
-        chunks, off, cap = [], 0, 0
-        tab[0], tab[1] = len(stages), k0p8
-        for s_, (hi, N) in enumerate(stages):
-            nfl = 2 * hi.size
-            tab[4 + 4 * s_: 8 + 4 * s_] = (off, nfl, N, 0)
-            chunks += [hi, np.where(hi >= 0, -2 - hi, -1)]
-            off += nfl
-            cap = max(cap, nfl)
-        return dict(src=np.concatenate(chunks).astype(np.int32), tab=tab.astype(np.int32),
-                    stage_cap=int((cap + 31) & ~31), n_words=int(off))
+            stages.append((hidden(int(t[L.R_BLK0 + 4 * b + 0]), 64, H), 64, 0))
+            stages.append((hidden(int(t[L.R_BLK0 + 4 * b + 2]), 64, H), 64, 0))
+        stages.append((hidden(int(t[L.R_WF]), 16, 1), 16, 0))
+        return _tc_assemble([(k0p8, stages)])
 
     def fill_struct(self, s: "L.RatioModel", nbuf: int):
         s.Dt, s.Dx, s.H, s.NB = self.Dt, self.Dx, self.H, self.NB
@@ -912,9 +742,6 @@ class RatioLayout(_LayoutOps):
         s.rpc0, s.rpc1 = self.rpc0, self.rpc1
         s.wcap, s.nbuf, s.n_params = self.wcap, nbuf, self.n_params
         return s
-
-
-RatioLayout.family = "ratio"
 
 
 @dataclass
@@ -930,8 +757,8 @@ class MlpRatioLayout(_LayoutOps):
     norm: Optional[str] = "layer"
     eps: float = 1e-5
     wcap_target: int = 4096
-    n_params: int = 0
-    index: Dict[str, np.ndarray] = field(default_factory=dict, repr=False)
+
+    family = "ratio_mlp"
 
     def __post_init__(self):
         Dt, Dx, H, NL = self.Dt, self.Dx, self.H, self.NL
@@ -941,38 +768,24 @@ class MlpRatioLayout(_LayoutOps):
         K0p, Hp = self.Dtp + self.Dxp, self.Hp
         KFp = Hp if NL else K0p
         cap = max(self.wcap_target, 4 * K0p, 4 * Hp)
-        self.rpc0 = max(4, min(Hp, (cap // K0p) & ~3))
-        self.rpc1 = max(4, min(Hp, (cap // Hp) & ~3))
-        self.wcap = (max(self.rpc0 * K0p, self.rpc1 * Hp, 4 * KFp) + 31) & ~31
-        off = 0
-
-        def take(n):
-            nonlocal off
-            o = off
-            off += round4(n)
-            return o
-
+        (self.rpc0, self.rpc1), self.wcap = _plan_ring(cap, [(K0p, Hp), (Hp, Hp)], [4 * KFp])
+        a = _Alloc()
         tab = np.zeros(10, np.int32)
-        idx: Dict[str, np.ndarray] = {}
         cols0 = np.concatenate([np.arange(Dt), self.Dtp + np.arange(Dx)])   # [theta | pad | x | pad]
         for l in range(NL):
-            Kp, cols = (K0p, cols0) if l == 0 else (Hp, np.arange(H))
-            o = tab[4 * l + L.RM_W0] = take(Hp * Kp)
-            idx[f"net.{3 * l}.weight"] = o + np.arange(H)[:, None] * Kp + cols[None, :]
-            o = tab[4 * l + L.RM_B0] = take(Hp)
-            idx[f"net.{3 * l}.bias"] = o + np.arange(H)
+            K, Kp, cols = (Dt + Dx, K0p, cols0) if l == 0 else (H, Hp, None)
+            a.linear(f"net.{3 * l}", tab, (4 * l + L.RM_W0, 4 * l + L.RM_B0), H, K, Kp, cols=cols)
             if self.norm == "layer":
-                o = tab[4 * l + L.RM_G0] = take(Hp)
-                idx[f"net.{3 * l + 1}.weight"] = o + np.arange(H)
-                o = tab[4 * l + L.RM_BE0] = take(Hp)
-                idx[f"net.{3 * l + 1}.bias"] = o + np.arange(H)
-        pre = "net.6." if NL else "net."
-        o = tab[L.RM_WF] = take(4 * KFp)
-        idx[pre + "weight"] = o + (np.arange(H) if NL else cols0)[None, :]
-        o = tab[L.RM_BF] = take(4)
-        idx[pre + "bias"] = o + np.arange(1)
-        self.n_params = off
-        self.index = idx
+                o = tab[4 * l + L.RM_G0] = a.take(Hp)
+                a.index[f"net.{3 * l + 1}.weight"] = o + np.arange(H)
+                o = tab[4 * l + L.RM_BE0] = a.take(Hp)
+                a.index[f"net.{3 * l + 1}.bias"] = o + np.arange(H)
+        if NL:
+            a.linear("net.6", tab, (L.RM_WF, L.RM_BF), 1, H, Hp)
+        else:
+            a.linear("net", tab, (L.RM_WF, L.RM_BF), 1, Dt + Dx, K0p, cols=cols0)
+        self.n_params = a.off
+        self.index = a.index
         self.tab = tab
         self.buffers = {}
 
@@ -986,13 +799,10 @@ class MlpRatioLayout(_LayoutOps):
         return s
 
 
-MlpRatioLayout.family = "ratio_mlp"
-
-
 @dataclass
 class FmLayout(_LayoutOps):
     """Packed layout of the flow-matching VectorFieldMLP (include/sbi_b200.h `sbi_fm_model`), tensor
-    names as in /root/reference/sbi/neural_nets/net_builders/vector_field_nets.py:610-719 under the
+    names as in sbi/neural_nets/net_builders/vector_field_nets.py:610-719 under the
     estimator attribute `net` (FlowMatchingEstimator.net)."""
     D: int
     C: int
@@ -1000,8 +810,8 @@ class FmLayout(_LayoutOps):
     NL: int = 5
     TE: int = 32
     wcap_target: int = 3200
-    n_params: int = 0
-    index: Dict[str, np.ndarray] = field(default_factory=dict, repr=False)
+
+    family = "fm"
 
     def __post_init__(self):
         D, C, H, NL, TE = self.D, self.C, self.H, self.NL, self.TE
@@ -1012,52 +822,25 @@ class FmLayout(_LayoutOps):
         self.Dp, self.Cp, self.Hp, self.TEp = round4(D), round4(C), round4(H), round4(TE)
         Hp = self.Hp
         cap = max(self.wcap_target, 4 * 2 * Hp)
-
-        def rows(rowlen, nmax):
-            return max(4, min(nmax, (cap // rowlen) & ~3))
-
-        self.rpc_i, self.rpc_c, self.rpc_m = rows(self.Dp, Hp), rows(self.Cp, Hp), rows(2 * Hp, Hp)
-        self.rpc_t, self.rpc_h, self.rpc_o = rows(self.TEp, Hp), rows(Hp, Hp), rows(Hp, self.Dp)
-        used = max(self.rpc_i * self.Dp, self.rpc_c * self.Cp, self.rpc_m * 2 * Hp, self.rpc_t * self.TEp,
-                   self.rpc_h * Hp, self.rpc_o * Hp)
-        self.wcap = (used + 31) & ~31
-        off = 0
-
-        def take(n):
-            nonlocal off
-            o = off
-            off += round4(n)
-            return o
-
+        (self.rpc_i, self.rpc_c, self.rpc_m, self.rpc_t, self.rpc_h, self.rpc_o), self.wcap = _plan_ring(
+            cap, [(self.Dp, Hp), (self.Cp, Hp), (2 * Hp, Hp), (self.TEp, Hp), (Hp, Hp), (Hp, self.Dp)])
+        a = _Alloc()
         tab = np.zeros(L.F_LAYER0 + 4 * 12, np.int32)
-        idx: Dict[str, np.ndarray] = {}
-
-        def lin(name, slot_w, slot_b, N, K, Kp, cols=None, Np=None):
-            Np = round4(N) if Np is None else Np
-            o = take(Np * Kp)
-            tab[slot_w] = o
-            c = np.arange(K) if cols is None else cols
-            idx[name + ".weight"] = o + np.arange(N)[:, None] * Kp + c[None, :]
-            o = take(Np)
-            tab[slot_b] = o
-            idx[name + ".bias"] = o + np.arange(N)
-
-        lin("net.input_layer", L.F_WI, L.F_BI, H, D, self.Dp)
-        lin("net.condition_layer", L.F_WC, L.F_BC, H, C, self.Cp)
-        lin("net.input_merge_layer", L.F_WM, L.F_BM, H, 2 * H, 2 * Hp,
-            cols=np.concatenate([np.arange(H), Hp + np.arange(H)]))
-        lin("net.time_linear_layer", L.F_WT, L.F_BT, H, TE, self.TEp)
-        lin("net.output_layer", L.F_WO, L.F_BO, D, H, Hp)
+        a.linear("net.input_layer", tab, (L.F_WI, L.F_BI), H, D, self.Dp)
+        a.linear("net.condition_layer", tab, (L.F_WC, L.F_BC), H, C, self.Cp)
+        a.linear("net.input_merge_layer", tab, (L.F_WM, L.F_BM), H, 2 * H, 2 * Hp,
+                 cols=np.concatenate([np.arange(H), Hp + np.arange(H)]))
+        a.linear("net.time_linear_layer", tab, (L.F_WT, L.F_BT), H, TE, self.TEp)
+        a.linear("net.output_layer", tab, (L.F_WO, L.F_BO), D, H, Hp)
         for i in range(NL):
-            lin(f"net.layers.{i}", L.F_LAYER0 + 4 * i, L.F_LAYER0 + 4 * i + 1, H, H, Hp)
-            o = take(Hp)
-            tab[L.F_LAYER0 + 4 * i + 2] = o
-            idx[f"net.layers_norm.{i}.weight"] = o + np.arange(H)
-            o = take(Hp)
-            tab[L.F_LAYER0 + 4 * i + 3] = o
-            idx[f"net.layers_norm.{i}.bias"] = o + np.arange(H)
-        self.n_params = off
-        self.index = idx
+            t = L.F_LAYER0 + 4 * i
+            a.linear(f"net.layers.{i}", tab, (t, t + 1), H, H, Hp)
+            o = tab[t + 2] = a.take(Hp)
+            a.index[f"net.layers_norm.{i}.weight"] = o + np.arange(H)
+            o = tab[t + 3] = a.take(Hp)
+            a.index[f"net.layers_norm.{i}.bias"] = o + np.arange(H)
+        self.n_params = a.off
+        self.index = a.index
         self.tab = tab
         self.buffers = {}
 
@@ -1069,6 +852,3 @@ class FmLayout(_LayoutOps):
         s.wcap, s.nbuf, s.n_params = self.wcap, nbuf, self.n_params
         s.noise_scale, s.ln_eps = 1e-3, 1e-5
         return s
-
-
-FmLayout.family = "fm"
