@@ -100,8 +100,8 @@ class FlowMatchingEstimator(_PackedEstimator):
         v = torch.empty_like(inp)
         m = self._model(nbuf=2)
         rows = L.Rows(inp.data_ptr(), cond.data_ptr(), None, R, 1 if shared else 0)
-        L.check(lib.sbi_b200_fm_forward(C.byref(m), C.byref(rows), L.ptr(tt), 1 if t_shared else 0, L.ptr(v),
-                                        L.stream_ptr()), "fm_forward")
+        self._check_rc(lib.sbi_b200_fm_forward(C.byref(m), C.byref(rows), L.ptr(tt), 1 if t_shared else 0, L.ptr(v),
+                                               L.stream_ptr()), "fm_forward")
         return v.reshape(*bshape, *self.input_shape)
 
     def forward_and_divergence(self, input: Tensor, condition: Tensor, time: Tensor):
@@ -121,8 +121,8 @@ class FlowMatchingEstimator(_PackedEstimator):
         div = torch.empty(R, dtype=torch.float32, device=inp.device)
         m = self._model(nbuf=2)
         rows = L.Rows(inp.data_ptr(), cond.data_ptr(), None, R, 1 if shared else 0)
-        L.check(lib.sbi_b200_fm_forward_div(C.byref(m), C.byref(rows), L.ptr(tt), 1 if t_shared else 0, L.ptr(v),
-                                            L.ptr(div), L.stream_ptr()), "fm_forward_div")
+        self._check_rc(lib.sbi_b200_fm_forward_div(C.byref(m), C.byref(rows), L.ptr(tt), 1 if t_shared else 0,
+                                                   L.ptr(v), L.ptr(div), L.stream_ptr()), "fm_forward_div")
         return v, div
 
     def ode_fn(self, input: Tensor, condition: Tensor, times: Tensor) -> Tensor:
@@ -191,9 +191,9 @@ class FlowMatchingEstimator(_PackedEstimator):
         gpart = self._gpart(n_part) if gpart is None else gpart
         m = self._model(nbuf=2)
         rows = L.Rows(inp.data_ptr(), cond.data_ptr(), None if index is None else index.data_ptr(), R, 0)
-        L.check(lib.sbi_b200_fm_loss_vjp_cond(C.byref(m), C.byref(rows), L.ptr(times), L.ptr(eps), None, g_const,
-                                              L.ptr(loss), L.ptr(gpart), L.ptr(loss_acc), L.ptr(gcond),
-                                              L.stream_ptr()), "fm_loss_vjp")
+        self._check_rc(lib.sbi_b200_fm_loss_vjp_cond(C.byref(m), C.byref(rows), L.ptr(times), L.ptr(eps), None,
+                                                     g_const, L.ptr(loss), L.ptr(gpart), L.ptr(loss_acc),
+                                                     L.ptr(gcond), L.stream_ptr()), "fm_loss_vjp")
         return loss, gpart, n_part
 
 
@@ -208,8 +208,8 @@ class _FmLoss(torch.autograd.Function):
         m = est._model(nbuf=2)
         rows = L.Rows(inp.data_ptr(), cond.data_ptr(), None, R, 0)
         # forward value only: g = 0 (the partial gradients written are zeros)
-        L.check(lib.sbi_b200_fm_loss_vjp(C.byref(m), C.byref(rows), L.ptr(times), L.ptr(eps), None, 0.0,
-                                         L.ptr(loss), L.ptr(gpart), None, L.stream_ptr()), "fm_loss")
+        est._check_rc(lib.sbi_b200_fm_loss_vjp(C.byref(m), C.byref(rows), L.ptr(times), L.ptr(eps), None, 0.0,
+                                               L.ptr(loss), L.ptr(gpart), None, L.stream_ptr()), "fm_loss")
         ctx.save_for_backward(inp, cond, times, eps)
         ctx.est = est
         return loss
@@ -226,8 +226,9 @@ class _FmLoss(torch.autograd.Function):
         rows = L.Rows(inp.data_ptr(), cond.data_ptr(), None, R, 0)
         g = g.contiguous().float()
         gcond = torch.empty_like(cond) if ctx.needs_input_grad[2] else None
-        L.check(lib.sbi_b200_fm_loss_vjp_cond(C.byref(m), C.byref(rows), L.ptr(times), L.ptr(eps), L.ptr(g), 0.0,
-                                              None, L.ptr(gpart), None, L.ptr(gcond), L.stream_ptr()), "fm_loss_vjp")
+        est._check_rc(lib.sbi_b200_fm_loss_vjp_cond(C.byref(m), C.byref(rows), L.ptr(times), L.ptr(eps), L.ptr(g),
+                                                    0.0, None, L.ptr(gpart), None, L.ptr(gcond), L.stream_ptr()),
+                      "fm_loss_vjp")
         gflat = L.reduce_partials(gpart, n_part, est.layout.n_params) if ctx.needs_input_grad[0] else None
         return gflat, None, gcond, None, None, None
 
@@ -433,11 +434,11 @@ def _fm_rhs(est: FlowMatchingEstimator, cond: Tensor, R: int, with_div: bool):
     def rhs(y: Tensor, t_ptr: int, out: Tensor):
         rows = L.Rows(y.data_ptr(), keep[1].data_ptr(), None, R, shared)
         if with_div:
-            L.check(lib.sbi_b200_fm_forward_div(C.byref(keep[0]), C.byref(rows), t_ptr, 1, out.data_ptr(),
-                                                out.data_ptr() + 4 * R * D, L.stream_ptr()), "fm_forward_div")
+            est._check_rc(lib.sbi_b200_fm_forward_div(C.byref(keep[0]), C.byref(rows), t_ptr, 1, out.data_ptr(),
+                                                      out.data_ptr() + 4 * R * D, L.stream_ptr()), "fm_forward_div")
         else:
-            L.check(lib.sbi_b200_fm_forward(C.byref(keep[0]), C.byref(rows), t_ptr, 1, out.data_ptr(),
-                                            L.stream_ptr()), "fm_forward")
+            est._check_rc(lib.sbi_b200_fm_forward(C.byref(keep[0]), C.byref(rows), t_ptr, 1, out.data_ptr(),
+                                                  L.stream_ptr()), "fm_forward")
     return rhs
 
 
@@ -627,8 +628,8 @@ def sample_sde(est: FlowMatchingEstimator, num_samples: int, condition: Tensor, 
     rows = L.Rows(theta.data_ptr(), cond.data_ptr(), None, R, 1 if B == 1 else 0)
 
     def step():
-        L.check(lib.sbi_b200_fm_forward(C.byref(m), C.byref(rows), ctrl.data_ptr(), 1, v.data_ptr(), L.stream_ptr()),
-                "fm_forward")
+        est._check_rc(lib.sbi_b200_fm_forward(C.byref(m), C.byref(rows), ctrl.data_ptr(), 1, v.data_ptr(),
+                                              L.stream_ptr()), "fm_forward")
         z.normal_()
         L.check(lib.sbi_b200_sde_em_step(theta.data_ptr(), v.data_ptr(), z.data_ptr(), n, ts.data_ptr(),
                                          ctrl.data_ptr(), float(eta), float(est.noise_scale), 0.99, L.stream_ptr()),

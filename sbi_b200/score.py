@@ -51,8 +51,8 @@ class _RawNet(torch.autograd.Function):
         m = est._model(nbuf=2)
         rows = L.Rows(inp.data_ptr(), cond.data_ptr(), None, R, 1 if cond.shape[0] == 1 and R > 1 else 0)
         g = g.contiguous().float()
-        L.check(lib.sbi_b200_fm_net_vjp(C.byref(m), C.byref(rows), L.ptr(tenc), L.ptr(g), L.ptr(gpart),
-                                        L.stream_ptr()), "fm_net_vjp")
+        est._check_rc(lib.sbi_b200_fm_net_vjp(C.byref(m), C.byref(rows), L.ptr(tenc), L.ptr(g), L.ptr(gpart),
+                                              L.stream_ptr()), "fm_net_vjp")
         return L.reduce_partials(gpart, n_part, est.layout.n_params), None, None, None, None
 
 
@@ -92,8 +92,8 @@ class ConditionalScoreEstimator(FlowMatchingEstimator):
         out = torch.empty_like(inp)
         m = self._model(nbuf=2)
         rows = L.Rows(inp.data_ptr(), cond.data_ptr(), None, R, 1 if cond.shape[0] == 1 and R > 1 else 0)
-        L.check(lib.sbi_b200_fm_forward(C.byref(m), C.byref(rows), L.ptr(tenc), 0, L.ptr(out), L.stream_ptr()),
-                "fm_forward(raw)")
+        self._check_rc(lib.sbi_b200_fm_forward(C.byref(m), C.byref(rows), L.ptr(tenc), 0, L.ptr(out),
+                                               L.stream_ptr()), "fm_forward(raw)")
         return out
 
     def _raw_forward_diag(self, inp: Tensor, cond: Tensor, tenc: Tensor):
@@ -104,8 +104,8 @@ class ConditionalScoreEstimator(FlowMatchingEstimator):
         out, diag = torch.empty_like(inp), torch.empty_like(inp)
         m = self._model(nbuf=2)
         rows = L.Rows(inp.data_ptr(), cond.data_ptr(), None, R, 1 if cond.shape[0] == 1 and R > 1 else 0)
-        L.check(lib.sbi_b200_fm_forward_div(C.byref(m), C.byref(rows), L.ptr(tenc), 0, L.ptr(out), L.ptr(diag),
-                                            L.stream_ptr()), "fm_forward_div(raw)")
+        self._check_rc(lib.sbi_b200_fm_forward_div(C.byref(m), C.byref(rows), L.ptr(tenc), 0, L.ptr(out),
+                                                   L.ptr(diag), L.stream_ptr()), "fm_forward_div(raw)")
         return out, diag
 
     def _net_call(self, input_enc: Tensor, condition: Tensor, time_enc: Tensor) -> Tensor:

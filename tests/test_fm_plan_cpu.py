@@ -59,3 +59,11 @@ def test_default_network_plan():
     assert ev[6] == 100 and tr[6] >= 48 and dv[6] >= 48
     for p in (ev, tr, dv):
         assert p[8] <= SMEM_MAX
+
+
+def test_shared_memory_limit_per_kernel():
+    """The largest hidden width each kernel fits at D = C = 20, num_layers = 5 (DESIGN.md §3.1): the 32-row
+    forward takes H = 224, the 16-row loss / network VJP 124 and the forward + divergence 120, so evaluation fits
+    models (H = 128) that training does not."""
+    limits = [max(H for H in range(4, 400, 4) if _plans(20, 20, H, 5, 32)[1][k][8] <= SMEM_MAX) for k in range(3)]
+    assert limits == [224, 124, 120]
