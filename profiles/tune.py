@@ -57,5 +57,5 @@ def logprob():
     L.check(lib.sbi_b200_nsf_logprob(C.byref(m), C.byref(rows), L.ptr(lp), None, L.stream_ptr()), "lp")
 
 
-print(f"{os.environ.get('SBI_B200_LIB', 'default')} tm={os.environ.get('SBI_B200_LOGPROB_TM', '-')} nbuf={nbuf_tr}/{nbuf_ev}: "
+print(f"{os.environ.get('SBI_B200_LIB', 'default')} nbuf={nbuf_tr}/{nbuf_ev}: "
       f"vjp {timeit(vjp) * 1e3:.1f} us   logprob(4.2M rows) {timeit(logprob, n=8, do_flush=False):.2f} ms")

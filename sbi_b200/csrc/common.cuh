@@ -143,16 +143,9 @@ __device__ __forceinline__ float warp_sum(float v) {
 // round trips per thread and tile).  Every address is written by ONE thread, first with a plain store, then with
 // REDs in tile order, so the sum order is fixed and nothing ever reads the slab inside the kernel (an L1-cached
 // load could not see the REDs).
-#ifndef SBI_DW_RED
-#define SBI_DW_RED 1
-#endif
 __device__ __forceinline__ void grad_out(float* dst, float v, bool accumulate) {
-#if SBI_DW_RED
   if (accumulate) asm volatile("red.global.add.f32 [%0], %1;" ::"l"(dst), "f"(v) : "memory");
   else *dst = v;
-#else
-  *dst = accumulate ? (*dst + v) : v;
-#endif
 }
 
 }  // namespace sbi

@@ -669,30 +669,22 @@ fm_vjp_kernel(const __grid_constant__ sbi_fm_model m, const __grid_constant__ sb
 
 using namespace sbi;
 
-static int fm_num_sms() { return sbi::dev_num_sms(); }
-
 // Launch-side tuning of the weight pipeline (the kernels read nbuf / wcap / rpc_* from the model struct, the
 // packed weights do not depend on them).  Measured on cfg4 (FMPE dim 20, batch 16384, trainer level, M samples/s;
-// profiles/r02_bench_cfg4*.json):
-//  * SBI_RING_AUTO >= 1: the ring the caller asked for is a lower bound; deepen it to what the 227 KB of shared
-//    memory leave after the activation tile.  ncu attributes ~25 % of fm_vjp's stall samples to the ring's `full`
-//    barrier (profiles/r02_fm_vjp.md), but depth alone only moved 9.80 -> 9.99.
-//  * SBI_RING_AUTO >= 2: re-chunk per kernel.  A forward chunk of `cnt` weight rows occupies cnt / RN of the
-//    256 / (TM / 4) output-thread groups, so the caller's 32-row chunks of a 100-wide layer kept 25 % (16-row
-//    tiles) to 50 % (32-row tiles) of the consumer threads busy, the 16-row chunks of the merge layer half of
-//    that.  Two stages of the largest chunk that fits (60 rows in training, whole layers in evaluation) with
-//    RN = SBI_FM_RN = 1 output row per thread fill them: 9.99 -> 12.5.  (RN = 1 with the 32-row chunks is SLOWER,
-//    7.67: five shared-memory wavefronts per 16 FMAs without the extra parallelism.)
-#ifndef SBI_RING_AUTO
-#define SBI_RING_AUTO 2
-#endif
-#ifndef SBI_FM_RN
-#define SBI_FM_RN 1
-#endif
+// profiles/r02_bench_cfg4*.json), in two steps:
+//  * Re-chunk per kernel.  A forward chunk of `cnt` weight rows occupies cnt / RN of the 256 / (TM / 4)
+//    output-thread groups, so the caller's 32-row chunks of a 100-wide layer kept 25 % (16-row tiles) to 50 %
+//    (32-row tiles) of the consumer threads busy, the 16-row chunks of the merge layer half of that.  Two stages of
+//    the largest chunk that fits (60 rows in training, whole layers in evaluation) with RN = kFmRN = 1 output row
+//    per thread fill them.  (RN = 1 with the 32-row chunks is SLOWER, 7.67: five shared-memory wavefronts per
+//    16 FMAs without the extra parallelism.)
+//  * Deepen the ring to what the 227 KB of shared memory leave after the activation tile.  ncu attributes ~25 % of
+//    fm_vjp's stall samples to the ring's `full` barrier (profiles/r02_fm_vjp.md).
+// Deepening alone moved 9.80 -> 9.99, re-chunking on top of it 9.99 -> 12.5.
+constexpr int kFmRN = 1;
 static sbi_fm_model fm_tune(const sbi_fm_model& m, int TM, int mode) {
   sbi_fm_model c = m;
-  constexpr int kBudget = 227 * 1024 - 1024;      // static shared memory of the kernels stays below 1 KB
-#if SBI_RING_AUTO >= 2
+  constexpr int kBudget = kMaxSmemBytes - 1024;   // static shared memory of the kernels stays below 1 KB
   {
     sbi_fm_model z = m;
     z.nbuf = 0;
@@ -716,15 +708,12 @@ static sbi_fm_model fm_tune(const sbi_fm_model& m, int TM, int mode) {
       if (fm_smem_layout(c, TM, mode).total_bytes > kBudget) c = m;   // (cannot happen; keep the caller's plan)
     }
   }
-#endif
-#if SBI_RING_AUTO >= 1
   const int nb0 = c.nbuf;
   for (int nb = 8; nb > nb0; --nb) {
     c.nbuf = nb;
     if (fm_smem_layout(c, TM, mode).total_bytes <= kBudget) return c;
   }
   c.nbuf = nb0;
-#endif
   return c;
 }
 
@@ -732,23 +721,10 @@ static int fm_check(const sbi_fm_model* m) {
   if (!m || !m->d_params || !m->d_tab || !m->d_stats) return SBI_EINVAL;
   if (m->D < 1 || m->C < 1 || m->H < 1 || m->NL < 2 || m->NL > SBI_FM_MAX_LAYERS || m->TE < 2 || (m->TE & 1)) return SBI_EINVAL;
   if (m->Dp != round4(m->D) || m->Cp != round4(m->C) || m->Hp != round4(m->H) || m->TEp != round4(m->TE)) return SBI_EINVAL;
-  const int rp[6] = {m->rpc_i, m->rpc_c, m->rpc_m, m->rpc_t, m->rpc_h, m->rpc_o};
-  const int rl[6] = {m->Dp, m->Cp, 2 * m->Hp, m->TEp, m->Hp, m->Hp};
-  for (int i = 0; i < 6; ++i)
-    if ((rp[i] & 3) || rp[i] < 4 || rp[i] * rl[i] > m->wcap) return SBI_EINVAL;
-  if (m->nbuf < 2 || m->nbuf > 8) return SBI_EINVAL;
-  return 0;
-}
-
-template <int ID, class K>
-static int fm_set_smem(K kernel, int bytes) {
-  static int granted_[sbi::kMaxDev] = {0};
-  int& granted = granted_[sbi::cur_dev()];
-  if (bytes > 227 * 1024) return SBI_ESMEM;
-  if (bytes <= granted) return 0;
-  cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
-  if (e != cudaSuccess) return (int)e;
-  granted = bytes;
+  if (!ring_ok({{m->rpc_i, m->Dp}, {m->rpc_c, m->Cp}, {m->rpc_m, 2 * m->Hp}, {m->rpc_t, m->TEp}, {m->rpc_h, m->Hp},
+                {m->rpc_o, m->Hp}},
+               m->nbuf, m->wcap))
+    return SBI_EINVAL;
   return 0;
 }
 
@@ -761,13 +737,8 @@ extern "C" int sbi_b200_fm_forward(const sbi_fm_model* m, const sbi_rows* rows, 
   if (rows->R == 0) return 0;
   constexpr int TM = 32;
   const sbi_fm_model md = fm_tune(*m, TM, kFmEval);
-  const FmSmem L = fm_smem_layout(md, TM, kFmEval);
-  auto k = fm_forward_kernel<TM, SBI_FM_RN>;
-  if ((rc = fm_set_smem<0>(k, L.total_bytes))) return rc;
-  const int64_t ntiles = (rows->R + TM - 1) / TM;
-  const int grid = (int)std::min<int64_t>(ntiles, fm_num_sms());
-  k<<<grid, kThreads, L.total_bytes, (cudaStream_t)stream>>>(md, *rows, d_time, time_shared, d_v);
-  return (int)cudaGetLastError();
+  return launch(fm_forward_kernel<TM, kFmRN>, tile_grid(rows->R, TM, 1), kThreads,
+                fm_smem_layout(md, TM, kFmEval).total_bytes, (cudaStream_t)stream, md, *rows, d_time, time_shared, d_v);
 }
 
 extern "C" int sbi_b200_fm_forward_div(const sbi_fm_model* m, const sbi_rows* rows, const float* d_time,
@@ -779,13 +750,9 @@ extern "C" int sbi_b200_fm_forward_div(const sbi_fm_model* m, const sbi_rows* ro
   if (rows->R == 0) return 0;
   constexpr int TM = 16;
   const sbi_fm_model md = fm_tune(*m, TM, kFmTrace);
-  const FmSmem L = fm_smem_layout(md, TM, kFmTrace);
-  auto k = fm_trace_kernel<TM, SBI_FM_RN>;
-  if ((rc = fm_set_smem<2>(k, L.total_bytes))) return rc;
-  const int64_t ntiles = (rows->R + TM - 1) / TM;
-  const int grid = (int)std::min<int64_t>(ntiles, fm_num_sms());
-  k<<<grid, kThreads, L.total_bytes, (cudaStream_t)stream>>>(md, *rows, d_time, time_shared, d_v, d_div);
-  return (int)cudaGetLastError();
+  return launch(fm_trace_kernel<TM, kFmRN>, tile_grid(rows->R, TM, 1), kThreads,
+                fm_smem_layout(md, TM, kFmTrace).total_bytes, (cudaStream_t)stream, md, *rows, d_time, time_shared, d_v,
+                d_div);
 }
 
 extern "C" int sbi_b200_fm_plan(const sbi_fm_model* m, int32_t kernel, int32_t* out10) {
@@ -797,15 +764,12 @@ extern "C" int sbi_b200_fm_plan(const sbi_fm_model* m, int32_t kernel, int32_t* 
   const int mode = kernel == 0 ? kFmEval : (kernel == 1 ? kFmTrain : kFmTrace);
   const sbi_fm_model c = fm_tune(*m, TM, mode);
   const int v[10] = {c.nbuf, c.wcap, c.rpc_i, c.rpc_c, c.rpc_m, c.rpc_t, c.rpc_h, c.rpc_o,
-                     fm_smem_layout(c, TM, mode).total_bytes, SBI_FM_RN};
+                     fm_smem_layout(c, TM, mode).total_bytes, kFmRN};
   for (int i = 0; i < 10; ++i) out10[i] = v[i];
   return 0;
 }
 
-extern "C" int sbi_b200_fm_vjp_parts(int64_t R) {
-  const int64_t ntiles = (R + 15) / 16;
-  return (int)std::max<int64_t>(1, std::min<int64_t>(ntiles, fm_num_sms()));
-}
+extern "C" int sbi_b200_fm_vjp_parts(int64_t R) { return vjp_parts(R, 16); }
 
 extern "C" int sbi_b200_fm_loss_vjp(const sbi_fm_model* m, const sbi_rows* rows, const float* d_time,
                                     const float* d_eps, const float* d_gout, float g_const, float* d_loss,
@@ -828,13 +792,9 @@ extern "C" int sbi_b200_fm_loss_vjp_cond(const sbi_fm_model* m, const sbi_rows* 
   }
   constexpr int TM = 16;
   const sbi_fm_model md = fm_tune(*m, TM, kFmTrain);
-  const FmSmem L = fm_smem_layout(md, TM, kFmTrain);
-  auto k = fm_vjp_kernel<TM, SBI_FM_RN, 2>;
-  if ((rc = fm_set_smem<1>(k, L.total_bytes))) return rc;
-  const int grid = sbi_b200_fm_vjp_parts(rows->R);
-  k<<<grid, kThreads, L.total_bytes, (cudaStream_t)stream>>>(md, *rows, d_time, d_eps, d_gout, g_const, d_loss,
-                                                           d_gpart, d_loss_acc, nullptr, d_gcond);
-  return (int)cudaGetLastError();
+  return launch(fm_vjp_kernel<TM, kFmRN, 2>, sbi_b200_fm_vjp_parts(rows->R), kThreads,
+                fm_smem_layout(md, TM, kFmTrain).total_bytes, (cudaStream_t)stream, md, *rows, d_time, d_eps, d_gout,
+                g_const, d_loss, d_gpart, d_loss_acc, nullptr, d_gcond);
 }
 
 extern "C" int sbi_b200_fm_net_vjp(const sbi_fm_model* m, const sbi_rows* rows, const float* d_time,
@@ -846,11 +806,7 @@ extern "C" int sbi_b200_fm_net_vjp(const sbi_fm_model* m, const sbi_rows* rows, 
     return SBI_EINVAL;
   constexpr int TM = 16;
   const sbi_fm_model md = fm_tune(*m, TM, kFmTrain);
-  const FmSmem L = fm_smem_layout(md, TM, kFmTrain);
-  auto k = fm_vjp_kernel<TM, SBI_FM_RN, 2>;
-  if ((rc = fm_set_smem<1>(k, L.total_bytes))) return rc;
-  const int grid = sbi_b200_fm_vjp_parts(rows->R);
-  k<<<grid, kThreads, L.total_bytes, (cudaStream_t)stream>>>(md, *rows, d_time, nullptr, nullptr, 0.f, nullptr, d_gpart,
-                                                           nullptr, d_dout, nullptr);
-  return (int)cudaGetLastError();
+  return launch(fm_vjp_kernel<TM, kFmRN, 2>, sbi_b200_fm_vjp_parts(rows->R), kThreads,
+                fm_smem_layout(md, TM, kFmTrain).total_bytes, (cudaStream_t)stream, md, *rows, d_time, nullptr, nullptr,
+                0.f, nullptr, d_gpart, nullptr, d_dout, nullptr);
 }

@@ -535,8 +535,6 @@ maf_vjp_kernel(const __grid_constant__ sbi_maf_model m, const __grid_constant__ 
 // =================================================================================================
 using namespace sbi;
 
-static int maf_num_sms() { return sbi::dev_num_sms(); }
-
 static int maf_check(const sbi_maf_model* m) {
   if (!m || !m->d_params || !m->d_layer_tab || !m->d_perm_tab || !m->d_stats) return SBI_EINVAL;
   if (m->D < 1 || m->C < 1 || m->H < 1 || m->T < 1 || m->NB < 0 || m->NB > 8) return SBI_EINVAL;
@@ -546,42 +544,10 @@ static int maf_check(const sbi_maf_model* m) {
   if (m->Dp != round4(m->D) || m->Cp != round4(m->C) || m->Hp != round4(m->H) ||
       m->OUTp != round4(m->OUTM * m->D))
     return SBI_EINVAL;
-  if ((m->rpc0 & 3) || (m->rpc1 & 3) || (m->rpcf & 3) || m->rpc0 < 4 || m->rpc1 < 4 || m->rpcf < 4) return SBI_EINVAL;
-  if (m->nbuf < 2 || m->nbuf > 8) return SBI_EINVAL;
-  if (m->rpc0 * (m->Dp + m->Cp) > m->wcap || m->rpc1 * m->Hp > m->wcap || m->rpcf * m->Hp > m->wcap)
+  if (!ring_ok({{m->rpc0, m->Dp + m->Cp}, {m->rpc1, m->Hp}, {m->rpcf, m->Hp}, {4, m->Cp}, {4, m->Dp}}, m->nbuf,
+               m->wcap))
     return SBI_EINVAL;
-  if (4 * m->Cp > m->wcap || 4 * m->Dp > m->wcap) return SBI_EINVAL;
   return 0;
-}
-
-template <int ID, class K>
-static int maf_set_smem(K kernel, int bytes) {
-  static int granted_[sbi::kMaxDev] = {0};
-  int& granted = granted_[sbi::cur_dev()];
-  if (bytes > 227 * 1024) return SBI_ESMEM;
-  if (bytes <= granted) return 0;
-  cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
-  if (e != cudaSuccess) return (int)e;
-  granted = bytes;
-  return 0;
-}
-
-template <int ID, int TM, int RN, class KF>
-static int maf_launch_rows(KF kernel, const sbi_maf_model* m, const sbi_rows* rows, float* a, float* b,
-                           cudaStream_t s) {
-  const MafSmem L = maf_smem_layout(*m, TM, false);
-  int rc = maf_set_smem<ID>(kernel, L.total_bytes);
-  if (rc) return rc;
-  const int64_t ntiles = (rows->R + TM - 1) / TM;
-  const int per_sm = (L.total_bytes <= 110 * 1024) ? 2 : 1;
-  const int grid = (int)std::min<int64_t>(ntiles, (int64_t)maf_num_sms() * per_sm);
-  kernel<<<grid, kThreads, L.total_bytes, s>>>(*m, *rows, a, b);
-  return (int)cudaGetLastError();
-}
-
-// large batches take 64-row tiles when the model's 64-row layout fits, else stay on 32-row tiles
-static bool maf_big_tile(const sbi_maf_model* m, const sbi_rows* rows) {
-  return rows->R >= (int64_t)64 * sbi::dev_num_sms() * 2 && maf_smem_layout(*m, 64, false).total_bytes <= 227 * 1024;
 }
 
 extern "C" int sbi_b200_maf_logprob(const sbi_maf_model* m, const sbi_rows* rows, float* d_logp,
@@ -591,9 +557,14 @@ extern "C" int sbi_b200_maf_logprob(const sbi_maf_model* m, const sbi_rows* rows
   if (rc) return rc;
   if (!rows || !rows->d_input || !rows->d_cond || rows->R < 0 || !d_logp) return SBI_EINVAL;
   if (rows->R == 0) return 0;
-  if (maf_big_tile(m, rows))
-    return maf_launch_rows<0, 64, 4>(maf_logprob_kernel<64, 4>, m, rows, d_logp, d_noise, (cudaStream_t)stream);
-  return maf_launch_rows<1, 32, 2>(maf_logprob_kernel<32, 2>, m, rows, d_logp, d_noise, (cudaStream_t)stream);
+  cudaStream_t s = (cudaStream_t)stream;
+  const int bytes64 = maf_smem_layout(*m, 64, false).total_bytes;
+  if (use_64_rows(rows->R, bytes64))
+    return launch(maf_logprob_kernel<64, 4>, tile_grid(rows->R, 64, per_sm_110k(bytes64)), kThreads, bytes64, s,
+                  *m, *rows, d_logp, d_noise);
+  const int bytes = maf_smem_layout(*m, 32, false).total_bytes;
+  return launch(maf_logprob_kernel<32, 2>, tile_grid(rows->R, 32, per_sm_110k(bytes)), kThreads, bytes, s, *m,
+                *rows, d_logp, d_noise);
 }
 
 extern "C" int sbi_b200_maf_inverse(const sbi_maf_model* m, const sbi_rows* rows, float* d_out,
@@ -603,15 +574,17 @@ extern "C" int sbi_b200_maf_inverse(const sbi_maf_model* m, const sbi_rows* rows
   if (rc) return rc;
   if (!rows || !rows->d_input || !rows->d_cond || rows->R < 0 || !d_out) return SBI_EINVAL;
   if (rows->R == 0) return 0;
-  if (maf_big_tile(m, rows))
-    return maf_launch_rows<2, 64, 4>(maf_inverse_kernel<64, 4>, m, rows, d_out, d_logabsdet, (cudaStream_t)stream);
-  return maf_launch_rows<3, 32, 2>(maf_inverse_kernel<32, 2>, m, rows, d_out, d_logabsdet, (cudaStream_t)stream);
+  cudaStream_t s = (cudaStream_t)stream;
+  const int bytes64 = maf_smem_layout(*m, 64, false).total_bytes;
+  if (use_64_rows(rows->R, bytes64))
+    return launch(maf_inverse_kernel<64, 4>, tile_grid(rows->R, 64, per_sm_110k(bytes64)), kThreads, bytes64, s,
+                  *m, *rows, d_out, d_logabsdet);
+  const int bytes = maf_smem_layout(*m, 32, false).total_bytes;
+  return launch(maf_inverse_kernel<32, 2>, tile_grid(rows->R, 32, per_sm_110k(bytes)), kThreads, bytes, s, *m,
+                *rows, d_out, d_logabsdet);
 }
 
-extern "C" int sbi_b200_maf_vjp_parts(int64_t R) {
-  const int64_t ntiles = (R + 31) / 32;
-  return (int)std::max<int64_t>(1, std::min<int64_t>(ntiles, maf_num_sms()));
-}
+extern "C" int sbi_b200_maf_vjp_parts(int64_t R) { return vjp_parts(R, 32); }
 
 extern "C" int sbi_b200_maf_vjp(const sbi_maf_model* m, const sbi_rows* rows, const float* d_gout,
                                 float g_const, float* d_logp, float* d_gpart, float* d_ginput,
@@ -620,12 +593,7 @@ extern "C" int sbi_b200_maf_vjp(const sbi_maf_model* m, const sbi_rows* rows, co
   int rc = maf_check(m);
   if (rc) return rc;
   if (!rows || !rows->d_input || !rows->d_cond || rows->R < 1 || !d_gpart) return SBI_EINVAL;
-  constexpr int TM = 32;
-  const MafSmem L = maf_smem_layout(*m, TM, true);
-  auto k = maf_vjp_kernel<TM, 2, 2>;
-  if ((rc = maf_set_smem<4>(k, L.total_bytes))) return rc;
-  const int grid = sbi_b200_maf_vjp_parts(rows->R);
-  k<<<grid, kThreads, L.total_bytes, (cudaStream_t)stream>>>(*m, *rows, d_gout, g_const, d_logp, d_gpart,
-                                                           d_ginput, d_gcond, d_loss_acc);
-  return (int)cudaGetLastError();
+  return launch(maf_vjp_kernel<32, 2, 2>, sbi_b200_maf_vjp_parts(rows->R), kThreads,
+                maf_smem_layout(*m, 32, true).total_bytes, (cudaStream_t)stream, *m, *rows, d_gout, g_const, d_logp,
+                d_gpart, d_ginput, d_gcond, d_loss_acc);
 }

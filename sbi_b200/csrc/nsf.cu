@@ -12,15 +12,8 @@ namespace sbi {
 // =================================================================================================
 // log_prob:  persistent over row tiles
 // =================================================================================================
-#ifndef SBI_EVAL_MINB32
-#define SBI_EVAL_MINB32 2
-#endif
-#ifndef SBI_VJP_SINGLE_COND
-#define SBI_VJP_SINGLE_COND 0
-#endif
-
 template <int TM, int RN>
-__global__ void __launch_bounds__(kThreads, (TM > 64 ? 1 : (TM == 32 ? SBI_EVAL_MINB32 : 2)))
+__global__ void __launch_bounds__(kThreads, 2)
 nsf_logprob_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_constant__ sbi_rows rows,
                    float* __restrict__ logp, float* __restrict__ noise) {
   constexpr int LD = Tile<TM>::LD;
@@ -618,8 +611,6 @@ made_sample_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_constan
 // =================================================================================================
 using namespace sbi;
 
-static int num_sms() { return sbi::dev_num_sms(); }
-
 static int check_model(const sbi_nsf_model* m) {
   if (!m || !m->d_params || !m->d_layer_tab || !m->d_feat_tab || !m->d_stats) return SBI_EINVAL;
   if (m->D < 1 || m->C < 1 || m->H < 1 || m->T < 1 || m->KB < 2 || m->NB < 0) return SBI_EINVAL;
@@ -631,13 +622,8 @@ static int check_model(const sbi_nsf_model* m) {
   if (m->head == SBI_NSF_MOG && (m->M < 1 || m->M > kMogMax || m->T != 1 || !(m->mog_eps > 0.f))) return SBI_EINVAL;
   if (m->PR != (m->head == SBI_NSF_MOG ? round4(3 * m->M) : round4(3 * m->KB - 1)) || (m->IDp & 3) || m->nf_chunk < 1)
     return SBI_EINVAL;
-  if ((m->rpc0 & 3) || (m->rpc1 & 3) || (m->rpc2 & 3) || m->rpc0 < 4 || m->rpc1 < 4 || m->rpc2 < 4)
-    return SBI_EINVAL;
-  if (m->nbuf < 2 || m->nbuf > 8) return SBI_EINVAL;
-  // every chunk must fit a ring slot
-  const int K0p = m->Cp + m->IDp;
-  if (m->rpc0 * K0p > m->wcap || m->rpc1 * m->Hp > m->wcap ||
-      m->rpc2 * (m->Hp + m->Cp) > m->wcap || m->nf_chunk * m->PR * m->Hp > m->wcap)
+  if (!ring_ok({{m->rpc0, m->Cp + m->IDp}, {m->rpc1, m->Hp}, {m->rpc2, m->Hp + m->Cp}, {m->nf_chunk * m->PR, m->Hp}},
+               m->nbuf, m->wcap))
     return SBI_EINVAL;
   return 0;
 }
@@ -652,12 +638,6 @@ extern "C" int sbi_b200_device_ok(void) {
   return (p.major == 9 && p.minor == 0) ? 1 : 0;
 }
 
-// Large batches take TM-row tiles (TM = 64, or 128 on request) when the model's TM-row layout fits; a
-// model that only fits a 32-row tile evaluates every batch on 32-row tiles.
-static bool use_big_tile(const sbi_nsf_model& m, int64_t R, int TM) {
-  return R >= (int64_t)64 * sbi::dev_num_sms() * 2 && nsf_smem_layout(m, TM, false).total_bytes <= 227 * 1024;
-}
-
 extern "C" int sbi_b200_nsf_logprob(const sbi_nsf_model* m, const sbi_rows* rows, float* d_logp,
                                     float* d_noise, void* stream) {
   sbi::DeviceGuard dev_guard_(m ? m->d_params : nullptr);
@@ -666,37 +646,14 @@ extern "C" int sbi_b200_nsf_logprob(const sbi_nsf_model* m, const sbi_rows* rows
   if (!rows || !rows->d_input || !rows->d_cond || rows->R < 0 || !d_logp) return SBI_EINVAL;
   if (rows->R == 0) return 0;
   cudaStream_t s = (cudaStream_t)stream;
-  static const int tm_env = getenv("SBI_B200_LOGPROB_TM") ? atoi(getenv("SBI_B200_LOGPROB_TM")) : 0;
-  if (tm_env == 128 && use_big_tile(*m, rows->R, 128)) {
-    constexpr int TM = 128;
-    const NsfSmem L = nsf_smem_layout(*m, TM, false);
-    auto k = nsf_logprob_kernel<TM, 4>;
-    if ((rc = set_smem<5>(k, L.total_bytes))) return rc;
-    const int64_t ntiles = (rows->R + TM - 1) / TM;
-    const int grid = (int)std::min<int64_t>(ntiles, (int64_t)num_sms());
-    k<<<grid, kThreads, L.total_bytes, s>>>(*m, *rows, d_logp, d_noise);
-    return (int)cudaGetLastError();
-  }
-  if (tm_env != 32 && use_big_tile(*m, rows->R, 64)) {
-    constexpr int TM = 64;
-    const NsfSmem L = nsf_smem_layout(*m, TM, false);
-    auto k = nsf_logprob_kernel<TM, 4>;
-    if ((rc = set_smem<0>(k, L.total_bytes))) return rc;
-    const int64_t ntiles = (rows->R + TM - 1) / TM;
-    const int per_sm = (L.total_bytes <= 110 * 1024) ? 2 : 1;
-    const int grid = (int)std::min<int64_t>(ntiles, (int64_t)num_sms() * per_sm);
-    k<<<grid, kThreads, L.total_bytes, s>>>(*m, *rows, d_logp, d_noise);
-  } else {
-    constexpr int TM = 32;
-    const NsfSmem L = nsf_smem_layout(*m, TM, false);
-    auto k = nsf_logprob_kernel<TM, 2>;
-    if ((rc = set_smem<1>(k, L.total_bytes))) return rc;
-    const int64_t ntiles = (rows->R + TM - 1) / TM;
-    const int per_sm = std::max(1, std::min(SBI_EVAL_MINB32, (227 * 1024) / (L.total_bytes + 1024)));
-    const int grid = (int)std::min<int64_t>(ntiles, (int64_t)num_sms() * per_sm);
-    k<<<grid, kThreads, L.total_bytes, s>>>(*m, *rows, d_logp, d_noise);
-  }
-  return (int)cudaGetLastError();
+  const int bytes64 = nsf_smem_layout(*m, 64, false).total_bytes;
+  if (use_64_rows(rows->R, bytes64))
+    return launch(nsf_logprob_kernel<64, 4>, tile_grid(rows->R, 64, per_sm_110k(bytes64)), kThreads,
+                  bytes64, s, *m, *rows, d_logp, d_noise);
+  const int bytes = nsf_smem_layout(*m, 32, false).total_bytes;
+  const int per_sm = std::max(1, std::min(2, kMaxSmemBytes / (bytes + 1024)));
+  return launch(nsf_logprob_kernel<32, 2>, tile_grid(rows->R, 32, per_sm), kThreads, bytes, s, *m, *rows, d_logp,
+                d_noise);
 }
 
 extern "C" int sbi_b200_made_sample(const sbi_nsf_model* m, const sbi_rows* rows, const float* d_uniform,
@@ -707,15 +664,9 @@ extern "C" int sbi_b200_made_sample(const sbi_nsf_model* m, const sbi_rows* rows
   if (m->head != SBI_NSF_MOG) return SBI_EINVAL;
   if (!rows || !rows->d_input || !rows->d_cond || rows->R < 0 || !d_uniform || !d_out) return SBI_EINVAL;
   if (rows->R == 0) return 0;
-  constexpr int TM = 32;
-  const NsfSmem L = nsf_smem_layout(*m, TM, false);
-  auto k = made_sample_kernel<TM, 2>;
-  if ((rc = set_smem<8>(k, L.total_bytes))) return rc;
-  const int64_t ntiles = (rows->R + TM - 1) / TM;
-  const int per_sm = (L.total_bytes <= 110 * 1024) ? 2 : 1;
-  const int grid = (int)std::min<int64_t>(ntiles, (int64_t)num_sms() * per_sm);
-  k<<<grid, kThreads, L.total_bytes, (cudaStream_t)stream>>>(*m, *rows, d_uniform, d_out);
-  return (int)cudaGetLastError();
+  const int bytes = nsf_smem_layout(*m, 32, false).total_bytes;
+  return launch(made_sample_kernel<32, 2>, tile_grid(rows->R, 32, per_sm_110k(bytes)), kThreads, bytes,
+                (cudaStream_t)stream, *m, *rows, d_uniform, d_out);
 }
 
 extern "C" int sbi_b200_nsf_inverse(const sbi_nsf_model* m, const sbi_rows* rows, float* d_out,
@@ -726,33 +677,16 @@ extern "C" int sbi_b200_nsf_inverse(const sbi_nsf_model* m, const sbi_rows* rows
   if (!rows || !rows->d_input || !rows->d_cond || rows->R < 0 || !d_out) return SBI_EINVAL;
   if (rows->R == 0) return 0;
   cudaStream_t s = (cudaStream_t)stream;
-  if (use_big_tile(*m, rows->R, 64)) {
-    constexpr int TM = 64;
-    const NsfSmem L = nsf_smem_layout(*m, TM, false);
-    auto k = nsf_inverse_kernel<TM, 4>;
-    if ((rc = set_smem<2>(k, L.total_bytes))) return rc;
-    const int64_t ntiles = (rows->R + TM - 1) / TM;
-    const int per_sm = (L.total_bytes <= 110 * 1024) ? 2 : 1;
-    const int grid = (int)std::min<int64_t>(ntiles, (int64_t)num_sms() * per_sm);
-    k<<<grid, kThreads, L.total_bytes, s>>>(*m, *rows, d_out, d_logabsdet);
-  } else {
-    constexpr int TM = 32;
-    const NsfSmem L = nsf_smem_layout(*m, TM, false);
-    auto k = nsf_inverse_kernel<TM, 2>;
-    if ((rc = set_smem<3>(k, L.total_bytes))) return rc;
-    const int64_t ntiles = (rows->R + TM - 1) / TM;
-    const int per_sm = (L.total_bytes <= 110 * 1024) ? 2 : 1;
-    const int grid = (int)std::min<int64_t>(ntiles, (int64_t)num_sms() * per_sm);
-    k<<<grid, kThreads, L.total_bytes, s>>>(*m, *rows, d_out, d_logabsdet);
-  }
-  return (int)cudaGetLastError();
+  const int bytes64 = nsf_smem_layout(*m, 64, false).total_bytes;
+  if (use_64_rows(rows->R, bytes64))
+    return launch(nsf_inverse_kernel<64, 4>, tile_grid(rows->R, 64, per_sm_110k(bytes64)), kThreads,
+                  bytes64, s, *m, *rows, d_out, d_logabsdet);
+  const int bytes = nsf_smem_layout(*m, 32, false).total_bytes;
+  return launch(nsf_inverse_kernel<32, 2>, tile_grid(rows->R, 32, per_sm_110k(bytes)), kThreads, bytes, s,
+                *m, *rows, d_out, d_logabsdet);
 }
 
-extern "C" int sbi_b200_nsf_vjp_parts(int64_t R) {
-  constexpr int TM = 32;
-  const int64_t ntiles = (R + TM - 1) / TM;
-  return (int)std::max<int64_t>(1, std::min<int64_t>(ntiles, num_sms()));
-}
+extern "C" int sbi_b200_nsf_vjp_parts(int64_t R) { return vjp_parts(R, 32); }
 
 // Scratch for the activation spill of the VJP kernel: one slab per (CTA, layer), owned by the
 // library and grown on demand (old, smaller buffers stay allocated).  It cannot be (re)allocated while the stream is being captured into
@@ -790,31 +724,18 @@ extern "C" int sbi_b200_nsf_vjp(const sbi_nsf_model* m, const sbi_rows* rows, co
   if (!rows || !rows->d_input || !rows->d_cond || rows->R < 1 || !d_gpart) return SBI_EINVAL;
   cudaStream_t s = (cudaStream_t)stream;
   constexpr int TM = 32;
-  const NsfSmem L = nsf_smem_layout(*m, TM, true);
+  const int bytes = nsf_smem_layout(*m, TM, true).total_bytes;
   const int grid = sbi_b200_nsf_vjp_parts(rows->R);
-  if (L.total_bytes > 227 * 1024) {
+  if (bytes > kMaxSmemBytes) {
     // deep conditioners (`made`: five residual blocks) keep too many intermediates for a 32-row tile:
-    // 16-row tiles, per-layer recompute; every CTA walks its tiles and accumulates into its slab
-    constexpr int TS = 16;
-    const NsfSmem Ls = nsf_smem_layout(*m, TS, true);
-    auto k = nsf_vjp_kernel<TS, 2, 2, false>;
-    if ((rc = set_smem<7>(k, Ls.total_bytes))) return rc;
-    k<<<grid, kThreads, Ls.total_bytes, s>>>(*m, *rows, d_gout, g_const, d_logp, d_gpart, d_ginput, d_gcond,
-                                             d_loss_acc, nullptr);
-    return (int)cudaGetLastError();
+    // 16-row tiles, per-layer recompute; every CTA walks its tiles and accumulates into its slab (the grid keeps
+    // the 32-row part count: the caller sized its slabs from sbi_b200_nsf_vjp_parts)
+    return launch(nsf_vjp_kernel<16, 2, 2, false>, grid, kThreads, nsf_smem_layout(*m, 16, true).total_bytes, s, *m,
+                  *rows, d_gout, g_const, d_logp, d_gpart, d_ginput, d_gcond, d_loss_acc, nullptr);
   }
   const size_t slab = (size_t)((4 * m->NB + 1) * m->Hp + m->TRmax * m->PR) * (TM + 4);
-  float* scratch = vjp_scratch(sizeof(float) * slab * m->T * (size_t)num_sms(), s);
-  if (scratch != nullptr) {
-    auto k = nsf_vjp_kernel<TM, 2, 2, true>;
-    if ((rc = set_smem<4>(k, L.total_bytes))) return rc;
-    k<<<grid, kThreads, L.total_bytes, s>>>(*m, *rows, d_gout, g_const, d_logp, d_gpart, d_ginput,
-                                            d_gcond, d_loss_acc, scratch);
-  } else {
-    auto k = nsf_vjp_kernel<TM, 2, 2, false>;
-    if ((rc = set_smem<6>(k, L.total_bytes))) return rc;
-    k<<<grid, kThreads, L.total_bytes, s>>>(*m, *rows, d_gout, g_const, d_logp, d_gpart, d_ginput,
-                                            d_gcond, d_loss_acc, scratch);
-  }
-  return (int)cudaGetLastError();
+  float* scratch = vjp_scratch(sizeof(float) * slab * m->T * (size_t)dev_num_sms(), s);
+  auto k = scratch != nullptr ? nsf_vjp_kernel<TM, 2, 2, true> : nsf_vjp_kernel<TM, 2, 2, false>;
+  return launch(k, grid, kThreads, bytes, s, *m, *rows, d_gout, g_const, d_logp, d_gpart, d_ginput, d_gcond,
+                d_loss_acc, scratch);
 }

@@ -541,8 +541,6 @@ int store_args(StoreArgs* out) {
 // =================================================================================================
 using namespace sbi;
 
-static int tc_num_sms() { return sbi::dev_num_sms(); }
-
 extern "C" int sbi_b200_nsf_tc_supported(const sbi_nsf_model* m, const sbi_nsf_tc* tc) {
   sbi::DeviceGuard dev_guard_(m ? m->d_params : nullptr);
   if (!m || !tc) return 0;
@@ -558,11 +556,7 @@ extern "C" int sbi_b200_nsf_tc_supported(const sbi_nsf_model* m, const sbi_nsf_t
 
 extern "C" int sbi_b200_nsf_tc_pack(const sbi_nsf_model* m, const sbi_nsf_tc* tc, void* stream) {
   sbi::DeviceGuard dev_guard_(m ? m->d_params : nullptr);
-  if (!m || !tc || !m->d_params || !tc->d_src || !tc->d_tcw || tc->n_words <= 0) return SBI_EINVAL;
-  const int threads = 256, blocks = (tc->n_words + threads - 1) / threads;
-  tc::tc_pack_kernel<<<blocks, threads, 0, (cudaStream_t)stream>>>(m->d_params, tc->d_src,
-                                                                       tc->d_tcw, tc->n_words);
-  return (int)cudaGetLastError();
+  return m ? tc::pack_weights(m->d_params, tc, (cudaStream_t)stream) : SBI_EINVAL;
 }
 
 extern "C" int sbi_b200_nsf_logprob_tc(const sbi_nsf_model* m, const sbi_nsf_tc* tc,
@@ -576,25 +570,18 @@ extern "C" int sbi_b200_nsf_logprob_tc(const sbi_nsf_model* m, const sbi_nsf_tc*
   if (rows->R == 0) return 0;
   tc::StoreArgs sa;
   if (int e = tc::store_args(&sa)) return e;
-  const tc::TcSmem L = tc::tc_smem_layout(*m, tc->stage_cap);
-  auto k = tc::nsf_logprob_tc_kernel<50, 10, false>;
-  if (int e = sbi::set_smem<0>(k, L.total_bytes)) return e;
-  const int64_t ntiles = (rows->R + tc::kRows - 1) / tc::kRows;
-  const int grid = (int)std::min<int64_t>(ntiles, (int64_t)tc_num_sms() * 2);
-  k<<<grid, tc::kThreads, L.total_bytes, (cudaStream_t)stream>>>(*m, *tc, *rows, d_logp, d_noise, nullptr, sa);
-  return (int)cudaGetLastError();
+  return launch(tc::nsf_logprob_tc_kernel<50, 10, false>, tile_grid(rows->R, tc::kRows, 2), tc::kThreads,
+                tc::tc_smem_layout(*m, tc->stage_cap).total_bytes, (cudaStream_t)stream, *m, *tc, *rows, d_logp,
+                d_noise, nullptr, sa);
 }
 
 int sbi::tc::launch_forward_save(const sbi_nsf_model* m, const sbi_nsf_tc* tc, const sbi_rows* rows, float* d_logp,
                                  float* d_save, cudaStream_t s) {
   tc::StoreArgs sa;
   if (int e = tc::store_args(&sa)) return e;
-  const tc::TcSmem L = tc::tc_smem_layout(*m, tc->stage_cap);
-  auto k = tc::nsf_logprob_tc_kernel<50, 10, false, true>;
-  if (int e = sbi::set_smem<1>(k, L.total_bytes)) return e;
   const int grid = (int)((rows->R + tc::kRows - 1) / tc::kRows);      // one tile per CTA: `d_save` slab = blockIdx
-  k<<<grid, tc::kThreads, L.total_bytes, s>>>(*m, *tc, *rows, d_logp, nullptr, d_save, sa);
-  return (int)cudaGetLastError();
+  return launch(tc::nsf_logprob_tc_kernel<50, 10, false, true>, grid, tc::kThreads,
+                tc::tc_smem_layout(*m, tc->stage_cap).total_bytes, s, *m, *tc, *rows, d_logp, nullptr, d_save, sa);
 }
 
 extern "C" int sbi_b200_nsf_inverse_tc(const sbi_nsf_model* m, const sbi_nsf_tc* tc,
@@ -608,13 +595,9 @@ extern "C" int sbi_b200_nsf_inverse_tc(const sbi_nsf_model* m, const sbi_nsf_tc*
   if (rows->R == 0) return 0;
   tc::StoreArgs sa;
   if (int e = tc::store_args(&sa)) return e;
-  const tc::TcSmem L = tc::tc_smem_layout(*m, tc->stage_cap);
-  auto k = tc::nsf_logprob_tc_kernel<50, 10, true>;
-  if (int e = sbi::set_smem<2>(k, L.total_bytes)) return e;
-  const int64_t ntiles = (rows->R + tc::kRows - 1) / tc::kRows;
-  const int grid = (int)std::min<int64_t>(ntiles, (int64_t)tc_num_sms() * 2);
-  k<<<grid, tc::kThreads, L.total_bytes, (cudaStream_t)stream>>>(*m, *tc, *rows, d_logabsdet, d_out, nullptr, sa);
-  return (int)cudaGetLastError();
+  return launch(tc::nsf_logprob_tc_kernel<50, 10, true>, tile_grid(rows->R, tc::kRows, 2), tc::kThreads,
+                tc::tc_smem_layout(*m, tc->stage_cap).total_bytes, (cudaStream_t)stream, *m, *tc, *rows, d_logabsdet,
+                d_out, nullptr, sa);
 }
 
 #ifdef SBI_TC_TIMELINE

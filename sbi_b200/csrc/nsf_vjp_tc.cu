@@ -705,7 +705,7 @@ static int vjp_tc_ok(const sbi_nsf_model* m, const sbi_nsf_tc* tcf, const sbi_ns
   if (!tcb || !tcb->d_tab || !tcb->d_tcw || tcb->stage_cap <= 0 || (tcb->stage_cap & 31)) return 0;
   if (m->IDp > 16 || m->Cp + m->IDp + 1 > 64 || m->Cp + 1 > 64) return 0;
   const tc::BwdSmem L = tc::bwd_smem_layout(tcb->stage_cap, tc::bwd_ldmax(*m));
-  return L.total_bytes <= 227 * 1024 ? 1 : 0;
+  return L.total_bytes <= kMaxSmemBytes ? 1 : 0;
 }
 
 extern "C" int sbi_b200_nsf_vjp_tc_supported(const sbi_nsf_model* m, const sbi_nsf_tc* tc_fwd,
@@ -723,10 +723,7 @@ extern "C" int sbi_b200_nsf_vjp_tc_cond_supported(const sbi_nsf_model* m, const 
 // rows of one forward + backward launch pair (one tile per CTA, every SM busy once)
 static int64_t vjp_tc_chunk_rows() { return (int64_t)tc::kRows * sbi::dev_num_sms(); }
 
-extern "C" int sbi_b200_nsf_vjp_tc_parts(int64_t R) {
-  const int64_t ntiles = (R + tc::kRows - 1) / tc::kRows;
-  return (int)std::max<int64_t>(1, std::min<int64_t>(ntiles, sbi::dev_num_sms()));
-}
+extern "C" int sbi_b200_nsf_vjp_tc_parts(int64_t R) { return vjp_parts(R, tc::kRows); }
 
 extern "C" int64_t sbi_b200_nsf_vjp_tc_save_bytes(const sbi_nsf_model* m, int64_t R) {
   if (!m || R < 1) return 0;
@@ -745,9 +742,9 @@ static int vjp_tc_launch(const sbi_nsf_model* m, const sbi_nsf_tc* tc_fwd, const
   if (!vjp_tc_ok(m, tc_fwd, tc_bwd)) return SBI_ESMEM;
   if (save_bytes < sbi_b200_nsf_vjp_tc_save_bytes(m, rows->R)) return SBI_EINVAL;
   cudaStream_t s = (cudaStream_t)stream;
-  const tc::BwdSmem Lb = tc::bwd_smem_layout(tc_bwd->stage_cap, tc::bwd_ldmax(*m));
-  auto kb = tc::nsf_vjp_tc_kernel<50, 10, COND>;
-  if (int e = sbi::set_smem<COND ? 1 : 0>(kb, Lb.total_bytes)) return e;
+  const int bwd_bytes = tc::bwd_smem_layout(tc_bwd->stage_cap, tc::bwd_ldmax(*m)).total_bytes;
+  // opt the backward kernel in before anything is launched: a failed opt-in leaves no forward sweep behind
+  if (int e = set_smem(reinterpret_cast<const void*>(tc::nsf_vjp_tc_kernel<50, 10, COND>), bwd_bytes)) return e;
   // chunks of one tile per SM: forward sweep (saves activations) then backward sweep of the same rows;
   // later chunks accumulate into the partial-gradient slabs
   tc::StoreArgs sa;
@@ -762,13 +759,13 @@ static int vjp_tc_launch(const sbi_nsf_model* m, const sbi_nsf_tc* tc_fwd, const
       if (!rows->cond_shared) rr.d_cond = rows->d_cond + r0 * m->C;
     }
     const int grid = (int)((rr.R + tc::kRows - 1) / tc::kRows);
-    const int rc = tc::launch_forward_save(m, tc_fwd, &rr, d_logp ? d_logp + r0 : nullptr, d_save, s);
-    if (rc) return rc;
-    kb<<<grid, tc::kThreads, Lb.total_bytes, s>>>(*m, *tc_bwd, rr, d_gout ? d_gout + r0 : nullptr, g_const,
-                                                  d_gpart, d_loss_acc, d_save, r0 > 0 ? 1 : 0, sa,
-                                                  COND ? d_gcond + r0 * m->C : nullptr);
+    if (int rc = tc::launch_forward_save(m, tc_fwd, &rr, d_logp ? d_logp + r0 : nullptr, d_save, s)) return rc;
+    if (int rc = launch(tc::nsf_vjp_tc_kernel<50, 10, COND>, grid, tc::kThreads, bwd_bytes, s, *m, *tc_bwd, rr,
+                        d_gout ? d_gout + r0 : nullptr, g_const, d_gpart, d_loss_acc, d_save, r0 > 0 ? 1 : 0, sa,
+                        COND ? d_gcond + r0 * m->C : nullptr))
+      return rc;
   }
-  return (int)cudaGetLastError();
+  return 0;
 }
 
 extern "C" int sbi_b200_nsf_vjp_tc(const sbi_nsf_model* m, const sbi_nsf_tc* tc_fwd, const sbi_nsf_tc* tc_bwd,

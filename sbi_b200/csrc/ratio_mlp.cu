@@ -341,10 +341,8 @@ static int ratio_mlp_check(const sbi_ratio_mlp_model* m) {
   if (m->norm != SBI_RM_NORM_NONE && m->norm != SBI_RM_NORM_LAYER) return SBI_EINVAL;
   if (m->norm == SBI_RM_NORM_LAYER && !(m->ln_eps > 0.f)) return SBI_EINVAL;
   if (m->Dtp != round4(m->Dt) || m->Dxp != round4(m->Dx) || m->Hp != round4(m->H)) return SBI_EINVAL;
-  if ((m->rpc0 & 3) || (m->rpc1 & 3) || m->rpc0 < 4 || m->rpc1 < 4 || m->nbuf < 2 || m->nbuf > 8) return SBI_EINVAL;
   const int K0p = m->Dtp + m->Dxp;
-  if (m->rpc0 * K0p > m->wcap || m->rpc1 * m->Hp > m->wcap || 4 * (m->NL > 0 ? m->Hp : K0p) > m->wcap)
-    return SBI_EINVAL;
+  if (!ring_ok({{m->rpc0, K0p}, {m->rpc1, m->Hp}, {4, m->NL > 0 ? m->Hp : K0p}}, m->nbuf, m->wcap)) return SBI_EINVAL;
   return 0;
 }
 
@@ -356,32 +354,16 @@ extern "C" int sbi_b200_ratio_mlp_forward(const sbi_ratio_mlp_model* m, const sb
   if (!pairs || !pairs->d_theta || !pairs->d_x || pairs->R < 0 || !d_logits) return SBI_EINVAL;
   if (pairs->R == 0) return 0;
   cudaStream_t s = (cudaStream_t)stream;
-  const int sms = sbi::dev_num_sms();
-  // large batches take 64-row tiles when the model's 64-row layout fits, else stay on 32-row tiles
-  if (pairs->R >= (int64_t)64 * sms * 2 && mlp_smem_layout(*m, 64, false).total_bytes <= 227 * 1024) {
-    constexpr int TM = 64;
-    const MlpSmem L = mlp_smem_layout(*m, TM, false);
-    auto k = ratio_mlp_forward_kernel<TM, 4>;
-    if ((rc = set_smem<0>(k, L.total_bytes))) return rc;
-    const int64_t ntiles = (pairs->R + TM - 1) / TM;
-    const int per_sm = (L.total_bytes <= 110 * 1024) ? 2 : 1;
-    k<<<(int)std::min<int64_t>(ntiles, (int64_t)sms * per_sm), kThreads, L.total_bytes, s>>>(*m, *pairs, d_logits);
-  } else {
-    constexpr int TM = 32;
-    const MlpSmem L = mlp_smem_layout(*m, TM, false);
-    auto k = ratio_mlp_forward_kernel<TM, 2>;
-    if ((rc = set_smem<1>(k, L.total_bytes))) return rc;
-    const int64_t ntiles = (pairs->R + TM - 1) / TM;
-    const int per_sm = (L.total_bytes <= 110 * 1024) ? 2 : 1;
-    k<<<(int)std::min<int64_t>(ntiles, (int64_t)sms * per_sm), kThreads, L.total_bytes, s>>>(*m, *pairs, d_logits);
-  }
-  return (int)cudaGetLastError();
+  const int bytes64 = mlp_smem_layout(*m, 64, false).total_bytes;
+  if (use_64_rows(pairs->R, bytes64))
+    return launch(ratio_mlp_forward_kernel<64, 4>, tile_grid(pairs->R, 64, per_sm_110k(bytes64)), kThreads, bytes64,
+                  s, *m, *pairs, d_logits);
+  const int bytes = mlp_smem_layout(*m, 32, false).total_bytes;
+  return launch(ratio_mlp_forward_kernel<32, 2>, tile_grid(pairs->R, 32, per_sm_110k(bytes)), kThreads, bytes, s,
+                *m, *pairs, d_logits);
 }
 
-extern "C" int sbi_b200_ratio_mlp_vjp_parts(int64_t R) {
-  const int64_t ntiles = (R + 31) / 32;
-  return (int)std::max<int64_t>(1, std::min<int64_t>(ntiles, sbi::dev_num_sms()));
-}
+extern "C" int sbi_b200_ratio_mlp_vjp_parts(int64_t R) { return vjp_parts(R, 32); }
 
 extern "C" int sbi_b200_ratio_mlp_vjp(const sbi_ratio_mlp_model* m, const sbi_pairs* pairs, const float* d_gout,
                                       float* d_logits, float* d_gpart, float* d_gtheta, void* stream) {
@@ -389,11 +371,7 @@ extern "C" int sbi_b200_ratio_mlp_vjp(const sbi_ratio_mlp_model* m, const sbi_pa
   int rc = ratio_mlp_check(m);
   if (rc) return rc;
   if (!pairs || !pairs->d_theta || !pairs->d_x || pairs->R < 1 || !d_gpart || !d_gout) return SBI_EINVAL;
-  constexpr int TM = 32;
-  const MlpSmem L = mlp_smem_layout(*m, TM, true);
-  auto k = ratio_mlp_vjp_kernel<TM, 2, 2>;
-  if ((rc = set_smem<2>(k, L.total_bytes))) return rc;
-  const int grid = sbi_b200_ratio_mlp_vjp_parts(pairs->R);
-  k<<<grid, kThreads, L.total_bytes, (cudaStream_t)stream>>>(*m, *pairs, d_gout, d_logits, d_gpart, d_gtheta);
-  return (int)cudaGetLastError();
+  return launch(ratio_mlp_vjp_kernel<32, 2, 2>, sbi_b200_ratio_mlp_vjp_parts(pairs->R), kThreads,
+                mlp_smem_layout(*m, 32, true).total_bytes, (cudaStream_t)stream, *m, *pairs, d_gout, d_logits, d_gpart,
+                d_gtheta);
 }

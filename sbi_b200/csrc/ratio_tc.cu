@@ -196,8 +196,6 @@ ratio_forward_tc_kernel(const __grid_constant__ sbi_ratio_model m, const __grid_
 
 using namespace sbi;
 
-static int rtc_num_sms() { return sbi::dev_num_sms(); }
-
 extern "C" int sbi_b200_ratio_tc_supported(const sbi_ratio_model* m, const sbi_nsf_tc* tc) {
   sbi::DeviceGuard dev_guard_(m ? m->d_params : nullptr);
   if (!m || !tc) return 0;
@@ -210,11 +208,7 @@ extern "C" int sbi_b200_ratio_tc_supported(const sbi_ratio_model* m, const sbi_n
 
 extern "C" int sbi_b200_ratio_tc_pack(const sbi_ratio_model* m, const sbi_nsf_tc* tc, void* stream) {
   sbi::DeviceGuard dev_guard_(m ? m->d_params : nullptr);
-  if (!m || !tc || !m->d_params || !tc->d_src || !tc->d_tcw || tc->n_words <= 0) return SBI_EINVAL;
-  const int threads = 256, blocks = (tc->n_words + threads - 1) / threads;
-  tc::tc_pack_kernel<<<blocks, threads, 0, (cudaStream_t)stream>>>(m->d_params, tc->d_src, tc->d_tcw,
-                                                                   tc->n_words);
-  return (int)cudaGetLastError();
+  return m ? tc::pack_weights(m->d_params, tc, (cudaStream_t)stream) : SBI_EINVAL;
 }
 
 extern "C" int sbi_b200_ratio_forward_tc(const sbi_ratio_model* m, const sbi_nsf_tc* tc,
@@ -224,13 +218,9 @@ extern "C" int sbi_b200_ratio_forward_tc(const sbi_ratio_model* m, const sbi_nsf
   if (!tc->d_tab || !tc->d_tcw) return SBI_EINVAL;
   if (!sbi_b200_ratio_tc_supported(m, tc)) return SBI_ESMEM;
   if (pairs->R == 0) return 0;
-  const tc::RatioTcSmem L = tc::ratio_tc_smem_layout(*m, tc->stage_cap);
   tc::StoreArgs sa;
   if (int e = tc::store_args(&sa)) return e;
-  auto k = tc::ratio_forward_tc_kernel<50>;
-  if (int e = sbi::set_smem<0>(k, L.total_bytes)) return e;
-  const int64_t ntiles = (pairs->R + tc::kRows - 1) / tc::kRows;
-  const int grid = (int)std::min<int64_t>(ntiles, (int64_t)rtc_num_sms() * 2);
-  k<<<grid, tc::kThreads, L.total_bytes, (cudaStream_t)stream>>>(*m, *tc, *pairs, d_logits, sa);
-  return (int)cudaGetLastError();
+  return launch(tc::ratio_forward_tc_kernel<50>, tile_grid(pairs->R, tc::kRows, 2), tc::kThreads,
+                tc::ratio_tc_smem_layout(*m, tc->stage_cap).total_bytes, (cudaStream_t)stream, *m, *tc, *pairs,
+                d_logits, sa);
 }

@@ -325,6 +325,14 @@ static __global__ void tc_pack_kernel(const float* __restrict__ params, const in
   tcw[i] = v;
 }
 
+// host: re-pack `params` into the operand blocks of `tc`; returns a C-ABI status code
+static int pack_weights(const float* params, const sbi_nsf_tc* tc, cudaStream_t s) {
+  if (!params || !tc || !tc->d_src || !tc->d_tcw || tc->n_words <= 0) return SBI_EINVAL;
+  const int threads = 256, blocks = (tc->n_words + threads - 1) / threads;
+  tc_pack_kernel<<<blocks, threads, 0, s>>>(params, tc->d_src, tc->d_tcw, tc->n_words);
+  return (int)cudaGetLastError();
+}
+
 // ---- the kernel ------------------------------------------------------------------------------------
 // Every thread runs begin / block / end: the MMAs of a stage take both warpgroups and are complete
 // once end() returns.  The weight stream rotates between the warps (stage k is fetched by the
