@@ -499,6 +499,18 @@ int sbi_b200_reject_compact(const float* d_cand, int32_t D, const float* d_log_t
                             const float* d_u, int64_t n, int64_t index_base, float* d_out, int64_t* d_out_idx,
                             int64_t cap, int32_t* d_count, int32_t* d_scratch, void* stream);
 
+/* ---- sampling-importance-resampling: one categorical draw per group of K proposals (csrc/compact.cu; reference
+ * sbi/samplers/importance/sir.py:59-63).  Candidates are (groups*K, D) rows; per group g, lw_k = log_target_k -
+ * log_proposal_k (fp32), w = softmax(lw), and the selected candidate is the first k with cumsum(w)_k >= u_g.  A
+ * group selects nothing when its softmax is NaN (a NaN or +inf log weight, or all -inf) or when the cumulative
+ * weights never reach u_g.  Selected rows are appended, in group order, at d_out[*d_count ...] (rows past `cap`
+ * are dropped but counted), their global group indices (index_base + g) at d_out_idx (optional); *d_count is
+ * advanced on the device.  d_scratch: sbi_b200_sir_scratch_ints(groups) int32. */
+int64_t sbi_b200_sir_scratch_ints(int64_t groups);
+int sbi_b200_sir_select(const float* d_cand, int32_t D, const float* d_log_target, const float* d_log_proposal,
+                        const float* d_u, int64_t groups, int32_t K, int64_t index_base, float* d_out,
+                        int64_t* d_out_idx, int64_t cap, int32_t* d_count, int32_t* d_scratch, void* stream);
+
 /* ---- multi-GPU: gradient sum over NVLink peer memory (csrc/peer.cu), replacing the NCCL all-reduce +
  * norm pass of the data-parallel step (reference semantics: clip_grad_norm_ + Adam on the summed
  * gradient, sbi/inference/trainers/base.py:1181-1187).  Each rank allocates a symmetric buffer

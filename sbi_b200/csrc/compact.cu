@@ -102,6 +102,95 @@ __global__ void scatter_kernel(const float* __restrict__ cand, int D, const floa
   }
 }
 
+// ---- sampling-importance-resampling: one categorical draw per group of K candidates ----------------------------
+// (/root/reference/sbi/samplers/importance/sir.py:59-63: `w = softmax(lw).cumsum(-1); mask = cumsum(w >= u) == 1;
+// thetas.reshape(b, K, D)[mask]`).  One warp per group, kGroups groups per block; lanes walk the group in
+// 32-candidate chunks, so any K >= 1 works.  The select kernel writes the chosen index of every group (-1: none)
+// and the block's selection count; scan_kernel above turns the counts into output offsets; the scatter kernel
+// copies the selected rows.
+constexpr int kGroups = kThreads / 32;        // groups per block
+
+__device__ __forceinline__ float log_weight(const float* lt, const float* lp, int64_t i) {
+  return lt[i] - lp[i];                       // fp32 subtraction, as importance_sample computes it
+}
+
+__global__ void sir_select_kernel(const float* __restrict__ lt, const float* __restrict__ lp,
+                                  const float* __restrict__ u, int64_t groups, int K, int32_t* __restrict__ sel,
+                                  int32_t* __restrict__ block_count) {
+  __shared__ int sh[kGroups];
+  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+  const int64_t g = (int64_t)blockIdx.x * kGroups + w;
+  int pick = -1;
+  if (g < groups) {
+    const int64_t row0 = g * K;
+    // pass 1: max; a NaN or +inf anywhere (or all -inf) makes torch's softmax NaN, which selects nothing
+    float m = -INFINITY;
+    bool bad = false;
+    for (int k0 = 0; k0 < K; k0 += 32) {
+      const int k = k0 + lane;
+      if (k < K) {
+        const float v = log_weight(lt, lp, row0 + k);
+        bad |= isnan(v) || v == INFINITY;
+        m = fmaxf(m, v);
+      }
+    }
+    for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
+    bad = __any_sync(0xffffffffu, bad) || m == -INFINITY;
+    if (!bad) {
+      // pass 2: softmax denominator
+      float s = 0.f;
+      for (int k0 = 0; k0 < K; k0 += 32) {
+        const int k = k0 + lane;
+        if (k < K) s += expf(log_weight(lt, lp, row0 + k) - m);
+      }
+      for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+      // pass 3: inclusive cumulative weights in index order; the first k with cumw_k >= u_g
+      const float ug = u[g];
+      float carry = 0.f;
+      for (int k0 = 0; k0 < K; k0 += 32) {
+        const int k = k0 + lane;
+        float c = k < K ? expf(log_weight(lt, lp, row0 + k) - m) / s : 0.f;
+        for (int o = 1; o < 32; o <<= 1) {
+          const float t = __shfl_up_sync(0xffffffffu, c, o);
+          if (lane >= o) c += t;
+        }
+        c += carry;
+        const unsigned hit = __ballot_sync(0xffffffffu, k < K && c >= ug);
+        if (hit) {
+          pick = k0 + __ffs(hit) - 1;
+          break;
+        }
+        carry = __shfl_sync(0xffffffffu, c, 31);
+      }
+    }
+    if (lane == 0) sel[g] = pick;
+  }
+  if (lane == 0) sh[w] = pick >= 0 ? 1 : 0;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    int t = 0;
+    for (int j = 0; j < kGroups; ++j) t += sh[j];
+    block_count[blockIdx.x] = t;
+  }
+}
+
+__global__ void sir_scatter_kernel(const float* __restrict__ cand, int D, int64_t groups, int K, int64_t index_base,
+                                   const int32_t* __restrict__ sel, const int32_t* __restrict__ block_off,
+                                   float* __restrict__ out, int64_t* __restrict__ out_idx, int64_t cap) {
+  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+  const int64_t g0 = (int64_t)blockIdx.x * kGroups;
+  const int64_t g = g0 + w;
+  const int pick = g < groups ? sel[g] : -1;
+  if (pick < 0) return;
+  // groups before this one in the block that selected a row (warps own consecutive groups: warp order = group order)
+  int64_t pos = block_off[blockIdx.x];
+  for (int j = 0; j < w; ++j) pos += (g0 + j < groups && sel[g0 + j] >= 0) ? 1 : 0;
+  if (pos >= cap) return;
+  const float* src = cand + (g * K + pick) * (int64_t)D;
+  for (int d = lane; d < D; d += 32) out[pos * D + d] = src[d];
+  if (lane == 0 && out_idx != nullptr) out_idx[pos] = index_base + g;
+}
+
 }  // namespace compact
 }  // namespace sbi
 
@@ -128,5 +217,34 @@ extern "C" int sbi_b200_reject_compact(const float* d_cand, int32_t D, const flo
   compact::scan_kernel<<<1, compact::kThreads, 0, s>>>(d_scratch, nb, d_count);
   compact::scatter_kernel<<<nb, compact::kThreads, 0, s>>>(d_cand, D, d_log_target, d_log_scaled, d_u, n, index_base,
                                                          d_scratch, d_out, d_out_idx, cap);
+  return (int)cudaGetLastError();
+}
+
+// scratch: one count per block of kGroups groups, then the selected index of every group
+extern "C" int64_t sbi_b200_sir_scratch_ints(int64_t groups) {
+  if (groups < 1) return 1;
+  return (groups + compact::kGroups - 1) / compact::kGroups + groups;
+}
+
+extern "C" int sbi_b200_sir_select(const float* d_cand, int32_t D, const float* d_log_target,
+                                   const float* d_log_proposal, const float* d_u, int64_t groups, int32_t K,
+                                   int64_t index_base, float* d_out, int64_t* d_out_idx, int64_t cap,
+                                   int32_t* d_count, int32_t* d_scratch, void* stream) {
+  if (!d_cand || !d_log_target || !d_log_proposal || !d_u || !d_out || !d_count || !d_scratch || D < 1 || K < 1 ||
+      groups < 0 || cap < 0)
+    return SBI_EINVAL;
+  sbi::DeviceGuard dev_guard_(d_cand);
+  if (groups == 0) return 0;
+  const int64_t nb64 = (groups + compact::kGroups - 1) / compact::kGroups;
+  if (nb64 > (1 << 30) || groups > INT64_MAX / K) return SBI_EINVAL;
+  const int nb = (int)nb64;
+  int32_t* block_count = d_scratch;
+  int32_t* sel = d_scratch + nb;
+  cudaStream_t s = (cudaStream_t)stream;
+  compact::sir_select_kernel<<<nb, compact::kThreads, 0, s>>>(d_log_target, d_log_proposal, d_u, groups, K, sel,
+                                                               block_count);
+  compact::scan_kernel<<<1, compact::kThreads, 0, s>>>(block_count, nb, d_count);
+  compact::sir_scatter_kernel<<<nb, compact::kThreads, 0, s>>>(d_cand, D, groups, K, index_base, sel, block_count,
+                                                                d_out, d_out_idx, cap);
   return (int)cudaGetLastError();
 }

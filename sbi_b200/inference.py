@@ -529,9 +529,10 @@ class _PotentialPosterior:
 
     def build_posterior(self, density_estimator=None, prior=None, sample_with: str = "mcmc",
                         mcmc_method: str = "slice_np_vectorized", mcmc_parameters: Optional[dict] = None,
-                        rejection_sampling_parameters: Optional[dict] = None, **kwargs):
-        """nle_base.py:274-378, nre_base.py:311-394 (`sample_with` in {"mcmc", "rejection"})."""
-        from .posteriors import MCMCPosterior, RejectionPosterior
+                        rejection_sampling_parameters: Optional[dict] = None,
+                        importance_sampling_parameters: Optional[dict] = None, **kwargs):
+        """nle_base.py:274-378, nre_base.py:311-394 (`sample_with` in {"mcmc", "rejection", "importance"})."""
+        from .posteriors import ImportanceSamplingPosterior, MCMCPosterior, RejectionPosterior
         est = deepcopy(density_estimator if density_estimator is not None else self._neural_net)
         prior = prior if prior is not None else self._prior
         potential_fn, theta_transform = self._potential(est, prior)
@@ -541,6 +542,9 @@ class _PotentialPosterior:
         if sample_with == "rejection":
             return RejectionPosterior(potential_fn, proposal=prior, device=self._device,
                                       **(rejection_sampling_parameters or {}))
+        if sample_with == "importance":   # trainers/base.py:1045-1053
+            return ImportanceSamplingPosterior(potential_fn, proposal=prior, device=self._device,
+                                               **(importance_sampling_parameters or {}))
         raise NotImplementedError(sample_with)
 
 
@@ -821,12 +825,19 @@ class NPE(_FlowTrainer):
                              dataloader_kwargs=dataloader_kwargs)
 
     def build_posterior(self, density_estimator: Optional[nn.Module] = None, prior=None,
-                        sample_with: str = "direct", **kwargs):
-        from .posteriors import DirectPosterior
-        if sample_with != "direct":
-            raise NotImplementedError("NPE.build_posterior supports sample_with='direct'")
+                        sample_with: str = "direct", importance_sampling_parameters: Optional[dict] = None,
+                        **kwargs):
+        """npe_base.py:425-509 (`sample_with` in {"direct", "importance"})."""
+        from .posteriors import DirectPosterior, ImportanceSamplingPosterior
+        if sample_with not in ("direct", "importance"):
+            raise NotImplementedError("NPE.build_posterior supports sample_with='direct' and 'importance'")
         est = density_estimator if density_estimator is not None else self._neural_net
         prior = prior if prior is not None else self._prior
+        if sample_with == "importance":
+            from .potentials import posterior_estimator_based_potential
+            potential_fn, _ = posterior_estimator_based_potential(deepcopy(est).to(self._device), prior)
+            return ImportanceSamplingPosterior(potential_fn, proposal=prior, device=self._device,
+                                               **(importance_sampling_parameters or {}))
         return DirectPosterior(deepcopy(est), prior, device=self._device)
 
 

@@ -583,6 +583,150 @@ class RejectionPosterior:
                                  track_gradients=track_gradients)
 
 
+class ImportanceSamplingPosterior:
+    """/root/reference/sbi/inference/posteriors/importance_posterior.py:18-380: samples by sampling-importance-
+    resampling from `proposal` (`method="sir"`), or returns the proposal draws with their log importance weights
+    (`method="importance"`); `log_prob` is the potential minus an importance-sampled log normalising constant.
+    The SIR selection runs in csrc/compact.cu (`samplers.sampling_importance_resampling`)."""
+
+    def __init__(self, potential_fn, proposal, theta_transform=None, method: str = "sir",
+                 oversampling_factor: int = 32, max_sampling_batch_size: int = 10_000,
+                 device: Optional[str] = None, x_shape=None):
+        self.potential_fn = potential_fn
+        self._device = device or potential_fn.device
+        self.proposal = prior_to_device(proposal, self._device)
+        self.theta_transform = theta_transform
+        self.method = method
+        self.oversampling_factor = oversampling_factor
+        self.max_sampling_batch_size = max_sampling_batch_size
+        self._normalization_constant = None
+        self._map = None
+        self.default_x = None
+
+    def set_default_x(self, x: Tensor):
+        self.default_x = self._batch_x(x)
+        self._normalization_constant = None     # the cached estimate belongs to the old default x
+        self._map = None
+        return self
+
+    def _batch_x(self, x) -> Tensor:
+        x = torch.as_tensor(x, dtype=torch.float32).to(self._device)
+        return x.unsqueeze(0) if x.dim() < 2 else x
+
+    def _x_else_default_x(self, x):
+        if x is not None:
+            return self._batch_x(x)
+        if self.default_x is None:
+            raise ValueError("Context `x` needed when a default has not been set."
+                             "If you'd like to have a default, use the `.set_default_x()` method.")
+        return self.default_x
+
+    def log_prob(self, theta: Tensor, x: Optional[Tensor] = None, track_gradients: bool = False,
+                 normalization_constant_params: Optional[dict] = None) -> Tensor:
+        """importance_posterior.py:109-149: potential(theta) - log Z(x)."""
+        x = self._x_else_default_x(x)
+        self.potential_fn.set_x(x)
+        theta = torch.as_tensor(theta)
+        if theta.dim() == 1:
+            theta = theta.unsqueeze(0)
+        with torch.set_grad_enabled(track_gradients):
+            potential_values = self.potential_fn(theta.to(self._device), track_gradients=track_gradients)
+            normalization_constant = self.estimate_normalization_constant(x, **(normalization_constant_params or {}))
+            return (potential_values - torch.log(normalization_constant)).to(self._device)
+
+    @torch.no_grad()
+    def estimate_normalization_constant(self, x: Tensor, num_samples: int = 10_000,
+                                        force_update: bool = False) -> Tensor:
+        """importance_posterior.py:151-185: Z = mean(exp(log w)) over `num_samples` proposal draws; kept only at
+        the default x (recomputed with `force_update`), computed unsaved at any other x."""
+        from .samplers import importance_sample
+        is_new_x = self.default_x is None or (x is not self.default_x and (x != self.default_x).any())
+        if is_new_x:
+            _, log_importance_weights = importance_sample(self.potential_fn, proposal=self.proposal,
+                                                          num_samples=num_samples)
+            return torch.mean(torch.exp(log_importance_weights))
+        if self._normalization_constant is None or force_update:
+            _, log_importance_weights = importance_sample(self.potential_fn, proposal=self.proposal,
+                                                          num_samples=num_samples)
+            self._normalization_constant = torch.mean(torch.exp(log_importance_weights))
+        return self._normalization_constant.to(self._device)
+
+    def sample(self, sample_shape=torch.Size(), x: Optional[Tensor] = None, method: Optional[str] = None,
+               oversampling_factor: int = 32, max_sampling_batch_size: int = 10_000,
+               show_progress_bars: bool = False) -> Union[Tensor, Tuple[Tensor, Tensor]]:
+        """importance_posterior.py:187-228.  As in the reference, `sample`'s own defaults are passed on: the
+        constructor's `oversampling_factor` / `max_sampling_batch_size` apply only when the caller passes None."""
+        method = self.method if method is None else method
+        self.potential_fn.set_x(self._x_else_default_x(x))
+        if method == "sir":
+            return self._sir_sample(sample_shape, oversampling_factor=oversampling_factor,
+                                    max_sampling_batch_size=max_sampling_batch_size,
+                                    show_progress_bars=show_progress_bars)
+        elif method == "importance":
+            return self._importance_sample(sample_shape)
+        else:
+            raise NameError
+
+    def sample_batched(self, sample_shape, x: Tensor, max_sampling_batch_size: int = 10_000,
+                       show_progress_bars: bool = True) -> Tensor:
+        """importance_posterior.py:230-241: not implemented, so batched callers fall back to one `sample` per x."""
+        raise NotImplementedError(
+            "Batched sampling is not implemented for ImportanceSamplingPosterior. \
+           Alternatively you can use `sample` in a loop \
+           [posterior.sample(theta, x_o) for x_o in x]."
+        )
+
+    def _importance_sample(self, sample_shape=torch.Size(), show_progress_bars: bool = False) -> Tuple[Tensor, Tensor]:
+        from .samplers import importance_sample
+        num_samples = torch.Size(sample_shape).numel()
+        samples, log_importance_weights = importance_sample(self.potential_fn, proposal=self.proposal,
+                                                            num_samples=num_samples,
+                                                            show_progress_bars=show_progress_bars)
+        samples = samples.reshape((*sample_shape, -1)).to(self._device)
+        return samples, log_importance_weights.to(self._device)
+
+    def _sir_sample(self, sample_shape=torch.Size(), oversampling_factor: Optional[int] = 32,
+                    max_sampling_batch_size: Optional[int] = 10_000, show_progress_bars: bool = False) -> Tensor:
+        from .samplers import sampling_importance_resampling
+        oversampling_factor = self.oversampling_factor if oversampling_factor is None else oversampling_factor
+        max_sampling_batch_size = (self.max_sampling_batch_size if max_sampling_batch_size is None
+                                   else max_sampling_batch_size)
+        num_samples = torch.Size(sample_shape).numel()
+        samples = sampling_importance_resampling(
+            self.potential_fn, proposal=self.proposal, num_samples=num_samples,
+            num_candidate_samples=oversampling_factor, show_progress_bars=show_progress_bars,
+            max_sampling_batch_size=max_sampling_batch_size, device=self._device)
+        return samples.reshape((*sample_shape, -1)).to(self._device)
+
+    def map(self, x: Optional[Tensor] = None, num_iter: int = 1_000, num_to_optimize: int = 100,
+            learning_rate: float = 0.01, init_method: Union[str, Tensor] = "proposal", num_init_samples: int = 1_000,
+            save_best_every: int = 10, show_progress_bars: bool = False, force_update: bool = False) -> Tensor:
+        """importance_posterior.py:315-380 -> base_posterior.py:216-323: gradient ascent on the potential from
+        the best of `num_init_samples` starting points; gradients come from the estimator kernels' VJP."""
+        from .samplers import gradient_ascent
+        if x is not None:
+            raise ValueError("Passing `x` directly to `.map()` has been deprecated."
+                             "Use `.self_default_x()` to set `x`, and then run `.map()` ")
+        if self.default_x is None:
+            raise ValueError("Default `x` has not been set."
+                             "To set the default, use the `.set_default_x()` method.")
+        if self._map is None or force_update:
+            self.potential_fn.set_x(self.default_x)
+            if isinstance(init_method, str) and init_method == "posterior":
+                inits = self.sample((num_init_samples,))
+            elif isinstance(init_method, str) and init_method == "proposal":
+                inits = self.proposal.sample((num_init_samples,))
+            elif isinstance(init_method, Tensor):
+                inits = init_method.to(self._device)
+            else:
+                raise ValueError
+            self._map = gradient_ascent(potential_fn=self.potential_fn, inits=inits,
+                                        theta_transform=self.theta_transform, num_iter=num_iter,
+                                        num_to_optimize=num_to_optimize, learning_rate=learning_rate,
+                                        save_best_every=save_best_every, show_progress_bars=show_progress_bars)[0]
+        return self._map
+
+
 class VectorFieldPosterior:
     """Posterior of a flow-matching estimator sampled by integrating its ODE or its reverse SDE
     (reference: /root/reference/sbi/inference/posteriors/vector_field_posterior.py: sample :155-329,

@@ -9,6 +9,8 @@
   `gradient_ascent` search for max(potential - log q) (sbiutils.py:1160-1285); the acceptance
   uniforms are drawn with the CPU generator and uploaded, exactly as the reference does (:178), so
   accepted-index sets are comparable.
+* `importance_sample` / `sampling_importance_resampling` -- importance_sampling.py:11-37 and sir.py:13-71; the SIR
+  selection and compaction is one kernel sequence (`sbi_b200_sir_select`).
 * `resample_given_potential_fn` / `sir_init` -- init strategies of
   /root/reference/sbi/samplers/mcmc/init_strategy.py:37-114.
 """
@@ -284,6 +286,67 @@ def rejection_sample(potential_fn: Callable, proposal: Any, theta_transform: Opt
     if return_indices:
         return samples, torch.as_tensor(acceptance_rate), out_idx
     return samples, torch.as_tensor(acceptance_rate)
+
+
+def _proposal_draws(proposal: Any, num_samples: int, show_progress_bars: bool) -> Tensor:
+    try:   # multi-round proposals take a progress-bar argument, torch distributions do not
+        return proposal.sample((num_samples,), show_progress_bar=show_progress_bars)
+    except TypeError:
+        return proposal.sample((num_samples,))
+
+
+def importance_sample(potential_fn: Callable, proposal: Any, num_samples: int = 1,
+                      show_progress_bars: bool = False) -> Tuple[Tensor, Tensor]:
+    """importance_sampling.py:11-37: proposal draws and their log importance weights, potential - log q."""
+    samples = _proposal_draws(proposal, num_samples, show_progress_bars)
+    potential_logprobs = potential_fn(samples)
+    proposal_logprobs = proposal.log_prob(samples)
+    log_importance_weights = potential_logprobs - proposal_logprobs
+    return samples, log_importance_weights
+
+
+def sampling_importance_resampling(potential_fn: Callable, proposal: Any, num_samples: int = 1,
+                                   num_candidate_samples: int = 32, max_sampling_batch_size: int = 10_000,
+                                   show_progress_bars: bool = False, device: str = "cuda", **kwargs: Any) -> Tensor:
+    """sir.py:13-71: every posterior sample is one categorical draw, by importance weight, among
+    `num_candidate_samples` proposal draws.  The proposal, potential and uniform draws are the reference's own
+    calls in its order, so a seed gives the reference's candidates and uniforms; the softmax, cumulative weights,
+    decision and compaction are one kernel sequence (csrc/compact.cu) appending the selected rows to a device
+    buffer, where the reference's boolean indexing synchronises through `nonzero`.  The host reads the running
+    count once per batch."""
+    dev = torch.device(device)
+    if dev.type != "cuda":
+        raise RuntimeError(f"sampling_importance_resampling selects on a CUDA device, got device={device!r} "
+                           "(no CPU fallback)")
+    lib = L.load()
+    K = int(num_candidate_samples)
+    sampling_batch_size = min(num_samples, max_sampling_batch_size)
+    num_remaining = num_samples
+    out = count = None
+    total = groups_done = 0
+    with torch.no_grad():
+        while num_remaining > 0:
+            batch_size = min(sampling_batch_size, num_remaining)
+            thetas = _proposal_draws(proposal, batch_size * K, show_progress_bars)
+            log_target = potential_fn(thetas)
+            log_proposal = proposal.log_prob(thetas)
+            uniform_decision = torch.rand(batch_size, 1, device=device)
+            cand = thetas.reshape(batch_size * K, -1).to(dev).float().contiguous()
+            if out is None:
+                out = torch.empty(num_samples, cand.shape[1], dtype=torch.float32, device=dev)
+                count = torch.zeros(1, dtype=torch.int32, device=dev)
+            scratch = torch.empty(int(lib.sbi_b200_sir_scratch_ints(batch_size)), dtype=torch.int32, device=dev)
+            lt = log_target.reshape(-1).to(dev).float().contiguous()
+            lq = log_proposal.reshape(-1).to(dev).float().contiguous()
+            u = uniform_decision.reshape(-1).to(dev).float().contiguous()
+            L.check(lib.sbi_b200_sir_select(
+                cand.data_ptr(), cand.shape[1], lt.data_ptr(), lq.data_ptr(), u.data_ptr(), batch_size, K,
+                groups_done, out.data_ptr(), None, num_samples, count.data_ptr(), scratch.data_ptr(),
+                L.stream_ptr()), "sir_select")
+            groups_done += batch_size
+            total = int(count.item())
+            num_remaining = num_samples - total
+    return out[:total]
 
 
 def resample_given_potential_fn(proposal: Any, potential_fn: Callable, transform: torch_tf.Transform,
