@@ -511,6 +511,63 @@ int sbi_b200_sir_select(const float* d_cand, int32_t D, const float* d_log_targe
                         const float* d_u, int64_t groups, int32_t K, int64_t index_base, float* d_out,
                         int64_t* d_out_idx, int64_t cap, int32_t* d_count, int32_t* d_scratch, void* stream);
 
+/* ---- L-C2ST classifiers (csrc/lc2st.cu; reference sbi/diagnostics/lc2st.py with scikit-learn's
+ * MLPClassifier(solver="adam", activation="relu")).  A network maps F = dim_theta + dim_x inputs through L ReLU
+ * hidden layers to one logistic output p = P(class 1).  Parameters are packed per model in sklearn's order:
+ * coefs_[0] (F x H[0], row-major), intercepts_[0], coefs_[1], intercepts_[1], ..., coefs_[L] (H[L-1] x 1),
+ * intercepts_[L]; P counts them.  Envelope: F <= SBI_LC2ST_MAX_F, 1 <= L <= SBI_LC2ST_MAX_HIDDEN, every width
+ * <= SBI_LC2ST_MAX_WIDTH, and the model's weights and gradient fit one CTA's shared memory with 8-row tiles
+ * (sbi_b200_lc2st_plan returns SBI_ESMEM otherwise). */
+#define SBI_LC2ST_MAX_HIDDEN 4
+#define SBI_LC2ST_MAX_F 64
+#define SBI_LC2ST_MAX_WIDTH 256
+typedef struct {
+  int32_t F, L;
+  int32_t H[SBI_LC2ST_MAX_HIDDEN];
+  int32_t P;
+} sbi_lc2st_net;
+
+/* sklearn's hyperparameters.  batch_size < 1 selects min(200, n_train); the float fields are the float32 values
+ * numpy applies (one_minus_beta* = float32(1 - beta) computed in float64), the double fields the Python floats. */
+typedef struct {
+  int32_t max_iter, n_iter_no_change, early_stopping, shuffle, batch_size;
+  float beta1, beta2, one_minus_beta1, one_minus_beta2, eps, alpha;
+  double lr_d, beta1_d, beta2_d, tol;
+} sbi_lc2st_opt;
+
+/* One model of a training launch.  Its samples are entries row0 .. row0 + n_train + n_val - 1 of d_rows (pairs
+ * (theta row, x row) of the shared tables) and d_labels (0 or 1): the n_train training samples, then the n_val
+ * validation samples.  Epoch `e` visits training sample d_order[order0 + e * n_train + i] at position i, or, with
+ * order0 < 0, a keyed bijection of [0, n_train) drawn from (key, e) on the device (identity when !shuffle). */
+typedef struct {
+  int64_t row0;
+  int32_t n_train, n_val;
+  int64_t order0;
+  uint64_t key;
+} sbi_lc2st_job;
+
+/* out3 = {training tile rows, evaluation tile rows, padded parameter count}; SBI_ESMEM when a model does not fit. */
+int sbi_b200_lc2st_plan(const sbi_lc2st_net* net, int32_t* out3);
+/* floats of the training workspace of M models (Adam moments and best weights) */
+int64_t sbi_b200_lc2st_ws_floats(const sbi_lc2st_net* net, int32_t M);
+/* Train M models to completion in one launch (one CTA each).  d_params (M, P): initial parameters in, final ones
+ * out (the best-validation ones when early_stopping).  Per model: d_n_iter = n_iter_, d_val_curve /
+ * d_loss_curve (M, max_iter) float64 = validation accuracy / epoch loss per epoch run, d_best = the best
+ * validation score (early stopping) or the best loss. */
+int sbi_b200_lc2st_train(const sbi_lc2st_net* net, const sbi_lc2st_opt* opt, const sbi_lc2st_job* d_jobs, int32_t M,
+                         const float* d_theta, int32_t dt, const float* d_x, int32_t dx, const int32_t* d_rows,
+                         const float* d_labels, const int32_t* d_order, float* d_params, float* d_ws,
+                         int32_t* d_n_iter, double* d_val_curve, double* d_loss_curve, double* d_best, void* stream);
+/* row chunks of an evaluation over S rows (the length of d_part per classifier) */
+int sbi_b200_lc2st_eval_chunks(const sbi_lc2st_net* net, int64_t S);
+/* Evaluate C classifiers of E consecutive parameter sets each (d_params: (C*E, P)) on S rows [theta_s, x]: theta
+ * from d_theta (G, S, dt) at block d_group[c] (block 0 when d_group is NULL), x = d_x (dx) for every row.
+ * d_prob (C, S) = mean over members of 1 - p; d_score (C) = sum_s (prob - 0.5)^2 / S in float64; d_part:
+ * (C, sbi_b200_lc2st_eval_chunks(net, S)) doubles of scratch. */
+int sbi_b200_lc2st_eval(const sbi_lc2st_net* net, const float* d_params, int32_t C, int32_t E, const float* d_theta,
+                        int32_t dt, int64_t S, const int32_t* d_group, const float* d_x, int32_t dx, float* d_prob,
+                        double* d_part, double* d_score, void* stream);
+
 /* ---- multi-GPU: gradient sum over NVLink peer memory (csrc/peer.cu), replacing the NCCL all-reduce +
  * norm pass of the data-parallel step (reference semantics: clip_grad_norm_ + Adam on the summed
  * gradient, sbi/inference/trainers/base.py:1181-1187).  Each rank allocates a symmetric buffer

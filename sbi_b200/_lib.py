@@ -146,6 +146,30 @@ class TrainWs(C.Structure):
     ]
 
 
+SBI_LC2ST_MAX_HIDDEN = 4
+SBI_LC2ST_MAX_F = 64
+SBI_LC2ST_MAX_WIDTH = 256
+
+
+class Lc2stNet(C.Structure):
+    _fields_ = [("F", C.c_int32), ("L", C.c_int32), ("H", C.c_int32 * SBI_LC2ST_MAX_HIDDEN), ("P", C.c_int32)]
+
+
+class Lc2stOpt(C.Structure):
+    _fields_ = [
+        ("max_iter", C.c_int32), ("n_iter_no_change", C.c_int32), ("early_stopping", C.c_int32),
+        ("shuffle", C.c_int32), ("batch_size", C.c_int32),
+        ("beta1", C.c_float), ("beta2", C.c_float), ("one_minus_beta1", C.c_float), ("one_minus_beta2", C.c_float),
+        ("eps", C.c_float), ("alpha", C.c_float),
+        ("lr_d", C.c_double), ("beta1_d", C.c_double), ("beta2_d", C.c_double), ("tol", C.c_double),
+    ]
+
+
+class Lc2stJob(C.Structure):
+    _fields_ = [("row0", C.c_int64), ("n_train", C.c_int32), ("n_val", C.c_int32), ("order0", C.c_int64),
+                ("key", C.c_uint64)]
+
+
 class PeerCtx(C.Structure):
     _fields_ = [("h_peer_ptrs", C.c_void_p), ("world", C.c_int), ("rank", C.c_int), ("d_grad_local", C.c_void_p)]
 
@@ -217,6 +241,16 @@ _EXPORTS = {
     "sbi_b200_sir_select": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64,
                                       C.c_int32, C.c_int64, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p,
                                       C.c_void_p, C.c_void_p]),
+    "sbi_b200_lc2st_plan": (C.c_int, [C.POINTER(Lc2stNet), C.POINTER(C.c_int32)]),
+    "sbi_b200_lc2st_ws_floats": (C.c_int64, [C.POINTER(Lc2stNet), C.c_int32]),
+    "sbi_b200_lc2st_train": (C.c_int, [C.POINTER(Lc2stNet), C.POINTER(Lc2stOpt), C.c_void_p, C.c_int32,
+                                       C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p,
+                                       C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                       C.c_void_p, C.c_void_p]),
+    "sbi_b200_lc2st_eval_chunks": (C.c_int, [C.POINTER(Lc2stNet), C.c_int64]),
+    "sbi_b200_lc2st_eval": (C.c_int, [C.POINTER(Lc2stNet), C.c_void_p, C.c_int32, C.c_int32, C.c_void_p,
+                                      C.c_int32, C.c_int64, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p,
+                                      C.c_void_p, C.c_void_p, C.c_void_p]),
     "sbi_b200_ode_red_size": (C.c_int, [C.c_int64]),
     "sbi_b200_ode_stage": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_int32, C.c_void_p,
                                      C.c_void_p]),

@@ -13,6 +13,16 @@ from typing import Callable, List, Optional, Tuple, Union
 import torch
 from torch import Tensor
 
+_LC2ST_NAMES = ("LC2ST", "LC2ST_NF", "LC2STScores", "LC2STState")
+
+
+def __getattr__(name):
+    """The local test (`sbi_b200.lc2st`) on first use: it needs scikit-learn, SBC and TARP do not."""
+    if name in _LC2ST_NAMES:
+        from . import lc2st
+        return getattr(lc2st, name)
+    raise AttributeError(f"module {__name__!r} has no attribute {name!r}")
+
 
 def _clean(thetas: Tensor, xs: Tensor) -> Tuple[Tensor, Tensor]:
     """remove_nans_and_infs_in_x (utils/diagnostics_utils.py:101-120)."""
