@@ -79,8 +79,8 @@ __host__ __device__ inline TcSmem tc_smem_layout(const sbi_nsf_model& m, int sta
 //
 // SAVE = true (training forward, INV = false): every layer's conditioner intermediates, raw spline
 // parameters, layer input and coupling output of the tile go to the activation scratch `save`
-// (layout: nsf_tc_save.cuh) for the tensor-core backward kernel (nsf_vjp_tc.cu), together with the
-// final base-space point and the row's log-density.
+// (layout: nsf_tc_save.cuh) for the tensor-core backward and weight-gradient kernels (nsf_vjp_tc.cu),
+// together with the final base-space point and the row's log-density.
 template <int H, int KB, bool INV, bool SAVE = false>
 __global__ void __launch_bounds__(kThreads, 2)
 nsf_logprob_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_constant__ sbi_nsf_tc tc,

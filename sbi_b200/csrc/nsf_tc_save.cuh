@@ -1,6 +1,7 @@
 // Activation scratch shared by the tensor-core training kernels: the forward sweep
-// (nsf_logprob_tc_kernel<.., SAVE = true>, nsf_tc.cu) writes it, the backward sweep
-// (nsf_vjp_tc_kernel, nsf_vjp_tc.cu) reads it.  One slab per 128-row tile:
+// (nsf_logprob_tc_kernel<.., SAVE = true>, nsf_tc.cu) writes the activations, the backward sweep
+// (nsf_vjp_tc_kernel, nsf_vjp_tc.cu) reads them and writes the output gradients dY, the weight-gradient
+// kernel (nsf_dw_tc_kernel, nsf_vjp_tc.cu) reads both.  One slab per 128-row tile:
 //
 //   per layer l (layer_stride floats):
 //     for each residual block b:  h_b | a1_b | t2_b | s_b     each [128 rows][64 columns]
@@ -10,6 +11,10 @@
 //     hf   = input of the final layer                         [128][64]
 //     prm  = raw spline parameters incl. bias                 [128][TRmax][32]
 //     zin  = layer input z_l,  v = coupling output (LULinear input)   each [128][16]
+//     dy   = output gradients dY of the layer's linears, written by the backward sweep and read by the
+//            weight-gradient kernel (nsf_dw_tc_kernel)        [128][64 npm + 192 NB + 64]:
+//            final-layer pass p (features 2p, 2p+1: 32 parameter rows each) at column 64p (npm passes),
+//            block b: dG (GLU context linear) | dT (W2) | dA (W1) at 64 npm + 192b, then dh (initial linear)
 //   then per tile:  zt = base-space point z_T [128][16],  lp = log q [128]
 //
 // Every array of a slab is stored as float4 groups with the ROW index fastest: group g of row r sits at
@@ -29,7 +34,8 @@ namespace tc {
 
 struct TcSave {
   int NB;
-  int hf, prm, zin, v;        // float offsets inside a layer slab
+  int npm;                    // final-layer passes of the widest layer, (TRmax + 1) / 2
+  int hf, prm, zin, v, dy;    // float offsets inside a layer slab
   int layer_stride;
   int zt, lp;                 // float offsets inside a tile slab (after the T layer slabs)
   int64_t tile_stride;
@@ -37,16 +43,22 @@ struct TcSave {
   __host__ __device__ int a1(int b) const { return (4 * b + 1) * 64 * 128; }
   __host__ __device__ int t2(int b) const { return (4 * b + 2) * 64 * 128; }
   __host__ __device__ int s(int b) const { return (4 * b + 3) * 64 * 128; }
+  // dY of final-layer pass p, of linear k (0: GLU context, 1: W2, 2: W1) of block b, of the initial linear
+  __host__ __device__ int dy_fin(int p) const { return dy + 64 * p * 128; }
+  __host__ __device__ int dy_blk(int b, int k) const { return dy + (64 * npm + 192 * b + 64 * k) * 128; }
+  __host__ __device__ int dy_init() const { return dy + (64 * npm + 192 * NB) * 128; }
 };
 
 __host__ __device__ inline TcSave tc_save_layout(int NB, int TRmax, int T) {
   TcSave L;
   L.NB = NB;
+  L.npm = (TRmax + 1) / 2;
   L.hf = 4 * NB * 64 * 128;
   L.prm = L.hf + 64 * 128;
   L.zin = L.prm + TRmax * 32 * 128;
   L.v = L.zin + 16 * 128;
-  L.layer_stride = L.v + 16 * 128;
+  L.dy = L.v + 16 * 128;
+  L.layer_stride = L.dy + (64 * L.npm + 192 * NB + 64) * 128;
   L.zt = T * L.layer_stride;
   L.lp = L.zt + 16 * 128;
   L.tile_stride = (int64_t)L.lp + 128;

@@ -5,37 +5,40 @@
 // for the parameter gradients, on the activations the tensor-core forward sweep
 // (nsf_logprob_tc_kernel<..., SAVE = true>, nsf_tc.cu) left in the activation scratch
 // (nsf_tc_save.cuh).  Replaces nsf_vjp_kernel (nsf.cu, FP32 SIMT) when only parameter gradients
-// are asked for -- the trainer's case.
+// are asked for -- the trainer's case.  Two kernels per chunk of rows, after the forward sweep:
 //
-// One CTA = 8 warps owns a tile of 128 rows (row = store lane, two threads per row splitting the
-// columns), walks the layers T-1 .. 0 and, per layer, the linears of the conditioner
-// (nflows ResidualNet, restated in oracle/nflows_port/nn/nets/resnet.py) in reverse:
+// nsf_vjp_tc_kernel: the chain of the backward sweep, which each layer waits on.  One CTA = 8 warps owns a
+// tile of 128 rows (row = store lane, two threads per row splitting the columns), walks the layers
+// T-1 .. 0 and, per layer, the linears of the conditioner (nflows ResidualNet, restated in
+// oracle/nflows_port/nn/nets/resnet.py) in reverse:
 //
 //   * input-gradient chain  dX = dY W  on wgmma kind tf32 (both warpgroups, 64 rows each): A = dY from
 //     the accumulator store of tc_common.cuh (written
 //     by the row threads, 3xTF32 hi/lo split), B = W^T streamed by TMA bulk copies from the
 //     pre-transposed operand blocks (pack.NsfLayout.tc_bwd_plan) through a 2-slot ring; relu / GLU
-//     masks, the spline backward (rqs.cuh) and the LULinear backward are per-thread code on the
-//     thread's own row between the MMAs;
+//     masks, the spline backward (rqs.cuh) and the LULinear backward (with its parameter gradients) are
+//     per-thread code on the thread's own row between the MMAs;
+//   * the output gradient dY of every linear goes to the dY region of the activation scratch, where the
+//     weight-gradient kernel picks it up;
 //   * COND instantiation only: the condition gradient d(sum g log q)/d ctx in raw condition space, accumulated
 //     per row over the T layers from the context columns of the initial layer (dh W0[:, :C]) and the GLU
-//     context layer of every residual block (dG Wc).  dh / dG of the whole row sit in the staged weight-gradient
-//     operand (A') once it is handed over, so each of the row's two threads takes half of the C features over
-//     all H columns, on the CUDA cores from the fp32 parameters (C is small next to H), and accumulates them in
-//     place in d_gcond: every entry has one owner thread and a fixed summation order.  No shared memory is
-//     added, so the parameter-only layout and plan serve both instantiations;
-//   * weight gradients  dW = dY^T X  (K = the 128 rows of the tile) on the same tensor core with BOTH
-//     operands from shared memory: the row threads write dY^T and X^T into K-major staging buffers
-//     ([row/4][feature][row%4], one padding row per slab so that the 32 rows of a warp hit 32 banks),
-//     one M = 64 MMA chain of 16 K-steps per linear (single TF32 pass: the sum over rows averages the
-//     operand rounding; the two warpgroups split N), accumulators stored in the accumulator store,
-//     read back by the 16 lanes per warp that hold them and written to this CTA's partial-gradient
-//     slab; a ones row appended to X^T yields the bias gradient in the same MMA.  Staging buffers and
-//     accumulators are double buffered; every MMA completes before the code after it runs.
+//     context layer of every residual block (dG Wc).  dh / dG of the whole row are read back from the dY region
+//     after the CTA barrier that follows their write, so each of the row's two threads takes half of the C
+//     features over all H columns, on the CUDA cores from the fp32 parameters (C is small next to H), and
+//     accumulates them in place in d_gcond: every entry has one owner thread and a fixed summation order.
 //
-// Store columns (512): [0,64) A_hi | [64,128) A_lo | [128,192) D | [192,256) G |
-//                     [256,320) A2_hi | [320,384) A2_lo (second A set: spline passes alternate) |
-//                     [384,448) dW slot 0 | [448,512) dW slot 1
+// nsf_dw_tc_kernel: the weight gradients  dW = dY^T X  (K = the 128 rows of a tile), which no layer waits on,
+// so they run on every SM instead of the one SM per tile of the chain.  One CTA per (tile, layer, linear):
+// the row threads write dY^T (dY region) and X^T (saved activations, the context, the identity features)
+// into K-major staging buffers ([row/4][feature][row%4], one padding row per slab so that the 32 rows of a
+// warp hit 32 banks) and one M = 64 MMA chain of 16 K-steps multiplies them (single TF32 pass: the sum over
+// rows averages the operand rounding; the two warpgroups split N); a ones row appended to X^T yields the bias
+// gradient in the same MMA.  The accumulators are written into a shared-memory image laid out like the block
+// in the parameter buffer, and ONE thread sends it to the tile's partial-gradient slab with two TMA bulk
+// copies (a reducing copy for every chunk after the first).
+//
+// Store columns of the backward (384): [0,64) A_hi | [64,128) A_lo | [128,192) D | [192,256) G |
+//                                      [256,320) A2_hi | [320,384) A2_lo (second A set: spline passes alternate)
 #include <cuda_runtime.h>
 #include <math.h>
 #include <algorithm>
@@ -52,39 +55,42 @@ namespace sbi {
 namespace tc {
 
 constexpr int kBwdSlots = 2;
-constexpr int kBwdCols = 512;
+constexpr int kBwdCols = 384;
 static_assert(kBwdCols <= kStoreCols, "one CTA's columns must fit one slab");
 constexpr int cA2 = 256;
-constexpr int cW = 384;
 constexpr int kStLd = 65;                       // feature rows per K-slab of a staging buffer (64 + 1 pad)
 constexpr int kStFloats = 32 * kStLd * 4;       // [128 rows / 4][65][4]
 
 struct BwdSmem {
-  int dz, ctx, gr, lum, stg, obuf, ring;   // float offsets
+  int dz, gr, lum, lus, ring;   // float offsets
   int bar_bytes, total_bytes;
 };
-// ldmax: longest packed weight row (floats) of the model, max(Hp, Cp + IDp, Cp)
-__host__ __device__ inline BwdSmem bwd_smem_layout(int stage_cap, int ldmax) {
+__host__ __device__ inline BwdSmem bwd_smem_layout(int stage_cap) {
   BwdSmem L;
   int fl = 0;
   L.dz = fl;  fl += 16 * kRows;
-  L.ctx = fl; fl += 16 * kRows;
   L.gr = fl;  fl += kRows;
   L.lum = fl; fl += 2 * kLuMax * kLuMax + 2 * kLuMax;
   fl = (fl + 31) & ~31;
-  L.stg = fl; fl += 4 * kStFloats;               // [A'0 | B'0 | A'1 | B'1]
-  fl = (fl + 31) & ~31;
-  L.obuf = fl; fl += 64 * ldmax + 64;            // one weight-gradient block [<= 64 rows][ld] + its bias row
+  L.lus = fl; fl += 3 * kLuMax * kRows;          // LULinear backward: v | y | dy, feature-major
   fl = (fl + 31) & ~31;
   L.ring = fl; fl += kBwdSlots * stage_cap;
   L.bar_bytes = fl * 4;
-  L.total_bytes = L.bar_bytes + (kBwdSlots + 1) * 8;
+  L.total_bytes = L.bar_bytes + kBwdSlots * 8;
   return L;
 }
-__host__ __device__ inline int bwd_ldmax(const sbi_nsf_model& m) {
+// ldmax: longest packed weight row (floats) of the model, max(Hp, Cp + IDp, Cp)
+__host__ __device__ inline int dw_ldmax(const sbi_nsf_model& m) {
   int a = m.Hp > m.Cp + m.IDp ? m.Hp : m.Cp + m.IDp;
   return a > m.Cp ? a : m.Cp;
 }
+// weight-gradient kernel: staging buffers A' | B', then the output image [<= 64 rows][ld] + its bias row
+__host__ __device__ inline int dw_smem_bytes(const sbi_nsf_model& m) {
+  return (2 * kStFloats + 64 * dw_ldmax(m) + 64) * 4;
+}
+// work units of the weight-gradient kernel per (tile, layer): the final-layer passes, three linears per
+// residual block (GLU context, W2, W1), the initial linear
+__host__ __device__ inline int dw_units(const sbi_nsf_model& m) { return (m.TRmax + 1) / 2 + 3 * m.NB + 1; }
 
 // where the accumulators of one weight-gradient MMA go in the partial-gradient slab
 struct DwGeo {
@@ -94,31 +100,146 @@ struct DwGeo {
   int Mv, N;       // rows of the block incl. zero padding rows (Mv % 4 == 0); accumulator columns (multiple of 16)
 };
 
-// accumulators of one weight-gradient MMA (M = 64: rows 16q .. 16q+15 sit in lanes 32q .. 32q+15, mma_ss64)
-// -> the shared-memory image of the block, laid out exactly like the block in the parameter buffer
-// ([Mv][ldw] weights, then the Mv bias entries), from where ONE thread sends it to the CTA's
-// partial-gradient slab with two TMA bulk copies (coalesced, asynchronous; scattered per-lane global
-// stores of the same data cost 1.3 us per weight gradient).  Columns >= nX of a row are padding and take
-// a zero gradient.  One copy of the code for all call sites (the kernel is instruction-fetch bound).
-__device__ __noinline__ void dw_read_fn(uint32_t row, uint32_t col, const DwGeo g, float* obuf, int mrow, int col0,
-                                        bool holds_rows) {
-  if (col0 >= g.N) return;                          // warp-uniform
-  float v[32];
-  ld_cols<4>(row, col + col0, v);
-  if (holds_rows && mrow < g.Mv) {
-    float4* orow = reinterpret_cast<float4*>(obuf + mrow * g.ldw + col0);
-    float bv = 0.f;
+// dW = A'^T-staged dY (M = 64 feature rows) x B'-staged X (N = 2 NH feature rows), K = 128 tile rows ->
+// the shared-memory image of the block, laid out exactly like the block in the parameter buffer ([Mv][ldw]
+// weights, then the Mv bias entries).  Columns >= nX of a row are padding and take a zero gradient.
+template <int NH>
+__device__ __forceinline__ void dw_mma_image(const float* As, const float* Bs, const DwGeo& g, float* obuf) {
+  const uint64_t da = make_bdesc(smem_u32(As), kStLd * 16u, 128u);
+  const uint64_t db = make_bdesc(smem_u32(Bs), kStLd * 16u, 128u);
+  float d[NH / 2];
+  mma_ss64_n<NH>(d, da, db, (uint64_t)((2u * kStLd * 16u) >> 4), kRows / 8);
+  const int lane = threadIdx.x & 31;
+  const int m0 = ((threadIdx.x >> 5) & 3) * 16 + (lane >> 2);
+  const int n0 = (threadIdx.x >> 7) * NH + 2 * (lane & 3);
 #pragma unroll
-    for (int c = 0; c < 8; ++c) {
-      const int n = col0 + 4 * c;
+  for (int j = 0; j < NH / 8; ++j) {
 #pragma unroll
-      for (int i = 0; i < 4; ++i)
-        if (n + i == g.ones) bv = v[4 * c + i];
-      if (n < g.ldw)
-        orow[c] = make_float4(n < g.nX ? v[4 * c] : 0.f, n + 1 < g.nX ? v[4 * c + 1] : 0.f,
-                              n + 2 < g.nX ? v[4 * c + 2] : 0.f, n + 3 < g.nX ? v[4 * c + 3] : 0.f);
+    for (int e = 0; e < 4; ++e) {
+      const int mr = m0 + 8 * (e >> 1), n = n0 + 8 * j + (e & 1);
+      const float val = d[4 * j + e];
+      if (mr < g.Mv) {
+        if (n < g.ldw) obuf[mr * g.ldw + n] = n < g.nX ? val : 0.f;
+        if (n == g.ones) obuf[g.Mv * g.ldw + mr] = val;
+      }
     }
-    if (g.ones >= col0 && g.ones < col0 + 32) obuf[g.Mv * g.ldw + mrow] = bv;
+  }
+}
+
+template <int H>
+__global__ void __launch_bounds__(kThreads, 2)
+nsf_dw_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_constant__ sbi_rows rows,
+                 const float* __restrict__ save, float* __restrict__ gpart, int accum) {
+  constexpr int HP8 = (H + 7) & ~7;
+  constexpr int NC = HP8 / 2;
+  extern __shared__ __align__(128) float sm[];
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int half = warp >> 2;
+  const int row = ((warp & 3) << 5) | lane;
+  const int cbase = half * NC;
+  const int q_one = H - cbase;                 // this thread's column that is X column H (the ones column)
+  const int C = m.C, Cp = m.Cp, Hp = m.Hp;
+  const int nu = dw_units(m);
+  const int u = blockIdx.x % nu, l = (blockIdx.x / nu) % m.T;
+  const int64_t tile = blockIdx.x / (nu * m.T);
+  const NsfLayerView v = layer_view(m, l);
+  const TcSave SV = tc_save_layout(m.NB, m.TRmax, m.T);
+  const float* svl = save + (size_t)tile * SV.tile_stride + (size_t)l * SV.layer_stride;
+  const int64_t gr = tile * kRows + row;
+  const bool live = gr < rows.R;               // rows past the end of the batch contribute nothing
+  float* As = sm;
+  float* Bs = sm + kStFloats;
+  float* obuf = sm + 2 * kStFloats;
+  auto st_put = [&](float* buf, int n, float val) { buf[((row >> 2) * kStLd + n) * 4 + (row & 3)] = val; };
+  // context feature n < C of the row, standardised like load_rows (stages.cuh)
+  auto ctx = [&](int n) {
+    const int64_t src = rows.cond_shared ? 0 : (rows.d_index ? __ldg(rows.d_index + gr) : gr);
+    return (__ldg(rows.d_cond + src * C + n) - __ldg(m.d_stats + 2 * m.Dp + n)) / __ldg(m.d_stats + 2 * m.Dp + Cp + n);
+  };
+  // A' = dY^T: the thread's NC hidden columns
+  auto put_dy = [&](int off) {
+    float a[NC];
+    tc_load_cols<NC>(svl + off, row, half, a);
+#pragma unroll
+    for (int q = 0; q < NC; ++q) st_put(As, cbase + q, live ? a[q] : 0.f);
+  };
+  // B' = X^T from a saved [128][64] activation array, ones column at H
+  auto put_x = [&](int off, bool relu) {
+    float x[NC];
+    tc_load_cols<NC>(svl + off, row, half, x);
+#pragma unroll
+    for (int q = 0; q < NC; ++q) st_put(Bs, cbase + q, !live ? 0.f : q == q_one ? 1.f : relu ? relu_f(x[q]) : x[q]);
+  };
+
+  DwGeo g;
+  const int npm = SV.npm;
+  if (u < npm) {
+    // ---- final layer, pass u: dW of the parameter rows of features 2u, 2u+1; X = the final-layer input
+    const int nf = min(2, v.n_tr - 2 * u);
+    if (nf <= 0) return;                       // (CTA-uniform) this layer transforms fewer features
+    if (half < nf) {
+      float a[32];
+      tc_load_prm(svl + SV.dy_fin(u), row, 0, half, a);
+#pragma unroll
+      for (int i = 0; i < 32; ++i) st_put(As, 32 * half + i, live ? a[i] : 0.f);
+    }
+    put_x(SV.hf, false);
+    g.oW = __ldg(v.LT + SBI_L_WF) + 2 * u * m.PR * Hp; g.ldw = Hp; g.oB = __ldg(v.LT + SBI_L_BF) + 2 * u * m.PR;
+    g.nX = H; g.ones = H; g.Mv = 32 * nf; g.N = 64;
+  } else if (u < npm + 3 * m.NB) {
+    const int b = (u - npm) / 3, k = (u - npm) % 3;
+    const int* BT = v.LT + SBI_L_BLK0 + 6 * b;
+    put_dy(SV.dy_blk(b, k));
+    if (k == 0) {
+      // ---- dWc = dG^T ctx  (GLU gate)
+      const int Nc = (Cp + 1 + 15) & ~15;
+      for (int n = half * (Nc / 2); n < (half + 1) * (Nc / 2); ++n)
+        st_put(Bs, n, !live ? 0.f : n < C ? ctx(n) : (n == Cp ? 1.f : 0.f));
+      g.oW = __ldg(BT + 4); g.ldw = Cp; g.oB = __ldg(BT + 5); g.nX = Cp; g.ones = Cp; g.Mv = Hp; g.N = Nc;
+    } else if (k == 1) {
+      // ---- dW2 = dT^T a1
+      put_x(SV.a1(b), false);
+      g.oW = __ldg(BT + 2); g.ldw = Hp; g.oB = __ldg(BT + 3); g.nX = H; g.ones = H; g.Mv = Hp; g.N = 64;
+    } else {
+      // ---- dW1 = dA1^T relu(h_b)
+      put_x(SV.h(b), true);
+      g.oW = __ldg(BT + 0); g.ldw = Hp; g.oB = __ldg(BT + 1); g.nX = H; g.ones = H; g.Mv = Hp; g.N = 64;
+    }
+  } else {
+    // ---- initial layer: dW0 = dh^T [ctx | id | 1]
+    const int K0p = Cp + m.IDp;
+    const int N0 = (K0p + 1 + 15) & ~15;
+    put_dy(SV.dy_init());
+    for (int n = half * (N0 / 2); n < (half + 1) * (N0 / 2); ++n) {
+      float val = 0.f;
+      if (!live) val = 0.f;
+      else if (n < Cp) val = n < C ? ctx(n) : 0.f;
+      else if (n < K0p) {
+        const int i = n - Cp;
+        if (i < v.n_id) val = tc_load_row16_at(svl + SV.zin, row, __ldg(v.idf + i));
+      } else if (n == K0p) val = 1.f;
+      st_put(Bs, n, val);
+    }
+    g.oW = __ldg(v.LT + SBI_L_W0); g.ldw = K0p; g.oB = __ldg(v.LT + SBI_L_B0); g.nX = K0p; g.ones = K0p;
+    g.Mv = Hp; g.N = N0;
+  }
+  fence_async_smem();
+  __syncthreads();
+  switch (g.N) {
+    case 16: dw_mma_image<8>(As, Bs, g, obuf); break;
+    case 32: dw_mma_image<16>(As, Bs, g, obuf); break;
+    case 48: dw_mma_image<24>(As, Bs, g, obuf); break;
+    case 64: dw_mma_image<32>(As, Bs, g, obuf); break;
+    default: __trap();      // weight-gradient blocks are planned with N in {16, 32, 48, 64}
+  }
+  fence_async_smem();
+  __syncthreads();
+  if (tid == 0) {
+    float* gp = gpart + (size_t)tile * m.n_params;
+    bulk_s2g(gp + g.oW, obuf, (uint32_t)(g.Mv * g.ldw) * 4u, accum != 0);
+    bulk_s2g(gp + g.oB, obuf + g.Mv * g.ldw, (uint32_t)g.Mv * 4u, accum != 0);
+    bulk_commit();
+    bulk_wait_all();
   }
 }
 
@@ -127,7 +248,7 @@ __global__ void __launch_bounds__(kThreads, 1)
 nsf_vjp_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_constant__ sbi_nsf_tc tcb,
                   const __grid_constant__ sbi_rows rows, const float* __restrict__ gout, float g_const,
                   float* __restrict__ gpart, float* __restrict__ loss_acc,
-                  const float* __restrict__ save, int accum_first, const StoreArgs sa,
+                  float* __restrict__ save, int accum_first, const StoreArgs sa,
                   float* __restrict__ dcond) {
   constexpr int HP8 = (H + 7) & ~7;
   constexpr int NCH = HP8 / 8;
@@ -135,107 +256,43 @@ nsf_vjp_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_constant
   constexpr int NG = NC / 4;
   static_assert(HP8 % 8 == 0 && NC % 4 == 0 && H > NC && H < HP8 + 1 && HP8 <= 64, "hidden width");
   extern __shared__ __align__(128) float sm[];
-  const BwdSmem L = bwd_smem_layout(tcb.stage_cap, bwd_ldmax(m));
+  const BwdSmem L = bwd_smem_layout(tcb.stage_cap);
   uint64_t* full = reinterpret_cast<uint64_t*>(reinterpret_cast<char*>(sm) + L.bar_bytes);
-  uint64_t* obar = full + kBwdSlots;          // the output image has been read by its bulk copies
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int C = m.C, D = m.D, Cp = m.Cp, Hp = m.Hp;
+  const int C = m.C, D = m.D;
   const int64_t ntiles = (rows.R + kRows - 1) / kRows;
   const TcSave SV = tc_save_layout(m.NB, m.TRmax, m.T);
 
-  if (tid == 0) mbar_init(obar, 1);
   IssuerT<kBwdSlots> iss = tc_begin<kBwdSlots>(full, sm + L.ring, tcb, m.T, ntiles, true, kBwdCols, sa);
   SBI_TL(100);
 
   const float* __restrict__ P = m.d_params;
   float* dzs = sm + L.dz;
-  float* ctx_s = sm + L.ctx;
   float* GRs = sm + L.gr;
-  float* stg = sm + L.stg;
   const int half = warp >> 2;
   const int row = ((warp & 3) << 5) | lane;
   const int cbase = half * NC;
-  const int q_one = H - cbase;                 // this thread's column that is X column H (the ones column)
   RqsConst rc = rqs_const(m);
   rc.K = KB;
   float* gp = gpart + (size_t)blockIdx.x * m.n_params;
-  // condition gradient: features [c_lo, c_hi) of this thread's row; dY = the handed-over A' operand
+  // condition gradient: features [c_lo, c_hi) of this thread's row; dY = the row's dY columns at `dy`
+  // (written by both threads of the row before the CTA barrier that precedes the call)
   const int c_half = (C + 1) >> 1;
   const int c_lo = half * c_half, c_hi = min(C, c_lo + c_half);
-  auto dctx_add = [&](const float* As, const float* W, int ldw, int64_t row0) {
+  auto dctx_add = [&](const float* dy, const float* W, int ldw, int64_t row0) {
     if (row0 + row >= rows.R) return;
-    const float* csd = m.d_stats + 2 * m.Dp + Cp;
+    const float* csd = m.d_stats + 2 * m.Dp + m.Cp;
     float* out = dcond + (row0 + row) * C;
     for (int c = c_lo; c < c_hi; ++c) {
       float a = 0.f;
-      for (int n = 0; n < H; ++n) a = fmaf(As[((row >> 2) * kStLd + n) * 4 + (row & 3)], __ldg(W + n * ldw + c), a);
+      for (int n = 0; n < H; ++n) a = fmaf(__ldcg(dy + ((n >> 2) * kRows + row) * 4 + (n & 3)), __ldg(W + n * ldw + c), a);
       out[c] += a / __ldg(csd + c);
     }
   };
-
-  uint32_t dwn = 0u;           // weight-gradient MMAs issued so far (slot = dwn & 1, issuing warp = dwn & 7)
-  bool pend0 = false, pend1 = false;
-  DwGeo geo0, geo1;
-  geo0.oW = geo0.ldw = geo0.oB = geo0.nX = geo0.ones = geo0.Mv = geo0.N = 0;
-  geo1 = geo0;
   bool accum = accum_first != 0;
 
-  // operands written (the staging buffers through the generic proxy): hand them over to the MMAs
-  auto hand_over = [&]() {
-    fence_async_smem();
-    group_sync();
-  };
-  // element (feature n, row) of a transposed staging buffer
-  auto st_put = [&](float* buf, int n, float v) { buf[((row >> 2) * kStLd + n) * 4 + (row & 3)] = v; };
-  // accumulators of the weight-gradient MMA in `slot` -> this CTA's partial gradients
-  float* obuf = sm + L.obuf;
-  bool opend = false;          // the output image holds a block that has not been sent yet
-  uint32_t nflush = 0u;        // blocks sent so far (phase of obar)
-  DwGeo ogeo = geo0;
-  // make `slot` reusable: move the accumulators of the MMA chain that last used it into the output
-  // image, once the previous block's bulk copies have read the image.  The caller passes a CTA barrier
-  // (hand_over / fence_async_smem + group_sync) and then dw_flush() before the next dw_free.
-  auto dw_free = [&](int slot) {
-    const bool pend = slot ? pend1 : pend0;
-    if (!pend) return;
-    if (nflush > 0u) {
-      // the previous block's copies were issued a whole stage ago: they have read the image by now
-      if (tid == 0) {
-        bulk_wait_read();
-        mbar_arrive(obar);
-      }
-      mbar_wait(obar, (nflush - 1u) & 1u);
-    }
-    ogeo = slot ? geo1 : geo0;
-    dw_read_fn(row, cW + 64 * slot, ogeo, obuf, (warp & 3) * 16 + lane, half * 32, lane < 16);
-    if (slot) pend1 = false; else pend0 = false;
-    opend = true;
-  };
-  // after the barrier that followed dw_free: one thread sends the image to the partial-gradient slab
-  auto dw_flush = [&]() {
-    if (!opend) return;
-    if (tid == 0) {
-      bulk_s2g(gp + ogeo.oW, obuf, (uint32_t)(ogeo.Mv * ogeo.ldw) * 4u, accum);
-      bulk_s2g(gp + ogeo.oB, obuf + ogeo.Mv * ogeo.ldw, (uint32_t)ogeo.Mv * 4u, accum);
-      bulk_commit();
-    }
-    opend = false;
-    ++nflush;
-  };
-  // dW = A'^T-staged dY (M = 64 feature rows) x B'-staged X (N feature rows), K = 128 tile rows
-  auto dw_issue = [&](int slot, const DwGeo& g) {
-    {
-      const uint32_t a_s = smem_u32(stg + (2 * slot) * kStFloats);
-      const uint32_t b_s = smem_u32(stg + (2 * slot + 1) * kStFloats);
-      const uint64_t da = make_bdesc(a_s, kStLd * 16u, 128u);
-      const uint64_t db = make_bdesc(b_s, kStLd * 16u, 128u);
-      const uint64_t dstep = (uint64_t)((2u * kStLd * 16u) >> 4);
-      mma_ss64(g.N, cW + 64 * slot, da, db, dstep, kRows / 8);
-      group_sync();
-    }
-    if (slot) { pend1 = true; geo1 = g; } else { pend0 = true; geo0 = g; }
-    ++dwn;
-  };
+  // operands written: hand them over to the MMAs
+  auto hand_over = [&]() { group_sync(); };
   auto write_a = [&](const float (&act)[NC], int col0) {
 #pragma unroll
     for (int g = 0; g < NG; ++g) {
@@ -254,22 +311,9 @@ nsf_vjp_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_constant
   for (int64_t tile = blockIdx.x; tile < ntiles; tile += gridDim.x, ++iter) {
     if (iter > 0) accum = true;
     const int64_t row0 = tile * kRows;
-    const float* svt = save + (size_t)tile * SV.tile_stride;
-    // ---- per-tile setup: context (standardised like load_rows, stages.cuh), upstream gradient,
-    //      loss statistics, d(sum g log q)/dz_T = -g z_T
+    float* svt = save + (size_t)tile * SV.tile_stride;
+    // ---- per-tile setup: upstream gradient, loss statistics, d(sum g log q)/dz_T = -g z_T
     {
-      const float* st = m.d_stats;
-      const int Dp = m.Dp;
-      for (int e = tid; e < kRows * Cp; e += kThreads) {
-        const int r = e / Cp, c = e % Cp;
-        const int64_t gr = row0 + r;
-        float val = 0.f;
-        if (c < C && gr < rows.R) {
-          const int64_t src = rows.cond_shared ? 0 : (rows.d_index ? __ldg(rows.d_index + gr) : gr);
-          val = (__ldg(rows.d_cond + src * C + c) - __ldg(st + 2 * Dp + c)) / __ldg(st + 2 * Dp + Cp + c);
-        }
-        ctx_s[c * kRows + r] = val;
-      }
       const bool live = row0 + row < rows.R;
       const float g = live ? (gout ? __ldg(gout + row0 + row) : g_const) : 0.f;
       if (half == 0) {
@@ -309,15 +353,14 @@ nsf_vjp_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_constant
       const int l = m.T - 1 - li;
       const NsfLayerView v = layer_view(m, l);
       const int32_t* tab = tcb.d_tab + l * SBI_NSF_TC_STRIDE;
-      const float* svl = svt + (size_t)l * SV.layer_stride;
+      float* svl = svt + (size_t)l * SV.layer_stride;
       int stage = 0;
       SBI_TL(1000 * (li + 1));
 
-      // saved activations travel from L2 while the LU section runs: the final-layer input (X of the
-      // final layer's weight gradient) and the spline parameters of this thread's first feature
-      float xh[NC], qn[32], xn = 0.f;
+      // saved activations travel from L2 while the LU section runs: the spline parameters of this
+      // thread's first feature
+      float qn[32], xn = 0.f;
       int jn = 0;
-      tc_load_cols<NC>(svl + SV.hf, row, half, xh);
 #pragma unroll
       for (int i = 0; i < 32; ++i) qn[i] = 0.f;
       if (half < v.n_tr) {
@@ -327,18 +370,13 @@ nsf_vjp_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_constant
       }
 
       // ================= LULinear backward (y = U v, z' = L y + b) =================
+      // (the scratch and the dense factors were last read before the barriers of the previous layer;
+      // the factors of this layer were built a layer ago: prep_lu below)
       if (__ldg(v.LT + SBI_L_HAS_LU)) {
         float vr[kLuMax];
-        if (half == 0) tc_load_row16(svl + SV.v, row, vr);      // in flight across the waits below
-        // the row-major scratch below lives in the staging buffers of the slot that is reused next
-        const int lslot = (int)(dwn & 1u);
-        dw_free(lslot);
-        SBI_TL(1000 * (li + 1) + 90);
-        fence_async_smem();
-        group_sync();            // (the dense factors of this layer were built a layer ago: prep_lu below)
-        dw_flush();
+        if (half == 0) tc_load_row16(svl + SV.v, row, vr);
         SBI_TL(1000 * (li + 1) + 91);
-        float* V = stg + (2 * lslot) * kStFloats;
+        float* V = sm + L.lus;
         float* Y = V + 16 * kRows;
         float* DY = Y + 16 * kRows;
         const float* U = sm + L.lum;
@@ -428,7 +466,7 @@ nsf_vjp_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_constant
             *dst = accum ? (*dst + a) : a;
           }
           // the arrays are padded to a multiple of 4 entries: padding takes a zero gradient (every
-          // entry of the slab is written by this kernel; nothing is zero-filled beforehand)
+          // entry of the slab is written by this kernel or nsf_dw_tc_kernel; nothing is zero-filled beforehand)
           if (!accum && tid >= kThreads - 4) {
             const int k = tid - (kThreads - 4);
             const int ntri = D * (D - 1) / 2;
@@ -459,7 +497,6 @@ nsf_vjp_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_constant
 
       // ================= final layer + spline backward, passes of <= 2 features =================
       const int np = __ldg(tab + 1);
-      const int oWF = __ldg(v.LT + SBI_L_WF), oBF = __ldg(v.LT + SBI_L_BF);
       {
         for (int p = 0; p < np; ++p) {
           const int f = 2 * p + half;
@@ -477,10 +514,6 @@ nsf_vjp_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_constant
             jn = __ldg(v.trf + f + 2);
             xn = tc_load_row16_at(svl + SV.zin, row, jn);
           }
-          const int slot = (int)(dwn & 1u);
-          dw_free(slot);
-          float* As = stg + (2 * slot) * kStFloats;
-          float* Bs = As + kStFloats;
           if (has) {
             float dq[32];
             const float gx = rqs_backward_fast<KB>(q, rc, x, dzs[j * kRows + row], GRs[row], dq);
@@ -492,12 +525,7 @@ nsf_vjp_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_constant
               for (int i = 0; i < 8; ++i) a[i] = dq[8 * c + i];
               store_a8(row, aset + 32 * half + 8 * c, a);
             }
-#pragma unroll
-            for (int i = 0; i < 32; ++i) st_put(As, 32 * half + i, dq[i]);
-          }
-          if (p < 2) {      // the X operand (final-layer input) of pass p - 2 is still in this slot
-#pragma unroll
-            for (int q = 0; q < NC; ++q) st_put(Bs, cbase + q, q == q_one ? 1.f : xh[q]);
+            tc_save_prm(svl + SV.dy_fin(p), row, 0, half, dq);
           }
           hand_over();
           {
@@ -506,11 +534,6 @@ nsf_vjp_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_constant
             iss.block(cD, aset, 4 * nf, 0, 64, acc);
             iss.end();
           }
-          DwGeo g;
-          g.oW = oWF + 2 * p * m.PR * Hp; g.ldw = Hp; g.oB = oBF + 2 * p * m.PR;
-          g.nX = H; g.ones = H; g.Mv = 32 * nf; g.N = 64;
-          dw_issue(slot, g);
-          dw_flush();
           SBI_TL(1000 * (li + 1) + 10 + p);
         }
         stage += np;
@@ -531,42 +554,25 @@ nsf_vjp_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_constant
         float dT[NC], a1[NC];
         tc_load_cols<NC>(svl + SV.a1(b), row, half, a1);
         {
-          // ---- dWc = dG^T ctx  (GLU gate; the COND instantiation also takes dctx += dG Wc)
-          const int slot = (int)(dwn & 1u);
-          dw_free(slot);
-          float* As = stg + (2 * slot) * kStFloats;
-          float* Bs = As + kStFloats;
-          const int Nc = (Cp + 1 + 15) & ~15;
+          // ---- dG = dh t2 s (1 - s): output gradient of the GLU context linear (the COND instantiation
+          //      also takes dctx += dG Wc)
+          float dG[NC];
 #pragma unroll
           for (int q = 0; q < NC; ++q) {
             const float dhq = dh[q], s = sv[q];
             dT[q] = dhq * s;
-            st_put(As, cbase + q, dhq * t2[q] * s * (1.f - s));
+            dG[q] = dhq * t2[q] * s * (1.f - s);
           }
-          for (int n = half * (Nc / 2); n < (half + 1) * (Nc / 2); ++n)
-            st_put(Bs, n, n < C ? ctx_s[n * kRows + row] : (n == Cp ? 1.f : 0.f));
-          fence_async_smem();
-          group_sync();
-          if (COND) dctx_add(As, P + __ldg(BT + 4), Cp, row0);     // dG Wc
-          DwGeo g;
-          g.oW = __ldg(BT + 4); g.ldw = Cp; g.oB = __ldg(BT + 5); g.nX = Cp; g.ones = Cp; g.Mv = Hp; g.N = Nc;
-          dw_issue(slot, g);
-          dw_flush();
+          tc_save_cols<NC>(svl + SV.dy_blk(b, 0), row, half, dG);
+          if (COND) {
+            group_sync();
+            dctx_add(svl + SV.dy_blk(b, 0), P + __ldg(BT + 4), m.Cp, row0);     // dG Wc
+          }
         }
         SBI_TL(1000 * (li + 1) + 30 + 10 * b);
-        // ---- dW2 = dT^T a1 ;  dA1 = (dT W2) * [a1 > 0]
+        // ---- dA1 = (dT W2) * [a1 > 0]
         {
-          const int slot = (int)(dwn & 1u);
-          dw_free(slot);
-          SBI_TL(1000 * (li + 1) + 70 + 10 * b);
-          float* As = stg + (2 * slot) * kStFloats;
-          float* Bs = As + kStFloats;
-#pragma unroll
-          for (int q = 0; q < NC; ++q) {
-            st_put(As, cbase + q, dT[q]);
-            st_put(Bs, cbase + q, q == q_one ? 1.f : a1[q]);
-          }
-          SBI_TL(1000 * (li + 1) + 71 + 10 * b);
+          tc_save_cols<NC>(svl + SV.dy_blk(b, 1), row, half, dT);
           write_a(dT, 0);
           SBI_TL(1000 * (li + 1) + 72 + 10 * b);
           hand_over();
@@ -579,10 +585,6 @@ nsf_vjp_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_constant
           }
           SBI_TL(1000 * (li + 1) + 74 + 10 * b);
           ++stage;
-          DwGeo g;
-          g.oW = __ldg(BT + 2); g.ldw = Hp; g.oB = __ldg(BT + 3); g.nX = H; g.ones = H; g.Mv = Hp; g.N = 64;
-          dw_issue(slot, g);
-          dw_flush();
         }
         SBI_TL(1000 * (li + 1) + 31 + 10 * b);
         float hb[NC];
@@ -592,17 +594,9 @@ nsf_vjp_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_constant
 #pragma unroll
         for (int q = 0; q < NC; ++q) dA[q] = a1[q] > 0.f ? dA[q] : 0.f;
         SBI_TL(1000 * (li + 1) + 32 + 10 * b);
-        // ---- dW1 = dA1^T relu(h_b) ;  dh += (dA1 W1) * [h_b > 0]
+        // ---- dh += (dA1 W1) * [h_b > 0]
         {
-          const int slot = (int)(dwn & 1u);
-          dw_free(slot);
-          float* As = stg + (2 * slot) * kStFloats;
-          float* Bs = As + kStFloats;
-#pragma unroll
-          for (int q = 0; q < NC; ++q) {
-            st_put(As, cbase + q, dA[q]);
-            st_put(Bs, cbase + q, q == q_one ? 1.f : relu_f(hb[q]));
-          }
+          tc_save_cols<NC>(svl + SV.dy_blk(b, 2), row, half, dA);
           write_a(dA, 0);
           hand_over();
           {
@@ -612,10 +606,6 @@ nsf_vjp_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_constant
             iss.end();
           }
           ++stage;
-          DwGeo g;
-          g.oW = __ldg(BT + 0); g.ldw = Hp; g.oB = __ldg(BT + 1); g.nX = H; g.ones = H; g.Mv = Hp; g.N = 64;
-          dw_issue(slot, g);
-          dw_flush();
         }
         SBI_TL(1000 * (li + 1) + 33 + 10 * b);
         if (b > 0) {
@@ -631,28 +621,13 @@ nsf_vjp_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_constant
         SBI_TL(1000 * (li + 1) + 34 + 10 * b);
       }
 
-      // ================= initial layer: dW0 = dh^T [ctx | id | 1], d(identity features) =================
+      // ================= initial layer: d(identity features) = dh W0[:, C:] =================
       {
-        const int K0p = Cp + m.IDp;
-        const int N0 = (K0p + 1 + 15) & ~15;
-        const int slot = (int)(dwn & 1u);
-        dw_free(slot);
-        float* As = stg + (2 * slot) * kStFloats;
-        float* Bs = As + kStFloats;
-#pragma unroll
-        for (int q = 0; q < NC; ++q) st_put(As, cbase + q, dh[q]);
-        for (int n = half * (N0 / 2); n < (half + 1) * (N0 / 2); ++n) {
-          float val = 0.f;
-          if (n < Cp) val = n < C ? ctx_s[n * kRows + row] : 0.f;
-          else if (n < K0p) {
-            const int i = n - Cp;
-            if (i < v.n_id) val = tc_load_row16_at(svl + SV.zin, row, __ldg(v.idf + i));
-          } else if (n == K0p) val = 1.f;
-          st_put(Bs, n, val);
-        }
+        const int K0p = m.Cp + m.IDp;
+        tc_save_cols<NC>(svl + SV.dy_init(), row, half, dh);
         write_a(dh, 0);
         hand_over();
-        if (COND) dctx_add(As, P + __ldg(v.LT + SBI_L_W0), K0p, row0);     // the context columns of dh W0
+        if (COND) dctx_add(svl + SV.dy_init(), P + __ldg(v.LT + SBI_L_W0), K0p, row0);     // the context columns of dh W0
         {
           uint32_t acc = 0u;
           iss.begin(__ldg(tab + 5 + 4 * stage));
@@ -660,11 +635,6 @@ nsf_vjp_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_constant
           iss.end();
         }
         ++stage;
-        DwGeo g;
-        g.oW = __ldg(v.LT + SBI_L_W0); g.ldw = K0p; g.oB = __ldg(v.LT + SBI_L_B0); g.nX = K0p; g.ones = K0p;
-        g.Mv = Hp; g.N = N0;
-        dw_issue(slot, g);
-        dw_flush();
         SBI_TL(1000 * (li + 1) + 60);
         if (half == 0) {
           float d[16];
@@ -678,17 +648,9 @@ nsf_vjp_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_constant
       }
     }
     SBI_TL(9000);
-    // the tile's last weight gradients
-    for (int k = 0; k < 2; ++k) {
-      dw_free((int)((dwn + k) & 1u));     // older slot first
-      fence_async_smem();
-      group_sync();
-      dw_flush();
-    }
   }
   SBI_TL(9001);
 
-  if (tid == 0) bulk_wait_all();
   tc_end(kBwdCols, sa);
 }
 
@@ -704,8 +666,8 @@ static int vjp_tc_ok(const sbi_nsf_model* m, const sbi_nsf_tc* tcf, const sbi_ns
   if (!sbi_b200_nsf_tc_supported(m, tcf)) return 0;
   if (!tcb || !tcb->d_tab || !tcb->d_tcw || tcb->stage_cap <= 0 || (tcb->stage_cap & 31)) return 0;
   if (m->IDp > 16 || m->Cp + m->IDp + 1 > 64 || m->Cp + 1 > 64) return 0;
-  const tc::BwdSmem L = tc::bwd_smem_layout(tcb->stage_cap, tc::bwd_ldmax(*m));
-  return L.total_bytes <= kMaxSmemBytes ? 1 : 0;
+  const tc::BwdSmem L = tc::bwd_smem_layout(tcb->stage_cap);
+  return L.total_bytes <= kMaxSmemBytes && tc::dw_smem_bytes(*m) <= kMaxSmemBytes ? 1 : 0;
 }
 
 extern "C" int sbi_b200_nsf_vjp_tc_supported(const sbi_nsf_model* m, const sbi_nsf_tc* tc_fwd,
@@ -742,11 +704,14 @@ static int vjp_tc_launch(const sbi_nsf_model* m, const sbi_nsf_tc* tc_fwd, const
   if (!vjp_tc_ok(m, tc_fwd, tc_bwd)) return SBI_ESMEM;
   if (save_bytes < sbi_b200_nsf_vjp_tc_save_bytes(m, rows->R)) return SBI_EINVAL;
   cudaStream_t s = (cudaStream_t)stream;
-  const int bwd_bytes = tc::bwd_smem_layout(tc_bwd->stage_cap, tc::bwd_ldmax(*m)).total_bytes;
-  // opt the backward kernel in before anything is launched: a failed opt-in leaves no forward sweep behind
+  const int bwd_bytes = tc::bwd_smem_layout(tc_bwd->stage_cap).total_bytes;
+  const int dw_bytes = tc::dw_smem_bytes(*m);
+  // opt the backward kernels in before anything is launched: a failed opt-in leaves no forward sweep behind
   if (int e = set_smem(reinterpret_cast<const void*>(tc::nsf_vjp_tc_kernel<50, 10, COND>), bwd_bytes)) return e;
-  // chunks of one tile per SM: forward sweep (saves activations) then backward sweep of the same rows;
-  // later chunks accumulate into the partial-gradient slabs
+  if (int e = set_smem(reinterpret_cast<const void*>(tc::nsf_dw_tc_kernel<50>), dw_bytes)) return e;
+  // chunks of one tile per SM: forward sweep (saves activations), backward sweep of the same rows (one CTA
+  // per tile, so tile t writes partial-gradient slab t), then their weight gradients (one CTA per tile,
+  // layer and linear); later chunks accumulate into the partial-gradient slabs
   tc::StoreArgs sa;
   if (int e = tc::store_args(&sa)) return e;
   const int64_t chunk = vjp_tc_chunk_rows();
@@ -763,6 +728,9 @@ static int vjp_tc_launch(const sbi_nsf_model* m, const sbi_nsf_tc* tc_fwd, const
     if (int rc = launch(tc::nsf_vjp_tc_kernel<50, 10, COND>, grid, tc::kThreads, bwd_bytes, s, *m, *tc_bwd, rr,
                         d_gout ? d_gout + r0 : nullptr, g_const, d_gpart, d_loss_acc, d_save, r0 > 0 ? 1 : 0, sa,
                         COND ? d_gcond + r0 * m->C : nullptr))
+      return rc;
+    if (int rc = launch(tc::nsf_dw_tc_kernel<50>, grid * m->T * tc::dw_units(*m), tc::kThreads, dw_bytes, s, *m, rr,
+                        d_save, d_gpart, r0 > 0 ? 1 : 0))
       return rc;
   }
   return 0;

@@ -205,19 +205,13 @@ __device__ __forceinline__ void mma_rows(int N, uint32_t dcol, uint32_t ahcol, u
   }
 }
 
-// D[store, M = 64] = A[smem]^T-staged * B[smem]^T over nk K-steps, single TF32 pass.  Rows 16q .. 16q+15
-// of D go to lanes 32q .. 32q+15 of the store, so that lanes 0..15 of warp q of each warpgroup read
-// them back as their own tile rows (dw_read_fn, nsf_vjp_tc.cu); warpgroup wg computes columns
-// [wg N/2, (wg + 1) N/2) (N % 16 == 0).
+// D[M = 64, N = 2 NH] = A[smem]^T-staged * B[smem]^T over nk K-steps, single TF32 pass, into registers:
+// warpgroup wg computes columns [wg NH, (wg + 1) NH); d holds the accumulator fragment of the
+// warpgroup's m64nNHk8 MMA (rows 16w + g and 16w + g + 8 of warp w, columns wg NH + 8j + 2t, + 1).
 template <int NH>
-__device__ __forceinline__ void mma_ss64_n(uint32_t dcol, uint64_t da, uint64_t db, uint64_t dstep, int nk) {
-  const int lane = threadIdx.x & 31, g = lane >> 2, t = lane & 3;
+__device__ __forceinline__ void mma_ss64_n(float (&d)[NH / 2], uint64_t da, uint64_t db, uint64_t dstep, int nk) {
   const int wg = threadIdx.x >> 7;
-  const uint32_t l0 = ((threadIdx.x >> 5) & 3) * 32 + g;
   db += (uint64_t)((wg * NH / 8) * 128 >> 4);      // 8-row groups of B are 128 B apart
-  dcol += s_store_col + wg * NH;
-  float* slab = s_store;
-  float d[NH / 2];
 #pragma unroll
   for (int i = 0; i < NH / 2; ++i) d[i] = 0.f;
   for (int kk = 0; kk < nk; ++kk) {
@@ -231,23 +225,6 @@ __device__ __forceinline__ void mma_ss64_n(uint32_t dcol, uint64_t da, uint64_t 
 #pragma unroll
     for (int i = 0; i < NH / 2; ++i) d[i] += p[i];
     da += dstep; db += dstep;
-  }
-#pragma unroll
-  for (int j = 0; j < NH / 8; ++j) {
-    const uint32_t c = dcol + 8 * j + 2 * t;
-    slab[c * kStoreLanes + l0] = d[4 * j + 0];
-    slab[(c + 1) * kStoreLanes + l0] = d[4 * j + 1];
-    slab[c * kStoreLanes + l0 + 8] = d[4 * j + 2];
-    slab[(c + 1) * kStoreLanes + l0 + 8] = d[4 * j + 3];
-  }
-}
-__device__ __forceinline__ void mma_ss64(int N, uint32_t dcol, uint64_t da, uint64_t db, uint64_t dstep, int nk) {
-  switch (N) {
-    case 16: mma_ss64_n<8>(dcol, da, db, dstep, nk); break;
-    case 32: mma_ss64_n<16>(dcol, da, db, dstep, nk); break;
-    case 48: mma_ss64_n<24>(dcol, da, db, dstep, nk); break;
-    case 64: mma_ss64_n<32>(dcol, da, db, dstep, nk); break;
-    default: __trap();      // weight-gradient blocks are planned with N in {16, 32, 48, 64}
   }
 }
 template <int NCHUNK>
