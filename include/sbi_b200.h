@@ -511,6 +511,24 @@ int sbi_b200_sir_select(const float* d_cand, int32_t D, const float* d_log_targe
                         const float* d_u, int64_t groups, int32_t K, int64_t index_base, float* d_out,
                         int64_t* d_out_idx, int64_t cap, int32_t* d_count, int32_t* d_scratch, void* stream);
 
+/* ---- MMD misspecification test (csrc/mmd.cu; reference sbi/diagnostics/misspecification.py:19-110) ----------------
+ * S index sets over the rows of d_z (R, D) fp32.  Set s takes rows d_idx[s*L + i] (int32, in [0, R)): its first
+ * nx_s rows form X and the next ny_s rows form Y (d_nxy: (S, 2) int32, nx_s <= max_nx, ny_s <= max_ny,
+ * nx_s + ny_s <= L <= SBI_MMD_MAX_ROWS, S <= SBI_MMD_MAX_SETS).  Unless `given_bw`, the bandwidth d_bw[s] is
+ * written as the exact lower median of the nx_s*ny_s X-Y distances (NaN for an empty X or Y); with `given_bw` it is
+ * read.  d_mmd[s] (fp64) receives the biased or, with `unbiased`, the reference's unbiased RBF MMD
+ * (K = exp(-d^2 / (2 h^2))); a null d_mmd computes the bandwidths only.  d_ws: sbi_b200_mmd_ws_bytes(S) bytes.
+ * The launch sequence does not depend on S, and a set's results depend only on its own rows. */
+#define SBI_MMD_MAX_ROWS 65536
+#define SBI_MMD_MAX_SETS 65536
+int64_t sbi_b200_mmd_ws_bytes(int32_t S);
+int sbi_b200_mmd(const float* d_z, int64_t R, int32_t D, const int32_t* d_idx, int32_t L, const int32_t* d_nxy,
+                 int32_t S, int32_t max_nx, int32_t max_ny, int32_t unbiased, int32_t given_bw, float* d_bw,
+                 double* d_mmd, void* d_ws, void* stream);
+/* out (nx, ny) = exp(-|x_i - y_j|^2 / (2 bandwidth^2)) for x (nx, D), y (ny, D) fp32. */
+int sbi_b200_rbf_matrix(const float* d_x, int64_t nx, const float* d_y, int64_t ny, int32_t D, double bandwidth,
+                        float* d_out, void* stream);
+
 /* ---- L-C2ST classifiers (csrc/lc2st.cu; reference sbi/diagnostics/lc2st.py with scikit-learn's
  * MLPClassifier(solver="adam", activation="relu")).  A network maps F = dim_theta + dim_x inputs through L ReLU
  * hidden layers to one logistic output p = P(class 1).  Parameters are packed per model in sklearn's order:

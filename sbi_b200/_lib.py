@@ -151,6 +151,10 @@ SBI_LC2ST_MAX_F = 64
 SBI_LC2ST_MAX_WIDTH = 256
 
 
+SBI_MMD_MAX_ROWS = 65536
+SBI_MMD_MAX_SETS = 65536
+
+
 class Lc2stNet(C.Structure):
     _fields_ = [("F", C.c_int32), ("L", C.c_int32), ("H", C.c_int32 * SBI_LC2ST_MAX_HIDDEN), ("P", C.c_int32)]
 
@@ -241,7 +245,13 @@ _EXPORTS = {
     "sbi_b200_sir_select": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64,
                                       C.c_int32, C.c_int64, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p,
                                       C.c_void_p, C.c_void_p]),
-    "sbi_b200_lc2st_plan": (C.c_int, [C.POINTER(Lc2stNet), C.POINTER(C.c_int32)]),
+    "sbi_b200_mmd_ws_bytes": (C.c_int64, [C.c_int32]),
+    "sbi_b200_mmd": (C.c_int, [C.c_void_p, C.c_int64, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p, C.c_int32,
+                               C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p,
+                               C.c_void_p]),
+    "sbi_b200_rbf_matrix": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_int32, C.c_double,
+                                      C.c_void_p, C.c_void_p]),
+    "sbi_b200_lc2st_plan":(C.c_int, [C.POINTER(Lc2stNet), C.POINTER(C.c_int32)]),
     "sbi_b200_lc2st_ws_floats": (C.c_int64, [C.POINTER(Lc2stNet), C.c_int32]),
     "sbi_b200_lc2st_train": (C.c_int, [C.POINTER(Lc2stNet), C.POINTER(Lc2stOpt), C.c_void_p, C.c_int32,
                                        C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p,

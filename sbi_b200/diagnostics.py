@@ -13,6 +13,8 @@ from typing import Callable, List, Optional, Tuple, Union
 import torch
 from torch import Tensor
 
+from .misspecification import calc_misspecification_mmd  # noqa: F401  (the MMD misspecification test)
+
 _LC2ST_NAMES = ("LC2ST", "LC2ST_NF", "LC2STScores", "LC2STState")
 
 
