@@ -390,6 +390,57 @@ int sbi_b200_slice_init(const sbi_slice_chains* s, float* d_params, void* stream
 int sbi_b200_slice_step(const sbi_slice_chains* s, const float* d_logp, float* d_params,
                         int32_t* d_n_done, void* stream);
 
+/* ---- lock-step HMC / NUTS (`mcmc_method="hmc_pyro"` / `"nuts_pyro"`): one thread per chain, one
+ * launch per lock-step, one leapfrog step per chain per lock-step.  Every chain runs its own
+ * adaptation (dual-averaged step size, diagonal mass matrix over Stan's windows).  Between two
+ * lock-steps the host evaluates log p and its gradient at d_params.  Layouts are column-per-chain
+ * so that the threads of a warp touch consecutive words:
+ *   d_vec    (SBI_HMC_NV0 + 4 * max_tree_depth, D, C) f64 working vectors (csrc/hmc.cu),
+ *   d_istate (SBI_HMC_NI, C) i32, d_fstate (SBI_HMC_NF0 + 2 * max_tree_depth, C) f64,
+ *   d_normal (D, C) f64 and d_uniform (max_tree_depth + 1, C) f64: this lock-step's draws.
+ * Random numbers: a chain draws a fresh momentum from d_normal (at most once per lock-step); the
+ * direction of a new doubling is d_uniform[0] < 0.5 (right); the progressive-sampling choice of the
+ * merge that forms a 2^(k+1)-leaf subtree uses d_uniform[1 + k]; the top-level NUTS choice and the
+ * HMC Metropolis test use d_uniform[max_tree_depth].  Other entries are left unused. */
+#define SBI_HMC_NV0 11
+#define SBI_HMC_NI 14
+#define SBI_HMC_NF0 10
+#define SBI_HMC_MAX_TREE_DEPTH 30
+#define SBI_HMC_MAX_WINDOWS 64
+#define SBI_HMC_TRACE_SCALARS 5
+enum { SBI_HMC_NUTS = 0, SBI_HMC_HMC = 1 };
+enum { SBI_HMC_PHASE_INIT = 0, SBI_HMC_PHASE_FIND = 1, SBI_HMC_PHASE_TRAJ = 2, SBI_HMC_PHASE_DONE = 3 };
+typedef struct {
+  int32_t C, D;
+  int32_t algo;                       /* SBI_HMC_NUTS or SBI_HMC_HMC */
+  int32_t max_tree_depth;             /* NUTS doublings per transition, 1..SBI_HMC_MAX_TREE_DEPTH */
+  int32_t warmup, num_samples;        /* adapted transitions, then recorded transitions */
+  int32_t adapt_step_size, adapt_mass_matrix;
+  int32_t n_windows;                  /* adaptation windows: window w ends at transition win_end[w] */
+  int32_t win_end[SBI_HMC_MAX_WINDOWS];
+  double step_size;                   /* initial step size */
+  double target_accept, trajectory_length;
+  double* d_z;                        /* (C, D) position: initial state in, last state out */
+  double* d_vec;
+  int32_t* d_istate;
+  double* d_fstate;
+  const double* d_normal;
+  const double* d_uniform;
+  const float* d_logp;                /* (C,) log p at d_params (written by the host) */
+  const float* d_grad;                /* (C, D) d log p / d params (written by the host) */
+  float* d_params;                    /* (C, D) next point to evaluate (written by the kernel) */
+  double* d_samples;                  /* (C, num_samples, D) recorded positions */
+  double* d_trace;                    /* optional (C, warmup + num_samples, 2 D + 5): position, inverse
+                                         mass, tree depth, leapfrog steps, divergent, accept stat, step
+                                         size of every transition (the last two sets as used by it) */
+} sbi_hmc_chains;
+
+/* initialise the chain state (unit inverse mass, initial step size) and write d_z to d_params */
+int sbi_b200_hmc_init(const sbi_hmc_chains* s, void* stream);
+/* one lock-step: consume d_logp / d_grad at d_params and this lock-step's draws, advance every chain
+ * by one potential evaluation, write the next d_params; d_n_done[0] = chains that are done */
+int sbi_b200_hmc_step(const sbi_hmc_chains* s, int32_t* d_n_done, void* stream);
+
 /* ---- flow matching (FMPE): VectorFieldMLP behind FlowMatchingEstimator
  * (net: sbi/neural_nets/net_builders/vector_field_nets.py:610-719, sinusoidal time embedding
  * :367-421; estimator: sbi/neural_nets/estimators/flowmatching_estimator.py:205-347). */

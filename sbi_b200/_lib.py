@@ -128,6 +128,25 @@ class SliceChains(C.Structure):
     ]
 
 
+SBI_HMC_NV0, SBI_HMC_NI, SBI_HMC_NF0 = 11, 14, 10
+SBI_HMC_MAX_TREE_DEPTH = 30
+SBI_HMC_MAX_WINDOWS = 64
+SBI_HMC_TRACE_SCALARS = 5
+SBI_HMC_NUTS, SBI_HMC_HMC = 0, 1
+
+
+class HmcChains(C.Structure):
+    _fields_ = [
+        ("C", C.c_int32), ("D", C.c_int32), ("algo", C.c_int32), ("max_tree_depth", C.c_int32),
+        ("warmup", C.c_int32), ("num_samples", C.c_int32), ("adapt_step_size", C.c_int32),
+        ("adapt_mass_matrix", C.c_int32), ("n_windows", C.c_int32), ("win_end", C.c_int32 * SBI_HMC_MAX_WINDOWS),
+        ("step_size", C.c_double), ("target_accept", C.c_double), ("trajectory_length", C.c_double),
+        ("d_z", C.c_void_p), ("d_vec", C.c_void_p), ("d_istate", C.c_void_p), ("d_fstate", C.c_void_p),
+        ("d_normal", C.c_void_p), ("d_uniform", C.c_void_p), ("d_logp", C.c_void_p), ("d_grad", C.c_void_p),
+        ("d_params", C.c_void_p), ("d_samples", C.c_void_p), ("d_trace", C.c_void_p),
+    ]
+
+
 class Rows(C.Structure):
     _fields_ = [
         ("d_input", C.c_void_p), ("d_cond", C.c_void_p), ("d_index", C.c_void_p),
@@ -276,6 +295,8 @@ _EXPORTS = {
                                             C.c_void_p]),
     "sbi_b200_slice_init": (C.c_int, [C.POINTER(SliceChains), C.c_void_p, C.c_void_p]),
     "sbi_b200_slice_step": (C.c_int, [C.POINTER(SliceChains), C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "sbi_b200_hmc_init": (C.c_int, [C.POINTER(HmcChains), C.c_void_p]),
+    "sbi_b200_hmc_step": (C.c_int, [C.POINTER(HmcChains), C.c_void_p, C.c_void_p]),
     "sbi_b200_reduce_partials": (C.c_int, [C.c_void_p, C.c_int, C.c_int64, C.c_void_p,
                                            C.c_void_p]),
     "sbi_b200_nll_stats": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p]),

@@ -371,18 +371,24 @@ class DirectPosterior:
         return self._leakage_density_correction_factor
 
 
+_HMC_OPTIONS = ("step_size", "adapt_step_size", "adapt_mass_matrix", "target_accept_prob", "max_tree_depth",
+                "trajectory_length")
+
+
 # =================================================================================================
 class MCMCPosterior:
-    """Posterior sampled with the lock-step vectorized slice sampler (reference:
-    /root/reference/sbi/inference/posteriors/mcmc_posterior.py: sample :237-367, _slice_np_mcmc
-    :737-811, _get_initial_params :590-659).  Supported method: `slice_np_vectorized`."""
+    """Posterior sampled with the lock-step vectorized slice sampler or with the lock-step NUTS / HMC sampler
+    (reference: /root/reference/sbi/inference/posteriors/mcmc_posterior.py: sample :237-367, _slice_np_mcmc
+    :737-811, _pyro_mcmc :813-878, _get_initial_params :590-659).  Supported methods: `slice_np_vectorized`
+    (`slice_np`), `nuts_pyro` and `hmc_pyro` (sbi_b200.hmc; pyro's defaults, run on the device)."""
 
     def __init__(self, potential_fn, proposal, theta_transform=None, method: str = "slice_np_vectorized",
                  thin: int = -1, warmup_steps: int = 200, num_chains: int = 20,
                  init_strategy: str = "resample", init_strategy_parameters: Optional[dict] = None,
                  num_workers: int = 1, device: Optional[str] = None, x_shape=None):
-        if method not in ("slice_np_vectorized", "slice_np"):
-            raise NotImplementedError("sbi_b200.MCMCPosterior implements method='slice_np_vectorized'")
+        if method not in ("slice_np_vectorized", "slice_np", "nuts_pyro", "hmc_pyro"):
+            raise NotImplementedError("sbi_b200.MCMCPosterior implements method='slice_np_vectorized', "
+                                      "'nuts_pyro' and 'hmc_pyro'")
         self.potential_fn = potential_fn
         self._device = device or potential_fn.device
         self.proposal = prior_to_device(proposal, self._device)
@@ -392,6 +398,7 @@ class MCMCPosterior:
             self.theta_transform = tt.IndependentTransform(tt.identity_transform, reinterpreted_batch_ndims=1)
         self.method, self.warmup_steps, self.num_chains = method, warmup_steps, num_chains
         self.thin = 10 if thin == -1 else thin       # reference default (mcmc_posterior.py: thin=-1 -> 10)
+        self._thin_arg = thin                        # the pyro methods read -1 as 1 (_process_thin_default)
         self.init_strategy = init_strategy
         self.init_strategy_parameters = init_strategy_parameters or {}
         self._mcmc_init_params = None
@@ -429,6 +436,10 @@ class MCMCPosterior:
         if x is None:
             raise ValueError("Context `x` needed when a default has not been set.")
         self.potential_fn.set_x(x, x_is_iid=True)
+        method = self.method if method is None else method
+        if method in ("nuts_pyro", "hmc_pyro"):
+            return self._sample_gradient_based(sample_shape, method, thin, warmup_steps, num_chains, init_strategy,
+                                               **kwargs)
         thin = self.thin if thin is None else thin
         warmup_steps = self.warmup_steps if warmup_steps is None else warmup_steps
         num_chains = self.num_chains if num_chains is None else num_chains
@@ -452,6 +463,44 @@ class MCMCPosterior:
         self._posterior_sampler = sampler
         self._mcmc_init_params = samples[:, -1, :].reshape(num_chains, dim).float().to(self._device)
         samples = samples.reshape(-1, dim)[:num_samples].type(torch.float32).to(self._device)
+        samples = self.theta_transform.inv(samples)
+        return samples.reshape((*torch.Size(sample_shape), -1))
+
+    def _sample_gradient_based(self, sample_shape, method: str, thin: Optional[int], warmup_steps: Optional[int],
+                               num_chains: Optional[int], init_strategy: Optional[str], **kwargs) -> Tensor:
+        """_pyro_mcmc (mcmc_posterior.py:813-878): `ceil(thin * n / num_chains)` transitions per chain after
+        `warmup_steps` warm-up transitions (not multiplied by `thin`), flattened chain-major, then `[::thin][:n]`.
+        The energy is minus the potential in unconstrained space, log|det J| included (`_prepare_potential` with
+        `track_gradients=True`).  The sampler options among `kwargs` (`step_size`, `adapt_step_size`,
+        `adapt_mass_matrix`, `target_accept_prob`, `max_tree_depth`, `trajectory_length`) go to
+        `HMCSamplerVectorized`; the others are ignored, as on the slice path."""
+        from math import ceil
+        from .hmc import HMCSamplerVectorized, frozen_parameters
+        from .potentials import transformed_potential
+        thin = self._thin_arg if thin is None else thin
+        thin = 1 if thin == -1 else thin
+        warmup_steps = self.warmup_steps if warmup_steps is None else warmup_steps
+        num_chains = self.num_chains if num_chains is None else num_chains
+        init_strategy = self.init_strategy if init_strategy is None else init_strategy
+        num_samples = torch.Size(sample_shape).numel()
+        initial_params = self._get_initial_params(init_strategy, num_chains)
+        dim = initial_params.shape[1]
+
+        def log_prob_fn(params):
+            return transformed_potential(params, self.potential_fn, self.theta_transform, self._device,
+                                         track_gradients=True).flatten()
+
+        sampler = HMCSamplerVectorized(log_prob_fn, initial_params.detach(), num_chains=num_chains,
+                                       method="nuts" if method == "nuts_pyro" else "hmc", warmup_steps=warmup_steps,
+                                       device=self._device, graph=True,
+                                       **{k: v for k, v in kwargs.items() if k in _HMC_OPTIONS})
+        with frozen_parameters(self.potential_fn):
+            samples = sampler.run(ceil((thin * num_samples) / num_chains))     # (chains, n, dim)
+        samples = torch.from_numpy(samples)
+        self._posterior_sampler = sampler
+        if samples.shape[1] > 0:
+            self._mcmc_init_params = samples[:, -1, :].reshape(num_chains, dim).float().to(self._device)
+        samples = samples.reshape(-1, dim)[::thin][:num_samples].type(torch.float32).to(self._device)
         samples = self.theta_transform.inv(samples)
         return samples.reshape((*torch.Size(sample_shape), -1))
 

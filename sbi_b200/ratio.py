@@ -166,9 +166,7 @@ class _RatioFn(torch.autograd.Function):
         if resnet:
             est._check_rc(L.load().sbi_b200_ratio_vjp_inputs(C.byref(m), C.byref(pr), L.ptr(g), None, L.ptr(gpart),
                                                             L.ptr(gth), L.ptr(gx), L.stream_ptr()), "ratio_vjp")
-        else:
-            if need_th and ctx.ti is not None:
-                raise NotImplementedError("theta gradients with an index gather are not needed by any caller")
+        else:   # per-pair theta gradients, summed onto the gathered rows below
             est._check_rc(est._entry("vjp")(C.byref(m), C.byref(pr), L.ptr(g), None, L.ptr(gpart), L.ptr(gth),
                                             L.stream_ptr()), f"{est.layout.family}_vjp")
         gflat = L.reduce_partials(gpart, n_part, est.layout.n_params) if need_flat else None
