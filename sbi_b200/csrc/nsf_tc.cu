@@ -25,7 +25,8 @@
 //
 // Store columns of a CTA:  [0,64) A_hi | [64,128) A_lo | [128,192) D | [192,256) G (GLU gate);
 // the final layer's spline parameters P (32 columns per feature, 2 features per pass)
-// alternate between D and G.
+// alternate between D and G.  The training forward (SAVE) runs one CTA per SM (one tile each), keeps
+// A_hi / A_lo in shared memory (tc_common.cuh) and reserves only [0,64) D | [64,128) G of the store.
 #include <cuda_runtime.h>
 #include <math.h>
 #include <algorithm>
@@ -43,10 +44,11 @@ namespace tc {
 
 // ---- shared memory plan -------------------------------------------------------------------------
 struct TcSmem {
-  int zs, ctx, lds, lum, bias, bias_stride, ring;   // float offsets
+  int zs, ctx, lds, lum, bias, bias_stride, a, ring;   // float offsets
   int bar_bytes, total_bytes;
 };
-__host__ __device__ inline TcSmem tc_smem_layout(const sbi_nsf_model& m, int stage_cap) {
+// a_smem: the training forward (SAVE) also keeps its A operands in shared memory (tc_common.cuh)
+__host__ __device__ inline TcSmem tc_smem_layout(const sbi_nsf_model& m, int stage_cap, bool a_smem) {
   TcSmem L;
   int fl = 0;
   L.zs = fl;  fl += m.Dp * kRows;
@@ -56,6 +58,7 @@ __host__ __device__ inline TcSmem tc_smem_layout(const sbi_nsf_model& m, int sta
   L.bias_stride = 64 + m.NB * 192 + m.TRmax * 32;
   L.bias = fl; fl += m.T * L.bias_stride;
   fl = (fl + 31) & ~31;
+  L.a = fl;   fl += a_smem ? kASmemFloats : 0;
   L.ring = fl; fl += kSlots * stage_cap;
   L.bar_bytes = fl * 4;
   L.total_bytes = L.bar_bytes + kSlots * 8;
@@ -82,7 +85,7 @@ __host__ __device__ inline TcSmem tc_smem_layout(const sbi_nsf_model& m, int sta
 // (layout: nsf_tc_save.cuh) for the tensor-core backward and weight-gradient kernels (nsf_vjp_tc.cu),
 // together with the final base-space point and the row's log-density.
 template <int H, int KB, bool INV, bool SAVE = false>
-__global__ void __launch_bounds__(kThreads, 2)
+__global__ void __launch_bounds__(kThreads, SAVE ? 1 : 2)
 nsf_logprob_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_constant__ sbi_nsf_tc tc,
                       const __grid_constant__ sbi_rows rows, float* __restrict__ logp,
                       float* __restrict__ noise, float* __restrict__ save, const StoreArgs sa) {
@@ -94,7 +97,7 @@ nsf_logprob_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_cons
   constexpr int QC = H - NC;        // first column offset of half 1 that is a context column
   static_assert(HP8 % 8 == 0 && NC % 4 == 0 && H > NC && H <= 64, "hidden width");
   extern __shared__ __align__(128) float sm[];
-  const TcSmem L = tc_smem_layout(m, tc.stage_cap);
+  const TcSmem L = tc_smem_layout(m, tc.stage_cap, SAVE);
   uint64_t* full = reinterpret_cast<uint64_t*>(reinterpret_cast<char*>(sm) + L.bar_bytes);
   const int tid = threadIdx.x, warp = tid >> 5;
   const int C = m.C;
@@ -102,7 +105,11 @@ nsf_logprob_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_cons
   const int64_t ntiles = (rows.R + kRows - 1) / kRows;
   const TcSave SV = tc_save_layout(m.NB, m.TRmax, m.T);
 
-  Issuer iss = tc_begin<kSlots>(full, sm + L.ring, tc, m.T, ntiles, INV, kCols, sa);
+  // SAVE: A in shared memory, the store holds D | G only
+  constexpr int ncols = SAVE ? kColsDG : kCols;
+  constexpr int kD = SAVE ? cDs : cD, kG = SAVE ? cGs : cG;
+  float* as = sm + L.a;
+  IssuerT<kSlots, SAVE> iss = tc_begin<kSlots, SAVE>(full, sm + L.ring, tc, m.T, ntiles, INV, ncols, sa, as);
 
   const float* __restrict__ P = m.d_params;
   float* zs = sm + L.zs;
@@ -151,6 +158,19 @@ nsf_logprob_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_cons
     ld_const = INV ? (-tot - m.ld_zscore) : (tot + m.ld_zscore - 0.5f * (float)D * 1.8378770664093453f);
   }
 
+  auto put_a4 = [&](int col, const float (&a)[4]) {
+    if constexpr (SAVE) smem_a4(as, row, col, a);
+    else store_a4(row, col, a);
+  };
+  auto put_a8 = [&](int col, const float (&a)[8]) {
+    if constexpr (SAVE) smem_a8(as, row, col, a);
+    else store_a8(row, col, a);
+  };
+  // operands written: hand them over to the MMAs
+  auto hand_over = [&]() {
+    if constexpr (SAVE) fence_async_smem();
+    group_sync();
+  };
   // A-operand column j of a hidden layer: activation (j < H), context (H <= j < H+C), zero
   auto acol = [&](int j, float act) -> float {
     const int c = j - H;
@@ -167,7 +187,7 @@ nsf_logprob_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_cons
         if (q < QC) a[i] = act[q];
         else a[i] = half ? ((q - QC < C) ? ctx_s[(q - QC) * kRows + row] : 0.f) : act[q];
       }
-      store_a4(row, cbase + 4 * g, a);
+      put_a4(cbase + 4 * g, a);
     }
   };
   auto read_acc = [&](int region, float (&d)[NC]) {
@@ -212,7 +232,7 @@ nsf_logprob_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_cons
         float v[8];
 #pragma unroll
         for (int i = 0; i < 8; ++i) v[i] = acol(8 * c + i, 0.f);
-        store_a8(row, 8 * c, v);
+        put_a8(8 * c, v);
       }
     }
     float ldacc = 0.f;
@@ -280,7 +300,7 @@ nsf_logprob_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_cons
             const int j = 8 * kk + i;
             a[i] = (j < v.n_id) ? zs[__ldg(v.idf + j) * kRows + row] : 0.f;
           }
-          store_a8(row, 8 * kk, a);
+          put_a8(8 * kk, a);
         }
       } else {
 #pragma unroll
@@ -288,15 +308,15 @@ nsf_logprob_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_cons
           float a[8];
 #pragma unroll
           for (int i = 0; i < 8; ++i) a[i] = acol(8 * c + i, 0.f);
-          store_a8(row, 8 * c, a);
+          put_a8(8 * c, a);
         }
       }
-      group_sync();
+      hand_over();
       {
         iss.begin(__ldg(tab + 5 + 4 * stage));
         uint32_t acc = 0u;
-        iss.block(cD, 0, kid8 / 8, 0, 64, acc);
-        iss.block(cD, 8 * KC0, nkc, 64 * kid8, 64, acc);
+        iss.block(kD, 0, kid8 / 8, 0, 64, acc);
+        iss.block(kD, 8 * KC0, nkc, 64 * kid8, 64, acc);
         iss.end();
       }
       ++stage;
@@ -309,7 +329,7 @@ nsf_logprob_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_cons
       const float* blh = bl + cbase;
       {
         float d[NC];
-        read_acc(cD, d);
+        read_acc(kD, d);
 #pragma unroll
         for (int q = 0; q < NC; ++q) h[q] = d[q] + blh[q];     // columns >= H: zero weights + zero bias
       }
@@ -328,15 +348,15 @@ nsf_logprob_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_cons
           for (int q = 0; q < NC; ++q) a[q] = relu_f(h[q]);
           write_a(a);
         }
-        group_sync();
+        hand_over();
         {
           uint32_t accg = 0u;
           iss.begin(__ldg(tab + 5 + 4 * stage));
-          iss.block(cG, 8 * KC0, nkc, 0, 64, accg);
+          iss.block(kG, 8 * KC0, nkc, 0, 64, accg);
           iss.end();
           uint32_t acc = 0u;
           iss.begin(__ldg(tab + 5 + 4 * (stage + 1)));
-          iss.block(cD, 0, NCH, 0, 64, acc);
+          iss.block(kD, 0, NCH, 0, 64, acc);
           iss.end();
         }
         stage += 2;
@@ -345,7 +365,7 @@ nsf_logprob_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_cons
         float sg[NC];
         {
           float g[NC];
-          read_acc(cG, g);
+          read_acc(kG, g);
 #pragma unroll
           for (int q = 0; q < NC; ++q) sg[q] = sigmoid_fast(g[q] + bc[q]);
           if (SAVE) tc_save_cols<NC>(svl + SV.s(b), row, half, sg);
@@ -353,17 +373,17 @@ nsf_logprob_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_cons
         SBI_TL(1000 * (li + 1) + 10 * b + 14);
         {
           float d[NC];
-          read_acc(cD, d);
+          read_acc(kD, d);
 #pragma unroll
           for (int q = 0; q < NC; ++q) d[q] = relu_f(d[q] + b1[q]);
           if (SAVE) tc_save_cols<NC>(svl + SV.a1(b), row, half, d);
           write_a(d);
         }
-        group_sync();
+        hand_over();
         {
           uint32_t acc = 0u;
           iss.begin(__ldg(tab + 5 + 4 * stage));
-          iss.block(cD, 0, NCH, 0, 64, acc);
+          iss.block(kD, 0, NCH, 0, 64, acc);
           iss.end();
         }
         ++stage;
@@ -371,7 +391,7 @@ nsf_logprob_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_cons
         {
           // h += (W2 a + b2) * gate
           float d[NC];
-          read_acc(cD, d);
+          read_acc(kD, d);
           if (SAVE) {
 #pragma unroll
             for (int q = 0; q < NC; ++q) d[q] += b2[q];
@@ -393,12 +413,12 @@ nsf_logprob_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_cons
         const float* bf = bl + 64 + m.NB * 192;
         const int ns = __ldg(tab);
         const int np = ns - stage;            // passes
-        group_sync();
+        hand_over();
         {
           for (int p = 0; p < 2 && p < np; ++p) {
             uint32_t acc = 0u;
             iss.begin(__ldg(tab + 5 + 4 * (stage + p)));
-            iss.block(cD + 64 * p, 0, NCH, 0, __ldg(tab + 6 + 4 * (stage + p)), acc);
+            iss.block(kD + 64 * p, 0, NCH, 0, __ldg(tab + 6 + 4 * (stage + p)), acc);
             iss.end();
           }
         }
@@ -409,7 +429,7 @@ nsf_logprob_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_cons
           for (int f = 0; f < nf; ++f) {
             if (((f0 + f) & 1) != half) continue;     // warp-uniform: features alternate between halves
             float q[32];
-            ld_cols<4>(row, cD + 64 * (p & 1) + 32 * f, q);
+            ld_cols<4>(row, kD + 64 * (p & 1) + 32 * f, q);
             const float* bff = bf + (f0 + f) * 32;
 #pragma unroll
             for (int i = 0; i < 32; ++i) q[i] = (i < 3 * KB - 1) ? q[i] + bff[i] : 0.f;
@@ -429,7 +449,7 @@ nsf_logprob_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_cons
             {
               uint32_t acc = 0u;
               iss.begin(__ldg(tab + 5 + 4 * (stage + p + 2)));
-              iss.block(cD + 64 * (p & 1), 0, NCH, 0, __ldg(tab + 6 + 4 * (stage + p + 2)), acc);
+              iss.block(kD + 64 * (p & 1), 0, NCH, 0, __ldg(tab + 6 + 4 * (stage + p + 2)), acc);
               iss.end();
             }
           }
@@ -512,7 +532,7 @@ nsf_logprob_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_cons
     group_sync();   // rows of the next tile are written cooperatively
   }
 
-  tc_end(kCols, sa);
+  tc_end(ncols, sa);
 }
 
 // the accumulator store of every tensor-core kernel of the library (tc_common.cuh)
@@ -551,7 +571,7 @@ extern "C" int sbi_b200_nsf_tc_supported(const sbi_nsf_model* m, const sbi_nsf_t
   if (m->NB < 1 || m->NB > SBI_NSF_MAX_BLOCKS) return 0;
   if (tc->stage_cap <= 0 || (tc->stage_cap & 31) || tc->n_words <= 0) return 0;
   // the weight ring has to fit next to a second CTA on the SM
-  return tc::tc_smem_layout(*m, tc->stage_cap).total_bytes <= 112 * 1024 ? 1 : 0;
+  return tc::tc_smem_layout(*m, tc->stage_cap, false).total_bytes <= 112 * 1024 ? 1 : 0;
 }
 
 extern "C" int sbi_b200_nsf_tc_pack(const sbi_nsf_model* m, const sbi_nsf_tc* tc, void* stream) {
@@ -571,7 +591,7 @@ extern "C" int sbi_b200_nsf_logprob_tc(const sbi_nsf_model* m, const sbi_nsf_tc*
   tc::StoreArgs sa;
   if (int e = tc::store_args(&sa)) return e;
   return launch(tc::nsf_logprob_tc_kernel<50, 10, false>, tile_grid(rows->R, tc::kRows, 2), tc::kThreads,
-                tc::tc_smem_layout(*m, tc->stage_cap).total_bytes, (cudaStream_t)stream, *m, *tc, *rows, d_logp,
+                tc::tc_smem_layout(*m, tc->stage_cap, false).total_bytes, (cudaStream_t)stream, *m, *tc, *rows, d_logp,
                 d_noise, nullptr, sa);
 }
 
@@ -581,7 +601,11 @@ int sbi::tc::launch_forward_save(const sbi_nsf_model* m, const sbi_nsf_tc* tc, c
   if (int e = tc::store_args(&sa)) return e;
   const int grid = (int)((rows->R + tc::kRows - 1) / tc::kRows);      // one tile per CTA: `d_save` slab = blockIdx
   return launch(tc::nsf_logprob_tc_kernel<50, 10, false, true>, grid, tc::kThreads,
-                tc::tc_smem_layout(*m, tc->stage_cap).total_bytes, s, *m, *tc, *rows, d_logp, nullptr, d_save, sa);
+                tc::forward_save_smem_bytes(*m, *tc), s, *m, *tc, *rows, d_logp, nullptr, d_save, sa);
+}
+
+int sbi::tc::forward_save_smem_bytes(const sbi_nsf_model& m, const sbi_nsf_tc& tc) {
+  return tc::tc_smem_layout(m, tc.stage_cap, true).total_bytes;
 }
 
 extern "C" int sbi_b200_nsf_inverse_tc(const sbi_nsf_model* m, const sbi_nsf_tc* tc,
@@ -596,7 +620,7 @@ extern "C" int sbi_b200_nsf_inverse_tc(const sbi_nsf_model* m, const sbi_nsf_tc*
   tc::StoreArgs sa;
   if (int e = tc::store_args(&sa)) return e;
   return launch(tc::nsf_logprob_tc_kernel<50, 10, true>, tile_grid(rows->R, tc::kRows, 2), tc::kThreads,
-                tc::tc_smem_layout(*m, tc->stage_cap).total_bytes, (cudaStream_t)stream, *m, *tc, *rows, d_logabsdet,
+                tc::tc_smem_layout(*m, tc->stage_cap, false).total_bytes, (cudaStream_t)stream, *m, *tc, *rows, d_logabsdet,
                 d_out, nullptr, sa);
 }
 

@@ -126,6 +126,8 @@ __device__ __forceinline__ float tc_load_row16_at(const float* q, int row, int j
 // (defined in nsf_tc.cu; returns a C-ABI status code)
 int launch_forward_save(const sbi_nsf_model* m, const sbi_nsf_tc* tc, const sbi_rows* rows, float* d_logp,
                         float* d_save, cudaStream_t s);
+// dynamic shared memory of that launch (its A operands live in shared memory)
+int forward_save_smem_bytes(const sbi_nsf_model& m, const sbi_nsf_tc& tc);
 
 }  // namespace tc
 }  // namespace sbi

@@ -13,8 +13,8 @@
 // oracle/nflows_port/nn/nets/resnet.py) in reverse:
 //
 //   * input-gradient chain  dX = dY W  on wgmma kind tf32 (both warpgroups, 64 rows each): A = dY from
-//     the accumulator store of tc_common.cuh (written
-//     by the row threads, 3xTF32 hi/lo split), B = W^T streamed by TMA bulk copies from the
+//     the shared-memory A region of tc_common.cuh (written by the row threads, 3xTF32 hi/lo split), the
+//     accumulators in the accumulator store; B = W^T streamed by TMA bulk copies from the
 //     pre-transposed operand blocks (pack.NsfLayout.tc_bwd_plan) through a 2-slot ring; relu / GLU
 //     masks, the spline backward (rqs.cuh) and the LULinear backward (with its parameter gradients) are
 //     per-thread code on the thread's own row between the MMAs;
@@ -37,8 +37,8 @@
 // in the parameter buffer, and ONE thread sends it to the tile's partial-gradient slab with two TMA bulk
 // copies (a reducing copy for every chunk after the first).
 //
-// Store columns of the backward (384): [0,64) A_hi | [64,128) A_lo | [128,192) D | [192,256) G |
-//                                      [256,320) A2_hi | [320,384) A2_lo (second A set: spline passes alternate)
+// Store columns of the backward (128): [0,64) D | [64,128) G.  One A set serves every MMA: each pass's MMAs
+// complete (wgmma wait) before the CTA barrier of Issuer::end(), and the next operands are written after it.
 #include <cuda_runtime.h>
 #include <math.h>
 #include <algorithm>
@@ -55,14 +55,11 @@ namespace sbi {
 namespace tc {
 
 constexpr int kBwdSlots = 2;
-constexpr int kBwdCols = 384;
-static_assert(kBwdCols <= kStoreCols, "one CTA's columns must fit one slab");
-constexpr int cA2 = 256;
 constexpr int kStLd = 65;                       // feature rows per K-slab of a staging buffer (64 + 1 pad)
 constexpr int kStFloats = 32 * kStLd * 4;       // [128 rows / 4][65][4]
 
 struct BwdSmem {
-  int dz, gr, lum, lus, ring;   // float offsets
+  int dz, gr, lum, lus, a, ring;   // float offsets
   int bar_bytes, total_bytes;
 };
 __host__ __device__ inline BwdSmem bwd_smem_layout(int stage_cap) {
@@ -74,6 +71,7 @@ __host__ __device__ inline BwdSmem bwd_smem_layout(int stage_cap) {
   fl = (fl + 31) & ~31;
   L.lus = fl; fl += 3 * kLuMax * kRows;          // LULinear backward: v | y | dy, feature-major
   fl = (fl + 31) & ~31;
+  L.a = fl;   fl += kASmemFloats;                 // A_hi | A_lo (tc_common.cuh)
   L.ring = fl; fl += kBwdSlots * stage_cap;
   L.bar_bytes = fl * 4;
   L.total_bytes = L.bar_bytes + kBwdSlots * 8;
@@ -263,7 +261,8 @@ nsf_vjp_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_constant
   const int64_t ntiles = (rows.R + kRows - 1) / kRows;
   const TcSave SV = tc_save_layout(m.NB, m.TRmax, m.T);
 
-  IssuerT<kBwdSlots> iss = tc_begin<kBwdSlots>(full, sm + L.ring, tcb, m.T, ntiles, true, kBwdCols, sa);
+  float* as = sm + L.a;
+  IssuerT<kBwdSlots, true> iss = tc_begin<kBwdSlots, true>(full, sm + L.ring, tcb, m.T, ntiles, true, kColsDG, sa, as);
   SBI_TL(100);
 
   const float* __restrict__ P = m.d_params;
@@ -292,14 +291,17 @@ nsf_vjp_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_constant
   bool accum = accum_first != 0;
 
   // operands written: hand them over to the MMAs
-  auto hand_over = [&]() { group_sync(); };
+  auto hand_over = [&]() {
+    fence_async_smem();
+    group_sync();
+  };
   auto write_a = [&](const float (&act)[NC], int col0) {
 #pragma unroll
     for (int g = 0; g < NG; ++g) {
       float a[4];
 #pragma unroll
       for (int i = 0; i < 4; ++i) a[i] = act[4 * g + i];
-      store_a4(row, col0 + cbase + 4 * g, a);
+      smem_a4(as, row, col0 + cbase + 4 * g, a);
     }
   };
   auto read_acc = [&](int region, float (&d)[NC]) {
@@ -502,7 +504,6 @@ nsf_vjp_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_constant
           const int f = 2 * p + half;
           const int nf = min(2, v.n_tr - 2 * p);
           const bool has = f < v.n_tr;                     // warp-uniform
-          const int aset = (p & 1) * cA2;
           // this pass's parameters were requested a pass (or the LU section) ago; request the next
           float q[32];
           const float x = xn;
@@ -523,7 +524,7 @@ nsf_vjp_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_constant
               float a[8];
 #pragma unroll
               for (int i = 0; i < 8; ++i) a[i] = dq[8 * c + i];
-              store_a8(row, aset + 32 * half + 8 * c, a);
+              smem_a8(as, row, 32 * half + 8 * c, a);
             }
             tc_save_prm(svl + SV.dy_fin(p), row, 0, half, dq);
           }
@@ -531,7 +532,7 @@ nsf_vjp_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_constant
           {
             uint32_t acc = p > 0 ? 1u : 0u;
             iss.begin(__ldg(tab + 5 + 4 * (stage + p)));
-            iss.block(cD, aset, 4 * nf, 0, 64, acc);
+            iss.block(cDs, 0, 4 * nf, 0, 64, acc);
             iss.end();
           }
           SBI_TL(1000 * (li + 1) + 10 + p);
@@ -545,7 +546,7 @@ nsf_vjp_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_constant
         tc_load_cols<NC>(svl + SV.t2(m.NB - 1), row, half, t2);
       }
       float dh[NC];
-      read_acc(cD, dh);
+      read_acc(cDs, dh);
       SBI_TL(1000 * (li + 1) + 20);
 
       // ================= residual blocks, last to first =================
@@ -580,7 +581,7 @@ nsf_vjp_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_constant
           {
             uint32_t acc = 0u;
             iss.begin(__ldg(tab + 5 + 4 * stage));
-            iss.block(cD, 0, NCH, 0, 64, acc);
+            iss.block(cDs, 0, NCH, 0, 64, acc);
             iss.end();
           }
           SBI_TL(1000 * (li + 1) + 74 + 10 * b);
@@ -590,7 +591,7 @@ nsf_vjp_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_constant
         float hb[NC];
         tc_load_cols<NC>(svl + SV.h(b), row, half, hb);
         float dA[NC];
-        read_acc(cD, dA);
+        read_acc(cDs, dA);
 #pragma unroll
         for (int q = 0; q < NC; ++q) dA[q] = a1[q] > 0.f ? dA[q] : 0.f;
         SBI_TL(1000 * (li + 1) + 32 + 10 * b);
@@ -602,7 +603,7 @@ nsf_vjp_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_constant
           {
             uint32_t acc = 0u;
             iss.begin(__ldg(tab + 5 + 4 * stage));
-            iss.block(cG, 0, NCH, 0, 64, acc);
+            iss.block(cGs, 0, NCH, 0, 64, acc);
             iss.end();
           }
           ++stage;
@@ -614,7 +615,7 @@ nsf_vjp_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_constant
         }
         {
           float d[NC];
-          read_acc(cG, d);
+          read_acc(cGs, d);
 #pragma unroll
           for (int q = 0; q < NC; ++q) dh[q] += hb[q] > 0.f ? d[q] : 0.f;
         }
@@ -631,15 +632,15 @@ nsf_vjp_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_constant
         {
           uint32_t acc = 0u;
           iss.begin(__ldg(tab + 5 + 4 * stage));
-          iss.block(cD, 0, NCH, 0, 16, acc);
+          iss.block(cDs, 0, NCH, 0, 16, acc);
           iss.end();
         }
         ++stage;
         SBI_TL(1000 * (li + 1) + 60);
         if (half == 0) {
           float d[16];
-          ld8(row, cD, d);
-          ld8(row, cD + 8, d + 8);
+          ld8(row, cDs, d);
+          ld8(row, cDs + 8, d + 8);
 #pragma unroll
           for (int j = 0; j < 16; ++j)
             if (j < v.n_id) dzs[__ldg(v.idf + j) * kRows + row] += d[j];
@@ -651,7 +652,7 @@ nsf_vjp_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_constant
   }
   SBI_TL(9001);
 
-  tc_end(kBwdCols, sa);
+  tc_end(kColsDG, sa);
 }
 
 }  // namespace tc
@@ -666,8 +667,13 @@ static int vjp_tc_ok(const sbi_nsf_model* m, const sbi_nsf_tc* tcf, const sbi_ns
   if (!sbi_b200_nsf_tc_supported(m, tcf)) return 0;
   if (!tcb || !tcb->d_tab || !tcb->d_tcw || tcb->stage_cap <= 0 || (tcb->stage_cap & 31)) return 0;
   if (m->IDp > 16 || m->Cp + m->IDp + 1 > 64 || m->Cp + 1 > 64) return 0;
-  const tc::BwdSmem L = tc::bwd_smem_layout(tcb->stage_cap);
-  return L.total_bytes <= kMaxSmemBytes && tc::dw_smem_bytes(*m) <= kMaxSmemBytes ? 1 : 0;
+  // the training pair runs one CTA per SM: the forward with activation save and the backward sweep may each
+  // opt into a whole SM's shared memory
+  return tc::forward_save_smem_bytes(*m, *tcf) <= kMaxSmemBytes &&
+                 tc::bwd_smem_layout(tcb->stage_cap).total_bytes <= kMaxSmemBytes &&
+                 tc::dw_smem_bytes(*m) <= kMaxSmemBytes
+             ? 1
+             : 0;
 }
 
 extern "C" int sbi_b200_nsf_vjp_tc_supported(const sbi_nsf_model* m, const sbi_nsf_tc* tc_fwd,

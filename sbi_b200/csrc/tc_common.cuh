@@ -35,9 +35,13 @@ constexpr int kLuMax = 16;        // LULinear runs on register-resident rows of 
 constexpr int kSlots = 3;         // weight ring: up to two stages in use + one prefetched
 constexpr int kCols = 256;        // accumulator-store columns per CTA
 constexpr int cAhi = 0, cAlo = 64, cD = 128, cG = 192;
+// kernels that keep A in shared memory (the training pair, below) reserve the accumulator columns only
+constexpr int kColsDG = 128;
+constexpr int cDs = 0, cGs = 64;
 
 // ---- accumulator store --------------------------------------------------------------------------
-// The kernels keep their MMA A operands and accumulators in columns of 128 lanes, lane = tile row.
+// The kernels keep their MMA accumulators, and all but the training pair (A in shared memory, below) their
+// A operands, in columns of 128 lanes, lane = tile row.
 // Hopper keeps wgmma accumulators in registers, and an SM's shared memory is taken by the weight ring
 // and the staging buffers, so the columns live in global memory: kStoreSlots slabs of kStoreCols
 // columns x 128 lanes (lane-contiguous, so the 32 threads of a warp touch one 128-byte line per column;
@@ -132,19 +136,35 @@ __device__ __forceinline__ void ld4(uint32_t row, uint32_t col, float* v) {
   for (int i = 0; i < 4; ++i) v[i] = p[i * kStoreLanes];
 }
 
+// ---- A operands in shared memory ------------------------------------------------------------------
+// The training pair (nsf_logprob_tc_kernel<..., SAVE>, nsf_vjp_tc_kernel) runs one CTA per SM, which leaves
+// room for A_hi | A_lo (128 rows x 64 K-columns each, 32 KB each) in shared memory, so the MMAs read A
+// through a descriptor instead of waiting for fragment loads from the L2-resident store in every K-step.
+// Layout: wgmma's K-major no-swizzle canonical layout [k/4][128 rows][4], the convention of make_bdesc for
+// B: a core matrix (8 rows x 4 K-columns) is 128 contiguous bytes, 8-row groups are 128 B apart (SBO),
+// K-adjacent core matrices 128 x 16 B = 2048 B apart (LBO); a K-step of 8 columns advances 4096 B, and
+// warpgroup 1 (rows 64 ..) starts 1024 B in.  A row thread writes 4 consecutive columns as one float4,
+// so the 32 rows of a warp cover 512 contiguous bytes.
+constexpr int kAFloats = 64 * kRows;          // one half
+constexpr int kASmemFloats = 2 * kAFloats;    // A_hi | A_lo
+constexpr uint64_t kAStep = 4096u >> 4;       // descriptor start-address advance per K-step
+
 // ---- the MMAs: both warpgroups of the CTA, synchronously ------------------------------------------
 // Accumulator fragment of wgmma m64nNk8 (f32): warp w of the warpgroup holds rows 16w + g and
 // 16w + g + 8 (g = lane / 4), columns 8j + 2t and 8j + 2t + 1 (t = lane % 4) in d[4j .. 4j+3].
 //
-// D[store, M = 128] (+)= A[store] * B[smem]^T over nk K-steps, 3xTF32 (A_hi B_hi + A_lo B_hi + A_hi B_lo):
-// warpgroup wg computes rows 64 wg .. 64 wg + 63; A_hi / A_lo fragments come straight from the store.
-template <int N>
-__device__ __forceinline__ void mma_rows_n(uint32_t dcol, uint32_t ahcol, uint32_t alcol, uint64_t dh,
+// D[store, M = 128] (+)= A * B[smem]^T over nk K-steps, 3xTF32 (A_hi B_hi + A_lo B_hi + A_hi B_lo):
+// warpgroup wg computes rows 64 wg .. 64 wg + 63.  ASMEM = false: ah / al are the A_hi / A_lo store
+// columns of the first K-step and the fragments come straight from the store; ASMEM = true: ah / al are
+// the shared-memory descriptors of the warpgroup's first K-step.  Same products in the same order.
+template <int N, bool ASMEM>
+__device__ __forceinline__ void mma_rows_n(uint32_t dcol, uint64_t ah, uint64_t al, uint64_t dh,
                                            uint64_t dl, uint64_t dstep, int nk, uint32_t acc) {
   const int lane = threadIdx.x & 31, g = lane >> 2, t = lane & 3;
   const uint32_t r0 = (threadIdx.x >> 7) * 64 + ((threadIdx.x >> 5) & 3) * 16 + g;
   const uint32_t c0 = s_store_col;
-  dcol += c0; ahcol += c0; alcol += c0;
+  dcol += c0;
+  const uint32_t ahcol = (uint32_t)ah + c0, alcol = (uint32_t)al + c0;
   float* slab = s_store;
   float d[N / 2];
 #pragma unroll
@@ -156,25 +176,33 @@ __device__ __forceinline__ void mma_rows_n(uint32_t dcol, uint32_t ahcol, uint32
     d[4 * j + 3] = acc ? slab[(c + 1) * kStoreLanes + r0 + 8] : 0.f;
   }
   for (int kk = 0; kk < nk; ++kk) {
-    uint32_t ah[4], al[4];
-    const uint32_t ch = ahcol + 8 * kk + t, cl = alcol + 8 * kk + t;
-    ah[0] = __float_as_uint(slab[ch * kStoreLanes + r0]);
-    ah[1] = __float_as_uint(slab[ch * kStoreLanes + r0 + 8]);
-    ah[2] = __float_as_uint(slab[(ch + 4) * kStoreLanes + r0]);
-    ah[3] = __float_as_uint(slab[(ch + 4) * kStoreLanes + r0 + 8]);
-    al[0] = __float_as_uint(slab[cl * kStoreLanes + r0]);
-    al[1] = __float_as_uint(slab[cl * kStoreLanes + r0 + 8]);
-    al[2] = __float_as_uint(slab[(cl + 4) * kStoreLanes + r0]);
-    al[3] = __float_as_uint(slab[(cl + 4) * kStoreLanes + r0 + 8]);
     // each K-step into a fresh accumulator, correction terms first; the running sum is then carried
     // with round-to-nearest adds (the tensor core's own fp32 accumulation truncates)
     float p[N / 2];
 #pragma unroll
     for (int i = 0; i < N / 2; ++i) p[i] = 0.f;
-    wgmma_fence();
-    wgmma_rs<N>(p, al, dh, 0u);
-    wgmma_rs<N>(p, ah, dl, 1u);
-    wgmma_rs<N>(p, ah, dh, 1u);
+    if constexpr (ASMEM) {
+      wgmma_fence();
+      wgmma_ss<N>(p, al, dh, 0u);
+      wgmma_ss<N>(p, ah, dl, 1u);
+      wgmma_ss<N>(p, ah, dh, 1u);
+      ah += kAStep; al += kAStep;
+    } else {
+      uint32_t fh[4], fl[4];
+      const uint32_t ch = ahcol + 8 * kk + t, cl = alcol + 8 * kk + t;
+      fh[0] = __float_as_uint(slab[ch * kStoreLanes + r0]);
+      fh[1] = __float_as_uint(slab[ch * kStoreLanes + r0 + 8]);
+      fh[2] = __float_as_uint(slab[(ch + 4) * kStoreLanes + r0]);
+      fh[3] = __float_as_uint(slab[(ch + 4) * kStoreLanes + r0 + 8]);
+      fl[0] = __float_as_uint(slab[cl * kStoreLanes + r0]);
+      fl[1] = __float_as_uint(slab[cl * kStoreLanes + r0 + 8]);
+      fl[2] = __float_as_uint(slab[(cl + 4) * kStoreLanes + r0]);
+      fl[3] = __float_as_uint(slab[(cl + 4) * kStoreLanes + r0 + 8]);
+      wgmma_fence();
+      wgmma_rs<N>(p, fl, dh, 0u);
+      wgmma_rs<N>(p, fh, dl, 1u);
+      wgmma_rs<N>(p, fh, dh, 1u);
+    }
     wgmma_commit();
     wgmma_wait_all();
 #pragma unroll
@@ -190,17 +218,18 @@ __device__ __forceinline__ void mma_rows_n(uint32_t dcol, uint32_t ahcol, uint32
     slab[(c + 1) * kStoreLanes + r0 + 8] = d[4 * j + 3];
   }
 }
-__device__ __forceinline__ void mma_rows(int N, uint32_t dcol, uint32_t ahcol, uint32_t alcol, uint64_t dh,
+template <bool ASMEM>
+__device__ __forceinline__ void mma_rows(int N, uint32_t dcol, uint64_t ah, uint64_t al, uint64_t dh,
                                          uint64_t dl, uint64_t dstep, int nk, uint32_t acc) {
   switch (N) {
-    case 8: mma_rows_n<8>(dcol, ahcol, alcol, dh, dl, dstep, nk, acc); break;
-    case 16: mma_rows_n<16>(dcol, ahcol, alcol, dh, dl, dstep, nk, acc); break;
-    case 24: mma_rows_n<24>(dcol, ahcol, alcol, dh, dl, dstep, nk, acc); break;
-    case 32: mma_rows_n<32>(dcol, ahcol, alcol, dh, dl, dstep, nk, acc); break;
-    case 40: mma_rows_n<40>(dcol, ahcol, alcol, dh, dl, dstep, nk, acc); break;
-    case 48: mma_rows_n<48>(dcol, ahcol, alcol, dh, dl, dstep, nk, acc); break;
-    case 56: mma_rows_n<56>(dcol, ahcol, alcol, dh, dl, dstep, nk, acc); break;
-    case 64: mma_rows_n<64>(dcol, ahcol, alcol, dh, dl, dstep, nk, acc); break;
+    case 8: mma_rows_n<8, ASMEM>(dcol, ah, al, dh, dl, dstep, nk, acc); break;
+    case 16: mma_rows_n<16, ASMEM>(dcol, ah, al, dh, dl, dstep, nk, acc); break;
+    case 24: mma_rows_n<24, ASMEM>(dcol, ah, al, dh, dl, dstep, nk, acc); break;
+    case 32: mma_rows_n<32, ASMEM>(dcol, ah, al, dh, dl, dstep, nk, acc); break;
+    case 40: mma_rows_n<40, ASMEM>(dcol, ah, al, dh, dl, dstep, nk, acc); break;
+    case 48: mma_rows_n<48, ASMEM>(dcol, ah, al, dh, dl, dstep, nk, acc); break;
+    case 56: mma_rows_n<56, ASMEM>(dcol, ah, al, dh, dl, dstep, nk, acc); break;
+    case 64: mma_rows_n<64, ASMEM>(dcol, ah, al, dh, dl, dstep, nk, acc); break;
     default: __trap();      // operand blocks are planned with N in {8, ..., 64}
   }
 }
@@ -253,6 +282,20 @@ __device__ __forceinline__ void store_a4(uint32_t row, int col, const float (&v)
   for (int i = 0; i < 4; ++i) split_tf32(v[i], hi[i], lo[i]);
   st4(row, cAhi + col, hi);
   st4(row, cAlo + col, lo);
+}
+// the same into the shared-memory A region `as` (col % 4 == 0); the writer issues fence_async_smem()
+// before the CTA barrier that hands the operands to the MMAs
+__device__ __forceinline__ void smem_a4(float* as, uint32_t row, int col, const float (&v)[4]) {
+  float hi[4], lo[4];
+#pragma unroll
+  for (int i = 0; i < 4; ++i) split_tf32(v[i], hi[i], lo[i]);
+  float4* p = reinterpret_cast<float4*>(as + ((col >> 2) * kRows + row) * 4);
+  p[0] = make_float4(hi[0], hi[1], hi[2], hi[3]);
+  p[kAFloats / 4] = make_float4(lo[0], lo[1], lo[2], lo[3]);
+}
+__device__ __forceinline__ void smem_a8(float* as, uint32_t row, int col, const float (&v)[8]) {
+  smem_a4(as, row, col, {v[0], v[1], v[2], v[3]});
+  smem_a4(as, row, col + 4, {v[4], v[5], v[6], v[7]});
 }
 __device__ __forceinline__ void group_sync() { asm volatile("bar.sync 1, 256;" ::: "memory"); }
 
@@ -315,11 +358,12 @@ static int pack_weights(const float* params, const sbi_nsf_tc* tc, cudaStream_t 
 // once end() returns.  The weight stream rotates between the warps (stage k is fetched by the
 // elected lane of warp (k + 4) % 8).  Stage k lives in ring slot k % NSLOT.  A stage is fetched
 // (TMA bulk copy, completion on full[slot]) by the end() of the stage that used its slot NSLOT stages
-// earlier.
-template <int NSLOT>
+// earlier.  ASMEM: A comes from the shared-memory A region at `abase`, else from the store.
+template <int NSLOT, bool ASMEM = false>
 struct IssuerT {
   bool leader;          // the elected lane of this warp
   int warp;             // this warp; stage k is fetched by warp (k+4) % 8
+  uint32_t abase;       // ASMEM: shared address of the A region
   float* ring;
   uint64_t* full;
   const float* tcw;
@@ -361,7 +405,15 @@ struct IssuerT {
     const uint64_t dh = make_bdesc(bh, slab, 128u);
     const uint64_t dl = make_bdesc(bh + lo_off, slab, 128u);
     const uint64_t dstep = (uint64_t)((2u * slab) >> 4);    // start-address field advance per K-step
-    if (nk > 0) mma_rows(N, dcol, cAhi + a0, cAlo + a0, dh, dl, dstep, nk, acc);
+    if constexpr (ASMEM) {
+      // column a0 (a multiple of 4) of the warpgroup's first row
+      const uint32_t ah = abase + (uint32_t)a0 * (kRows * 4u) + (threadIdx.x >> 7) * 1024u;
+      if (nk > 0)
+        mma_rows<true>(N, dcol, make_bdesc(ah, kRows * 16u, 128u), make_bdesc(ah + kAFloats * 4u, kRows * 16u, 128u),
+                       dh, dl, dstep, nk, acc);
+    } else {
+      if (nk > 0) mma_rows<false>(N, dcol, cAhi + a0, cAlo + a0, dh, dl, dstep, nk, acc);
+    }
     if (nk > 0) acc = 1u;
   }
   // close the stage: after the CTA barrier its accumulators are in the store and its ring slot is free
@@ -376,20 +428,23 @@ using Issuer = IssuerT<kSlots>;
 // Kernel prologue, all threads: thread 0 initialises the ring's mbarriers full[0 .. NSLOT) (and any
 // other mbarrier the kernel initialised before the call), warp 0 reserves `ncols` store columns, and
 // after the CTA barrier the issuer starts fetching the first NSLOT stages of the CTA's first tile.
-template <int NSLOT>
-__device__ __forceinline__ IssuerT<NSLOT> tc_begin(uint64_t* full, float* ring, const sbi_nsf_tc& tc, int T,
-                                                   int64_t ntiles, bool reverse, int ncols, const StoreArgs& sa) {
+// ASMEM: `as` is the shared-memory A region (kASmemFloats floats, 16-byte aligned).
+template <int NSLOT, bool ASMEM = false>
+__device__ __forceinline__ IssuerT<NSLOT, ASMEM> tc_begin(uint64_t* full, float* ring, const sbi_nsf_tc& tc, int T,
+                                                          int64_t ntiles, bool reverse, int ncols, const StoreArgs& sa,
+                                                          float* as = nullptr) {
   if (threadIdx.x == 0) {
     for (int s = 0; s < NSLOT; ++s) mbar_init(&full[s], 1);
     fence_barrier_init();
   }
   if (threadIdx.x < 32) store_alloc(ncols, sa);
   __syncthreads();
-  IssuerT<NSLOT> iss;
+  IssuerT<NSLOT, ASMEM> iss;
   uint32_t el = 0;
   asm volatile("{\n\t.reg .pred p;\n\telect.sync _|p, 0xffffffff;\n\tselp.u32 %0, 1, 0, p;\n\t}" : "=r"(el));
   iss.leader = el != 0;
   iss.warp = threadIdx.x >> 5;
+  iss.abase = ASMEM ? smem_u32(as) : 0u;
   iss.ring = ring; iss.full = full;
   iss.tcw = tc.d_tcw; iss.tab = tc.d_tab; iss.cap = tc.stage_cap; iss.T = T;
   iss.it = 0; iss.fetched = 0;
