@@ -71,11 +71,33 @@ inline int set_smem(const void* kernel, int bytes) {
   return 0;
 }
 
+// Grid of a launch: `ctas` CTAs along x, in clusters of `cluster` CTAs (1: no clusters).
+struct Grid {
+  int ctas, cluster;
+  Grid(int n, int c = 1) : ctas(n), cluster(c) {}
+};
+
 // Opt `kernel` into `smem_bytes` of dynamic shared memory, launch it and return the launch status.
 template <class... P, class... A>
-int launch(void (*kernel)(P...), int grid, int threads, int smem_bytes, cudaStream_t s, A&&... args) {
+int launch(void (*kernel)(P...), Grid grid, int threads, int smem_bytes, cudaStream_t s, A&&... args) {
   if (int e = set_smem(reinterpret_cast<const void*>(kernel), smem_bytes)) return e;
-  kernel<<<grid, threads, smem_bytes, s>>>(std::forward<A>(args)...);
+  if (grid.cluster > 1) {
+    cudaLaunchAttribute at;
+    at.id = cudaLaunchAttributeClusterDimension;
+    at.val.clusterDim.x = (unsigned)grid.cluster;
+    at.val.clusterDim.y = 1;
+    at.val.clusterDim.z = 1;
+    cudaLaunchConfig_t cfg = {};
+    cfg.gridDim = dim3((unsigned)grid.ctas);
+    cfg.blockDim = dim3((unsigned)threads);
+    cfg.dynamicSmemBytes = (size_t)smem_bytes;
+    cfg.stream = s;
+    cfg.attrs = &at;
+    cfg.numAttrs = 1;
+    cudaLaunchKernelEx(&cfg, kernel, std::forward<A>(args)...);
+  } else {
+    kernel<<<grid.ctas, threads, smem_bytes, s>>>(std::forward<A>(args)...);
+  }
   return (int)cudaGetLastError();
 }
 

@@ -27,6 +27,9 @@
 // the final layer's spline parameters P (32 columns per feature, 2 features per pass)
 // alternate between D and G.  The training forward (SAVE) runs one CTA per SM (one tile each), keeps
 // A_hi / A_lo in shared memory (tc_common.cuh) and reserves only [0,64) D | [64,128) G of the store.
+// When a chunk of tiles would leave SMs idle, the training forward runs two CTAs per tile, one per 64-row
+// half (RPC = 64): four threads per row, both warpgroups on the CTA's 64 rows (tc_common.cuh), lanes 0..63
+// of the store columns, and the tile's save slab at lanes [64 r, 64 r + 64) for half r.
 #include <cuda_runtime.h>
 #include <math.h>
 #include <algorithm>
@@ -44,30 +47,36 @@ namespace tc {
 
 // ---- shared memory plan -------------------------------------------------------------------------
 struct TcSmem {
-  int zs, ctx, lds, lum, bias, bias_stride, a, ring;   // float offsets
+  int zs, ctx, lds, ldf, lum, bias, bias_stride, a, ring;   // float offsets
   int bar_bytes, total_bytes;
 };
-// a_smem: the training forward (SAVE) also keeps its A operands in shared memory (tc_common.cuh)
-__host__ __device__ inline TcSmem tc_smem_layout(const sbi_nsf_model& m, int stage_cap, bool a_smem) {
+// a_smem: the training forward (SAVE) also keeps its A operands in shared memory (tc_common.cuh);
+// rpc: rows per CTA (128, or 64 for the training forward's half tiles)
+__host__ __device__ inline TcSmem tc_smem_layout(const sbi_nsf_model& m, int stage_cap, bool a_smem, int rpc = kRows) {
   TcSmem L;
   int fl = 0;
-  L.zs = fl;  fl += m.Dp * kRows;
-  L.ctx = fl; fl += m.Cp * kRows;
-  L.lds = fl; fl += kRows;
+  L.zs = fl;  fl += m.Dp * rpc;
+  L.ctx = fl; fl += m.Cp * rpc;
+  L.lds = fl; fl += rpc;
+  L.ldf = fl; fl += rpc < kRows ? kLuMax * rpc : 0;     // half tiles: log|det| per spline feature of a layer
   L.lum = fl; fl += 2 * kLuMax * kLuMax + 2 * kLuMax;   // [U 16x16 | L 16x16 | bias 16 | diag 16]
   L.bias_stride = 64 + m.NB * 192 + m.TRmax * 32;
   L.bias = fl; fl += m.T * L.bias_stride;
   fl = (fl + 31) & ~31;
-  L.a = fl;   fl += a_smem ? kASmemFloats : 0;
+  L.a = fl;   fl += a_smem ? a_smem_floats(rpc) : 0;
   L.ring = fl; fl += kSlots * stage_cap;
   L.bar_bytes = fl * 4;
   L.total_bytes = L.bar_bytes + kSlots * 8;
   return L;
 }
 
-// Two threads share a row: `half` 0 owns hidden columns [0, HP8/2), `half` 1 owns [HP8/2, HP8)
+// Two threads share a row: part `tq` 0 owns hidden columns [0, HP8/2), part 1 owns [HP8/2, HP8)
 // (which end in the first context columns).  All epilogues are column-wise, so the
-// halves never exchange activations; the spline features of a layer alternate between them.
+// parts never exchange activations; the spline features of a layer alternate between them.
+// Half tiles (RPC = 64, training forward only) have four threads per row, part tq owning columns
+// [16 tq, 16 tq + 16); part 3 holds the last hidden columns, the context and the zero tail.  The spline
+// features go round-robin over the four parts, which leave each feature's log|det| in shared memory;
+// parts 0 and 1 add them up in the order of the two-part split, so every row's result is bit-identical.
 //
 // Per coupling layer the tensor core sees these stages (result columns after the arrow):
 //   initial layer -> D
@@ -84,7 +93,7 @@ __host__ __device__ inline TcSmem tc_smem_layout(const sbi_nsf_model& m, int sta
 // parameters, layer input and coupling output of the tile go to the activation scratch `save`
 // (layout: nsf_tc_save.cuh) for the tensor-core backward and weight-gradient kernels (nsf_vjp_tc.cu),
 // together with the final base-space point and the row's log-density.
-template <int H, int KB, bool INV, bool SAVE = false>
+template <int H, int KB, bool INV, bool SAVE = false, int RPC = kRows>
 __global__ void __launch_bounds__(kThreads, SAVE ? 1 : 2)
 nsf_logprob_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_constant__ sbi_nsf_tc tc,
                       const __grid_constant__ sbi_rows rows, float* __restrict__ logp,
@@ -92,33 +101,38 @@ nsf_logprob_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_cons
   constexpr int HP8 = (H + 7) & ~7;
   constexpr int NCH = HP8 / 8;      // K-steps / 8-column chunks of the hidden operand
   constexpr int KC0 = H / 8;        // first chunk that holds context columns
-  constexpr int NC = HP8 / 2;       // hidden columns per thread (half 0: [0,NC), half 1: [NC,HP8))
+  constexpr int TPR = kThreads / RPC;                   // threads per row
+  constexpr int UPT = kRows / RPC;                      // CTAs per tile
+  constexpr int NC = TPR == 2 ? HP8 / 2 : 16;           // hidden columns per thread ([tq NC, tq NC + NC))
   constexpr int NG = NC / 4;        // groups of 4 columns
-  constexpr int QC = H - NC;        // first column offset of half 1 that is a context column
-  static_assert(HP8 % 8 == 0 && NC % 4 == 0 && H > NC && H <= 64, "hidden width");
+  constexpr int QC = H - (TPR - 1) * NC;                // first column offset of the last part that is context
+  static_assert(HP8 % 8 == 0 && NC % 4 == 0 && QC > 0 && QC <= NC && H <= 64, "hidden width");
+  static_assert(!(RPC < kRows) || (SAVE && !INV), "half tiles are a layout of the training forward");
   extern __shared__ __align__(128) float sm[];
-  const TcSmem L = tc_smem_layout(m, tc.stage_cap, SAVE);
+  const TcSmem L = tc_smem_layout(m, tc.stage_cap, SAVE, RPC);
   uint64_t* full = reinterpret_cast<uint64_t*>(reinterpret_cast<char*>(sm) + L.bar_bytes);
   const int tid = threadIdx.x, warp = tid >> 5;
   const int C = m.C;
   const int nkc = (H + C + 7) / 8 - KC0;     // K-steps that cover the context columns
-  const int64_t ntiles = (rows.R + kRows - 1) / kRows;
+  const int64_t nunits = (rows.R + kRows - 1) / kRows * UPT;     // CTA tiles of RPC rows
   const TcSave SV = tc_save_layout(m.NB, m.TRmax, m.T);
 
   // SAVE: A in shared memory, the store holds D | G only
   constexpr int ncols = SAVE ? kColsDG : kCols;
   constexpr int kD = SAVE ? cDs : cD, kG = SAVE ? cGs : cG;
   float* as = sm + L.a;
-  IssuerT<kSlots, SAVE> iss = tc_begin<kSlots, SAVE>(full, sm + L.ring, tc, m.T, ntiles, INV, ncols, sa, as);
+  IssuerT<kSlots, SAVE, RPC> iss = tc_begin<kSlots, SAVE, RPC>(full, sm + L.ring, tc, m.T, nunits, INV, ncols, sa, as);
 
   const float* __restrict__ P = m.d_params;
   float* zs = sm + L.zs;
   float* ctx_s = sm + L.ctx;
   float* lds = sm + L.lds;
+  float* ldf = sm + L.ldf;
   const float* bias_s = sm + L.bias;
-  const int half = warp >> 2;                          // which column half of the row
-  const int row = ((warp & 3) << 5) | (tid & 31);      // row of the tile = store lane
-  const int cbase = half * NC;                          // first hidden column of this thread
+  const int tq = RPC == kRows ? warp >> 2 : warp >> 1;                      // which column part of the row
+  const int row = ((RPC == kRows ? warp & 3 : warp & 1) << 5) | (tid & 31);  // row of the CTA = store lane
+  const int cbase = tq * NC;                               // first hidden column of this thread
+  const int last = TPR == 2 ? tq : tq == TPR - 1;          // nonzero: the part that holds the context columns
   RqsConst rc = rqs_const(m);
   rc.K = KB;
   const int D = m.D;
@@ -145,7 +159,7 @@ nsf_logprob_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_cons
   }
   // batch-constant part of the log-density, summed in the order of lu_logdet_total (nsf.cuh)
   float ld_const = 0.f;
-  if (half == 1) {
+  if (tq == 1) {
     float tot = 0.f;
     for (int l = 0; l < m.T; ++l) {
       const int* LT = m.d_layer_tab + l * SBI_NSF_LAYER_STRIDE;
@@ -159,11 +173,11 @@ nsf_logprob_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_cons
   }
 
   auto put_a4 = [&](int col, const float (&a)[4]) {
-    if constexpr (SAVE) smem_a4(as, row, col, a);
+    if constexpr (SAVE) smem_a4<RPC>(as, row, col, a);
     else store_a4(row, col, a);
   };
   auto put_a8 = [&](int col, const float (&a)[8]) {
-    if constexpr (SAVE) smem_a8(as, row, col, a);
+    if constexpr (SAVE) smem_a8<RPC>(as, row, col, a);
     else store_a8(row, col, a);
   };
   // operands written: hand them over to the MMAs
@@ -174,18 +188,20 @@ nsf_logprob_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_cons
   // A-operand column j of a hidden layer: activation (j < H), context (H <= j < H+C), zero
   auto acol = [&](int j, float act) -> float {
     const int c = j - H;
-    return j < H ? act : ((c < C) ? ctx_s[c * kRows + row] : 0.f);
+    return j < H ? act : ((c < C) ? ctx_s[c * RPC + row] : 0.f);
   };
-  // this thread's NC columns of a hidden-layer A operand; half 1's last columns are context
+  // this thread's NC columns of a hidden-layer A operand; the last part's last columns are context
+  // (columns from HP8 on are the tail, written once per tile)
   auto write_a = [&](const float (&act)[NC]) {
 #pragma unroll
     for (int g = 0; g < NG; ++g) {
+      if (TPR * NC > HP8 && cbase + 4 * g >= HP8) continue;
       float a[4];
 #pragma unroll
       for (int i = 0; i < 4; ++i) {
         const int q = 4 * g + i;
         if (q < QC) a[i] = act[q];
-        else a[i] = half ? ((q - QC < C) ? ctx_s[(q - QC) * kRows + row] : 0.f) : act[q];
+        else a[i] = last ? ((q - QC < C) ? ctx_s[(q - QC) * RPC + row] : 0.f) : act[q];
       }
       put_a4(cbase + 4 * g, a);
     }
@@ -195,13 +211,15 @@ nsf_logprob_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_cons
     for (int g = 0; g < NG; ++g) ld4(row, region + cbase + 4 * g, d + 4 * g);
   };
 
-  for (int64_t tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
-    const int64_t row0 = tile * kRows;
-    // ---- load + standardise the tile's rows (arithmetic of load_rows, stages.cuh) ----
+  for (int64_t unit = blockIdx.x; unit < nunits; unit += gridDim.x) {
+    const int64_t tile = unit / UPT;                        // 128-row tile (save slab)
+    const int srow = (int)(unit % UPT) * RPC + row;         // lane of the row in the tile's save slab
+    const int64_t row0 = unit * RPC;
+    // ---- load + standardise the CTA's rows (arithmetic of load_rows, stages.cuh) ----
     {
       const float* st = m.d_stats;
       const int Dp = m.Dp, Cp = m.Cp;
-      for (int e = tid; e < kRows * Dp; e += kThreads) {
+      for (int e = tid; e < RPC * Dp; e += kThreads) {
         const int r = e / Dp, d = e % Dp;
         const int64_t gr = row0 + r;
         float val = 0.f;
@@ -210,9 +228,9 @@ nsf_logprob_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_cons
           const float x = __ldg(rows.d_input + src * D + d);
           val = INV ? x : __fadd_rn(__fmul_rn(x, __ldg(st + Dp + d)), __ldg(st + d));
         }
-        zs[d * kRows + r] = val;
+        zs[d * RPC + r] = val;
       }
-      for (int e = tid; e < kRows * Cp; e += kThreads) {
+      for (int e = tid; e < RPC * Cp; e += kThreads) {
         const int r = e / Cp, c = e % Cp;
         const int64_t gr = row0 + r;
         float val = 0.f;
@@ -220,13 +238,13 @@ nsf_logprob_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_cons
           const int64_t src = rows.cond_shared ? 0 : (rows.d_index ? __ldg(rows.d_index + gr) : gr);
           val = (__ldg(rows.d_cond + src * C + c) - __ldg(st + 2 * Dp + c)) / __ldg(st + 2 * Dp + Cp + c);
         }
-        ctx_s[c * kRows + r] = val;
+        ctx_s[c * RPC + r] = val;
       }
       if (INV) prep_lu(m, m.T - 1, sm + L.lum);
       group_sync();
     }
     // context tail columns [HP8, 64) never change within a tile
-    if (half == 0) {
+    if (tq == 0) {
 #pragma unroll
       for (int c = NCH; c < 8; ++c) {
         float v[8];
@@ -247,17 +265,17 @@ nsf_logprob_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_cons
       int stage = 0;
       float h[NC];
       float* svl = SAVE ? save + (size_t)tile * SV.tile_stride + (size_t)l * SV.layer_stride : nullptr;
-      if (SAVE && half == 1) tc_save_row16(svl + SV.zin, row, zs, D);      // layer input z_l
+      if (SAVE && tq == 1) tc_save_row16<RPC>(svl + SV.zin, srow, zs, row, D);      // layer input z_l
 
       // ---- sampling: z <- U^{-1} L^{-1} (z - b) on the thread's row (order of lu_inverse, nsf.cuh)
-      if (INV && half == 1 && __ldg(v.LT + SBI_L_HAS_LU)) {
+      if (INV && tq == 1 && __ldg(v.LT + SBI_L_HAS_LU)) {
         const float4* U4 = reinterpret_cast<const float4*>(sm + L.lum);
         const float4* L4 = U4 + kLuMax * kLuMax / 4;
         const float* bias = sm + L.lum + 2 * kLuMax * kLuMax;
         const float* diag = bias + kLuMax;
         float zr[kLuMax];
 #pragma unroll
-        for (int j = 0; j < kLuMax; ++j) zr[j] = (j < D) ? zs[j * kRows + row] : 0.f;
+        for (int j = 0; j < kLuMax; ++j) zr[j] = (j < D) ? zs[j * RPC + row] : 0.f;
 #pragma unroll
         for (int i = 0; i < kLuMax; ++i) {
           if (i < D) {
@@ -286,23 +304,23 @@ nsf_logprob_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_cons
               if (4 * j4 + 3 > i) a -= w.w * zr[4 * j4 + 3];
             }
             zr[i] = a / diag[i];
-            zs[i * kRows + row] = zr[i];
+            zs[i * RPC + row] = zr[i];
           }
         }
       }
       // ---- initial layer: A = [identity features | 0 ... | context] ----
-      // (half 1 ran the LU on this row, so it also writes the identity columns)
-      if (half == 1) {
+      // (part 1 ran the LU on this row, so it also writes the identity columns)
+      if (tq == 1) {
         for (int kk = 0; kk < kid8 / 8; ++kk) {
           float a[8];
 #pragma unroll
           for (int i = 0; i < 8; ++i) {
             const int j = 8 * kk + i;
-            a[i] = (j < v.n_id) ? zs[__ldg(v.idf + j) * kRows + row] : 0.f;
+            a[i] = (j < v.n_id) ? zs[__ldg(v.idf + j) * RPC + row] : 0.f;
           }
           put_a8(8 * kk, a);
         }
-      } else {
+      } else if (TPR == 2 || tq == 0) {
 #pragma unroll
         for (int c = KC0; c < NCH; ++c) {
           float a[8];
@@ -341,7 +359,7 @@ nsf_logprob_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_cons
         const float* b2 = b1 + 64;
         const float* bc = b1 + 128;
         // A = [relu(h) | ctx]
-        if (SAVE) tc_save_cols<NC>(svl + SV.h(b), row, half, h);
+        if (SAVE) tc_save_cols<NC>(svl + SV.h(b), srow, tq, h);
         {
           float a[NC];
 #pragma unroll
@@ -368,7 +386,7 @@ nsf_logprob_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_cons
           read_acc(kG, g);
 #pragma unroll
           for (int q = 0; q < NC; ++q) sg[q] = sigmoid_fast(g[q] + bc[q]);
-          if (SAVE) tc_save_cols<NC>(svl + SV.s(b), row, half, sg);
+          if (SAVE) tc_save_cols<NC>(svl + SV.s(b), srow, tq, sg);
         }
         SBI_TL(1000 * (li + 1) + 10 * b + 14);
         {
@@ -376,7 +394,7 @@ nsf_logprob_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_cons
           read_acc(kD, d);
 #pragma unroll
           for (int q = 0; q < NC; ++q) d[q] = relu_f(d[q] + b1[q]);
-          if (SAVE) tc_save_cols<NC>(svl + SV.a1(b), row, half, d);
+          if (SAVE) tc_save_cols<NC>(svl + SV.a1(b), srow, tq, d);
           write_a(d);
         }
         hand_over();
@@ -395,7 +413,7 @@ nsf_logprob_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_cons
           if (SAVE) {
 #pragma unroll
             for (int q = 0; q < NC; ++q) d[q] += b2[q];
-            tc_save_cols<NC>(svl + SV.t2(b), row, half, d);
+            tc_save_cols<NC>(svl + SV.t2(b), srow, tq, d);
 #pragma unroll
             for (int q = 0; q < NC; ++q) h[q] = fmaf(d[q], sg[q], h[q]);
           } else {
@@ -408,7 +426,7 @@ nsf_logprob_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_cons
 
       // ---- final layer passes + spline on the transformed features ----
       {
-        if (SAVE) tc_save_cols<NC>(svl + SV.hf, row, half, h);
+        if (SAVE) tc_save_cols<NC>(svl + SV.hf, srow, tq, h);
         write_a(h);
         const float* bf = bl + 64 + m.NB * 192;
         const int ns = __ldg(tab);
@@ -427,20 +445,21 @@ nsf_logprob_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_cons
           const int aux = __ldg(tab + 7 + 4 * (stage + p));
           const int f0 = aux & 0xffff, nf = aux >> 16;
           for (int f = 0; f < nf; ++f) {
-            if (((f0 + f) & 1) != half) continue;     // warp-uniform: features alternate between halves
+            if (((f0 + f) & (TPR - 1)) != tq) continue;     // warp-uniform: features go round-robin over the parts
             float q[32];
             ld_cols<4>(row, kD + 64 * (p & 1) + 32 * f, q);
             const float* bff = bf + (f0 + f) * 32;
 #pragma unroll
             for (int i = 0; i < 32; ++i) q[i] = (i < 3 * KB - 1) ? q[i] + bff[i] : 0.f;
-            if (SAVE) tc_save_prm(svl + SV.prm, row, m.TRmax, f0 + f, q);
+            if (SAVE) tc_save_prm(svl + SV.prm, srow, m.TRmax, f0 + f, q);
             const int j = __ldg(v.trf + f0 + f);
-            const float x = zs[j * kRows + row];
+            const float x = zs[j * RPC + row];
             float y, ld;
             if (INV) rqs_inverse_fast<KB>(q, rc, x, y, ld);
             else rqs_forward_fast<KB>(q, rc, x, y, ld);
-            zs[j * kRows + row] = y;
-            ldacc += ld;
+            zs[j * RPC + row] = y;
+            if (TPR == 2) ldacc += ld;
+            else ldf[(f0 + f) * RPC + row] = ld;
           }
           SBI_TL(1000 * (li + 1) + 41 + p);
           if (p + 2 < np) {
@@ -456,18 +475,20 @@ nsf_logprob_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_cons
         }
       }
 
-      // ---- LULinear on the row (half 1: it has one spline feature less, and it also writes the
+      // ---- LULinear on the row (part 1: it has one spline feature less, and it also writes the
       //      next layer's identity columns):  z <- L (U z) + b, in place ----
-      group_sync();      // both halves' spline outputs are in zs
+      group_sync();      // all parts' spline outputs are in zs
       SBI_TL(1000 * (li + 1) + 50);
-      if (SAVE && half == 1) tc_save_row16(svl + SV.v, row, zs, D);         // coupling output v_l
-      if (!INV && half == 1 && __ldg(v.LT + SBI_L_HAS_LU)) {
+      if (TPR > 2 && tq < 2)      // parts 0 / 1 take the even / odd features' log|det|, in feature order
+        for (int k = tq; k < v.n_tr; k += 2) ldacc += ldf[k * RPC + row];
+      if (SAVE && tq == 1) tc_save_row16<RPC>(svl + SV.v, srow, zs, row, D);         // coupling output v_l
+      if (!INV && tq == 1 && __ldg(v.LT + SBI_L_HAS_LU)) {
         const float4* U4 = reinterpret_cast<const float4*>(sm + L.lum);
         const float4* L4 = U4 + kLuMax * kLuMax / 4;
         const float* bias = sm + L.lum + 2 * kLuMax * kLuMax;
         float zr[kLuMax];
 #pragma unroll
-        for (int j = 0; j < kLuMax; ++j) zr[j] = (j < D) ? zs[j * kRows + row] : 0.f;
+        for (int j = 0; j < kLuMax; ++j) zr[j] = (j < D) ? zs[j * RPC + row] : 0.f;
         // y = U z (upper triangular incl. diagonal; padded entries are zero), same j order as
         // lu_forward (nsf.cuh)
 #pragma unroll
@@ -499,7 +520,7 @@ nsf_logprob_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_cons
               if (4 * j4 + 3 < i) a = fmaf(w.w, zr[4 * j4 + 3], a);
             }
             zr[i] = a + bias[i];
-            zs[i * kRows + row] = zr[i];
+            zs[i * RPC + row] = zr[i];
           }
         }
       }
@@ -507,25 +528,25 @@ nsf_logprob_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_cons
 
     // ---- base density ----
     SBI_TL(9000);
-    if (half == 0) lds[row] = ldacc;
+    if (tq == 0) lds[row] = ldacc;
     group_sync();
-    if (half == 1 && row0 + row < rows.R) {
+    if (tq == 1 && row0 + row < rows.R) {
       if (!INV) {
         float ss = 0.f;
-        for (int d = 0; d < D; ++d) ss = fmaf(zs[d * kRows + row], zs[d * kRows + row], ss);
+        for (int d = 0; d < D; ++d) ss = fmaf(zs[d * RPC + row], zs[d * RPC + row], ss);
         const float lp = -0.5f * ss + (lds[row] + ldacc) + ld_const;
         if (logp != nullptr) logp[row0 + row] = lp;
         if (SAVE) {
-          tc_save_row16(save + (size_t)tile * SV.tile_stride + SV.zt, row, zs, D);
+          tc_save_row16<RPC>(save + (size_t)tile * SV.tile_stride + SV.zt, srow, zs, row, D);
           float* lpt = save + (size_t)tile * SV.tile_stride + SV.lp;
-          lpt[row] = lp;
+          lpt[srow] = lp;
         }
         if (noise != nullptr)
-          for (int d = 0; d < D; ++d) noise[(row0 + row) * D + d] = zs[d * kRows + row];
+          for (int d = 0; d < D; ++d) noise[(row0 + row) * D + d] = zs[d * RPC + row];
       } else {
         const float* st = m.d_stats;
         for (int d = 0; d < D; ++d)
-          noise[(row0 + row) * D + d] = (zs[d * kRows + row] - __ldg(st + d)) / __ldg(st + m.Dp + d);
+          noise[(row0 + row) * D + d] = (zs[d * RPC + row] - __ldg(st + d)) / __ldg(st + m.Dp + d);
         if (logp != nullptr) logp[row0 + row] = (lds[row] + ldacc) + ld_const;
       }
     }
@@ -596,16 +617,20 @@ extern "C" int sbi_b200_nsf_logprob_tc(const sbi_nsf_model* m, const sbi_nsf_tc*
 }
 
 int sbi::tc::launch_forward_save(const sbi_nsf_model* m, const sbi_nsf_tc* tc, const sbi_rows* rows, float* d_logp,
-                                 float* d_save, cudaStream_t s) {
+                                 float* d_save, bool half_tiles, cudaStream_t s) {
   tc::StoreArgs sa;
   if (int e = tc::store_args(&sa)) return e;
-  const int grid = (int)((rows->R + tc::kRows - 1) / tc::kRows);      // one tile per CTA: `d_save` slab = blockIdx
-  return launch(tc::nsf_logprob_tc_kernel<50, 10, false, true>, grid, tc::kThreads,
-                tc::forward_save_smem_bytes(*m, *tc), s, *m, *tc, *rows, d_logp, nullptr, d_save, sa);
+  // one tile per CTA (`d_save` slab = blockIdx), or two CTAs per tile (slab = blockIdx / 2)
+  const int tiles = (int)((rows->R + tc::kRows - 1) / tc::kRows);
+  if (half_tiles)
+    return launch(tc::nsf_logprob_tc_kernel<50, 10, false, true, 64>, 2 * tiles, tc::kThreads,
+                  tc::forward_save_smem_bytes(*m, *tc, 64), s, *m, *tc, *rows, d_logp, nullptr, d_save, sa);
+  return launch(tc::nsf_logprob_tc_kernel<50, 10, false, true>, tiles, tc::kThreads,
+                tc::forward_save_smem_bytes(*m, *tc, tc::kRows), s, *m, *tc, *rows, d_logp, nullptr, d_save, sa);
 }
 
-int sbi::tc::forward_save_smem_bytes(const sbi_nsf_model& m, const sbi_nsf_tc& tc) {
-  return tc::tc_smem_layout(m, tc.stage_cap, true).total_bytes;
+int sbi::tc::forward_save_smem_bytes(const sbi_nsf_model& m, const sbi_nsf_tc& tc, int rpc) {
+  return tc::tc_smem_layout(m, tc.stage_cap, true, rpc).total_bytes;
 }
 
 extern "C" int sbi_b200_nsf_inverse_tc(const sbi_nsf_model* m, const sbi_nsf_tc* tc,

@@ -100,14 +100,15 @@ __device__ __forceinline__ void tc_load_prm(const float* q, int row, int TRmax, 
     v[4 * i] = t.x; v[4 * i + 1] = t.y; v[4 * i + 2] = t.z; v[4 * i + 3] = t.w;
   }
 }
-// the row's D <= 16 values of a feature-major shared tile zs[d][128]
-__device__ __forceinline__ void tc_save_row16(float* q, int row, const float* zs, int D) {
+// the D <= 16 values of row `row` of a feature-major shared array zs[d][RPC], into lane `lane`
+template <int RPC>
+__device__ __forceinline__ void tc_save_row16(float* q, int lane, const float* zs, int row, int D) {
 #pragma unroll
   for (int i = 0; i < 4; ++i) {
     float t[4];
 #pragma unroll
-    for (int j = 0; j < 4; ++j) t[j] = (4 * i + j < D) ? zs[(4 * i + j) * 128 + row] : 0.f;
-    __stcg(tc_grp(q, i, row), make_float4(t[0], t[1], t[2], t[3]));
+    for (int j = 0; j < 4; ++j) t[j] = (4 * i + j < D) ? zs[(4 * i + j) * RPC + row] : 0.f;
+    __stcg(tc_grp(q, i, lane), make_float4(t[0], t[1], t[2], t[3]));
   }
 }
 __device__ __forceinline__ void tc_load_row16(const float* q, int row, float (&v)[16]) {
@@ -122,12 +123,12 @@ __device__ __forceinline__ float tc_load_row16_at(const float* q, int row, int j
   return __ldcg(q + ((j >> 2) * 128 + row) * 4 + (j & 3));
 }
 
-// forward sweep of a training step: nsf_logprob_tc_kernel<50, 10, false, SAVE = true>, one tile per CTA
-// (defined in nsf_tc.cu; returns a C-ABI status code)
+// forward sweep of a training step: nsf_logprob_tc_kernel<50, 10, false, SAVE = true>, one tile per CTA, or
+// with `half_tiles` two CTAs of 64 rows per tile (defined in nsf_tc.cu; returns a C-ABI status code)
 int launch_forward_save(const sbi_nsf_model* m, const sbi_nsf_tc* tc, const sbi_rows* rows, float* d_logp,
-                        float* d_save, cudaStream_t s);
-// dynamic shared memory of that launch (its A operands live in shared memory)
-int forward_save_smem_bytes(const sbi_nsf_model& m, const sbi_nsf_tc& tc);
+                        float* d_save, bool half_tiles, cudaStream_t s);
+// dynamic shared memory of that launch with `rpc` rows per CTA (its A operands live in shared memory)
+int forward_save_smem_bytes(const sbi_nsf_model& m, const sbi_nsf_tc& tc, int rpc);
 
 }  // namespace tc
 }  // namespace sbi

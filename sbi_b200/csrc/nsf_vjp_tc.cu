@@ -23,7 +23,7 @@
 //   * COND instantiation only: the condition gradient d(sum g log q)/d ctx in raw condition space, accumulated
 //     per row over the T layers from the context columns of the initial layer (dh W0[:, :C]) and the GLU
 //     context layer of every residual block (dG Wc).  dh / dG of the whole row are read back from the dY region
-//     after the CTA barrier that follows their write, so each of the row's two threads takes half of the C
+//     after the CTA barrier that follows their write, so each of the row's threads takes its share of the C
 //     features over all H columns, on the CUDA cores from the fp32 parameters (C is small next to H), and
 //     accumulates them in place in d_gcond: every entry has one owner thread and a fixed summation order.
 //
@@ -39,6 +39,12 @@
 //
 // Store columns of the backward (128): [0,64) D | [64,128) G.  One A set serves every MMA: each pass's MMAs
 // complete (wgmma wait) before the CTA barrier of Issuer::end(), and the next operands are written after it.
+//
+// Half tiles (RPC = 64, when a chunk of tiles would leave SMs idle): two CTAs per tile, launched as a
+// 2-CTA cluster, CTA r owning tile rows [64 r, 64 r + 64) with four threads per row (the layout of the
+// forward's half tiles, nsf_tc.cu).  Everything is per row except the LULinear parameter gradients, which
+// sum over the tile's 128 rows: after a cluster barrier CTA 0 reads CTA 1's rows through distributed shared
+// memory and runs the same reductions in the same order.
 #include <cuda_runtime.h>
 #include <math.h>
 #include <algorithm>
@@ -62,16 +68,17 @@ struct BwdSmem {
   int dz, gr, lum, lus, a, ring;   // float offsets
   int bar_bytes, total_bytes;
 };
-__host__ __device__ inline BwdSmem bwd_smem_layout(int stage_cap) {
+// rpc: rows per CTA (128, or 64 for half tiles)
+__host__ __device__ inline BwdSmem bwd_smem_layout(int stage_cap, int rpc) {
   BwdSmem L;
   int fl = 0;
-  L.dz = fl;  fl += 16 * kRows;
-  L.gr = fl;  fl += kRows;
+  L.dz = fl;  fl += 16 * rpc;
+  L.gr = fl;  fl += rpc;
   L.lum = fl; fl += 2 * kLuMax * kLuMax + 2 * kLuMax;
   fl = (fl + 31) & ~31;
-  L.lus = fl; fl += 3 * kLuMax * kRows;          // LULinear backward: v | y | dy, feature-major
+  L.lus = fl; fl += 3 * kLuMax * rpc;            // LULinear backward: v | y | dy, feature-major
   fl = (fl + 31) & ~31;
-  L.a = fl;   fl += kASmemFloats;                 // A_hi | A_lo (tc_common.cuh)
+  L.a = fl;   fl += a_smem_floats(rpc);           // A_hi | A_lo (tc_common.cuh)
   L.ring = fl; fl += kBwdSlots * stage_cap;
   L.bar_bytes = fl * 4;
   L.total_bytes = L.bar_bytes + kBwdSlots * 8;
@@ -241,7 +248,7 @@ nsf_dw_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_constant_
   }
 }
 
-template <int H, int KB, bool COND>
+template <int H, int RPC, int KB, bool COND>
 __global__ void __launch_bounds__(kThreads, 1)
 nsf_vjp_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_constant__ sbi_nsf_tc tcb,
                   const __grid_constant__ sbi_rows rows, const float* __restrict__ gout, float g_const,
@@ -250,41 +257,45 @@ nsf_vjp_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_constant
                   float* __restrict__ dcond) {
   constexpr int HP8 = (H + 7) & ~7;
   constexpr int NCH = HP8 / 8;
-  constexpr int NC = HP8 / 2;
+  constexpr int TPR = kThreads / RPC;                   // threads per row
+  constexpr int UPT = kRows / RPC;                      // CTAs per tile (= cluster size)
+  constexpr int NC = TPR == 2 ? HP8 / 2 : 16;           // columns per thread ([tq NC, tq NC + NC))
   constexpr int NG = NC / 4;
-  static_assert(HP8 % 8 == 0 && NC % 4 == 0 && H > NC && H < HP8 + 1 && HP8 <= 64, "hidden width");
+  static_assert(HP8 % 8 == 0 && NC % 4 == 0 && H > (TPR - 1) * NC && H < HP8 + 1 && HP8 <= 64, "hidden width");
   extern __shared__ __align__(128) float sm[];
-  const BwdSmem L = bwd_smem_layout(tcb.stage_cap);
+  const BwdSmem L = bwd_smem_layout(tcb.stage_cap, RPC);
   uint64_t* full = reinterpret_cast<uint64_t*>(reinterpret_cast<char*>(sm) + L.bar_bytes);
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int C = m.C, D = m.D;
-  const int64_t ntiles = (rows.R + kRows - 1) / kRows;
+  const int64_t nunits = (rows.R + kRows - 1) / kRows * UPT;     // CTA tiles of RPC rows
   const TcSave SV = tc_save_layout(m.NB, m.TRmax, m.T);
 
   float* as = sm + L.a;
-  IssuerT<kBwdSlots, true> iss = tc_begin<kBwdSlots, true>(full, sm + L.ring, tcb, m.T, ntiles, true, kColsDG, sa, as);
+  IssuerT<kBwdSlots, true, RPC> iss =
+      tc_begin<kBwdSlots, true, RPC>(full, sm + L.ring, tcb, m.T, nunits, true, kColsDG, sa, as);
   SBI_TL(100);
 
   const float* __restrict__ P = m.d_params;
   float* dzs = sm + L.dz;
   float* GRs = sm + L.gr;
-  const int half = warp >> 2;
-  const int row = ((warp & 3) << 5) | lane;
-  const int cbase = half * NC;
+  const int tq = warp / (RPC / 32);                        // which column part of the row
+  const int row = ((warp % (RPC / 32)) << 5) | lane;       // row of the CTA = store lane
+  const int cbase = tq * NC;
+  const int rank = (int)(blockIdx.x % UPT);                // half of the tile (= rank in the cluster)
   RqsConst rc = rqs_const(m);
   rc.K = KB;
-  float* gp = gpart + (size_t)blockIdx.x * m.n_params;
+  float* gp = gpart + (size_t)(blockIdx.x / UPT) * m.n_params;
   // condition gradient: features [c_lo, c_hi) of this thread's row; dY = the row's dY columns at `dy`
-  // (written by both threads of the row before the CTA barrier that precedes the call)
-  const int c_half = (C + 1) >> 1;
-  const int c_lo = half * c_half, c_hi = min(C, c_lo + c_half);
-  auto dctx_add = [&](const float* dy, const float* W, int ldw, int64_t row0) {
+  // (written by all threads of the row before the CTA barrier that precedes the call)
+  const int c_part = (C + TPR - 1) / TPR;
+  const int c_lo = tq * c_part, c_hi = min(C, c_lo + c_part);
+  auto dctx_add = [&](const float* dy, const float* W, int ldw, int64_t row0, int srow) {
     if (row0 + row >= rows.R) return;
     const float* csd = m.d_stats + 2 * m.Dp + m.Cp;
     float* out = dcond + (row0 + row) * C;
     for (int c = c_lo; c < c_hi; ++c) {
       float a = 0.f;
-      for (int n = 0; n < H; ++n) a = fmaf(__ldcg(dy + ((n >> 2) * kRows + row) * 4 + (n & 3)), __ldg(W + n * ldw + c), a);
+      for (int n = 0; n < H; ++n) a = fmaf(__ldcg(dy + ((n >> 2) * kRows + srow) * 4 + (n & 3)), __ldg(W + n * ldw + c), a);
       out[c] += a / __ldg(csd + c);
     }
   };
@@ -298,10 +309,11 @@ nsf_vjp_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_constant
   auto write_a = [&](const float (&act)[NC], int col0) {
 #pragma unroll
     for (int g = 0; g < NG; ++g) {
+      if (TPR * NC > HP8 && cbase + 4 * g >= HP8) continue;     // no MMA reads columns from HP8 on
       float a[4];
 #pragma unroll
       for (int i = 0; i < 4; ++i) a[i] = act[4 * g + i];
-      smem_a4(as, row, col0 + cbase + 4 * g, a);
+      smem_a4<RPC>(as, row, col0 + cbase + 4 * g, a);
     }
   };
   auto read_acc = [&](int region, float (&d)[NC]) {
@@ -310,19 +322,21 @@ nsf_vjp_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_constant
   };
 
   int iter = 0;
-  for (int64_t tile = blockIdx.x; tile < ntiles; tile += gridDim.x, ++iter) {
+  for (int64_t unit = blockIdx.x; unit < nunits; unit += gridDim.x, ++iter) {
     if (iter > 0) accum = true;
-    const int64_t row0 = tile * kRows;
+    const int64_t tile = unit / UPT;                        // 128-row tile (save slab)
+    const int srow = rank * RPC + row;                      // lane of the row in the tile's save slab
+    const int64_t row0 = unit * RPC;
     float* svt = save + (size_t)tile * SV.tile_stride;
     // ---- per-tile setup: upstream gradient, loss statistics, d(sum g log q)/dz_T = -g z_T
     {
       const bool live = row0 + row < rows.R;
       const float g = live ? (gout ? __ldg(gout + row0 + row) : g_const) : 0.f;
-      if (half == 0) {
+      if (tq == 0) {
         GRs[row] = g;
         float nll = 0.f, bad = 0.f;
         if (live) {
-          const float lp = __ldcg(svt + SV.lp + row);
+          const float lp = __ldcg(svt + SV.lp + srow);
           if (isfinite(lp)) nll = -lp; else bad = 1.f;
         }
         if (loss_acc != nullptr) {
@@ -333,15 +347,15 @@ nsf_vjp_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_constant
             if (bad != 0.f) atomicAdd(loss_acc + 1, bad);
           }
         }
-      } else {
+      } else if (TPR == 2 || tq == 1) {
 #pragma unroll
         for (int i = 0; i < 4; ++i) {
-          const float4 t = __ldcg(tc_grp(svt + SV.zt, i, row));
+          const float4 t = __ldcg(tc_grp(svt + SV.zt, i, srow));
           // (rows past the end of the batch were never saved: their gradient is exactly zero)
-          dzs[(4 * i + 0) * kRows + row] = live ? -g * t.x : 0.f;
-          dzs[(4 * i + 1) * kRows + row] = live ? -g * t.y : 0.f;
-          dzs[(4 * i + 2) * kRows + row] = live ? -g * t.z : 0.f;
-          dzs[(4 * i + 3) * kRows + row] = live ? -g * t.w : 0.f;
+          dzs[(4 * i + 0) * RPC + row] = live ? -g * t.x : 0.f;
+          dzs[(4 * i + 1) * RPC + row] = live ? -g * t.y : 0.f;
+          dzs[(4 * i + 2) * RPC + row] = live ? -g * t.z : 0.f;
+          dzs[(4 * i + 3) * RPC + row] = live ? -g * t.w : 0.f;
         }
       }
       if (COND && live)
@@ -360,15 +374,15 @@ nsf_vjp_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_constant
       SBI_TL(1000 * (li + 1));
 
       // saved activations travel from L2 while the LU section runs: the spline parameters of this
-      // thread's first feature
+      // thread's first feature (the features go round-robin over the row's parts)
       float qn[32], xn = 0.f;
       int jn = 0;
 #pragma unroll
       for (int i = 0; i < 32; ++i) qn[i] = 0.f;
-      if (half < v.n_tr) {
-        tc_load_prm(svl + SV.prm, row, m.TRmax, half, qn);
-        jn = __ldg(v.trf + half);
-        xn = tc_load_row16_at(svl + SV.zin, row, jn);
+      if (tq < v.n_tr) {
+        tc_load_prm(svl + SV.prm, srow, m.TRmax, tq, qn);
+        jn = __ldg(v.trf + tq);
+        xn = tc_load_row16_at(svl + SV.zin, srow, jn);
       }
 
       // ================= LULinear backward (y = U v, z' = L y + b) =================
@@ -376,16 +390,16 @@ nsf_vjp_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_constant
       // the factors of this layer were built a layer ago: prep_lu below)
       if (__ldg(v.LT + SBI_L_HAS_LU)) {
         float vr[kLuMax];
-        if (half == 0) tc_load_row16(svl + SV.v, row, vr);
+        if (tq == 0) tc_load_row16(svl + SV.v, srow, vr);
         SBI_TL(1000 * (li + 1) + 91);
         float* V = sm + L.lus;
-        float* Y = V + 16 * kRows;
-        float* DY = Y + 16 * kRows;
+        float* Y = V + 16 * RPC;
+        float* DY = Y + 16 * RPC;
         const float* U = sm + L.lum;
         const float* Lw = U + kLuMax * kLuMax;
         float dyr[kLuMax];
-        if (half == 0) {
-          // y = U v on the thread's row (half 1 does dy meanwhile)
+        if (tq == 0) {
+          // y = U v on the thread's row (part 1 does dy meanwhile)
 #pragma unroll
           for (int i = 0; i < kLuMax; ++i) {
             float y = 0.f;
@@ -393,15 +407,15 @@ nsf_vjp_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_constant
             for (int j = 0; j < kLuMax; ++j)
               if (j >= i) y = fmaf(U[i * kLuMax + j], vr[j], y);        // padded entries are zero
             if (i < D) {
-              V[i * kRows + row] = vr[i];
-              Y[i * kRows + row] = y;
+              V[i * RPC + row] = vr[i];
+              Y[i * RPC + row] = y;
             }
           }
-        } else {
+        } else if (TPR == 2 || tq == 1) {
           // dy = dz + L^T dz (strictly lower part)
           float dzr[kLuMax];
 #pragma unroll
-          for (int i = 0; i < kLuMax; ++i) dzr[i] = (i < D) ? dzs[i * kRows + row] : 0.f;
+          for (int i = 0; i < kLuMax; ++i) dzr[i] = (i < D) ? dzs[i * RPC + row] : 0.f;
 #pragma unroll
           for (int i = 0; i < kLuMax; ++i) {
             float dy = dzr[i];
@@ -409,14 +423,20 @@ nsf_vjp_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_constant
             for (int j = 0; j < kLuMax; ++j)
               if (j > i) dy = fmaf(Lw[j * kLuMax + i], dzr[j], dy);
             dyr[i] = dy;
-            if (i < D) DY[i * kRows + row] = dy;
+            if (i < D) DY[i * RPC + row] = dy;
           }
         }
-        group_sync();
+        if constexpr (UPT == 1) group_sync();
+        else cluster_sync();      // both halves' rows are in their CTA's shared memory
         SBI_TL(1000 * (li + 1) + 92);
         // parameter gradients: one (i,j) pair per thread, reduction over the tile rows (order of
-        // lu_backward, nsf.cu)
-        {
+        // lu_backward, nsf.cu); half tiles: CTA 0 of the cluster, rows 64.. from CTA 1
+        if (UPT == 1 || rank == 0) {
+          const float* peer = UPT == 1 ? sm : cluster_peer(sm, 1);
+          // float4 of tile rows [rr, rr + 4) of the feature-major array at p (local address)
+          auto at4 = [&](const float* p, int rr) {
+            return *reinterpret_cast<const float4*>(UPT == 1 || rr < RPC ? p + rr : peer + (p - sm) + (rr - RPC));
+          };
           const int o_lo = __ldg(v.LT + SBI_L_LU_LOWER), o_up = __ldg(v.LT + SBI_L_LU_UPPER);
           const int o_dg = __ldg(v.LT + SBI_L_LU_DIAG), o_bi = __ldg(v.LT + SBI_L_LU_BIAS);
           for (int t = tid; t < D * D + D; t += kThreads) {
@@ -430,8 +450,8 @@ nsf_vjp_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_constant
 #pragma unroll 4
               for (int r = 0; r < kRows; r += 4) {
                 const int rr = (r + rot) & (kRows - 1);
-                const float4 x4 = *reinterpret_cast<const float4*>(p + rr);
-                const float4 y4 = *reinterpret_cast<const float4*>(q + rr);
+                const float4 x4 = at4(p, rr);
+                const float4 y4 = at4(q, rr);
                 a0 = fmaf(x4.x, y4.x, a0); a1 = fmaf(x4.y, y4.y, a1);
                 a2 = fmaf(x4.z, y4.z, a2); a3 = fmaf(x4.w, y4.w, a3);
               }
@@ -441,7 +461,7 @@ nsf_vjp_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_constant
               float a0 = 0.f, a1 = 0.f, a2 = 0.f, a3 = 0.f;
 #pragma unroll 4
               for (int r = 0; r < kRows; r += 4) {
-                const float4 x4 = *reinterpret_cast<const float4*>(p + ((r + rot) & (kRows - 1)));
+                const float4 x4 = at4(p, (r + rot) & (kRows - 1));
                 a0 += x4.x; a1 += x4.y; a2 += x4.z; a3 += x4.w;
               }
               return (a0 + a1) + (a2 + a3);
@@ -449,20 +469,20 @@ nsf_vjp_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_constant
             if (t < D * D) {
               const int i = t / D, j = t % D;
               if (i > j) {
-                a = dot(dzs + i * kRows, Y + j * kRows);
+                a = dot(dzs + i * RPC, Y + j * RPC);
                 dst = gp + o_lo + i * (i - 1) / 2 + j;
               } else if (i < j) {
-                a = dot(DY + i * kRows, V + j * kRows);
+                a = dot(DY + i * RPC, V + j * RPC);
                 dst = gp + o_up + i * D - i * (i + 1) / 2 + (j - i - 1);
               } else {
-                a = dot(DY + i * kRows, V + i * kRows);
+                a = dot(DY + i * RPC, V + i * RPC);
                 const float gs = rsum(GRs);
                 a = (a + gs / U[i * kLuMax + i]) * sigmoid_f(__ldg(P + o_dg + i));
                 dst = gp + o_dg + i;
               }
             } else {
               const int i = t - D * D;
-              a = rsum(dzs + i * kRows);
+              a = rsum(dzs + i * RPC);
               dst = gp + o_bi + i;
             }
             *dst = accum ? (*dst + a) : a;
@@ -477,9 +497,10 @@ nsf_vjp_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_constant
             for (int e = n; e < ((n + 3) & ~3); ++e) gp[o + e] = 0.f;
           }
         }
-        group_sync();
+        if constexpr (UPT == 1) group_sync();
+        else cluster_sync();      // CTA 1's rows have been read
         SBI_TL(1000 * (li + 1) + 93);
-        if (half == 1) {
+        if (tq == 1) {
           // dv = U^T dy
 #pragma unroll
           for (int j = 0; j < kLuMax; ++j) {
@@ -488,7 +509,7 @@ nsf_vjp_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_constant
 #pragma unroll
               for (int i = 0; i < kLuMax; ++i)
                 if (i <= j) a = fmaf(U[i * kLuMax + j], dyr[i], a);
-              dzs[j * kRows + row] = a;
+              dzs[j * RPC + row] = a;
             }
           }
         }
@@ -501,32 +522,34 @@ nsf_vjp_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_constant
       const int np = __ldg(tab + 1);
       {
         for (int p = 0; p < np; ++p) {
-          const int f = 2 * p + half;
+          // feature f of pass p is feature f & 1 of the pass, taken by part f % TPR (warp-uniform)
+          const int f = 2 * p + (tq & 1);
           const int nf = min(2, v.n_tr - 2 * p);
-          const bool has = f < v.n_tr;                     // warp-uniform
-          // this pass's parameters were requested a pass (or the LU section) ago; request the next
+          const bool mine = TPR == 2 || ((p ^ (tq >> 1)) & 1) == 0;
+          const bool has = mine && f < v.n_tr;
+          // this feature's parameters were requested a feature (or the LU section) ago; request the next
           float q[32];
           const float x = xn;
           const int j = jn;
 #pragma unroll
           for (int i = 0; i < 32; ++i) q[i] = qn[i];
-          if (f + 2 < v.n_tr) {
-            tc_load_prm(svl + SV.prm, row, m.TRmax, f + 2, qn);
-            jn = __ldg(v.trf + f + 2);
-            xn = tc_load_row16_at(svl + SV.zin, row, jn);
+          if (mine && f + TPR < v.n_tr) {
+            tc_load_prm(svl + SV.prm, srow, m.TRmax, f + TPR, qn);
+            jn = __ldg(v.trf + f + TPR);
+            xn = tc_load_row16_at(svl + SV.zin, srow, jn);
           }
           if (has) {
             float dq[32];
-            const float gx = rqs_backward_fast<KB>(q, rc, x, dzs[j * kRows + row], GRs[row], dq);
-            dzs[j * kRows + row] = gx;
+            const float gx = rqs_backward_fast<KB>(q, rc, x, dzs[j * RPC + row], GRs[row], dq);
+            dzs[j * RPC + row] = gx;
 #pragma unroll
             for (int c = 0; c < 4; ++c) {
               float a[8];
 #pragma unroll
               for (int i = 0; i < 8; ++i) a[i] = dq[8 * c + i];
-              smem_a8(as, row, 32 * half + 8 * c, a);
+              smem_a8<RPC>(as, row, 32 * (tq & 1) + 8 * c, a);
             }
-            tc_save_prm(svl + SV.dy_fin(p), row, 0, half, dq);
+            tc_save_prm(svl + SV.dy_fin(p), srow, 0, tq & 1, dq);
           }
           hand_over();
           {
@@ -542,8 +565,8 @@ nsf_vjp_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_constant
       // (loads of saved activations are requested one wait ahead of their use throughout the blocks)
       float sv[NC], t2[NC];
       if (m.NB > 0) {
-        tc_load_cols<NC>(svl + SV.s(m.NB - 1), row, half, sv);
-        tc_load_cols<NC>(svl + SV.t2(m.NB - 1), row, half, t2);
+        tc_load_cols<NC>(svl + SV.s(m.NB - 1), srow, tq, sv);
+        tc_load_cols<NC>(svl + SV.t2(m.NB - 1), srow, tq, t2);
       }
       float dh[NC];
       read_acc(cDs, dh);
@@ -553,7 +576,7 @@ nsf_vjp_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_constant
       for (int b = m.NB - 1; b >= 0; --b) {
         const int* BT = v.LT + SBI_L_BLK0 + 6 * b;
         float dT[NC], a1[NC];
-        tc_load_cols<NC>(svl + SV.a1(b), row, half, a1);
+        tc_load_cols<NC>(svl + SV.a1(b), srow, tq, a1);
         {
           // ---- dG = dh t2 s (1 - s): output gradient of the GLU context linear (the COND instantiation
           //      also takes dctx += dG Wc)
@@ -564,16 +587,16 @@ nsf_vjp_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_constant
             dT[q] = dhq * s;
             dG[q] = dhq * t2[q] * s * (1.f - s);
           }
-          tc_save_cols<NC>(svl + SV.dy_blk(b, 0), row, half, dG);
+          tc_save_cols<NC>(svl + SV.dy_blk(b, 0), srow, tq, dG);
           if (COND) {
             group_sync();
-            dctx_add(svl + SV.dy_blk(b, 0), P + __ldg(BT + 4), m.Cp, row0);     // dG Wc
+            dctx_add(svl + SV.dy_blk(b, 0), P + __ldg(BT + 4), m.Cp, row0, srow);     // dG Wc
           }
         }
         SBI_TL(1000 * (li + 1) + 30 + 10 * b);
         // ---- dA1 = (dT W2) * [a1 > 0]
         {
-          tc_save_cols<NC>(svl + SV.dy_blk(b, 1), row, half, dT);
+          tc_save_cols<NC>(svl + SV.dy_blk(b, 1), srow, tq, dT);
           write_a(dT, 0);
           SBI_TL(1000 * (li + 1) + 72 + 10 * b);
           hand_over();
@@ -589,7 +612,7 @@ nsf_vjp_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_constant
         }
         SBI_TL(1000 * (li + 1) + 31 + 10 * b);
         float hb[NC];
-        tc_load_cols<NC>(svl + SV.h(b), row, half, hb);
+        tc_load_cols<NC>(svl + SV.h(b), srow, tq, hb);
         float dA[NC];
         read_acc(cDs, dA);
 #pragma unroll
@@ -597,7 +620,7 @@ nsf_vjp_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_constant
         SBI_TL(1000 * (li + 1) + 32 + 10 * b);
         // ---- dh += (dA1 W1) * [h_b > 0]
         {
-          tc_save_cols<NC>(svl + SV.dy_blk(b, 2), row, half, dA);
+          tc_save_cols<NC>(svl + SV.dy_blk(b, 2), srow, tq, dA);
           write_a(dA, 0);
           hand_over();
           {
@@ -610,8 +633,8 @@ nsf_vjp_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_constant
         }
         SBI_TL(1000 * (li + 1) + 33 + 10 * b);
         if (b > 0) {
-          tc_load_cols<NC>(svl + SV.s(b - 1), row, half, sv);
-          tc_load_cols<NC>(svl + SV.t2(b - 1), row, half, t2);
+          tc_load_cols<NC>(svl + SV.s(b - 1), srow, tq, sv);
+          tc_load_cols<NC>(svl + SV.t2(b - 1), srow, tq, t2);
         }
         {
           float d[NC];
@@ -625,10 +648,10 @@ nsf_vjp_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_constant
       // ================= initial layer: d(identity features) = dh W0[:, C:] =================
       {
         const int K0p = m.Cp + m.IDp;
-        tc_save_cols<NC>(svl + SV.dy_init(), row, half, dh);
+        tc_save_cols<NC>(svl + SV.dy_init(), srow, tq, dh);
         write_a(dh, 0);
         hand_over();
-        if (COND) dctx_add(svl + SV.dy_init(), P + __ldg(v.LT + SBI_L_W0), K0p, row0);     // the context columns of dh W0
+        if (COND) dctx_add(svl + SV.dy_init(), P + __ldg(v.LT + SBI_L_W0), K0p, row0, srow);     // the context columns of dh W0
         {
           uint32_t acc = 0u;
           iss.begin(__ldg(tab + 5 + 4 * stage));
@@ -637,13 +660,13 @@ nsf_vjp_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_constant
         }
         ++stage;
         SBI_TL(1000 * (li + 1) + 60);
-        if (half == 0) {
+        if (tq == 0) {
           float d[16];
           ld8(row, cDs, d);
           ld8(row, cDs + 8, d + 8);
 #pragma unroll
           for (int j = 0; j < 16; ++j)
-            if (j < v.n_id) dzs[__ldg(v.idf + j) * kRows + row] += d[j];
+            if (j < v.n_id) dzs[__ldg(v.idf + j) * RPC + row] += d[j];
         }
         group_sync();
       }
@@ -668,12 +691,12 @@ static int vjp_tc_ok(const sbi_nsf_model* m, const sbi_nsf_tc* tcf, const sbi_ns
   if (!tcb || !tcb->d_tab || !tcb->d_tcw || tcb->stage_cap <= 0 || (tcb->stage_cap & 31)) return 0;
   if (m->IDp > 16 || m->Cp + m->IDp + 1 > 64 || m->Cp + 1 > 64) return 0;
   // the training pair runs one CTA per SM: the forward with activation save and the backward sweep may each
-  // opt into a whole SM's shared memory
-  return tc::forward_save_smem_bytes(*m, *tcf) <= kMaxSmemBytes &&
-                 tc::bwd_smem_layout(tcb->stage_cap).total_bytes <= kMaxSmemBytes &&
-                 tc::dw_smem_bytes(*m) <= kMaxSmemBytes
-             ? 1
-             : 0;
+  // opt into a whole SM's shared memory, on whole tiles and on half tiles
+  for (int rpc : {tc::kRows, 64})
+    if (tc::forward_save_smem_bytes(*m, *tcf, rpc) > kMaxSmemBytes ||
+        tc::bwd_smem_layout(tcb->stage_cap, rpc).total_bytes > kMaxSmemBytes)
+      return 0;
+  return tc::dw_smem_bytes(*m) <= kMaxSmemBytes ? 1 : 0;
 }
 
 extern "C" int sbi_b200_nsf_vjp_tc_supported(const sbi_nsf_model* m, const sbi_nsf_tc* tc_fwd,
@@ -710,14 +733,19 @@ static int vjp_tc_launch(const sbi_nsf_model* m, const sbi_nsf_tc* tc_fwd, const
   if (!vjp_tc_ok(m, tc_fwd, tc_bwd)) return SBI_ESMEM;
   if (save_bytes < sbi_b200_nsf_vjp_tc_save_bytes(m, rows->R)) return SBI_EINVAL;
   cudaStream_t s = (cudaStream_t)stream;
-  const int bwd_bytes = tc::bwd_smem_layout(tc_bwd->stage_cap).total_bytes;
+  const int bwd_bytes = tc::bwd_smem_layout(tc_bwd->stage_cap, tc::kRows).total_bytes;
+  const int bwd_bytes_half = tc::bwd_smem_layout(tc_bwd->stage_cap, 64).total_bytes;
   const int dw_bytes = tc::dw_smem_bytes(*m);
   // opt the backward kernels in before anything is launched: a failed opt-in leaves no forward sweep behind
-  if (int e = set_smem(reinterpret_cast<const void*>(tc::nsf_vjp_tc_kernel<50, 10, COND>), bwd_bytes)) return e;
+  if (int e = set_smem(reinterpret_cast<const void*>(tc::nsf_vjp_tc_kernel<50, tc::kRows, 10, COND>), bwd_bytes))
+    return e;
+  if (int e = set_smem(reinterpret_cast<const void*>(tc::nsf_vjp_tc_kernel<50, 64, 10, COND>), bwd_bytes_half))
+    return e;
   if (int e = set_smem(reinterpret_cast<const void*>(tc::nsf_dw_tc_kernel<50>), dw_bytes)) return e;
-  // chunks of one tile per SM: forward sweep (saves activations), backward sweep of the same rows (one CTA
-  // per tile, so tile t writes partial-gradient slab t), then their weight gradients (one CTA per tile,
-  // layer and linear); later chunks accumulate into the partial-gradient slabs
+  // chunks of one tile per SM: forward sweep (saves activations), backward sweep of the same rows (tile t
+  // writes partial-gradient slab t), then their weight gradients (one CTA per tile, layer and linear); later
+  // chunks accumulate into the partial-gradient slabs.  A chunk of at most half as many tiles as SMs runs
+  // the two sweeps on half tiles (two CTAs per tile), so that twice as many SMs take part.
   tc::StoreArgs sa;
   if (int e = tc::store_args(&sa)) return e;
   const int64_t chunk = vjp_tc_chunk_rows();
@@ -730,10 +758,16 @@ static int vjp_tc_launch(const sbi_nsf_model* m, const sbi_nsf_tc* tc_fwd, const
       if (!rows->cond_shared) rr.d_cond = rows->d_cond + r0 * m->C;
     }
     const int grid = (int)((rr.R + tc::kRows - 1) / tc::kRows);
-    if (int rc = tc::launch_forward_save(m, tc_fwd, &rr, d_logp ? d_logp + r0 : nullptr, d_save, s)) return rc;
-    if (int rc = launch(tc::nsf_vjp_tc_kernel<50, 10, COND>, grid, tc::kThreads, bwd_bytes, s, *m, *tc_bwd, rr,
-                        d_gout ? d_gout + r0 : nullptr, g_const, d_gpart, d_loss_acc, d_save, r0 > 0 ? 1 : 0, sa,
-                        COND ? d_gcond + r0 * m->C : nullptr))
+    const bool half_tiles = 2 * grid <= sbi::dev_num_sms();
+    if (int rc = tc::launch_forward_save(m, tc_fwd, &rr, d_logp ? d_logp + r0 : nullptr, d_save, half_tiles, s))
+      return rc;
+    if (int rc = half_tiles ? launch(tc::nsf_vjp_tc_kernel<50, 64, 10, COND>, Grid(2 * grid, 2), tc::kThreads,
+                                     bwd_bytes_half, s, *m, *tc_bwd, rr, d_gout ? d_gout + r0 : nullptr, g_const,
+                                     d_gpart, d_loss_acc, d_save, r0 > 0 ? 1 : 0, sa,
+                                     COND ? d_gcond + r0 * m->C : nullptr)
+                            : launch(tc::nsf_vjp_tc_kernel<50, tc::kRows, 10, COND>, grid, tc::kThreads, bwd_bytes, s, *m,
+                                     *tc_bwd, rr, d_gout ? d_gout + r0 : nullptr, g_const, d_gpart, d_loss_acc,
+                                     d_save, r0 > 0 ? 1 : 0, sa, COND ? d_gcond + r0 * m->C : nullptr))
       return rc;
     if (int rc = launch(tc::nsf_dw_tc_kernel<50>, grid * m->T * tc::dw_units(*m), tc::kThreads, dw_bytes, s, *m, rr,
                         d_save, d_gpart, r0 > 0 ? 1 : 0))

@@ -138,30 +138,32 @@ __device__ __forceinline__ void ld4(uint32_t row, uint32_t col, float* v) {
 
 // ---- A operands in shared memory ------------------------------------------------------------------
 // The training pair (nsf_logprob_tc_kernel<..., SAVE>, nsf_vjp_tc_kernel) runs one CTA per SM, which leaves
-// room for A_hi | A_lo (128 rows x 64 K-columns each, 32 KB each) in shared memory, so the MMAs read A
-// through a descriptor instead of waiting for fragment loads from the L2-resident store in every K-step.
-// Layout: wgmma's K-major no-swizzle canonical layout [k/4][128 rows][4], the convention of make_bdesc for
+// room for A_hi | A_lo (RPC rows x 64 K-columns each) in shared memory, so the MMAs read A through a
+// descriptor instead of waiting for fragment loads from the L2-resident store in every K-step.  RPC, the
+// rows of a CTA, is 128 (a whole tile) or 64 (half a tile, when a chunk of tiles would leave SMs idle).
+// Layout: wgmma's K-major no-swizzle canonical layout [k/4][RPC rows][4], the convention of make_bdesc for
 // B: a core matrix (8 rows x 4 K-columns) is 128 contiguous bytes, 8-row groups are 128 B apart (SBO),
-// K-adjacent core matrices 128 x 16 B = 2048 B apart (LBO); a K-step of 8 columns advances 4096 B, and
-// warpgroup 1 (rows 64 ..) starts 1024 B in.  A row thread writes 4 consecutive columns as one float4,
-// so the 32 rows of a warp cover 512 contiguous bytes.
-constexpr int kAFloats = 64 * kRows;          // one half
-constexpr int kASmemFloats = 2 * kAFloats;    // A_hi | A_lo
-constexpr uint64_t kAStep = 4096u >> 4;       // descriptor start-address advance per K-step
+// K-adjacent core matrices RPC x 16 B apart (LBO); a K-step of 8 columns advances RPC x 32 B, and with
+// RPC = 128 warpgroup 1 (rows 64 ..) starts 1024 B in.  A row thread writes 4 consecutive columns as one
+// float4, so the 32 rows of a warp cover 512 contiguous bytes.
+__host__ __device__ constexpr int a_smem_floats(int rpc) { return 2 * 64 * rpc; }   // A_hi | A_lo
 
 // ---- the MMAs: both warpgroups of the CTA, synchronously ------------------------------------------
 // Accumulator fragment of wgmma m64nNk8 (f32): warp w of the warpgroup holds rows 16w + g and
 // 16w + g + 8 (g = lane / 4), columns 8j + 2t and 8j + 2t + 1 (t = lane % 4) in d[4j .. 4j+3].
 //
-// D[store, M = 128] (+)= A * B[smem]^T over nk K-steps, 3xTF32 (A_hi B_hi + A_lo B_hi + A_hi B_lo):
-// warpgroup wg computes rows 64 wg .. 64 wg + 63.  ASMEM = false: ah / al are the A_hi / A_lo store
-// columns of the first K-step and the fragments come straight from the store; ASMEM = true: ah / al are
-// the shared-memory descriptors of the warpgroup's first K-step.  Same products in the same order.
-template <int N, bool ASMEM>
+// D[store, M = RPC] (+)= A * B[smem]^T over nk K-steps, 3xTF32 (A_hi B_hi + A_lo B_hi + A_hi B_lo):
+// RPC = 128: warpgroup wg computes rows 64 wg .. 64 wg + 63; RPC = 64: both warpgroups compute the CTA's
+// 64 rows, each its own N columns (the caller offsets dcol and the B descriptors).  ASMEM = false: ah / al
+// are the A_hi / A_lo store columns of the first K-step and the fragments come straight from the store;
+// ASMEM = true: ah / al are the shared-memory descriptors of the warpgroup's first K-step.  Same products in
+// the same order.
+template <int N, bool ASMEM, int RPC = kRows>
 __device__ __forceinline__ void mma_rows_n(uint32_t dcol, uint64_t ah, uint64_t al, uint64_t dh,
                                            uint64_t dl, uint64_t dstep, int nk, uint32_t acc) {
+  constexpr uint64_t kAStep = (RPC * 32u) >> 4;       // descriptor start-address advance per K-step
   const int lane = threadIdx.x & 31, g = lane >> 2, t = lane & 3;
-  const uint32_t r0 = (threadIdx.x >> 7) * 64 + ((threadIdx.x >> 5) & 3) * 16 + g;
+  const uint32_t r0 = (RPC == kRows ? (threadIdx.x >> 7) * 64 : 0) + ((threadIdx.x >> 5) & 3) * 16 + g;
   const uint32_t c0 = s_store_col;
   dcol += c0;
   const uint32_t ahcol = (uint32_t)ah + c0, alcol = (uint32_t)al + c0;
@@ -218,18 +220,18 @@ __device__ __forceinline__ void mma_rows_n(uint32_t dcol, uint64_t ah, uint64_t 
     slab[(c + 1) * kStoreLanes + r0 + 8] = d[4 * j + 3];
   }
 }
-template <bool ASMEM>
+template <bool ASMEM, int RPC = kRows>
 __device__ __forceinline__ void mma_rows(int N, uint32_t dcol, uint64_t ah, uint64_t al, uint64_t dh,
                                          uint64_t dl, uint64_t dstep, int nk, uint32_t acc) {
   switch (N) {
-    case 8: mma_rows_n<8, ASMEM>(dcol, ah, al, dh, dl, dstep, nk, acc); break;
-    case 16: mma_rows_n<16, ASMEM>(dcol, ah, al, dh, dl, dstep, nk, acc); break;
-    case 24: mma_rows_n<24, ASMEM>(dcol, ah, al, dh, dl, dstep, nk, acc); break;
-    case 32: mma_rows_n<32, ASMEM>(dcol, ah, al, dh, dl, dstep, nk, acc); break;
-    case 40: mma_rows_n<40, ASMEM>(dcol, ah, al, dh, dl, dstep, nk, acc); break;
-    case 48: mma_rows_n<48, ASMEM>(dcol, ah, al, dh, dl, dstep, nk, acc); break;
-    case 56: mma_rows_n<56, ASMEM>(dcol, ah, al, dh, dl, dstep, nk, acc); break;
-    case 64: mma_rows_n<64, ASMEM>(dcol, ah, al, dh, dl, dstep, nk, acc); break;
+    case 8: mma_rows_n<8, ASMEM, RPC>(dcol, ah, al, dh, dl, dstep, nk, acc); break;
+    case 16: mma_rows_n<16, ASMEM, RPC>(dcol, ah, al, dh, dl, dstep, nk, acc); break;
+    case 24: mma_rows_n<24, ASMEM, RPC>(dcol, ah, al, dh, dl, dstep, nk, acc); break;
+    case 32: mma_rows_n<32, ASMEM, RPC>(dcol, ah, al, dh, dl, dstep, nk, acc); break;
+    case 40: mma_rows_n<40, ASMEM, RPC>(dcol, ah, al, dh, dl, dstep, nk, acc); break;
+    case 48: mma_rows_n<48, ASMEM, RPC>(dcol, ah, al, dh, dl, dstep, nk, acc); break;
+    case 56: mma_rows_n<56, ASMEM, RPC>(dcol, ah, al, dh, dl, dstep, nk, acc); break;
+    case 64: mma_rows_n<64, ASMEM, RPC>(dcol, ah, al, dh, dl, dstep, nk, acc); break;
     default: __trap();      // operand blocks are planned with N in {8, ..., 64}
   }
 }
@@ -283,21 +285,34 @@ __device__ __forceinline__ void store_a4(uint32_t row, int col, const float (&v)
   st4(row, cAhi + col, hi);
   st4(row, cAlo + col, lo);
 }
-// the same into the shared-memory A region `as` (col % 4 == 0); the writer issues fence_async_smem()
-// before the CTA barrier that hands the operands to the MMAs
+// the same into the shared-memory A region `as` of an RPC-row CTA (col % 4 == 0); the writer issues
+// fence_async_smem() before the CTA barrier that hands the operands to the MMAs
+template <int RPC>
 __device__ __forceinline__ void smem_a4(float* as, uint32_t row, int col, const float (&v)[4]) {
   float hi[4], lo[4];
 #pragma unroll
   for (int i = 0; i < 4; ++i) split_tf32(v[i], hi[i], lo[i]);
-  float4* p = reinterpret_cast<float4*>(as + ((col >> 2) * kRows + row) * 4);
+  float4* p = reinterpret_cast<float4*>(as + ((col >> 2) * RPC + row) * 4);
   p[0] = make_float4(hi[0], hi[1], hi[2], hi[3]);
-  p[kAFloats / 4] = make_float4(lo[0], lo[1], lo[2], lo[3]);
+  p[a_smem_floats(RPC) / 8] = make_float4(lo[0], lo[1], lo[2], lo[3]);
 }
+template <int RPC>
 __device__ __forceinline__ void smem_a8(float* as, uint32_t row, int col, const float (&v)[8]) {
-  smem_a4(as, row, col, {v[0], v[1], v[2], v[3]});
-  smem_a4(as, row, col + 4, {v[4], v[5], v[6], v[7]});
+  smem_a4<RPC>(as, row, col, {v[0], v[1], v[2], v[3]});
+  smem_a4<RPC>(as, row, col + 4, {v[4], v[5], v[6], v[7]});
 }
 __device__ __forceinline__ void group_sync() { asm volatile("bar.sync 1, 256;" ::: "memory"); }
+// barrier of every thread of the CTA's cluster; orders the shared-memory writes before it with the reads
+// of other CTAs after it
+__device__ __forceinline__ void cluster_sync() {
+  asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
+}
+// generic address of the same shared-memory location in CTA `rank` of the cluster
+__device__ __forceinline__ const float* cluster_peer(const float* p, uint32_t rank) {
+  uint64_t r;
+  asm("mapa.u64 %0, %1, %2;" : "=l"(r) : "l"(p), "r"(rank));
+  return reinterpret_cast<const float*>(r);
+}
 
 // dense LU factors of NSF layer l, zero-padded to 16x16, into lum = [U | L | bias 16 | diag 16]
 // (all threads; the unit diagonal of L is implicit)
@@ -358,8 +373,8 @@ static int pack_weights(const float* params, const sbi_nsf_tc* tc, cudaStream_t 
 // once end() returns.  The weight stream rotates between the warps (stage k is fetched by the
 // elected lane of warp (k + 4) % 8).  Stage k lives in ring slot k % NSLOT.  A stage is fetched
 // (TMA bulk copy, completion on full[slot]) by the end() of the stage that used its slot NSLOT stages
-// earlier.  ASMEM: A comes from the shared-memory A region at `abase`, else from the store.
-template <int NSLOT, bool ASMEM = false>
+// earlier.  ASMEM: A comes from the shared-memory A region of an RPC-row CTA at `abase`, else from the store.
+template <int NSLOT, bool ASMEM = false, int RPC = kRows>
 struct IssuerT {
   bool leader;          // the elected lane of this warp
   int warp;             // this warp; stage k is fetched by warp (k+4) % 8
@@ -405,12 +420,22 @@ struct IssuerT {
     const uint64_t dh = make_bdesc(bh, slab, 128u);
     const uint64_t dl = make_bdesc(bh + lo_off, slab, 128u);
     const uint64_t dstep = (uint64_t)((2u * slab) >> 4);    // start-address field advance per K-step
-    if constexpr (ASMEM) {
+    if constexpr (ASMEM && RPC == kRows) {
       // column a0 (a multiple of 4) of the warpgroup's first row
       const uint32_t ah = abase + (uint32_t)a0 * (kRows * 4u) + (threadIdx.x >> 7) * 1024u;
       if (nk > 0)
-        mma_rows<true>(N, dcol, make_bdesc(ah, kRows * 16u, 128u), make_bdesc(ah + kAFloats * 4u, kRows * 16u, 128u),
-                       dh, dl, dstep, nk, acc);
+        mma_rows<true>(N, dcol, make_bdesc(ah, kRows * 16u, 128u),
+                       make_bdesc(ah + a_smem_floats(kRows) * 2u, kRows * 16u, 128u), dh, dl, dstep, nk, acc);
+    } else if constexpr (ASMEM) {
+      // both warpgroups on the CTA's rows from column a0; warpgroup wg takes result columns
+      // [wg N/2, (wg + 1) N/2), whose B rows start wg N/16 8-row groups (128 B each) in
+      const uint32_t ah = abase + (uint32_t)a0 * (RPC * 4u);
+      const uint32_t nh = (uint32_t)N / 2u, wg = threadIdx.x >> 7;
+      const uint64_t boff = (uint64_t)((wg * nh / 8u) * 128u >> 4);
+      if (nk > 0)
+        mma_rows<true, RPC>((int)nh, dcol + wg * nh, make_bdesc(ah, RPC * 16u, 128u),
+                            make_bdesc(ah + a_smem_floats(RPC) * 2u, RPC * 16u, 128u), dh + boff, dl + boff, dstep,
+                            nk, acc);
     } else {
       if (nk > 0) mma_rows<false>(N, dcol, cAhi + a0, cAlo + a0, dh, dl, dstep, nk, acc);
     }
@@ -428,9 +453,10 @@ using Issuer = IssuerT<kSlots>;
 // Kernel prologue, all threads: thread 0 initialises the ring's mbarriers full[0 .. NSLOT) (and any
 // other mbarrier the kernel initialised before the call), warp 0 reserves `ncols` store columns, and
 // after the CTA barrier the issuer starts fetching the first NSLOT stages of the CTA's first tile.
-// ASMEM: `as` is the shared-memory A region (kASmemFloats floats, 16-byte aligned).
-template <int NSLOT, bool ASMEM = false>
-__device__ __forceinline__ IssuerT<NSLOT, ASMEM> tc_begin(uint64_t* full, float* ring, const sbi_nsf_tc& tc, int T,
+// `ntiles` counts the CTA tiles of RPC rows.  ASMEM: `as` is the shared-memory A region
+// (a_smem_floats(RPC) floats, 16-byte aligned).
+template <int NSLOT, bool ASMEM = false, int RPC = kRows>
+__device__ __forceinline__ IssuerT<NSLOT, ASMEM, RPC> tc_begin(uint64_t* full, float* ring, const sbi_nsf_tc& tc, int T,
                                                           int64_t ntiles, bool reverse, int ncols, const StoreArgs& sa,
                                                           float* as = nullptr) {
   if (threadIdx.x == 0) {
@@ -439,7 +465,7 @@ __device__ __forceinline__ IssuerT<NSLOT, ASMEM> tc_begin(uint64_t* full, float*
   }
   if (threadIdx.x < 32) store_alloc(ncols, sa);
   __syncthreads();
-  IssuerT<NSLOT, ASMEM> iss;
+  IssuerT<NSLOT, ASMEM, RPC> iss;
   uint32_t el = 0;
   asm volatile("{\n\t.reg .pred p;\n\telect.sync _|p, 0xffffffff;\n\tselp.u32 %0, 1, 0, p;\n\t}" : "=r"(el));
   iss.leader = el != 0;
