@@ -215,6 +215,13 @@ nsf_logprob_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_cons
     const int64_t tile = unit / UPT;                        // 128-row tile (save slab)
     const int srow = (int)(unit % UPT) * RPC + row;         // lane of the row in the tile's save slab
     const int64_t row0 = unit * RPC;
+    // the tile's ready counters of the weight-gradient units start at zero (nsf_tc_save.cuh)
+    if constexpr (SAVE) {
+      if (unit % UPT == 0)
+        for (int e = tid; e < m.T * SV.units(); e += kThreads)
+          reinterpret_cast<unsigned*>(save + (size_t)tile * SV.tile_stride + (size_t)(e / SV.units()) * SV.layer_stride +
+                                      SV.ready())[e % SV.units()] = 0u;
+    }
     // ---- load + standardise the CTA's rows (arithmetic of load_rows, stages.cuh) ----
     {
       const float* st = m.d_stats;

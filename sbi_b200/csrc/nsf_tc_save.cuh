@@ -15,6 +15,10 @@
 //            weight-gradient kernel (nsf_dw_tc_kernel)        [128][64 npm + 192 NB + 64]:
 //            final-layer pass p (features 2p, 2p+1: 32 parameter rows each) at column 64p (npm passes),
 //            block b: dG (GLU context linear) | dT (W2) | dA (W1) at 64 npm + 192b, then dh (initial linear)
+//     ready = one counter per weight-gradient unit of the layer (u32, indexed like nsf_dw_tc_kernel's units),
+//            in columns [kDyCols, 64) of dh, which hold no gradient: the backward sweep adds 1 per CTA of
+//            the tile once the unit's dY is written, the weight-gradient kernel waits for the unit's count
+//            and the forward sweep zeroes the counters of its tile
 //   then per tile:  zt = base-space point z_T [128][16],  lp = log q [128]
 //
 // Every array of a slab is stored as float4 groups with the ROW index fastest: group g of row r sits at
@@ -32,6 +36,11 @@
 namespace sbi {
 namespace tc {
 
+// dY columns that are written and read (hidden width <= 56); columns [kDyCols, 64) of the dY arrays are free
+constexpr int kDyCols = 56;
+// a layer's counters (<= 8 final-layer passes of <= 16 features, 3 per block, the initial linear) fit them
+static_assert(8 + 3 * SBI_NSF_MAX_BLOCKS + 1 <= (64 - kDyCols) * 128, "ready counters");
+
 struct TcSave {
   int NB;
   int npm;                    // final-layer passes of the widest layer, (TRmax + 1) / 2
@@ -47,6 +56,11 @@ struct TcSave {
   __host__ __device__ int dy_fin(int p) const { return dy + 64 * p * 128; }
   __host__ __device__ int dy_blk(int b, int k) const { return dy + (64 * npm + 192 * b + 64 * k) * 128; }
   __host__ __device__ int dy_init() const { return dy + (64 * npm + 192 * NB) * 128; }
+  // weight-gradient units of a layer: the final-layer passes, three linears per residual block (GLU context,
+  // W2, W1), the initial linear
+  __host__ __device__ int units() const { return npm + 3 * NB + 1; }
+  // ready counters of the layer, units() of the (64 - kDyCols) * 128 free words
+  __host__ __device__ int ready() const { return dy_init() + kDyCols * 128; }
 };
 
 __host__ __device__ inline TcSave tc_save_layout(int NB, int TRmax, int T) {

@@ -93,9 +93,8 @@ __host__ __device__ inline int dw_ldmax(const sbi_nsf_model& m) {
 __host__ __device__ inline int dw_smem_bytes(const sbi_nsf_model& m) {
   return (2 * kStFloats + 64 * dw_ldmax(m) + 64) * 4;
 }
-// work units of the weight-gradient kernel per (tile, layer): the final-layer passes, three linears per
-// residual block (GLU context, W2, W1), the initial linear
-__host__ __device__ inline int dw_units(const sbi_nsf_model& m) { return (m.TRmax + 1) / 2 + 3 * m.NB + 1; }
+// work units of the weight-gradient kernel per (tile, layer) (TcSave::units)
+__host__ __device__ inline int dw_units(const sbi_nsf_model& m) { return tc_save_layout(m.NB, m.TRmax, m.T).units(); }
 
 // where the accumulators of one weight-gradient MMA go in the partial-gradient slab
 struct DwGeo {
@@ -131,12 +130,42 @@ __device__ __forceinline__ void dw_mma_image(const float* As, const float* Bs, c
   }
 }
 
+__device__ __forceinline__ void fence_acq_rel_gpu() { asm volatile("fence.acq_rel.gpu;" ::: "memory"); }
+__device__ __forceinline__ void red_add_gpu(unsigned* p, unsigned v) {
+  asm volatile("red.relaxed.gpu.global.add.u32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
+}
+__device__ __forceinline__ unsigned ld_acquire_gpu(const unsigned* p) {
+  unsigned v;
+  asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
+  return v;
+}
+
+// On half tiles (the chunk leaves SMs idle) it is launched right behind the backward sweep with programmatic
+// stream serialization: it may start once every backward CTA has run griddepcontrol.launch_dependents, and
+// each CTA waits for its own unit's dY instead of for the whole backward grid.  Its CTAs are then numbered in
+// the order the backward produces their dY: layer T-1 .. 0, then the unit in write order (final-layer passes,
+// blocks NB-1 .. 0 with GLU context, W2, W1, the initial linear), then the tile, so the CTAs dispatched first
+// are the first to find their unit ready.  On whole tiles every SM runs a backward CTA, so it is an ordinary
+// launch after the backward (`upt` = 0: no wait) with the CTAs tile-major.  Every unit writes a disjoint
+// block of its tile's partial-gradient slab, so neither order changes a value.
+// The wait cannot deadlock:
+//   * the grid launches only after every backward CTA has run launch_dependents, so the whole backward
+//     grid is resident (one CTA per SM: the chunk never has more backward CTAs than SMs);
+//   * the backward never waits on this kernel, so every counter reaches its count.
+// A backward CTA takes its SM's whole register file (255 registers x 256 threads), so these CTAs run only on
+// SMs the backward does not use, or after its CTA there has exited: they never take issue slots from it.
+// The dY loads are ld.global.cg (L2, coherent) after an acquire of the counter and a CTA barrier; nothing
+// the backward writes is read through the non-coherent path.  The counters start at zero in every run --
+// graph replays included -- because the forward sweep of the same chunk zeroes them, and stream order puts
+// that forward after the previous chunk's (or step's) weight-gradient kernel and before this backward.
+// `upt`: the count at which a unit is ready (2, one per CTA of the tile, on half tiles; 0 on whole tiles).
 template <int H>
 __global__ void __launch_bounds__(kThreads, 2)
 nsf_dw_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_constant__ sbi_rows rows,
-                 const float* __restrict__ save, float* __restrict__ gpart, int accum) {
+                 const float* __restrict__ save, float* __restrict__ gpart, int accum, unsigned upt) {
   constexpr int HP8 = (H + 7) & ~7;
   constexpr int NC = HP8 / 2;
+  static_assert(HP8 <= kDyCols, "the dY columns from kDyCols on hold the ready counters");
   extern __shared__ __align__(128) float sm[];
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int half = warp >> 2;
@@ -144,11 +173,24 @@ nsf_dw_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_constant_
   const int cbase = half * NC;
   const int q_one = H - cbase;                 // this thread's column that is X column H (the ones column)
   const int C = m.C, Cp = m.Cp, Hp = m.Hp;
-  const int nu = dw_units(m);
-  const int u = blockIdx.x % nu, l = (blockIdx.x / nu) % m.T;
-  const int64_t tile = blockIdx.x / (nu * m.T);
-  const NsfLayerView v = layer_view(m, l);
   const TcSave SV = tc_save_layout(m.NB, m.TRmax, m.T);
+  const int nu = SV.units(), npm = SV.npm;
+  int64_t tile;
+  int l, u;
+  if (upt > 0) {
+    const int ntiles = gridDim.x / (nu * m.T);
+    const int j = (blockIdx.x / ntiles) % nu;  // unit in write order
+    tile = blockIdx.x % ntiles;
+    l = m.T - 1 - (int)(blockIdx.x / (ntiles * nu));
+    u = j < npm || j == npm + 3 * m.NB ? j : npm + 3 * (m.NB - 1 - (j - npm) / 3) + (j - npm) % 3;
+  } else {
+    // after the backward: tile-major, so that the CTAs running together read and write one tile's slabs
+    tile = blockIdx.x / (nu * m.T);
+    l = (blockIdx.x / nu) % m.T;
+    u = blockIdx.x % nu;
+  }
+  const NsfLayerView v = layer_view(m, l);
+  if (u < npm && v.n_tr <= 2 * u) return;      // (CTA-uniform) this layer has fewer final-layer passes
   const float* svl = save + (size_t)tile * SV.tile_stride + (size_t)l * SV.layer_stride;
   const int64_t gr = tile * kRows + row;
   const bool live = gr < rows.R;               // rows past the end of the batch contribute nothing
@@ -176,25 +218,36 @@ nsf_dw_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_constant_
     for (int q = 0; q < NC; ++q) st_put(Bs, cbase + q, !live ? 0.f : q == q_one ? 1.f : relu ? relu_f(x[q]) : x[q]);
   };
 
+  // X comes from the forward sweep and the condition; dY only after the backward has counted the unit ready
+  auto wait_ready = [&]() {
+    if (tid == 0 && upt > 0) {
+      const unsigned* rdy = reinterpret_cast<const unsigned*>(svl + SV.ready()) + u;
+      unsigned ns = 32;
+      while (ld_acquire_gpu(rdy) < upt) {
+        __nanosleep(ns);
+        ns = min(2 * ns, 512u);
+      }
+    }
+    __syncthreads();
+  };
+
   DwGeo g;
-  const int npm = SV.npm;
   if (u < npm) {
     // ---- final layer, pass u: dW of the parameter rows of features 2u, 2u+1; X = the final-layer input
     const int nf = min(2, v.n_tr - 2 * u);
-    if (nf <= 0) return;                       // (CTA-uniform) this layer transforms fewer features
+    put_x(SV.hf, false);
+    wait_ready();
     if (half < nf) {
       float a[32];
       tc_load_prm(svl + SV.dy_fin(u), row, 0, half, a);
 #pragma unroll
       for (int i = 0; i < 32; ++i) st_put(As, 32 * half + i, live ? a[i] : 0.f);
     }
-    put_x(SV.hf, false);
     g.oW = __ldg(v.LT + SBI_L_WF) + 2 * u * m.PR * Hp; g.ldw = Hp; g.oB = __ldg(v.LT + SBI_L_BF) + 2 * u * m.PR;
     g.nX = H; g.ones = H; g.Mv = 32 * nf; g.N = 64;
   } else if (u < npm + 3 * m.NB) {
     const int b = (u - npm) / 3, k = (u - npm) % 3;
     const int* BT = v.LT + SBI_L_BLK0 + 6 * b;
-    put_dy(SV.dy_blk(b, k));
     if (k == 0) {
       // ---- dWc = dG^T ctx  (GLU gate)
       const int Nc = (Cp + 1 + 15) & ~15;
@@ -210,11 +263,12 @@ nsf_dw_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_constant_
       put_x(SV.h(b), true);
       g.oW = __ldg(BT + 0); g.ldw = Hp; g.oB = __ldg(BT + 1); g.nX = H; g.ones = H; g.Mv = Hp; g.N = 64;
     }
+    wait_ready();
+    put_dy(SV.dy_blk(b, k));
   } else {
     // ---- initial layer: dW0 = dh^T [ctx | id | 1]
     const int K0p = Cp + m.IDp;
     const int N0 = (K0p + 1 + 15) & ~15;
-    put_dy(SV.dy_init());
     for (int n = half * (N0 / 2); n < (half + 1) * (N0 / 2); ++n) {
       float val = 0.f;
       if (!live) val = 0.f;
@@ -227,6 +281,8 @@ nsf_dw_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_constant_
     }
     g.oW = __ldg(v.LT + SBI_L_W0); g.ldw = K0p; g.oB = __ldg(v.LT + SBI_L_B0); g.nX = K0p; g.ones = K0p;
     g.Mv = Hp; g.N = N0;
+    wait_ready();
+    put_dy(SV.dy_init());
   }
   fence_async_smem();
   __syncthreads();
@@ -246,6 +302,10 @@ nsf_dw_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_constant_
     bulk_commit();
     bulk_wait_all();
   }
+  // the last CTA (its unit is among the last the backward writes) holds the grid open until the backward grid
+  // has completed, so that stream work after this kernel also finds the backward's other outputs (LULinear
+  // gradients, condition gradients, loss statistics) in memory
+  if (blockIdx.x == gridDim.x - 1) asm volatile("griddepcontrol.wait;" ::: "memory");
 }
 
 template <int H, int RPC, int KB, bool COND>
@@ -261,7 +321,7 @@ nsf_vjp_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_constant
   constexpr int UPT = kRows / RPC;                      // CTAs per tile (= cluster size)
   constexpr int NC = TPR == 2 ? HP8 / 2 : 16;           // columns per thread ([tq NC, tq NC + NC))
   constexpr int NG = NC / 4;
-  static_assert(HP8 % 8 == 0 && NC % 4 == 0 && H > (TPR - 1) * NC && H < HP8 + 1 && HP8 <= 64, "hidden width");
+  static_assert(HP8 % 8 == 0 && NC % 4 == 0 && H > (TPR - 1) * NC && H < HP8 + 1 && HP8 <= kDyCols, "hidden width");
   extern __shared__ __align__(128) float sm[];
   const BwdSmem L = bwd_smem_layout(tcb.stage_cap, RPC);
   uint64_t* full = reinterpret_cast<uint64_t*>(reinterpret_cast<char*>(sm) + L.bar_bytes);
@@ -273,6 +333,8 @@ nsf_vjp_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_constant
   float* as = sm + L.a;
   IssuerT<kBwdSlots, true, RPC> iss =
       tc_begin<kBwdSlots, true, RPC>(full, sm + L.ring, tcb, m.T, nunits, true, kColsDG, sa, as);
+  // half tiles: the weight-gradient kernel may start once every CTA of this grid is resident (it waits per unit)
+  if constexpr (UPT > 1) asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
   SBI_TL(100);
 
   const float* __restrict__ P = m.d_params;
@@ -319,6 +381,27 @@ nsf_vjp_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_constant
   auto read_acc = [&](int region, float (&d)[NC]) {
 #pragma unroll
     for (int g = 0; g < NG; ++g) ld4(row, region + cbase + 4 * g, d + 4 * g);
+  };
+  // the thread's dY columns of a [128][64] dY array (none from kDyCols on: they hold the ready counters)
+  auto save_dy = [&](float* q, int srow, const float (&d)[NC]) {
+#pragma unroll
+    for (int g = 0; g < NG; ++g) {
+      if (TPR * NC > kDyCols && cbase + 4 * g >= kDyCols) continue;
+      __stcg(tc_grp(q, tq * NG + g, srow), make_float4(d[4 * g], d[4 * g + 1], d[4 * g + 2], d[4 * g + 3]));
+    }
+  };
+  // half tiles, after the CTA barrier that follows the write-out of units [u0, u0 + n) of the layer at svl:
+  // count this CTA in their ready counters (release at gpu scope, which the CTA barrier makes cover every
+  // thread's dY).  Releasing unit by unit spreads the weight-gradient work over the chain.  Whole tiles leave
+  // no SM idle and release nothing: their weight-gradient kernel is an ordinary launch after the backward.
+  auto publish = [&](float* svl, int u0, int n) {
+    if constexpr (UPT > 1) {
+      if (tid == 0) {
+        unsigned* rdy = reinterpret_cast<unsigned*>(svl + SV.ready());
+        fence_acq_rel_gpu();
+        for (int i = 0; i < n; ++i) red_add_gpu(rdy + u0 + i, 1u);
+      }
+    }
   };
 
   int iter = 0;
@@ -552,6 +635,7 @@ nsf_vjp_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_constant
             tc_save_prm(svl + SV.dy_fin(p), srow, 0, tq & 1, dq);
           }
           hand_over();
+          publish(svl, p, 1);
           {
             uint32_t acc = p > 0 ? 1u : 0u;
             iss.begin(__ldg(tab + 5 + 4 * (stage + p)));
@@ -587,19 +671,22 @@ nsf_vjp_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_constant
             dT[q] = dhq * s;
             dG[q] = dhq * t2[q] * s * (1.f - s);
           }
-          tc_save_cols<NC>(svl + SV.dy_blk(b, 0), srow, tq, dG);
+          save_dy(svl + SV.dy_blk(b, 0), srow, dG);
           if (COND) {
             group_sync();
+            publish(svl, SV.npm + 3 * b, 1);
             dctx_add(svl + SV.dy_blk(b, 0), P + __ldg(BT + 4), m.Cp, row0, srow);     // dG Wc
           }
         }
         SBI_TL(1000 * (li + 1) + 30 + 10 * b);
         // ---- dA1 = (dT W2) * [a1 > 0]
         {
-          tc_save_cols<NC>(svl + SV.dy_blk(b, 1), srow, tq, dT);
+          save_dy(svl + SV.dy_blk(b, 1), srow, dT);
           write_a(dT, 0);
           SBI_TL(1000 * (li + 1) + 72 + 10 * b);
           hand_over();
+          if (COND) publish(svl, SV.npm + 3 * b + 1, 1);
+          else publish(svl, SV.npm + 3 * b, 2);
           SBI_TL(1000 * (li + 1) + 73 + 10 * b);
           {
             uint32_t acc = 0u;
@@ -620,9 +707,10 @@ nsf_vjp_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_constant
         SBI_TL(1000 * (li + 1) + 32 + 10 * b);
         // ---- dh += (dA1 W1) * [h_b > 0]
         {
-          tc_save_cols<NC>(svl + SV.dy_blk(b, 2), srow, tq, dA);
+          save_dy(svl + SV.dy_blk(b, 2), srow, dA);
           write_a(dA, 0);
           hand_over();
+          publish(svl, SV.npm + 3 * b + 2, 1);
           {
             uint32_t acc = 0u;
             iss.begin(__ldg(tab + 5 + 4 * stage));
@@ -648,9 +736,10 @@ nsf_vjp_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_constant
       // ================= initial layer: d(identity features) = dh W0[:, C:] =================
       {
         const int K0p = m.Cp + m.IDp;
-        tc_save_cols<NC>(svl + SV.dy_init(), srow, tq, dh);
+        save_dy(svl + SV.dy_init(), srow, dh);
         write_a(dh, 0);
         hand_over();
+        publish(svl, SV.npm + 3 * m.NB, 1);
         if (COND) dctx_add(svl + SV.dy_init(), P + __ldg(v.LT + SBI_L_W0), K0p, row0, srow);     // the context columns of dh W0
         {
           uint32_t acc = 0u;
@@ -743,9 +832,10 @@ static int vjp_tc_launch(const sbi_nsf_model* m, const sbi_nsf_tc* tc_fwd, const
     return e;
   if (int e = set_smem(reinterpret_cast<const void*>(tc::nsf_dw_tc_kernel<50>), dw_bytes)) return e;
   // chunks of one tile per SM: forward sweep (saves activations), backward sweep of the same rows (tile t
-  // writes partial-gradient slab t), then their weight gradients (one CTA per tile, layer and linear); later
-  // chunks accumulate into the partial-gradient slabs.  A chunk of at most half as many tiles as SMs runs
-  // the two sweeps on half tiles (two CTAs per tile), so that twice as many SMs take part.
+  // writes partial-gradient slab t), then their weight gradients (one CTA per tile, layer and linear), which on
+  // half tiles start while the backward runs and take each unit as soon as its dY is written; later chunks accumulate
+  // into the partial-gradient slabs.  A chunk of at most half as many tiles as SMs runs the two sweeps on
+  // half tiles (two CTAs per tile), so that twice as many SMs take part.
   tc::StoreArgs sa;
   if (int e = tc::store_args(&sa)) return e;
   const int64_t chunk = vjp_tc_chunk_rows();
@@ -769,8 +859,8 @@ static int vjp_tc_launch(const sbi_nsf_model* m, const sbi_nsf_tc* tc_fwd, const
                                      *tc_bwd, rr, d_gout ? d_gout + r0 : nullptr, g_const, d_gpart, d_loss_acc,
                                      d_save, r0 > 0 ? 1 : 0, sa, COND ? d_gcond + r0 * m->C : nullptr))
       return rc;
-    if (int rc = launch(tc::nsf_dw_tc_kernel<50>, grid * m->T * tc::dw_units(*m), tc::kThreads, dw_bytes, s, *m, rr,
-                        d_save, d_gpart, r0 > 0 ? 1 : 0))
+    if (int rc = launch(tc::nsf_dw_tc_kernel<50>, Grid(grid * m->T * tc::dw_units(*m), 1, half_tiles), tc::kThreads,
+                        dw_bytes, s, *m, rr, d_save, d_gpart, r0 > 0 ? 1 : 0, half_tiles ? 2u : 0u))
       return rc;
   }
   return 0;
