@@ -109,11 +109,19 @@ int sbi_b200_nsf_logprob(const sbi_nsf_model* m, const sbi_rows* rows, float* d_
  *   d_gpart  (n_part, n_params) per-CTA partial parameter gradients (written, not
  *            accumulated); n_part = sbi_b200_nsf_vjp_parts(R).
  *   d_ginput (R, D), d_gcond (R, C) optional input / condition gradients.
- *   d_loss_acc optional: [0] += sum_r -logp_r , [1] += #non-finite rows.              */
+ *   d_loss_acc optional: [0] += sum_r -logp_r , [1] += #non-finite rows.
+ *   d_save  optional caller-owned activation scratch of save_bytes bytes.  With it the forward sweep keeps each
+ *           layer's conditioner intermediates there and the backward sweep reads them back; with NULL the
+ *           backward sweep recomputes them.  Both give bit-identical results.  A buffer smaller than
+ *           sbi_b200_nsf_vjp_save_bytes(m, R) is rejected with SBI_EINVAL before anything is launched.  Calls
+ *           that may run concurrently need buffers of their own.
+ * sbi_b200_nsf_vjp_save_bytes is 0 for models whose VJP always recomputes (16-row tiles, e.g. deep `made`
+ * conditioners), and for an invalid model or R < 1. */
 int sbi_b200_nsf_vjp_parts(int64_t R);
+int64_t sbi_b200_nsf_vjp_save_bytes(const sbi_nsf_model* m, int64_t R);
 int sbi_b200_nsf_vjp(const sbi_nsf_model* m, const sbi_rows* rows, const float* d_gout,
                      float g_const, float* d_logp, float* d_gpart, float* d_ginput,
-                     float* d_gcond, float* d_loss_acc, void* stream);
+                     float* d_gcond, float* d_loss_acc, float* d_save, int64_t save_bytes, void* stream);
 
 /* x = flow^{-1}(noise | cond): sampling path.  d_noise (R, D) -> d_out (R, D);
  * d_logabsdet (R,) optional = log|det d x / d noise|. */
@@ -218,9 +226,8 @@ int sbi_b200_nsf_vjp_tc(const sbi_nsf_model* m, const sbi_nsf_tc* tc_fwd, const 
 /* The same step plus the condition gradient d_gcond (R, C) of sum_r g_r log q_r in raw condition space (the
  * context columns of every layer's initial linear and the GLU context linear of every residual block, accumulated
  * per row over the layers; one writer per entry, repeated calls are bit-identical).  The parameter partials are
- * those of sbi_b200_nsf_vjp_tc.  The instantiation adds no shared memory, so _cond_supported applies the same layout
- * check as sbi_b200_nsf_vjp_tc_supported; models it declines run sbi_b200_nsf_vjp with d_gcond. */
-int sbi_b200_nsf_vjp_tc_cond_supported(const sbi_nsf_model* m, const sbi_nsf_tc* tc_fwd, const sbi_nsf_tc* tc_bwd);
+ * those of sbi_b200_nsf_vjp_tc.  The instantiation adds no shared memory, so sbi_b200_nsf_vjp_tc_supported covers it;
+ * models it declines run sbi_b200_nsf_vjp with d_gcond. */
 int sbi_b200_nsf_vjp_tc_cond(const sbi_nsf_model* m, const sbi_nsf_tc* tc_fwd, const sbi_nsf_tc* tc_bwd,
                              const sbi_rows* rows, const float* d_gout, float g_const, float* d_logp,
                              float* d_gpart, float* d_loss_acc, float* d_gcond, float* d_save, int64_t save_bytes,
@@ -682,6 +689,8 @@ typedef struct {
   const sbi_nsf_tc* tc_pack;
   const sbi_nsf_tc* tc_fwd;
   const sbi_nsf_tc* tc_bwd;
+  /* activation scratch of whichever kernel runs the step: required by the tensor-core step; optional for the SIMT
+   * kernel (NULL: it recomputes), which then needs sbi_b200_nsf_vjp_save_bytes(m, B) bytes */
   float* d_save;
   int64_t save_bytes;
 } sbi_train_ws;

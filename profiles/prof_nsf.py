@@ -23,12 +23,13 @@ gpart = est._gpart(n_part)
 grad = torch.zeros(P, device="cuda"); state = torch.zeros(2 * P, device="cuda")
 step = torch.zeros(2, dtype=torch.int32, device="cuda")
 idx = torch.randperm(90000, device="cuda")[:BATCH]
+save = torch.empty(lib.sbi_b200_nsf_vjp_save_bytes(C.byref(est._model(nbuf=3)), BATCH) // 4, device="cuda")
 for it in range(4):
     if which in ("all", "vjp"):
         m = est._model(nbuf=3)
         rows = L.Rows(th.data_ptr(), xx.data_ptr(), idx.data_ptr(), BATCH, 0)
         L.check(lib.sbi_b200_nsf_vjp(C.byref(m), C.byref(rows), None, -1.0 / BATCH, None, L.ptr(gpart), None, None,
-                                     None, L.stream_ptr()), "vjp")
+                                     None, L.ptr(save), save.numel() * 4, L.stream_ptr()), "vjp")
         L.check(lib.sbi_b200_reduce_partials(L.ptr(gpart), n_part, P, L.ptr(grad), L.stream_ptr()), "red")
         L.check(lib.sbi_b200_adam_clip_step(L.ptr(est.flat.data), L.ptr(grad), L.ptr(state), L.ptr(step),
                                             L.ptr(est.net._mask), P, 5e-4, .9, .999, 1e-8, 5.0, 1.0, L.stream_ptr()), "adam")

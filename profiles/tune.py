@@ -20,6 +20,7 @@ P = est.layout.n_params
 n_part = lib.sbi_b200_nsf_vjp_parts(BATCH)
 gpart = est._gpart(n_part)
 idx = torch.randperm(90000, device="cuda")[:BATCH]
+save = torch.empty(lib.sbi_b200_nsf_vjp_save_bytes(C.byref(est._model(nbuf=3)), BATCH) // 4, device="cuda")
 flush = torch.empty(256 << 20, dtype=torch.uint8, device="cuda")
 nbuf_tr = int(os.environ.get("NBUF_TRAIN", "3"))
 nbuf_ev = int(os.environ.get("NBUF_EVAL", "2"))
@@ -42,7 +43,7 @@ def vjp():
     m = est._model(nbuf=nbuf_tr)
     rows = L.Rows(th.data_ptr(), xx.data_ptr(), idx.data_ptr(), BATCH, 0)
     L.check(lib.sbi_b200_nsf_vjp(C.byref(m), C.byref(rows), None, -1.0 / BATCH, None, L.ptr(gpart), None, None, None,
-                                 L.stream_ptr()), "vjp")
+                                 L.ptr(save), save.numel() * 4, L.stream_ptr()), "vjp")
 
 
 R = 1 << 22

@@ -203,9 +203,10 @@ _EXPORTS = {
     "sbi_b200_nsf_logprob": (C.c_int, [C.POINTER(NsfModel), C.POINTER(Rows), C.c_void_p,
                                        C.c_void_p, C.c_void_p]),
     "sbi_b200_nsf_vjp_parts": (C.c_int, [C.c_int64]),
+    "sbi_b200_nsf_vjp_save_bytes": (C.c_int64, [C.POINTER(NsfModel), C.c_int64]),
     "sbi_b200_nsf_vjp": (C.c_int, [C.POINTER(NsfModel), C.POINTER(Rows), C.c_void_p, C.c_float,
                                    C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
-                                   C.c_void_p]),
+                                   C.c_void_p, C.c_int64, C.c_void_p]),
     "sbi_b200_nsf_inverse": (C.c_int, [C.POINTER(NsfModel), C.POINTER(Rows), C.c_void_p,
                                        C.c_void_p, C.c_void_p]),
     "sbi_b200_nsf_tc_supported": (C.c_int, [C.POINTER(NsfModel), C.POINTER(NsfTc)]),
@@ -220,7 +221,6 @@ _EXPORTS = {
     "sbi_b200_nsf_vjp_tc": (C.c_int, [C.POINTER(NsfModel), C.POINTER(NsfTc), C.POINTER(NsfTc), C.POINTER(Rows),
                                       C.c_void_p, C.c_float, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                       C.c_int64, C.c_void_p]),
-    "sbi_b200_nsf_vjp_tc_cond_supported": (C.c_int, [C.POINTER(NsfModel), C.POINTER(NsfTc), C.POINTER(NsfTc)]),
     "sbi_b200_nsf_vjp_tc_cond": (C.c_int, [C.POINTER(NsfModel), C.POINTER(NsfTc), C.POINTER(NsfTc), C.POINTER(Rows),
                                            C.c_void_p, C.c_float, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                            C.c_void_p, C.c_int64, C.c_void_p]),

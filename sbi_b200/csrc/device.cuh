@@ -1,6 +1,6 @@
 // Host side of the C-ABI entry points: every entry runs on the device that owns its first device pointer (not on
-// whatever device happens to be current), every per-process cache (SM count, granted dynamic shared memory,
-// scratch) is kept per device, and every row-tile kernel is sized and launched through the helpers below.
+// whatever device happens to be current), every per-process cache (SM count, granted dynamic shared memory)
+// is kept per device, and every row-tile kernel is sized and launched through the helpers below.
 #pragma once
 #include <cuda_runtime.h>
 

@@ -11,7 +11,8 @@
   } while (0)
 
 // forward+backward of the staged batch: tensor-core kernels when the workspace carries their operand
-// descriptors, else the SIMT kernel.  Returns the number of partial-gradient slabs written in *n_part.
+// descriptors, else the SIMT kernel, which spills its activations to ws->d_save when the workspace has one.
+// Returns the number of partial-gradient slabs written in *n_part.
 static int vjp_staged(const sbi_nsf_model* m, const sbi_train_ws* ws, int64_t B, float g_const, int* n_part,
                       void* stream) {
   sbi_rows rows;
@@ -29,7 +30,7 @@ static int vjp_staged(const sbi_nsf_model* m, const sbi_train_ws* ws, int64_t B,
   }
   *n_part = sbi_b200_nsf_vjp_parts(B);
   return sbi_b200_nsf_vjp(m, &rows, nullptr, g_const, nullptr, ws->d_gpart, nullptr, nullptr, ws->d_loss_acc,
-                          stream);
+                          ws->d_save, ws->save_bytes, stream);
 }
 
 // partial-gradient reduction (+ per-block sum of squares when the workspace has room) -> clip + Adam

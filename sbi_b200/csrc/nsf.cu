@@ -2,7 +2,6 @@
 #include <cuda_runtime.h>
 #include <math.h>
 #include <algorithm>
-#include <cstdlib>
 
 #include "nsf.cuh"
 #include "device.cuh"
@@ -688,54 +687,35 @@ extern "C" int sbi_b200_nsf_inverse(const sbi_nsf_model* m, const sbi_rows* rows
 
 extern "C" int sbi_b200_nsf_vjp_parts(int64_t R) { return vjp_parts(R, 32); }
 
-// Scratch for the activation spill of the VJP kernel: one slab per (CTA, layer), owned by the
-// library and grown on demand (old, smaller buffers stay allocated).  It cannot be (re)allocated while the stream is being captured into
-// a CUDA graph; then -- or with SBI_B200_VJP_SPILL=0 -- the kernel recomputes instead.
-static float* g_vjp_scratch[sbi::kMaxDev] = {nullptr};
-static size_t g_vjp_scratch_bytes[sbi::kMaxDev] = {0};
-static float* vjp_scratch(size_t bytes, cudaStream_t s) {
-  static const bool off = [] {
-    const char* e = getenv("SBI_B200_VJP_SPILL");
-    return e && e[0] == '0';
-  }();
-  if (off) return nullptr;
-  const int dev = sbi::cur_dev();      // one scratch per device: switching devices never reallocates
-  if (g_vjp_scratch[dev] && bytes <= g_vjp_scratch_bytes[dev]) return g_vjp_scratch[dev];
-  cudaStreamCaptureStatus st = cudaStreamCaptureStatusNone;
-  if (cudaStreamIsCapturing(s, &st) != cudaSuccess || st != cudaStreamCaptureStatusNone) return nullptr;
-  // a smaller buffer handed out earlier is NOT freed: a CUDA graph captured with it may still be
-  // replayed (growth happens at most a few times per process and device, with model size)
-  float* p = nullptr;
-  if (cudaMalloc(&p, bytes) != cudaSuccess) {
-    cudaGetLastError();
-    return nullptr;
-  }
-  g_vjp_scratch[dev] = p;
-  g_vjp_scratch_bytes[dev] = bytes;
-  return p;
+// Whether the VJP of `m` runs on 32-row tiles.  Deep conditioners (`made`: five residual blocks) keep too many
+// intermediates for a 32-row tile and take 16-row tiles that recompute each layer's conditioner (no spill).
+static bool vjp_32_rows(const sbi_nsf_model& m) { return nsf_smem_layout(m, 32, true).total_bytes <= kMaxSmemBytes; }
+
+extern "C" int64_t sbi_b200_nsf_vjp_save_bytes(const sbi_nsf_model* m, int64_t R) {
+  if (check_model(m) || R < 1 || !vjp_32_rows(*m)) return 0;
+  // the slab nsf_vjp_kernel spills per (CTA, layer): HS | A1S | T2S | SS and the spline parameters
+  const int64_t slab = (int64_t)((4 * m->NB + 1) * m->Hp + m->TRmax * m->PR) * Tile<32>::LD;
+  return (int64_t)sizeof(float) * slab * m->T * sbi_b200_nsf_vjp_parts(R);
 }
 
 extern "C" int sbi_b200_nsf_vjp(const sbi_nsf_model* m, const sbi_rows* rows, const float* d_gout,
                                 float g_const, float* d_logp, float* d_gpart, float* d_ginput,
-                                float* d_gcond, float* d_loss_acc, void* stream) {
+                                float* d_gcond, float* d_loss_acc, float* d_save, int64_t save_bytes,
+                                void* stream) {
   sbi::DeviceGuard dev_guard_(m ? m->d_params : nullptr);
   int rc = check_model(m);
   if (rc) return rc;
   if (!rows || !rows->d_input || !rows->d_cond || rows->R < 1 || !d_gpart) return SBI_EINVAL;
+  if (d_save && save_bytes < sbi_b200_nsf_vjp_save_bytes(m, rows->R)) return SBI_EINVAL;
   cudaStream_t s = (cudaStream_t)stream;
-  constexpr int TM = 32;
-  const int bytes = nsf_smem_layout(*m, TM, true).total_bytes;
   const int grid = sbi_b200_nsf_vjp_parts(rows->R);
-  if (bytes > kMaxSmemBytes) {
-    // deep conditioners (`made`: five residual blocks) keep too many intermediates for a 32-row tile:
-    // 16-row tiles, per-layer recompute; every CTA walks its tiles and accumulates into its slab (the grid keeps
-    // the 32-row part count: the caller sized its slabs from sbi_b200_nsf_vjp_parts)
+  if (!vjp_32_rows(*m)) {
+    // every CTA walks its 16-row tiles and accumulates into its slab (the grid keeps the 32-row part count: the
+    // caller sized its slabs from sbi_b200_nsf_vjp_parts)
     return launch(nsf_vjp_kernel<16, 2, 2, false>, grid, kThreads, nsf_smem_layout(*m, 16, true).total_bytes, s, *m,
                   *rows, d_gout, g_const, d_logp, d_gpart, d_ginput, d_gcond, d_loss_acc, nullptr);
   }
-  const size_t slab = (size_t)((4 * m->NB + 1) * m->Hp + m->TRmax * m->PR) * (TM + 4);
-  float* scratch = vjp_scratch(sizeof(float) * slab * m->T * (size_t)dev_num_sms(), s);
-  auto k = scratch != nullptr ? nsf_vjp_kernel<TM, 2, 2, true> : nsf_vjp_kernel<TM, 2, 2, false>;
-  return launch(k, grid, kThreads, bytes, s, *m, *rows, d_gout, g_const, d_logp, d_gpart, d_ginput, d_gcond,
-                d_loss_acc, scratch);
+  auto k = d_save ? nsf_vjp_kernel<32, 2, 2, true> : nsf_vjp_kernel<32, 2, 2, false>;
+  return launch(k, grid, kThreads, nsf_smem_layout(*m, 32, true).total_bytes, s, *m, *rows, d_gout, g_const, d_logp,
+                d_gpart, d_ginput, d_gcond, d_loss_acc, d_save);
 }

@@ -794,12 +794,6 @@ extern "C" int sbi_b200_nsf_vjp_tc_supported(const sbi_nsf_model* m, const sbi_n
   return vjp_tc_ok(m, tc_fwd, tc_bwd);
 }
 
-extern "C" int sbi_b200_nsf_vjp_tc_cond_supported(const sbi_nsf_model* m, const sbi_nsf_tc* tc_fwd,
-                                                  const sbi_nsf_tc* tc_bwd) {
-  if (!m || !tc_fwd || !tc_bwd) return 0;
-  return vjp_tc_ok(m, tc_fwd, tc_bwd);
-}
-
 // rows of one forward + backward launch pair (one tile per CTA, every SM busy once)
 static int64_t vjp_tc_chunk_rows() { return (int64_t)tc::kRows * sbi::dev_num_sms(); }
 

@@ -524,13 +524,21 @@ class FlowEstimator(_PackedEstimator):
 
     def vjp_cond_uses_tc(self, R: int) -> bool:
         """Whether the trainer's step with a condition gradient (embedding net) runs on the tensor cores
-        (`sbi_b200_nsf_vjp_tc_cond`): same row threshold and switches as the parameter-only step, and the model
-        must fit that instantiation's shared-memory layout.  `log_prob().backward()` does not use this path."""
-        if not self._vjp_uses_tc(R, True):
-            return False
-        tcs = self._tc_train_state(self._model(nbuf=3), pack=False)
-        return tcs is not None and bool(L.load().sbi_b200_nsf_vjp_tc_cond_supported(
-            C.byref(self._model(nbuf=3)), C.byref(tcs[0]), C.byref(tcs[1])))
+        (`sbi_b200_nsf_vjp_tc_cond`): that instantiation adds no shared memory, so it runs wherever the
+        parameter-only step does.  `log_prob().backward()` does not use this path."""
+        return self._vjp_uses_tc(R, True)
+
+    def _vjp_save(self, nbytes: int):
+        """(pointer, bytes) of the VJP kernels' activation scratch, grown to at least `nbytes` bytes on the
+        parameter device, or (None, 0) when `nbytes` is 0 (the kernel keeps nothing)."""
+        if nbytes == 0:
+            return None, 0
+        dev = self.net.flat.device
+        save = self._cache.get("vjp_save")
+        if save is None or save.numel() * 4 < nbytes or save.device != dev:
+            save = torch.empty((nbytes + 3) // 4, dtype=torch.float32, device=dev)
+            self._cache["vjp_save"] = save
+        return save.data_ptr(), save.numel() * 4
 
     def vjp(self, m, rows, R: int, gout, g_const: float, logp, gpart, ginput=None, gcond=None, loss_acc=None,
             cond_tc: bool = False):
@@ -543,24 +551,23 @@ class FlowEstimator(_PackedEstimator):
         if ginput is None and (gcond is None or cond_tc) and self._vjp_uses_tc(R, True):
             tcs = self._tc_train_state(m)
             if tcs is not None:
-                nbytes = int(lib.sbi_b200_nsf_vjp_tc_save_bytes(C.byref(m), R))
-                save = self._cache.get("vjp_save")
-                if save is None or save.numel() * 4 < nbytes or save.device != self.net.flat.device:
-                    save = torch.empty((nbytes + 3) // 4, dtype=torch.float32, device=self.net.flat.device)
-                    self._cache["vjp_save"] = save
+                save, nbytes = self._vjp_save(lib.sbi_b200_nsf_vjp_tc_save_bytes(C.byref(m), R))
                 if gcond is not None:
                     L.check(lib.sbi_b200_nsf_vjp_tc_cond(
                         C.byref(m), C.byref(tcs[0]), C.byref(tcs[1]), C.byref(rows), L.ptr(gout), g_const, L.ptr(logp),
-                        L.ptr(gpart), L.ptr(loss_acc), L.ptr(gcond), L.ptr(save), save.numel() * 4, L.stream_ptr()),
+                        L.ptr(gpart), L.ptr(loss_acc), L.ptr(gcond), save, nbytes, L.stream_ptr()),
                         "nsf_vjp_tc_cond")
                     return
                 L.check(lib.sbi_b200_nsf_vjp_tc(C.byref(m), C.byref(tcs[0]), C.byref(tcs[1]), C.byref(rows), L.ptr(gout),
-                                                g_const, L.ptr(logp), L.ptr(gpart), L.ptr(loss_acc), L.ptr(save),
-                                                save.numel() * 4, L.stream_ptr()), "nsf_vjp_tc")
+                                                g_const, L.ptr(logp), L.ptr(gpart), L.ptr(loss_acc), save, nbytes,
+                                                L.stream_ptr()), "nsf_vjp_tc")
                 return
-        self._check_rc(self._entry("vjp")(C.byref(m), C.byref(rows), L.ptr(gout), g_const, L.ptr(logp),
-                                          L.ptr(gpart), L.ptr(ginput), L.ptr(gcond), L.ptr(loss_acc),
-                                          L.stream_ptr()), f"{self.layout.family}_vjp")
+        args = (C.byref(m), C.byref(rows), L.ptr(gout), g_const, L.ptr(logp), L.ptr(gpart), L.ptr(ginput),
+                L.ptr(gcond), L.ptr(loss_acc))
+        if self._family.prefix == "nsf":       # `nsf` and `made`: the SIMT kernel spills its activations
+            save, nbytes = self._vjp_save(lib.sbi_b200_nsf_vjp_save_bytes(C.byref(m), R))
+            args += (save, nbytes)
+        self._check_rc(self._entry("vjp")(*args, L.stream_ptr()), f"{self.layout.family}_vjp")
 
     # ---- raw kernel entry (no autograd) --------------------------------------------------------------
     def _logprob_raw(self, inp: Tensor, ctx: Tensor, shared: bool, want_noise=False,

@@ -625,7 +625,7 @@ class _FlowTrainer(_Trainer):
         perm_buf = torch.empty(steps * B, dtype=torch.int64, device=dev)
         vperm_buf = torch.empty(max(vsteps * Bv, 1), dtype=torch.int64, device=dev)
         cond_tc = train_emb and net.vjp_cond_uses_tc(Bl)
-        n_part = lib.sbi_b200_nsf_vjp_tc_parts(Bl) if cond_tc else net.vjp_parts(Bl, param_grads_only=not train_emb)
+        n_part = net.vjp_parts(Bl, param_grads_only=cond_tc or not train_emb)
         gpart = net._gpart(n_part)
         gcond = torch.empty(Bl, net.layout.C, dtype=torch.float32, device=dev) if train_emb else None
         loss_acc = torch.zeros(2, dtype=torch.float32, device=dev)

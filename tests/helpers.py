@@ -26,6 +26,25 @@ def b200_from_oracle(flow, theta, x, device="cuda", **kw):
     return est.to(device)
 
 
+def nsf_vjp_raw(est, inp, cond, g, save, fill=0.0):
+    """sbi_b200_nsf_vjp of sum_r g_r log q(inp_r | cond_r) on the current stream, with `save` (a CUDA tensor, or
+    None) as the activation scratch: (return code, per-CTA partials, input gradient, condition gradient,
+    log-probs), the four outputs allocated and filled with `fill` before the call."""
+    import ctypes as C
+    from sbi_b200 import _lib as L
+    lib = L.load()
+    R = inp.shape[0]
+    m = est._model(nbuf=3)
+    rows = L.Rows(inp.data_ptr(), cond.data_ptr(), None, R, 0)
+    gpart = torch.full((lib.sbi_b200_nsf_vjp_parts(R), est.layout.n_params), fill, device=inp.device)
+    ginp, gcond = torch.full_like(inp, fill), torch.full_like(cond, fill)
+    logp = torch.full((R,), fill, device=inp.device)
+    rc = lib.sbi_b200_nsf_vjp(C.byref(m), C.byref(rows), L.ptr(g), 0.0, L.ptr(logp), L.ptr(gpart), L.ptr(ginp),
+                              L.ptr(gcond), None, L.ptr(save), 0 if save is None else save.numel() * 4,
+                              torch.cuda.current_stream().cuda_stream)
+    return rc, gpart, ginp, gcond, logp
+
+
 def oracle_maf(D=3, C=2, n=2000, seed=0, perturb=0.1, scale_fn="softplus", rqs=False, **kw):
     """Oracle MAF, or with `rqs` MAF-RQS (spline element-wise maps), with perturbed weights."""
     from oracle.nflows_port.transforms import autoregressive as _ar

@@ -155,3 +155,37 @@ def test_vector_field_trainers_refuse_later_rounds_like_the_reference():
         with pytest.raises(NotImplementedError, match=f"Multi-round {cls.__name__}"):
             t._vf_check_rounds({})
         t._vf_check_rounds({"force_first_round_loss": True})
+
+
+def _nsf_model_on_host(lay):
+    """The kernels' model struct of `lay` with its pointers on host buffers: enough for the host-side queries,
+    which read the struct and never dereference its pointers."""
+    from sbi_b200 import _lib as L
+    keep = [torch.zeros(lay.n_params), *(torch.from_numpy(t) for t in lay.tables()),
+            torch.ones(2 * lay.Dp + 2 * lay.Cp)]
+    m = lay.fill_struct(L.NsfModel(), 3)
+    m.d_params, m.d_layer_tab, m.d_feat_tab, m.d_stats = (t.data_ptr() for t in keep)
+    return m, keep
+
+
+def test_nsf_vjp_save_bytes(lib):
+    """The SIMT VJP's activation scratch: one slab of (4 NB + 1) Hp + TRmax PR rows of 36 floats per layer and
+    partial-gradient slab; none for the models that run 16-row tiles, an invalid model or R < 1."""
+    import ctypes as C
+    m, _keep = _nsf_model_on_host(NsfLayout(D=10, C=10))
+    slab = ((4 * m.NB + 1) * m.Hp + m.TRmax * m.PR) * 36
+    query = lambda R: lib.sbi_b200_nsf_vjp_save_bytes(C.byref(m), R)   # noqa: E731
+    for R in (1, 31, 32, 33, 300, 4096, 10 ** 6):
+        assert query(R) == 4 * slab * m.T * lib.sbi_b200_nsf_vjp_parts(R), R
+    n_sat = lib.sbi_b200_nsf_vjp_parts(10 ** 9)
+    assert n_sat > 1
+    sizes = [query(32 * k) for k in range(1, n_sat + 3)]
+    assert all(a < b for a, b in zip(sizes[:n_sat], sizes[1:n_sat])), "grows with R while the parts count does"
+    assert sizes[n_sat - 1] == sizes[n_sat] == sizes[n_sat + 1] == query(10 ** 9)
+    assert query(0) == 0 and query(-5) == 0
+    assert lib.sbi_b200_nsf_vjp_save_bytes(None, 4096) == 0
+    m.d_params = None
+    assert query(4096) == 0
+    for kw in (dict(H=64), dict(NB=4)):
+        m16, _keep16 = _nsf_model_on_host(NsfLayout(D=10, C=10, **kw))
+        assert lib.sbi_b200_nsf_vjp_save_bytes(C.byref(m16), 4096) == 0, kw

@@ -19,7 +19,7 @@ import torch
 from torch import nn
 
 from oracle import sbi_port
-from tests.helpers import b200_from_oracle, b200_maf_from_oracle, oracle_maf, oracle_nsf
+from tests.helpers import b200_from_oracle, b200_maf_from_oracle, nsf_vjp_raw, oracle_maf, oracle_nsf
 
 pytestmark = pytest.mark.gpu
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -232,13 +232,19 @@ def test_maf_row_tiles_match_oracle(cuda_lib, kw):
 _VJP_KERNEL = re.compile(r"nsf_vjp_kernel<\d+, \d+, \d+, (true|false)>")
 
 
-def _vjp_kernels_seen(est, inp, cond):
+def _vjp_kernels_seen(fn, repeat=1):
+    """(the NSF VJP kernels `repeat` calls of `fn()` launch, what the last call returns).  The window is padded on
+    both sides: a kernel that starts right after the profiler does is now and then missing from its trace."""
+    import time
     from torch.profiler import ProfilerActivity, profile
-    ic = inp.cuda().requires_grad_(True)
+    torch.cuda.synchronize()
     with profile(activities=[ProfilerActivity.CUDA]) as prof:
-        est.log_prob(ic, cond.cuda())[0].sum().backward()
+        time.sleep(0.02)
+        for _ in range(repeat):
+            out = fn()
         torch.cuda.synchronize()
-    return sorted({m.group(0) for e in prof.key_averages() for m in [_VJP_KERNEL.search(e.key)] if m})
+        time.sleep(0.02)
+    return sorted({m.group(0) for e in prof.key_averages() for m in [_VJP_KERNEL.search(e.key)] if m}), out
 
 
 @pytest.mark.parametrize("kw,want", [({}, "nsf_vjp_kernel<32, 2, 2, true>"),
@@ -248,35 +254,42 @@ def _vjp_kernels_seen(est, inp, cond):
 def test_nsf_vjp_regime_kernels(cuda_lib, kw, want):
     flow, theta, x = oracle_nsf(10, 10, n=500, **kw)
     est = b200_from_oracle(flow, theta, x, **kw)
-    seen = _vjp_kernels_seen(est, theta[:300] * 1.3, x[:300])
+    ic = (theta[:300] * 1.3).cuda().requires_grad_(True)
+    seen, _ = _vjp_kernels_seen(lambda: est.log_prob(ic, x[:300].cuda())[0].sum().backward())
     print(f"{kw}: VJP kernels seen {seen}")
     assert seen == [want]
     _flow_vjp(f"vjp regime {kw}", flow, est, theta[:300] * 1.3, x[:300])
+
+
+def test_nsf_vjp_kernel_follows_the_callers_scratch(cuda_lib):
+    """With the caller's activation scratch the 32-row VJP spills (nsf_vjp_kernel<32, 2, 2, true>); without one the
+    32-row recompute kernel runs and its gradients match the fp64 oracle."""
+    from sbi_b200 import _lib as L
+    flow, theta, x = oracle_nsf(10, 10, n=500)
+    est = b200_from_oracle(flow, theta, x)
+    R = 300
+    inp, cond = theta[:R] * 1.3, x[:R]
+    g = torch.randn(R, dtype=torch.float64, generator=torch.Generator().manual_seed(7))
+    ic, cc, gc = inp.float().cuda(), cond.float().cuda(), g.float().cuda()
+    save = torch.empty(cuda_lib.sbi_b200_nsf_vjp_save_bytes(C.byref(est._model(nbuf=3)), R) // 4, device="cuda")
+    seen, _ = _vjp_kernels_seen(lambda: nsf_vjp_raw(est, ic, cc, gc, save), repeat=3)
+    assert seen == ["nsf_vjp_kernel<32, 2, 2, true>"], seen
+    seen, (rc, gpart, ginp, gcond, _) = _vjp_kernels_seen(lambda: nsf_vjp_raw(est, ic, cc, gc, None), repeat=3)
+    print(f"no scratch: VJP kernels seen {seen}")
+    assert seen == ["nsf_vjp_kernel<32, 2, 2, false>"] and rc == 0
+    r32 = _oracle_grads(flow, est, inp, cond, g, torch.float32)
+    r64 = _oracle_grads(flow, est, inp, cond, g, torch.float64)
+    gflat = L.reduce_partials(gpart, gpart.shape[0], est.layout.n_params).cpu().double()
+    assert (gflat[_padding(est)] == 0).all(), "padding entries must receive zero gradient"
+    for name, a, b32, b64 in zip(("param", "input", "cond"), (gflat, ginp.cpu().double(), gcond.cpu().double()),
+                                 r32, r64):
+        _rel(f"vjp recompute {name}-grad", a, b32, b64)
 
 
 def _run_script(script, env_extra, out):
     env = dict(os.environ, **env_extra)
     subprocess.run([sys.executable, "-c", script, ROOT, str(out)], check=True, env=env, timeout=600)
     return torch.load(out)
-
-
-def test_nsf_vjp_recompute_regime_kernel(cuda_lib, tmp_path):
-    """SBI_B200_VJP_SPILL=0 (read once per process -> subprocess): the 32-row recompute kernel runs and its
-    gradients match the fp64 oracle."""
-    script = r'''
-import sys, torch
-sys.path.insert(0, sys.argv[1])
-from tests.helpers import b200_from_oracle, oracle_nsf
-from tests.test_kernel_envelope_gpu import _flow_vjp, _vjp_kernels_seen
-flow, theta, x = oracle_nsf(10, 10, n=500)
-est = b200_from_oracle(flow, theta, x)
-seen = _vjp_kernels_seen(est, theta[:300] * 1.3, x[:300])
-_flow_vjp("vjp recompute", flow, est, theta[:300] * 1.3, x[:300])
-torch.save(seen, sys.argv[2])
-'''
-    seen = _run_script(script, {"SBI_B200_VJP_SPILL": "0"}, tmp_path / "seen.pt")
-    print(f"SBI_B200_VJP_SPILL=0: VJP kernels seen {seen}")
-    assert seen == ["nsf_vjp_kernel<32, 2, 2, false>"]
 
 
 # --------------------------------------------------------------------------------- weight ring

@@ -7,7 +7,7 @@ samples |dx| <= 2e-3, parameter gradients <= 2e-3 relative to the gradient's max
 import pytest
 import torch
 
-from tests.helpers import b200_from_oracle, oracle_nsf
+from tests.helpers import b200_from_oracle, nsf_vjp_raw, oracle_nsf
 
 pytestmark = pytest.mark.gpu
 
@@ -123,33 +123,104 @@ def test_sample_shapes_and_roundtrip(cuda_lib):
     assert torch.isfinite(est.log_prob(s.reshape(14, 3, 10), cond)).all()
 
 
-def test_vjp_activation_spill_equals_recompute(cuda_lib, tmp_path):
-    """The VJP kernel's activation spill (conditioner intermediates written to an L2-resident
-    scratch in the forward sweep, read back in the backward sweep) must give bit-identical
-    gradients to the recompute path (SBI_B200_VJP_SPILL=0, read once per process -> subprocess)."""
-    import os
-    import subprocess
-    import sys
-    script = r'''
-import sys, torch
-sys.path.insert(0, %r)
-from tests.helpers import b200_from_oracle, oracle_nsf
-flow, theta, x = oracle_nsf(10, 10, n=5000)
-est = b200_from_oracle(flow, theta, x)
-inp = theta[:4096].cuda().requires_grad_(True)
-cond = x[:4096].cuda().requires_grad_(True)
-g = torch.Generator().manual_seed(9)
-w = torch.randn(4096, generator=g).cuda()
-lp = est.log_prob(inp, cond)[0]
-(lp * w).sum().backward()
-torch.save({"flat": est.flat.grad.cpu(), "inp": inp.grad.cpu(), "cond": cond.grad.cpu()}, sys.argv[1])
-''' % os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    outs = {}
-    for mode in ("1", "0"):
-        env = dict(os.environ, SBI_B200_VJP_SPILL=mode)
-        f = tmp_path / f"g{mode}.pt"
-        subprocess.run([sys.executable, "-c", script, str(f)], check=True, env=env, timeout=300)
-        outs[mode] = torch.load(f)
-    for k in ("flat", "inp", "cond"):
-        assert torch.equal(outs["1"][k], outs["0"][k]), k
-    assert outs["1"]["flat"].abs().max() > 0
+def _seeded_batch(R, seed=0, D=10, C=10):
+    """An estimator and R of its rows on the GPU, with a seeded upstream gradient per row."""
+    flow, theta, x = oracle_nsf(D, C, n=max(R, 500), seed=seed)
+    est = b200_from_oracle(flow, theta, x)
+    w = torch.randn(R, generator=torch.Generator().manual_seed(9))
+    return est, theta[:R].float().cuda().contiguous(), x[:R].float().cuda().contiguous(), w.cuda()
+
+
+def _scratch(est, R):
+    import ctypes as C
+    from sbi_b200 import _lib as L
+    nbytes = L.load().sbi_b200_nsf_vjp_save_bytes(C.byref(est._model(nbuf=3)), R)
+    assert nbytes > 0 and nbytes % 4 == 0
+    return torch.empty(nbytes // 4, device="cuda")
+
+
+def test_vjp_activation_spill_equals_recompute(cuda_lib):
+    """The VJP kernel's activation spill (conditioner intermediates written to the caller's scratch in the forward
+    sweep, read back in the backward sweep) gives bit-identical partial gradients, input and condition gradients
+    and log-probs to the recompute path (no scratch)."""
+    R = 4096
+    est, inp, cond, w = _seeded_batch(R)
+    spill = nsf_vjp_raw(est, inp, cond, w, _scratch(est, R))
+    recompute = nsf_vjp_raw(est, inp, cond, w, None)
+    assert spill[0] == 0 and recompute[0] == 0
+    for name, a, b in zip(("gpart", "ginput", "gcond", "logp"), spill[1:], recompute[1:]):
+        assert torch.isfinite(a).all() and torch.equal(a, b), name
+    assert spill[1].abs().max() > 0
+
+
+def test_vjp_undersized_scratch_is_rejected(cuda_lib):
+    """A scratch one float smaller than sbi_b200_nsf_vjp_save_bytes: SBI_EINVAL, and nothing is written."""
+    R = 1000
+    est, inp, cond, w = _seeded_batch(R)
+    save = _scratch(est, R)
+    rc, *outs = nsf_vjp_raw(est, inp, cond, w, save[:-1], fill=float("nan"))
+    torch.cuda.synchronize()
+    assert rc == -1                      # SBI_EINVAL
+    for name, t in zip(("gpart", "ginput", "gcond", "logp"), outs):
+        assert torch.isnan(t).all(), name
+    rc, *outs = nsf_vjp_raw(est, inp, cond, w, save, fill=float("nan"))
+    assert rc == 0 and torch.isfinite(outs[1]).all()
+
+
+def _vjp_outputs(est, inp, cond):
+    R = inp.shape[0]
+    return (torch.zeros(est.vjp_parts(R, False), est.layout.n_params, device="cuda"), torch.empty_like(inp),
+            torch.empty_like(cond), torch.empty(R, device="cuda"))
+
+
+def _est_vjp(est, inp, cond, w, outs):
+    from sbi_b200 import _lib as L
+    R = inp.shape[0]
+    gpart, ginp, gcond, logp = outs
+    rows = L.Rows(inp.data_ptr(), cond.data_ptr(), None, R, 0)
+    est.vjp(est._model(nbuf=3), rows, R, w, 0.0, logp, gpart, ginp, gcond)
+
+
+def test_vjp_first_call_captured_in_a_graph_spills(cuda_lib):
+    """A fresh estimator whose first SIMT VJP is captured in a CUDA graph allocates its activation scratch during
+    the capture; the replay equals an eager call bit for bit."""
+    import ctypes as C
+    R = 300
+    est, inp, cond, w = _seeded_batch(R)
+    assert nsf_vjp_raw(est, inp, cond, w, _scratch(est, R))[0] == 0    # kernel attributes set outside the capture
+    assert "vjp_save" not in est._cache
+    captured, eager = _vjp_outputs(est, inp, cond), _vjp_outputs(est, inp, cond)
+    graph, side = torch.cuda.CUDAGraph(), torch.cuda.Stream()
+    side.wait_stream(torch.cuda.current_stream())
+    with torch.cuda.graph(graph, stream=side):
+        _est_vjp(est, inp, cond, w, captured)
+    torch.cuda.current_stream().wait_stream(side)
+    graph.replay()
+    _est_vjp(est, inp, cond, w, eager)
+    torch.cuda.synchronize()
+    nbytes = cuda_lib.sbi_b200_nsf_vjp_save_bytes(C.byref(est._model(nbuf=3)), R)
+    assert est._cache["vjp_save"].numel() * 4 >= nbytes > 0
+    for name, a, b in zip(("gpart", "ginput", "gcond", "logp"), captured, eager):
+        assert torch.isfinite(a).all() and torch.equal(a, b), name
+
+
+def test_vjp_of_two_estimators_on_two_streams(cuda_lib):
+    """Two estimators run their SIMT VJPs at the same time on two streams, each grid small enough that both fit
+    the GPU at once: each gives the gradients it gives alone (every estimator owns its activation scratch)."""
+    R = 32 * (torch.cuda.get_device_properties(0).multi_processor_count // 2 - 4)
+    runs = [_seeded_batch(R, seed=s) for s in (0, 1)]
+    alone = []
+    for est, inp, cond, w in runs:
+        alone.append(_vjp_outputs(est, inp, cond))
+        _est_vjp(est, inp, cond, w, alone[-1])
+    together = [_vjp_outputs(est, inp, cond) for est, inp, cond, w in runs]
+    streams = [torch.cuda.Stream(), torch.cuda.Stream()]
+    for s in streams:
+        s.wait_stream(torch.cuda.current_stream())
+    for s, (est, inp, cond, w), outs in zip(streams, runs, together):
+        with torch.cuda.stream(s):
+            _est_vjp(est, inp, cond, w, outs)
+    torch.cuda.synchronize()
+    for i, (a_outs, t_outs) in enumerate(zip(alone, together)):
+        for name, a, b in zip(("gpart", "ginput", "gcond", "logp"), a_outs, t_outs):
+            assert torch.equal(a, b), (i, name)

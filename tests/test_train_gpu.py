@@ -55,8 +55,9 @@ def test_adam_clip_kernel_matches_torch(cuda_lib):
     assert (outs[0] - outs[1]).abs().max() <= 1e-7
 
 
-def test_fused_train_step_matches_oracle_step(cuda_lib):
-    """One full optimisation step (loss -> backward -> clip -> Adam) against the oracle."""
+def test_fused_train_step_with_scratch_matches_oracle_step(cuda_lib):
+    """One full optimisation step (loss -> backward with an activation scratch -> clip -> Adam) against the
+    oracle."""
     from sbi_b200 import _lib as L
     flow, theta, x = oracle_nsf(10, 10, n=2000)
     est = b200_from_oracle(flow, theta, x)
@@ -70,6 +71,7 @@ def test_fused_train_step_matches_oracle_step(cuda_lib):
     loss_acc = torch.zeros(2, device="cuda")
     n_part = cuda_lib.sbi_b200_nsf_vjp_parts(B)
     gpart = est._gpart(n_part)
+    save = torch.empty(cuda_lib.sbi_b200_nsf_vjp_save_bytes(C.byref(est._model(nbuf=3)), B) // 4, device="cuda")
     th_d, x_d = theta.cuda(), x.cuda()
     for it in range(3):
         idx = torch.randperm(2000)[:B]
@@ -84,7 +86,7 @@ def test_fused_train_step_matches_oracle_step(cuda_lib):
         rows = L.Rows(th_d.data_ptr(), x_d.data_ptr(), idx_d.data_ptr(), B, 0)
         loss_acc.zero_()
         L.check(cuda_lib.sbi_b200_nsf_vjp(C.byref(m), C.byref(rows), None, -1.0 / B, None, L.ptr(gpart), None,
-                                          None, L.ptr(loss_acc), L.stream_ptr()), "vjp")
+                                          None, L.ptr(loss_acc), L.ptr(save), save.numel() * 4, L.stream_ptr()), "vjp")
         L.check(cuda_lib.sbi_b200_reduce_partials(L.ptr(gpart), n_part, P, L.ptr(grad), L.stream_ptr()), "red")
         # unclipped gradient parity (the oracle's was clipped in place: compare direction + norm)
         g = grad.cpu()
@@ -103,8 +105,9 @@ def test_fused_train_step_matches_oracle_step(cuda_lib):
     assert (diff > 5e-5).float().mean() < 0.02
 
 
-def test_train_step_host_entry(cuda_lib):
-    """Host-buffer C-ABI step == device-resident step on the same batch."""
+def test_train_step_host_entry_matches_device_step(cuda_lib):
+    """Host-buffer C-ABI step == device-resident step on the same batch: the workspace has no activation
+    scratch, so the host step recomputes where the device step spills, bit-identically."""
     from sbi_b200 import _lib as L
     flow, theta, x = oracle_nsf(10, 10, n=1000)
     outs = []
@@ -120,8 +123,10 @@ def test_train_step_host_entry(cuda_lib):
         if mode == "device":
             th_d, x_d = theta[:B].cuda(), x[:B].cuda()
             rows = L.Rows(th_d.data_ptr(), x_d.data_ptr(), None, B, 0)
+            save = torch.empty(cuda_lib.sbi_b200_nsf_vjp_save_bytes(C.byref(m), B) // 4, device="cuda")
             L.check(cuda_lib.sbi_b200_nsf_vjp(C.byref(m), C.byref(rows), None, -1.0 / B, None, L.ptr(gpart),
-                                              None, None, L.ptr(loss_acc), L.stream_ptr()), "vjp")
+                                              None, None, L.ptr(loss_acc), L.ptr(save), save.numel() * 4,
+                                              L.stream_ptr()), "vjp")
             L.check(cuda_lib.sbi_b200_reduce_partials(L.ptr(gpart), n_part, P, L.ptr(grad), L.stream_ptr()), "r")
             L.check(cuda_lib.sbi_b200_adam_clip_step(L.ptr(est.flat.data), L.ptr(grad), L.ptr(state), L.ptr(step),
                                                      L.ptr(est.net._mask), P, 5e-4, 0.9, 0.999, 1e-8, 5.0, 1.0,
