@@ -9,7 +9,8 @@
 //   * one CTA = 8 warps (128 rows = 128 lanes of the accumulator store, two threads per row
 //     splitting the columns of every epilogue), two CTAs per SM (256 store columns each); the
 //     warps take turns issuing the TMA copies of the weight stages (tc_common.cuh);
-//   * wgmma.mma_async kind tf32, both warpgroups together (64 rows each), synchronously: the row
+//   * wgmma.mma_async kind tf32, both warpgroups together (64 rows each), synchronously (the training forward
+//     keeps two K-steps in flight, tc_common.cuh): the row
 //     threads put A (activations) into the accumulator store (tc_common.cuh) after splitting every
 //     fp32 value into hi = tf32(x) and lo = x - hi, the warpgroups load their A fragments from it;
 //     B (weights, pre-split hi/lo and pre-arranged in the K-major no-swizzle layout by
@@ -28,8 +29,8 @@
 // alternate between D and G.  The training forward (SAVE) runs one CTA per SM (one tile each), keeps
 // A_hi / A_lo in shared memory (tc_common.cuh) and reserves only [0,64) D | [64,128) G of the store.
 // When a chunk of tiles would leave SMs idle, the training forward runs two CTAs per tile, one per 64-row
-// half (RPC = 64): four threads per row, both warpgroups on the CTA's 64 rows (tc_common.cuh), lanes 0..63
-// of the store columns, and the tile's save slab at lanes [64 r, 64 r + 64) for half r.
+// half (RPC = 64): four threads per row, both warpgroups on the CTA's 64 rows (tc_common.cuh), D | G in shared
+// memory instead of the store, and the tile's save slab at lanes [64 r, 64 r + 64) for half r.
 #include <cuda_runtime.h>
 #include <math.h>
 #include <algorithm>
@@ -47,11 +48,11 @@ namespace tc {
 
 // ---- shared memory plan -------------------------------------------------------------------------
 struct TcSmem {
-  int zs, ctx, lds, ldf, lum, bias, bias_stride, a, ring;   // float offsets
+  int zs, ctx, lds, ldf, lum, bias, bias_stride, a, acc, ring;   // float offsets
   int bar_bytes, total_bytes;
 };
-// a_smem: the training forward (SAVE) also keeps its A operands in shared memory (tc_common.cuh);
-// rpc: rows per CTA (128, or 64 for the training forward's half tiles)
+// a_smem: the training forward (SAVE) also keeps its A operands in shared memory (tc_common.cuh), and on half
+// tiles its accumulator columns; rpc: rows per CTA (128, or 64 for the training forward's half tiles)
 __host__ __device__ inline TcSmem tc_smem_layout(const sbi_nsf_model& m, int stage_cap, bool a_smem, int rpc = kRows) {
   TcSmem L;
   int fl = 0;
@@ -64,6 +65,7 @@ __host__ __device__ inline TcSmem tc_smem_layout(const sbi_nsf_model& m, int sta
   L.bias = fl; fl += m.T * L.bias_stride;
   fl = (fl + 31) & ~31;
   L.a = fl;   fl += a_smem ? a_smem_floats(rpc) : 0;
+  L.acc = fl; fl += a_smem && rpc < kRows ? acc_smem_floats() : 0;
   L.ring = fl; fl += kSlots * stage_cap;
   L.bar_bytes = fl * 4;
   L.total_bytes = L.bar_bytes + kSlots * 8;
@@ -117,11 +119,13 @@ nsf_logprob_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_cons
   const int64_t nunits = (rows.R + kRows - 1) / kRows * UPT;     // CTA tiles of RPC rows
   const TcSave SV = tc_save_layout(m.NB, m.TRmax, m.T);
 
-  // SAVE: A in shared memory, the store holds D | G only
-  constexpr int ncols = SAVE ? kColsDG : kCols;
+  // SAVE: A in shared memory, the store holds D | G only; half tiles keep D | G in shared memory too
+  constexpr int ncols = RPC < kRows ? 0 : SAVE ? kColsDG : kCols;
   constexpr int kD = SAVE ? cDs : cD, kG = SAVE ? cGs : cG;
   float* as = sm + L.a;
-  IssuerT<kSlots, SAVE, RPC> iss = tc_begin<kSlots, SAVE, RPC>(full, sm + L.ring, tc, m.T, nunits, INV, ncols, sa, as);
+  float* accs = sm + L.acc;
+  IssuerT<kSlots, SAVE, RPC> iss =
+      tc_begin<kSlots, SAVE, RPC>(full, sm + L.ring, tc, m.T, nunits, INV, ncols, sa, as, accs);
 
   const float* __restrict__ P = m.d_params;
   float* zs = sm + L.zs;
@@ -208,7 +212,7 @@ nsf_logprob_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_cons
   };
   auto read_acc = [&](int region, float (&d)[NC]) {
 #pragma unroll
-    for (int g = 0; g < NG; ++g) ld4(row, region + cbase + 4 * g, d + 4 * g);
+    for (int g = 0; g < NG; ++g) ld4<RPC>(row, region + cbase + 4 * g, d + 4 * g, accs);
   };
 
   for (int64_t unit = blockIdx.x; unit < nunits; unit += gridDim.x) {
@@ -454,7 +458,7 @@ nsf_logprob_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_cons
           for (int f = 0; f < nf; ++f) {
             if (((f0 + f) & (TPR - 1)) != tq) continue;     // warp-uniform: features go round-robin over the parts
             float q[32];
-            ld_cols<4>(row, kD + 64 * (p & 1) + 32 * f, q);
+            ld_cols<4, RPC>(row, kD + 64 * (p & 1) + 32 * f, q, accs);
             const float* bff = bf + (f0 + f) * 32;
 #pragma unroll
             for (int i = 0; i < 32; ++i) q[i] = (i < 3 * KB - 1) ? q[i] + bff[i] : 0.f;

@@ -13,8 +13,9 @@
 // oracle/nflows_port/nn/nets/resnet.py) in reverse:
 //
 //   * input-gradient chain  dX = dY W  on wgmma kind tf32 (both warpgroups, 64 rows each): A = dY from
-//     the shared-memory A region of tc_common.cuh (written by the row threads, 3xTF32 hi/lo split), the
-//     accumulators in the accumulator store; B = W^T streamed by TMA bulk copies from the
+//     the shared-memory A region of tc_common.cuh (written by the row threads, 3xTF32 hi/lo split), two
+//     K-steps in flight, the accumulators in the accumulator store (in shared memory on half tiles); B = W^T
+//     streamed by TMA bulk copies from the
 //     pre-transposed operand blocks (pack.NsfLayout.tc_bwd_plan) through a 2-slot ring; relu / GLU
 //     masks, the spline backward (rqs.cuh) and the LULinear backward (with its parameter gradients) are
 //     per-thread code on the thread's own row between the MMAs;
@@ -37,8 +38,9 @@
 // in the parameter buffer, and ONE thread sends it to the tile's partial-gradient slab with two TMA bulk
 // copies (a reducing copy for every chunk after the first).
 //
-// Store columns of the backward (128): [0,64) D | [64,128) G.  One A set serves every MMA: each pass's MMAs
-// complete (wgmma wait) before the CTA barrier of Issuer::end(), and the next operands are written after it.
+// Accumulator columns of the backward (128): [0,64) D | [64,128) G, in the store on whole tiles and in shared
+// memory on half tiles.  One A set serves every MMA: each pass's MMAs complete (wgmma wait) before the CTA
+// barrier of Issuer::end(), and the next operands are written after it.
 //
 // Half tiles (RPC = 64, when a chunk of tiles would leave SMs idle): two CTAs per tile, launched as a
 // 2-CTA cluster, CTA r owning tile rows [64 r, 64 r + 64) with four threads per row (the layout of the
@@ -65,10 +67,10 @@ constexpr int kStLd = 65;                       // feature rows per K-slab of a 
 constexpr int kStFloats = 32 * kStLd * 4;       // [128 rows / 4][65][4]
 
 struct BwdSmem {
-  int dz, gr, lum, lus, a, ring;   // float offsets
+  int dz, gr, lum, lus, a, acc, ring;   // float offsets
   int bar_bytes, total_bytes;
 };
-// rpc: rows per CTA (128, or 64 for half tiles)
+// rpc: rows per CTA (128, or 64 for half tiles, which also keep their accumulator columns here)
 __host__ __device__ inline BwdSmem bwd_smem_layout(int stage_cap, int rpc) {
   BwdSmem L;
   int fl = 0;
@@ -79,6 +81,7 @@ __host__ __device__ inline BwdSmem bwd_smem_layout(int stage_cap, int rpc) {
   L.lus = fl; fl += 3 * kLuMax * rpc;            // LULinear backward: v | y | dy, feature-major
   fl = (fl + 31) & ~31;
   L.a = fl;   fl += a_smem_floats(rpc);           // A_hi | A_lo (tc_common.cuh)
+  L.acc = fl; fl += rpc < kRows ? acc_smem_floats() : 0;
   L.ring = fl; fl += kBwdSlots * stage_cap;
   L.bar_bytes = fl * 4;
   L.total_bytes = L.bar_bytes + kBwdSlots * 8;
@@ -330,9 +333,12 @@ nsf_vjp_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_constant
   const int64_t nunits = (rows.R + kRows - 1) / kRows * UPT;     // CTA tiles of RPC rows
   const TcSave SV = tc_save_layout(m.NB, m.TRmax, m.T);
 
+  // whole tiles: D | G in the store; half tiles: in shared memory
+  constexpr int ncols = RPC < kRows ? 0 : kColsDG;
   float* as = sm + L.a;
+  float* accs = sm + L.acc;
   IssuerT<kBwdSlots, true, RPC> iss =
-      tc_begin<kBwdSlots, true, RPC>(full, sm + L.ring, tcb, m.T, nunits, true, kColsDG, sa, as);
+      tc_begin<kBwdSlots, true, RPC>(full, sm + L.ring, tcb, m.T, nunits, true, ncols, sa, as, accs);
   // half tiles: the weight-gradient kernel may start once every CTA of this grid is resident (it waits per unit)
   if constexpr (UPT > 1) asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
   SBI_TL(100);
@@ -380,7 +386,7 @@ nsf_vjp_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_constant
   };
   auto read_acc = [&](int region, float (&d)[NC]) {
 #pragma unroll
-    for (int g = 0; g < NG; ++g) ld4(row, region + cbase + 4 * g, d + 4 * g);
+    for (int g = 0; g < NG; ++g) ld4<RPC>(row, region + cbase + 4 * g, d + 4 * g, accs);
   };
   // the thread's dY columns of a [128][64] dY array (none from kDyCols on: they hold the ready counters)
   auto save_dy = [&](float* q, int srow, const float (&d)[NC]) {
@@ -751,8 +757,8 @@ nsf_vjp_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_constant
         SBI_TL(1000 * (li + 1) + 60);
         if (tq == 0) {
           float d[16];
-          ld8(row, cDs, d);
-          ld8(row, cDs + 8, d + 8);
+          ld8<RPC>(row, cDs, d, accs);
+          ld8<RPC>(row, cDs + 8, d + 8, accs);
 #pragma unroll
           for (int j = 0; j < 16; ++j)
             if (j < v.n_id) dzs[__ldg(v.idf + j) * RPC + row] += d[j];
@@ -764,7 +770,7 @@ nsf_vjp_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_constant
   }
   SBI_TL(9001);
 
-  tc_end(kColsDG, sa);
+  tc_end(ncols, sa);
 }
 
 }  // namespace tc

@@ -38,12 +38,18 @@ constexpr int cAhi = 0, cAlo = 64, cD = 128, cG = 192;
 // kernels that keep A in shared memory (the training pair, below) reserve the accumulator columns only
 constexpr int kColsDG = 128;
 constexpr int cDs = 0, cGs = 64;
+// On half tiles (RPC = 64, below) the training pair keeps those columns in shared memory instead of the
+// store: kColsDG columns of kAccLd floats, column-major like the store.  64 lanes + 4 of padding: in the
+// fragment write-back the 4 threads of a quad write columns 2t apart, which a stride of 64 would put in
+// one bank.
+constexpr int kAccLd = 64 + 4;
+__host__ __device__ constexpr int acc_smem_floats() { return kColsDG * kAccLd; }
 
 // ---- accumulator store --------------------------------------------------------------------------
 // The kernels keep their MMA accumulators, and all but the training pair (A in shared memory, below) their
 // A operands, in columns of 128 lanes, lane = tile row.
 // Hopper keeps wgmma accumulators in registers, and an SM's shared memory is taken by the weight ring
-// and the staging buffers, so the columns live in global memory: kStoreSlots slabs of kStoreCols
+// and the staging buffers (except on the training pair's half tiles, above), so the columns live in global memory: kStoreSlots slabs of kStoreCols
 // columns x 128 lanes (lane-contiguous, so the 32 threads of a warp touch one 128-byte line per column;
 // 34.6 MB per device, defined once in nsf_tc.cu and mostly L2-resident while a kernel runs), handed out
 // in 64-column units through one mask per slab.  A CTA picks the slab of the SM it starts on (for
@@ -120,20 +126,25 @@ __device__ __forceinline__ void st8(uint32_t row, uint32_t col, const float (&v)
 #pragma unroll
   for (int i = 0; i < 8; ++i) p[i * kStoreLanes] = v[i];
 }
-__device__ __forceinline__ void ld8(uint32_t row, uint32_t col, float* v) {
-  const float* p = store_at(row, col);
+// accumulator reads of an RPC-row CTA: from the store, or on half tiles from the shared-memory columns `accs`
+template <int RPC = kRows>
+__device__ __forceinline__ void ld8(uint32_t row, uint32_t col, float* v, const float* accs = nullptr) {
+  constexpr int ld = RPC < kRows ? kAccLd : kStoreLanes;
+  const float* p = RPC < kRows ? accs + col * kAccLd + row : store_at(row, col);
 #pragma unroll
-  for (int i = 0; i < 8; ++i) v[i] = p[i * kStoreLanes];
+  for (int i = 0; i < 8; ++i) v[i] = p[i * ld];
 }
 __device__ __forceinline__ void st4(uint32_t row, uint32_t col, const float (&v)[4]) {
   float* p = store_at(row, col);
 #pragma unroll
   for (int i = 0; i < 4; ++i) p[i * kStoreLanes] = v[i];
 }
-__device__ __forceinline__ void ld4(uint32_t row, uint32_t col, float* v) {
-  const float* p = store_at(row, col);
+template <int RPC = kRows>
+__device__ __forceinline__ void ld4(uint32_t row, uint32_t col, float* v, const float* accs = nullptr) {
+  constexpr int ld = RPC < kRows ? kAccLd : kStoreLanes;
+  const float* p = RPC < kRows ? accs + col * kAccLd + row : store_at(row, col);
 #pragma unroll
-  for (int i = 0; i < 4; ++i) v[i] = p[i * kStoreLanes];
+  for (int i = 0; i < 4; ++i) v[i] = p[i * ld];
 }
 
 // ---- A operands in shared memory ------------------------------------------------------------------
@@ -148,48 +159,84 @@ __device__ __forceinline__ void ld4(uint32_t row, uint32_t col, float* v) {
 // float4, so the 32 rows of a warp cover 512 contiguous bytes.
 __host__ __device__ constexpr int a_smem_floats(int rpc) { return 2 * 64 * rpc; }   // A_hi | A_lo
 
-// ---- the MMAs: both warpgroups of the CTA, synchronously ------------------------------------------
+// ---- the MMAs: both warpgroups of the CTA, complete on return ------------------------------------
 // Accumulator fragment of wgmma m64nNk8 (f32): warp w of the warpgroup holds rows 16w + g and
 // 16w + g + 8 (g = lane / 4), columns 8j + 2t and 8j + 2t + 1 (t = lane % 4) in d[4j .. 4j+3].
 //
-// D[store, M = RPC] (+)= A * B[smem]^T over nk K-steps, 3xTF32 (A_hi B_hi + A_lo B_hi + A_hi B_lo):
+// D[M = RPC] (+)= A * B[smem]^T over nk K-steps, 3xTF32 (A_hi B_hi + A_lo B_hi + A_hi B_lo):
 // RPC = 128: warpgroup wg computes rows 64 wg .. 64 wg + 63; RPC = 64: both warpgroups compute the CTA's
 // 64 rows, each its own N columns (the caller offsets dcol and the B descriptors).  ASMEM = false: ah / al
 // are the A_hi / A_lo store columns of the first K-step and the fragments come straight from the store;
 // ASMEM = true: ah / al are the shared-memory descriptors of the warpgroup's first K-step.  Same products in
-// the same order.
+// the same order.  D is in the store, or on half tiles (RPC = 64) in the shared-memory columns `accs`.
+// ASMEM keeps the next K-step's MMAs in flight while the running sum takes the current one.
 template <int N, bool ASMEM, int RPC = kRows>
 __device__ __forceinline__ void mma_rows_n(uint32_t dcol, uint64_t ah, uint64_t al, uint64_t dh,
-                                           uint64_t dl, uint64_t dstep, int nk, uint32_t acc) {
+                                           uint64_t dl, uint64_t dstep, int nk, uint32_t acc, float* accs) {
   constexpr uint64_t kAStep = (RPC * 32u) >> 4;       // descriptor start-address advance per K-step
+  constexpr bool kDSmem = RPC < kRows;
+  constexpr uint32_t kLd = kDSmem ? kAccLd : kStoreLanes;
   const int lane = threadIdx.x & 31, g = lane >> 2, t = lane & 3;
   const uint32_t r0 = (RPC == kRows ? (threadIdx.x >> 7) * 64 : 0) + ((threadIdx.x >> 5) & 3) * 16 + g;
-  const uint32_t c0 = s_store_col;
+  const uint32_t c0 = kDSmem ? 0u : s_store_col;
   dcol += c0;
   const uint32_t ahcol = (uint32_t)ah + c0, alcol = (uint32_t)al + c0;
-  float* slab = s_store;
+  float* slab = kDSmem ? accs : s_store;
   float d[N / 2];
 #pragma unroll
   for (int j = 0; j < N / 8; ++j) {
     const uint32_t c = dcol + 8 * j + 2 * t;
-    d[4 * j + 0] = acc ? slab[c * kStoreLanes + r0] : 0.f;
-    d[4 * j + 1] = acc ? slab[(c + 1) * kStoreLanes + r0] : 0.f;
-    d[4 * j + 2] = acc ? slab[c * kStoreLanes + r0 + 8] : 0.f;
-    d[4 * j + 3] = acc ? slab[(c + 1) * kStoreLanes + r0 + 8] : 0.f;
+    d[4 * j + 0] = acc ? slab[c * kLd + r0] : 0.f;
+    d[4 * j + 1] = acc ? slab[(c + 1) * kLd + r0] : 0.f;
+    d[4 * j + 2] = acc ? slab[c * kLd + r0 + 8] : 0.f;
+    d[4 * j + 3] = acc ? slab[(c + 1) * kLd + r0 + 8] : 0.f;
   }
-  for (int kk = 0; kk < nk; ++kk) {
-    // each K-step into a fresh accumulator, correction terms first; the running sum is then carried
-    // with round-to-nearest adds (the tensor core's own fp32 accumulation truncates)
-    float p[N / 2];
-#pragma unroll
-    for (int i = 0; i < N / 2; ++i) p[i] = 0.f;
-    if constexpr (ASMEM) {
+  if constexpr (ASMEM) {
+    // each K-step into a fresh accumulator (two alternate), correction terms first; K-step k + 1 is issued
+    // before the running sum takes K-step k, with the round-to-nearest adds of the synchronous loop below in
+    // the same order
+    float p0[N / 2], p1[N / 2];
+    auto issue = [&](float (&p)[N / 2]) {
       wgmma_fence();
       wgmma_ss<N>(p, al, dh, 0u);
       wgmma_ss<N>(p, ah, dl, 1u);
       wgmma_ss<N>(p, ah, dh, 1u);
+      wgmma_commit();
       ah += kAStep; al += kAStep;
+      dh += dstep; dl += dstep;
+    };
+    auto take = [&](float (&p)[N / 2]) {
+      wgmma_fence_operand(p);
+#pragma unroll
+      for (int i = 0; i < N / 2; ++i) d[i] += p[i];
+    };
+    issue(p0);
+    int kk = 1;
+    for (; kk + 1 < nk; kk += 2) {
+      issue(p1);
+      wgmma_wait<1>();
+      take(p0);
+      issue(p0);
+      wgmma_wait<1>();
+      take(p1);
+    }
+    if (kk < nk) {
+      issue(p1);
+      wgmma_wait<1>();
+      take(p0);
+      wgmma_wait<0>();
+      take(p1);
     } else {
+      wgmma_wait<0>();
+      take(p0);
+    }
+  } else {
+    for (int kk = 0; kk < nk; ++kk) {
+      // each K-step into a fresh accumulator, correction terms first; the running sum is then carried
+      // with round-to-nearest adds (the tensor core's own fp32 accumulation truncates)
+      float p[N / 2];
+#pragma unroll
+      for (int i = 0; i < N / 2; ++i) p[i] = 0.f;
       uint32_t fh[4], fl[4];
       const uint32_t ch = ahcol + 8 * kk + t, cl = alcol + 8 * kk + t;
       fh[0] = __float_as_uint(slab[ch * kStoreLanes + r0]);
@@ -204,34 +251,34 @@ __device__ __forceinline__ void mma_rows_n(uint32_t dcol, uint64_t ah, uint64_t 
       wgmma_rs<N>(p, fl, dh, 0u);
       wgmma_rs<N>(p, fh, dl, 1u);
       wgmma_rs<N>(p, fh, dh, 1u);
-    }
-    wgmma_commit();
-    wgmma_wait_all();
+      wgmma_commit();
+      wgmma_wait_all();
 #pragma unroll
-    for (int i = 0; i < N / 2; ++i) d[i] += p[i];
-    dh += dstep; dl += dstep;
+      for (int i = 0; i < N / 2; ++i) d[i] += p[i];
+      dh += dstep; dl += dstep;
+    }
   }
 #pragma unroll
   for (int j = 0; j < N / 8; ++j) {
     const uint32_t c = dcol + 8 * j + 2 * t;
-    slab[c * kStoreLanes + r0] = d[4 * j + 0];
-    slab[(c + 1) * kStoreLanes + r0] = d[4 * j + 1];
-    slab[c * kStoreLanes + r0 + 8] = d[4 * j + 2];
-    slab[(c + 1) * kStoreLanes + r0 + 8] = d[4 * j + 3];
+    slab[c * kLd + r0] = d[4 * j + 0];
+    slab[(c + 1) * kLd + r0] = d[4 * j + 1];
+    slab[c * kLd + r0 + 8] = d[4 * j + 2];
+    slab[(c + 1) * kLd + r0 + 8] = d[4 * j + 3];
   }
 }
 template <bool ASMEM, int RPC = kRows>
 __device__ __forceinline__ void mma_rows(int N, uint32_t dcol, uint64_t ah, uint64_t al, uint64_t dh,
-                                         uint64_t dl, uint64_t dstep, int nk, uint32_t acc) {
+                                         uint64_t dl, uint64_t dstep, int nk, uint32_t acc, float* accs) {
   switch (N) {
-    case 8: mma_rows_n<8, ASMEM, RPC>(dcol, ah, al, dh, dl, dstep, nk, acc); break;
-    case 16: mma_rows_n<16, ASMEM, RPC>(dcol, ah, al, dh, dl, dstep, nk, acc); break;
-    case 24: mma_rows_n<24, ASMEM, RPC>(dcol, ah, al, dh, dl, dstep, nk, acc); break;
-    case 32: mma_rows_n<32, ASMEM, RPC>(dcol, ah, al, dh, dl, dstep, nk, acc); break;
-    case 40: mma_rows_n<40, ASMEM, RPC>(dcol, ah, al, dh, dl, dstep, nk, acc); break;
-    case 48: mma_rows_n<48, ASMEM, RPC>(dcol, ah, al, dh, dl, dstep, nk, acc); break;
-    case 56: mma_rows_n<56, ASMEM, RPC>(dcol, ah, al, dh, dl, dstep, nk, acc); break;
-    case 64: mma_rows_n<64, ASMEM, RPC>(dcol, ah, al, dh, dl, dstep, nk, acc); break;
+    case 8: mma_rows_n<8, ASMEM, RPC>(dcol, ah, al, dh, dl, dstep, nk, acc, accs); break;
+    case 16: mma_rows_n<16, ASMEM, RPC>(dcol, ah, al, dh, dl, dstep, nk, acc, accs); break;
+    case 24: mma_rows_n<24, ASMEM, RPC>(dcol, ah, al, dh, dl, dstep, nk, acc, accs); break;
+    case 32: mma_rows_n<32, ASMEM, RPC>(dcol, ah, al, dh, dl, dstep, nk, acc, accs); break;
+    case 40: mma_rows_n<40, ASMEM, RPC>(dcol, ah, al, dh, dl, dstep, nk, acc, accs); break;
+    case 48: mma_rows_n<48, ASMEM, RPC>(dcol, ah, al, dh, dl, dstep, nk, acc, accs); break;
+    case 56: mma_rows_n<56, ASMEM, RPC>(dcol, ah, al, dh, dl, dstep, nk, acc, accs); break;
+    case 64: mma_rows_n<64, ASMEM, RPC>(dcol, ah, al, dh, dl, dstep, nk, acc, accs); break;
     default: __trap();      // operand blocks are planned with N in {8, ..., 64}
   }
 }
@@ -258,10 +305,10 @@ __device__ __forceinline__ void mma_ss64_n(float (&d)[NH / 2], uint64_t da, uint
     da += dstep; db += dstep;
   }
 }
-template <int NCHUNK>
-__device__ __forceinline__ void ld_cols(uint32_t row, uint32_t col, float* v) {
+template <int NCHUNK, int RPC = kRows>
+__device__ __forceinline__ void ld_cols(uint32_t row, uint32_t col, float* v, const float* accs = nullptr) {
 #pragma unroll
-  for (int c = 0; c < NCHUNK; ++c) ld8(row, col + 8 * c, v + 8 * c);
+  for (int c = 0; c < NCHUNK; ++c) ld8<RPC>(row, col + 8 * c, v + 8 * c, accs);
 }
 
 // hi = x rounded to tf32 (10 explicit mantissa bits, round half away in the integer domain),
@@ -373,12 +420,14 @@ static int pack_weights(const float* params, const sbi_nsf_tc* tc, cudaStream_t 
 // once end() returns.  The weight stream rotates between the warps (stage k is fetched by the
 // elected lane of warp (k + 4) % 8).  Stage k lives in ring slot k % NSLOT.  A stage is fetched
 // (TMA bulk copy, completion on full[slot]) by the end() of the stage that used its slot NSLOT stages
-// earlier.  ASMEM: A comes from the shared-memory A region of an RPC-row CTA at `abase`, else from the store.
+// earlier.  ASMEM: A comes from the shared-memory A region of an RPC-row CTA at `abase`, else from the store;
+// half tiles (RPC = 64) keep D | G in the shared-memory columns `accs`.
 template <int NSLOT, bool ASMEM = false, int RPC = kRows>
 struct IssuerT {
   bool leader;          // the elected lane of this warp
   int warp;             // this warp; stage k is fetched by warp (k+4) % 8
   uint32_t abase;       // ASMEM: shared address of the A region
+  float* accs;          // half tiles: the shared-memory accumulator columns (acc_smem_floats() floats)
   float* ring;
   uint64_t* full;
   const float* tcw;
@@ -425,7 +474,7 @@ struct IssuerT {
       const uint32_t ah = abase + (uint32_t)a0 * (kRows * 4u) + (threadIdx.x >> 7) * 1024u;
       if (nk > 0)
         mma_rows<true>(N, dcol, make_bdesc(ah, kRows * 16u, 128u),
-                       make_bdesc(ah + a_smem_floats(kRows) * 2u, kRows * 16u, 128u), dh, dl, dstep, nk, acc);
+                       make_bdesc(ah + a_smem_floats(kRows) * 2u, kRows * 16u, 128u), dh, dl, dstep, nk, acc, accs);
     } else if constexpr (ASMEM) {
       // both warpgroups on the CTA's rows from column a0; warpgroup wg takes result columns
       // [wg N/2, (wg + 1) N/2), whose B rows start wg N/16 8-row groups (128 B each) in
@@ -435,13 +484,13 @@ struct IssuerT {
       if (nk > 0)
         mma_rows<true, RPC>((int)nh, dcol + wg * nh, make_bdesc(ah, RPC * 16u, 128u),
                             make_bdesc(ah + a_smem_floats(RPC) * 2u, RPC * 16u, 128u), dh + boff, dl + boff, dstep,
-                            nk, acc);
+                            nk, acc, accs);
     } else {
-      if (nk > 0) mma_rows<false>(N, dcol, cAhi + a0, cAlo + a0, dh, dl, dstep, nk, acc);
+      if (nk > 0) mma_rows<false>(N, dcol, cAhi + a0, cAlo + a0, dh, dl, dstep, nk, acc, nullptr);
     }
     if (nk > 0) acc = 1u;
   }
-  // close the stage: after the CTA barrier its accumulators are in the store and its ring slot is free
+  // close the stage: after the CTA barrier its accumulators are in place and its ring slot is free
   __device__ __forceinline__ void end() {
     group_sync();
     ++it;
@@ -451,19 +500,19 @@ struct IssuerT {
 using Issuer = IssuerT<kSlots>;
 
 // Kernel prologue, all threads: thread 0 initialises the ring's mbarriers full[0 .. NSLOT) (and any
-// other mbarrier the kernel initialised before the call), warp 0 reserves `ncols` store columns, and
-// after the CTA barrier the issuer starts fetching the first NSLOT stages of the CTA's first tile.
-// `ntiles` counts the CTA tiles of RPC rows.  ASMEM: `as` is the shared-memory A region
-// (a_smem_floats(RPC) floats, 16-byte aligned).
+// other mbarrier the kernel initialised before the call), warp 0 reserves `ncols` store columns (none on
+// half tiles), and after the CTA barrier the issuer starts fetching the first NSLOT stages of the CTA's
+// first tile.  `ntiles` counts the CTA tiles of RPC rows.  ASMEM: `as` is the shared-memory A region
+// (a_smem_floats(RPC) floats, 16-byte aligned); half tiles: `accs` the shared-memory accumulator columns.
 template <int NSLOT, bool ASMEM = false, int RPC = kRows>
 __device__ __forceinline__ IssuerT<NSLOT, ASMEM, RPC> tc_begin(uint64_t* full, float* ring, const sbi_nsf_tc& tc, int T,
                                                           int64_t ntiles, bool reverse, int ncols, const StoreArgs& sa,
-                                                          float* as = nullptr) {
+                                                          float* as = nullptr, float* accs = nullptr) {
   if (threadIdx.x == 0) {
     for (int s = 0; s < NSLOT; ++s) mbar_init(&full[s], 1);
     fence_barrier_init();
   }
-  if (threadIdx.x < 32) store_alloc(ncols, sa);
+  if (ncols > 0 && threadIdx.x < 32) store_alloc(ncols, sa);
   __syncthreads();
   IssuerT<NSLOT, ASMEM, RPC> iss;
   uint32_t el = 0;
@@ -471,6 +520,7 @@ __device__ __forceinline__ IssuerT<NSLOT, ASMEM, RPC> tc_begin(uint64_t* full, f
   iss.leader = el != 0;
   iss.warp = threadIdx.x >> 5;
   iss.abase = ASMEM ? smem_u32(as) : 0u;
+  iss.accs = accs;
   iss.ring = ring; iss.full = full;
   iss.tcw = tc.d_tcw; iss.tab = tc.d_tab; iss.cap = tc.stage_cap; iss.T = T;
   iss.it = 0; iss.fetched = 0;
@@ -483,7 +533,7 @@ __device__ __forceinline__ IssuerT<NSLOT, ASMEM, RPC> tc_begin(uint64_t* full, f
 // Kernel epilogue, all threads: release the store columns once every thread is done with them.
 __device__ __forceinline__ void tc_end(int ncols, const StoreArgs& sa) {
   group_sync();
-  if (threadIdx.x < 32) store_dealloc(ncols, sa);
+  if (ncols > 0 && threadIdx.x < 32) store_dealloc(ncols, sa);
 }
 
 // generic-proxy shared-memory writes -> visible to the async proxy (wgmma operand reads)

@@ -142,6 +142,16 @@ template <> __device__ __forceinline__ void wgmma_ss<64>(float* d, uint64_t a, u
 __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+// all but the newest `N` committed groups are complete
+template <int N> __device__ __forceinline__ void wgmma_wait() {
+  asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
+}
+// pin the accumulator registers `d` to this point of the instruction stream (after a wait, before their reads),
+// so that the compiler cannot move their reads above the wait
+template <int K> __device__ __forceinline__ void wgmma_fence_operand(float (&d)[K]) {
+#pragma unroll
+  for (int i = 0; i < K; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
 
 }  // namespace tc
 }  // namespace sbi
