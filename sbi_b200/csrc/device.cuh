@@ -71,41 +71,30 @@ inline int set_smem(const void* kernel, int bytes) {
   return 0;
 }
 
-// Grid of a launch: `ctas` CTAs along x, in clusters of `cluster` CTAs (1: no clusters).  `early`: programmatic
-// stream serialization -- the grid may start once every CTA of the kernel before it in the stream has run
-// griddepcontrol.launch_dependents, so it must itself wait for whatever of that kernel's output it reads.
+// Grid of a launch: `ctas` CTAs along x.  `early`: programmatic stream serialization -- the grid may start once
+// every CTA of the kernel before it in the stream has run griddepcontrol.launch_dependents, so it must itself
+// wait for whatever of that kernel's output it reads.
 struct Grid {
-  int ctas, cluster;
+  int ctas;
   bool early;
-  Grid(int n, int c = 1, bool e = false) : ctas(n), cluster(c), early(e) {}
+  Grid(int n, bool e = false) : ctas(n), early(e) {}
 };
 
 // Opt `kernel` into `smem_bytes` of dynamic shared memory, launch it and return the launch status.
 template <class... P, class... A>
 int launch(void (*kernel)(P...), Grid grid, int threads, int smem_bytes, cudaStream_t s, A&&... args) {
   if (int e = set_smem(reinterpret_cast<const void*>(kernel), smem_bytes)) return e;
-  if (grid.cluster > 1 || grid.early) {
-    cudaLaunchAttribute at[2];
-    int n = 0;
-    if (grid.cluster > 1) {
-      at[n].id = cudaLaunchAttributeClusterDimension;
-      at[n].val.clusterDim.x = (unsigned)grid.cluster;
-      at[n].val.clusterDim.y = 1;
-      at[n].val.clusterDim.z = 1;
-      ++n;
-    }
-    if (grid.early) {
-      at[n].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-      at[n].val.programmaticStreamSerializationAllowed = 1;
-      ++n;
-    }
+  if (grid.early) {
+    cudaLaunchAttribute at[1];
+    at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    at[0].val.programmaticStreamSerializationAllowed = 1;
     cudaLaunchConfig_t cfg = {};
     cfg.gridDim = dim3((unsigned)grid.ctas);
     cfg.blockDim = dim3((unsigned)threads);
     cfg.dynamicSmemBytes = (size_t)smem_bytes;
     cfg.stream = s;
     cfg.attrs = at;
-    cfg.numAttrs = n;
+    cfg.numAttrs = 1;
     cudaLaunchKernelEx(&cfg, kernel, std::forward<A>(args)...);
   } else {
     kernel<<<grid.ctas, threads, smem_bytes, s>>>(std::forward<A>(args)...);

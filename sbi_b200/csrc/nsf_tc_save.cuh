@@ -19,6 +19,11 @@
 //            in columns [kDyCols, 64) of dh, which hold no gradient: the backward sweep adds 1 per CTA of
 //            the tile once the unit's dY is written, the weight-gradient kernel waits for the unit's count
 //            and the forward sweep zeroes the counters of its tile
+//     dz of layer l-1 (l > 0): the gradient at layer l-1's LULinear output, [128][16], in columns [0, 16) of
+//            THIS layer's prm (prm has >= 32 columns).  The backward sweep writes it at the end of layer l,
+//            after layer l's spline backward -- the only reader of prm_l after the forward sweep; the
+//            weight-gradient kernel never reads prm -- and the weight-gradient kernel's LULinear unit of
+//            layer l-1 reads it.  The top layer's dz is -g z_T, which that unit computes from zt.
 //   then per tile:  zt = base-space point z_T [128][16],  lp = log q [128]
 //
 // Every array of a slab is stored as float4 groups with the ROW index fastest: group g of row r sits at
@@ -38,8 +43,9 @@ namespace tc {
 
 // dY columns that are written and read (hidden width <= 56); columns [kDyCols, 64) of the dY arrays are free
 constexpr int kDyCols = 56;
-// a layer's counters (<= 8 final-layer passes of <= 16 features, 3 per block, the initial linear) fit them
-static_assert(8 + 3 * SBI_NSF_MAX_BLOCKS + 1 <= (64 - kDyCols) * 128, "ready counters");
+// a layer's counters (<= 8 final-layer passes of <= 16 features, 3 per block, the initial linear, the LULinear)
+// fit them
+static_assert(8 + 3 * SBI_NSF_MAX_BLOCKS + 2 <= (64 - kDyCols) * 128, "ready counters");
 
 struct TcSave {
   int NB;
@@ -57,8 +63,11 @@ struct TcSave {
   __host__ __device__ int dy_blk(int b, int k) const { return dy + (64 * npm + 192 * b + 64 * k) * 128; }
   __host__ __device__ int dy_init() const { return dy + (64 * npm + 192 * NB) * 128; }
   // weight-gradient units of a layer: the final-layer passes, three linears per residual block (GLU context,
-  // W2, W1), the initial linear
-  __host__ __device__ int units() const { return npm + 3 * NB + 1; }
+  // W2, W1), the initial linear, the LULinear parameters
+  __host__ __device__ int units() const { return npm + 3 * NB + 2; }
+  __host__ __device__ int lu_unit() const { return npm + 3 * NB + 1; }
+  // dz at the LULinear output of layer l - 1, in layer l's slab (l > 0)
+  __host__ __device__ int dz_below() const { return prm; }
   // ready counters of the layer, units() of the (64 - kDyCols) * 128 free words
   __host__ __device__ int ready() const { return dy_init() + kDyCols * 128; }
 };

@@ -17,10 +17,11 @@
 //     K-steps in flight, the accumulators in the accumulator store (in shared memory on half tiles); B = W^T
 //     streamed by TMA bulk copies from the
 //     pre-transposed operand blocks (pack.NsfLayout.tc_bwd_plan) through a 2-slot ring; relu / GLU
-//     masks, the spline backward (rqs.cuh) and the LULinear backward (with its parameter gradients) are
-//     per-thread code on the thread's own row between the MMAs;
-//   * the output gradient dY of every linear goes to the dY region of the activation scratch, where the
-//     weight-gradient kernel picks it up;
+//     masks, the spline backward (rqs.cuh) and the LULinear input gradient are per-thread code on the
+//     thread's own row between the MMAs;
+//   * the output gradient dY of every linear goes to the dY region of the activation scratch, and the gradient
+//     dz at every LULinear output below the top layer to the prm region of the layer above (nsf_tc_save.cuh),
+//     where the weight-gradient kernel picks them up;
 //   * COND instantiation only: the condition gradient d(sum g log q)/d ctx in raw condition space, accumulated
 //     per row over the T layers from the context columns of the initial layer (dh W0[:, :C]) and the GLU
 //     context layer of every residual block (dG Wc).  dh / dG of the whole row are read back from the dY region
@@ -36,17 +37,17 @@
 // rows averages the operand rounding; the two warpgroups split N); a ones row appended to X^T yields the bias
 // gradient in the same MMA.  The accumulators are written into a shared-memory image laid out like the block
 // in the parameter buffer, and ONE thread sends it to the tile's partial-gradient slab with two TMA bulk
-// copies (a reducing copy for every chunk after the first).
+// copies (a reducing copy for every chunk after the first).  One more CTA per (tile, layer) takes the LULinear
+// parameter gradients: dot products over the tile's 128 rows of dz, y = U v, dy = dz + L^T dz and v, on the
+// CUDA cores (D^2 + D sums of 128 terms).
 //
 // Accumulator columns of the backward (128): [0,64) D | [64,128) G, in the store on whole tiles and in shared
 // memory on half tiles.  One A set serves every MMA: each pass's MMAs complete (wgmma wait) before the CTA
 // barrier of Issuer::end(), and the next operands are written after it.
 //
-// Half tiles (RPC = 64, when a chunk of tiles would leave SMs idle): two CTAs per tile, launched as a
-// 2-CTA cluster, CTA r owning tile rows [64 r, 64 r + 64) with four threads per row (the layout of the
-// forward's half tiles, nsf_tc.cu).  Everything is per row except the LULinear parameter gradients, which
-// sum over the tile's 128 rows: after a cluster barrier CTA 0 reads CTA 1's rows through distributed shared
-// memory and runs the same reductions in the same order.
+// Half tiles (RPC = 64, when a chunk of tiles would leave SMs idle): two CTAs per tile, CTA r owning tile rows
+// [64 r, 64 r + 64) with four threads per row (the layout of the forward's half tiles, nsf_tc.cu).  Everything
+// the backward computes is per row, so the two CTAs never talk to each other.
 #include <cuda_runtime.h>
 #include <math.h>
 #include <algorithm>
@@ -67,7 +68,7 @@ constexpr int kStLd = 65;                       // feature rows per K-slab of a 
 constexpr int kStFloats = 32 * kStLd * 4;       // [128 rows / 4][65][4]
 
 struct BwdSmem {
-  int dz, gr, lum, lus, a, acc, ring;   // float offsets
+  int dz, gr, lum, a, acc, ring;   // float offsets
   int bar_bytes, total_bytes;
 };
 // rpc: rows per CTA (128, or 64 for half tiles, which also keep their accumulator columns here)
@@ -77,8 +78,6 @@ __host__ __device__ inline BwdSmem bwd_smem_layout(int stage_cap, int rpc) {
   L.dz = fl;  fl += 16 * rpc;
   L.gr = fl;  fl += rpc;
   L.lum = fl; fl += 2 * kLuMax * kLuMax + 2 * kLuMax;
-  fl = (fl + 31) & ~31;
-  L.lus = fl; fl += 3 * kLuMax * rpc;            // LULinear backward: v | y | dy, feature-major
   fl = (fl + 31) & ~31;
   L.a = fl;   fl += a_smem_floats(rpc);           // A_hi | A_lo (tc_common.cuh)
   L.acc = fl; fl += rpc < kRows ? acc_smem_floats() : 0;
@@ -146,11 +145,12 @@ __device__ __forceinline__ unsigned ld_acquire_gpu(const unsigned* p) {
 // On half tiles (the chunk leaves SMs idle) it is launched right behind the backward sweep with programmatic
 // stream serialization: it may start once every backward CTA has run griddepcontrol.launch_dependents, and
 // each CTA waits for its own unit's dY instead of for the whole backward grid.  Its CTAs are then numbered in
-// the order the backward produces their dY: layer T-1 .. 0, then the unit in write order (final-layer passes,
-// blocks NB-1 .. 0 with GLU context, W2, W1, the initial linear), then the tile, so the CTAs dispatched first
-// are the first to find their unit ready.  On whole tiles every SM runs a backward CTA, so it is an ordinary
-// launch after the backward (`upt` = 0: no wait) with the CTAs tile-major.  Every unit writes a disjoint
-// block of its tile's partial-gradient slab, so neither order changes a value.
+// the order the backward produces their dY: layer T-1 .. 0, then the unit in write order (the LULinear, whose dz
+// the backward publishes after the layer's LU section, final-layer passes, blocks NB-1 .. 0 with GLU context,
+// W2, W1, the initial linear), then the tile, so the CTAs dispatched first are the first to find their unit
+// ready.  On whole tiles every SM runs a backward CTA, so it is an ordinary launch after the backward (`upt` = 0:
+// no wait) with the CTAs tile-major.  Every unit writes a disjoint block of its tile's partial-gradient slab, so
+// neither order changes a value.
 // The wait cannot deadlock:
 //   * the grid launches only after every backward CTA has run launch_dependents, so the whole backward
 //     grid is resident (one CTA per SM: the chunk never has more backward CTAs than SMs);
@@ -162,10 +162,12 @@ __device__ __forceinline__ unsigned ld_acquire_gpu(const unsigned* p) {
 // graph replays included -- because the forward sweep of the same chunk zeroes them, and stream order puts
 // that forward after the previous chunk's (or step's) weight-gradient kernel and before this backward.
 // `upt`: the count at which a unit is ready (2, one per CTA of the tile, on half tiles; 0 on whole tiles).
+// `gout` / `g_const`: the row weights of the chunk's rows, as given to the backward sweep.
 template <int H>
 __global__ void __launch_bounds__(kThreads, 2)
 nsf_dw_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_constant__ sbi_rows rows,
-                 const float* __restrict__ save, float* __restrict__ gpart, int accum, unsigned upt) {
+                 const float* __restrict__ save, float* __restrict__ gpart, int accum, unsigned upt,
+                 const float* __restrict__ gout, float g_const) {
   constexpr int HP8 = (H + 7) & ~7;
   constexpr int NC = HP8 / 2;
   static_assert(HP8 <= kDyCols, "the dY columns from kDyCols on hold the ready counters");
@@ -182,10 +184,11 @@ nsf_dw_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_constant_
   int l, u;
   if (upt > 0) {
     const int ntiles = gridDim.x / (nu * m.T);
-    const int j = (blockIdx.x / ntiles) % nu;  // unit in write order
+    const int j = (blockIdx.x / ntiles) % nu - 1;  // unit in write order, the LULinear (-1) first
     tile = blockIdx.x % ntiles;
     l = m.T - 1 - (int)(blockIdx.x / (ntiles * nu));
-    u = j < npm || j == npm + 3 * m.NB ? j : npm + 3 * (m.NB - 1 - (j - npm) / 3) + (j - npm) % 3;
+    u = j < 0 ? SV.lu_unit()
+              : j < npm || j == npm + 3 * m.NB ? j : npm + 3 * (m.NB - 1 - (j - npm) / 3) + (j - npm) % 3;
   } else {
     // after the backward: tile-major, so that the CTAs running together read and write one tile's slabs
     tile = blockIdx.x / (nu * m.T);
@@ -234,6 +237,127 @@ nsf_dw_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_constant_
     __syncthreads();
   };
 
+  if (u == SV.lu_unit()) {
+    // ---- LULinear (y = U v, z' = L y + b): parameter gradients summed over the tile's 128 rows, each in the
+    //      order of lu_backward (nsf.cu).  It returns before the end of the kernel: in production order it is
+    //      never the grid's last CTA, and on whole tiles (tile-major, an ordinary launch) that CTA waits for nothing.
+    if (!__ldg(v.LT + SBI_L_HAS_LU)) return;
+    static_assert(4 * kLuMax * kRows + kRows + 2 * kLuMax * kLuMax + 2 * kLuMax <= 2 * kStFloats, "LU unit");
+    const int D = m.D;
+    float* DZ = sm;                  // feature-major [16][128]: dz, y, dy, v; then the row weights and U | L
+    float* Y = DZ + kLuMax * kRows;
+    float* DY = Y + kLuMax * kRows;
+    float* V = DY + kLuMax * kRows;
+    float* GR = V + kLuMax * kRows;
+    float* U = GR + kRows;
+    const float* Lw = U + kLuMax * kLuMax;
+    const float g = live ? (gout ? __ldg(gout + gr) : g_const) : 0.f;
+    prep_lu(m, l, U);
+    // dz of the top layer is d(sum g log q)/dz_T = -g z_T; below it, the backward writes dz as it enters the layer
+    if (l < m.T - 1) wait_ready();
+    else __syncthreads();
+    if (half == 0) {
+      float vr[kLuMax];
+      tc_load_row16(svl + SV.v, row, vr);
+#pragma unroll
+      for (int i = 0; i < kLuMax; ++i) {
+        float y = 0.f;
+#pragma unroll
+        for (int j = 0; j < kLuMax; ++j)
+          if (j >= i) y = fmaf(U[i * kLuMax + j], vr[j], y);        // padded entries are zero
+        if (i < D) {
+          V[i * kRows + row] = vr[i];
+          Y[i * kRows + row] = y;
+        }
+      }
+      GR[row] = g;
+    } else {
+      float dzr[kLuMax];
+      if (l == m.T - 1) {
+        tc_load_row16(save + (size_t)tile * SV.tile_stride + SV.zt, row, dzr);
+#pragma unroll
+        for (int i = 0; i < kLuMax; ++i) dzr[i] = live ? -g * dzr[i] : 0.f;
+      } else {
+        tc_load_row16(svl + SV.layer_stride + SV.dz_below(), row, dzr);
+      }
+#pragma unroll
+      for (int i = 0; i < kLuMax; ++i) dzr[i] = (i < D) ? dzr[i] : 0.f;
+      // dy = dz + L^T dz (strictly lower part)
+#pragma unroll
+      for (int i = 0; i < kLuMax; ++i) {
+        float dy = dzr[i];
+#pragma unroll
+        for (int j = 0; j < kLuMax; ++j)
+          if (j > i) dy = fmaf(Lw[j * kLuMax + i], dzr[j], dy);
+        if (i < D) {
+          DZ[i * kRows + row] = dzr[i];
+          DY[i * kRows + row] = dy;
+        }
+      }
+    }
+    __syncthreads();
+    // one (i,j) pair per thread; four independent partial sums; the lanes of a warp read different feature rows
+    // (same bank at the same offset), so entry t starts 4 (t % 32) rows in
+    float* gp = gpart + (size_t)tile * m.n_params;
+    const int o_lo = __ldg(v.LT + SBI_L_LU_LOWER), o_up = __ldg(v.LT + SBI_L_LU_UPPER);
+    const int o_dg = __ldg(v.LT + SBI_L_LU_DIAG), o_bi = __ldg(v.LT + SBI_L_LU_BIAS);
+    for (int t = tid; t < D * D + D; t += kThreads) {
+      const int rot = 4 * (t & 31);
+      auto dot = [&](const float* p, const float* q) {
+        float a0 = 0.f, a1 = 0.f, a2 = 0.f, a3 = 0.f;
+#pragma unroll 4
+        for (int r = 0; r < kRows; r += 4) {
+          const int rr = (r + rot) & (kRows - 1);
+          const float4 x4 = *reinterpret_cast<const float4*>(p + rr);
+          const float4 y4 = *reinterpret_cast<const float4*>(q + rr);
+          a0 = fmaf(x4.x, y4.x, a0); a1 = fmaf(x4.y, y4.y, a1);
+          a2 = fmaf(x4.z, y4.z, a2); a3 = fmaf(x4.w, y4.w, a3);
+        }
+        return (a0 + a1) + (a2 + a3);
+      };
+      auto rsum = [&](const float* p) {
+        float a0 = 0.f, a1 = 0.f, a2 = 0.f, a3 = 0.f;
+#pragma unroll 4
+        for (int r = 0; r < kRows; r += 4) {
+          const float4 x4 = *reinterpret_cast<const float4*>(p + ((r + rot) & (kRows - 1)));
+          a0 += x4.x; a1 += x4.y; a2 += x4.z; a3 += x4.w;
+        }
+        return (a0 + a1) + (a2 + a3);
+      };
+      float a;
+      float* dst;
+      if (t < D * D) {
+        const int i = t / D, j = t % D;
+        if (i > j) {
+          a = dot(DZ + i * kRows, Y + j * kRows);
+          dst = gp + o_lo + i * (i - 1) / 2 + j;
+        } else if (i < j) {
+          a = dot(DY + i * kRows, V + j * kRows);
+          dst = gp + o_up + i * D - i * (i + 1) / 2 + (j - i - 1);
+        } else {
+          a = dot(DY + i * kRows, V + i * kRows);
+          const float gs = rsum(GR);
+          a = (a + gs / U[i * kLuMax + i]) * sigmoid_f(__ldg(m.d_params + o_dg + i));
+          dst = gp + o_dg + i;
+        }
+      } else {
+        const int i = t - D * D;
+        a = rsum(DZ + i * kRows);
+        dst = gp + o_bi + i;
+      }
+      *dst = accum ? (*dst + a) : a;
+    }
+    // the arrays are padded to a multiple of 4 entries: padding takes a zero gradient (every entry of the slab is
+    // written by this kernel; nothing is zero-filled beforehand)
+    if (!accum && tid >= kThreads - 4) {
+      const int k = tid - (kThreads - 4);
+      const int ntri = D * (D - 1) / 2;
+      const int o = k == 0 ? o_lo : k == 1 ? o_up : k == 2 ? o_dg : o_bi;
+      const int n = k < 2 ? ntri : D;
+      for (int e = n; e < ((n + 3) & ~3); ++e) gp[o + e] = 0.f;
+    }
+    return;
+  }
   DwGeo g;
   if (u < npm) {
     // ---- final layer, pass u: dW of the parameter rows of features 2u, 2u+1; X = the final-layer input
@@ -306,8 +430,8 @@ nsf_dw_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_constant_
     bulk_wait_all();
   }
   // the last CTA (its unit is among the last the backward writes) holds the grid open until the backward grid
-  // has completed, so that stream work after this kernel also finds the backward's other outputs (LULinear
-  // gradients, condition gradients, loss statistics) in memory
+  // has completed, so that stream work after this kernel also finds the backward's other outputs (condition
+  // gradients, loss statistics) in memory
   if (blockIdx.x == gridDim.x - 1) asm volatile("griddepcontrol.wait;" ::: "memory");
 }
 
@@ -315,13 +439,12 @@ template <int H, int RPC, int KB, bool COND>
 __global__ void __launch_bounds__(kThreads, 1)
 nsf_vjp_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_constant__ sbi_nsf_tc tcb,
                   const __grid_constant__ sbi_rows rows, const float* __restrict__ gout, float g_const,
-                  float* __restrict__ gpart, float* __restrict__ loss_acc,
-                  float* __restrict__ save, int accum_first, const StoreArgs sa,
+                  float* __restrict__ loss_acc, float* __restrict__ save, const StoreArgs sa,
                   float* __restrict__ dcond) {
   constexpr int HP8 = (H + 7) & ~7;
   constexpr int NCH = HP8 / 8;
   constexpr int TPR = kThreads / RPC;                   // threads per row
-  constexpr int UPT = kRows / RPC;                      // CTAs per tile (= cluster size)
+  constexpr int UPT = kRows / RPC;                      // CTAs per tile
   constexpr int NC = TPR == 2 ? HP8 / 2 : 16;           // columns per thread ([tq NC, tq NC + NC))
   constexpr int NG = NC / 4;
   static_assert(HP8 % 8 == 0 && NC % 4 == 0 && H > (TPR - 1) * NC && H < HP8 + 1 && HP8 <= kDyCols, "hidden width");
@@ -349,10 +472,8 @@ nsf_vjp_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_constant
   const int tq = warp / (RPC / 32);                        // which column part of the row
   const int row = ((warp % (RPC / 32)) << 5) | lane;       // row of the CTA = store lane
   const int cbase = tq * NC;
-  const int rank = (int)(blockIdx.x % UPT);                // half of the tile (= rank in the cluster)
   RqsConst rc = rqs_const(m);
   rc.K = KB;
-  float* gp = gpart + (size_t)(blockIdx.x / UPT) * m.n_params;
   // condition gradient: features [c_lo, c_hi) of this thread's row; dY = the row's dY columns at `dy`
   // (written by all threads of the row before the CTA barrier that precedes the call)
   const int c_part = (C + TPR - 1) / TPR;
@@ -367,7 +488,6 @@ nsf_vjp_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_constant
       out[c] += a / __ldg(csd + c);
     }
   };
-  bool accum = accum_first != 0;
 
   // operands written: hand them over to the MMAs
   auto hand_over = [&]() {
@@ -410,11 +530,9 @@ nsf_vjp_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_constant
     }
   };
 
-  int iter = 0;
-  for (int64_t unit = blockIdx.x; unit < nunits; unit += gridDim.x, ++iter) {
-    if (iter > 0) accum = true;
+  for (int64_t unit = blockIdx.x; unit < nunits; unit += gridDim.x) {
     const int64_t tile = unit / UPT;                        // 128-row tile (save slab)
-    const int srow = rank * RPC + row;                      // lane of the row in the tile's save slab
+    const int srow = (int)(unit % UPT) * RPC + row;         // lane of the row in the tile's save slab
     const int64_t row0 = unit * RPC;
     float* svt = save + (size_t)tile * SV.tile_stride;
     // ---- per-tile setup: upstream gradient, loss statistics, d(sum g log q)/dz_T = -g z_T
@@ -462,8 +580,8 @@ nsf_vjp_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_constant
       int stage = 0;
       SBI_TL(1000 * (li + 1));
 
-      // saved activations travel from L2 while the LU section runs: the spline parameters of this
-      // thread's first feature (the features go round-robin over the row's parts)
+      // the spline parameters of this thread's first feature (the features go round-robin over the row's
+      // parts), requested before the LU section
       float qn[32], xn = 0.f;
       int jn = 0;
 #pragma unroll
@@ -474,37 +592,17 @@ nsf_vjp_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_constant
         xn = tc_load_row16_at(svl + SV.zin, srow, jn);
       }
 
-      // ================= LULinear backward (y = U v, z' = L y + b) =================
-      // (the scratch and the dense factors were last read before the barriers of the previous layer;
-      // the factors of this layer were built a layer ago: prep_lu below)
+      // ================= LULinear backward (y = U v, z' = L y + b): dv = U^T (dz + L^T dz) =================
+      // (the dense factors of this layer were built a layer ago: prep_lu below; the parameter gradients are the
+      // weight-gradient kernel's LULinear unit, which reads the dz written here)
       if (__ldg(v.LT + SBI_L_HAS_LU)) {
-        float vr[kLuMax];
-        if (tq == 0) tc_load_row16(svl + SV.v, srow, vr);
-        SBI_TL(1000 * (li + 1) + 91);
-        float* V = sm + L.lus;
-        float* Y = V + 16 * RPC;
-        float* DY = Y + 16 * RPC;
-        const float* U = sm + L.lum;
-        const float* Lw = U + kLuMax * kLuMax;
-        float dyr[kLuMax];
-        if (tq == 0) {
-          // y = U v on the thread's row (part 1 does dy meanwhile)
-#pragma unroll
-          for (int i = 0; i < kLuMax; ++i) {
-            float y = 0.f;
-#pragma unroll
-            for (int j = 0; j < kLuMax; ++j)
-              if (j >= i) y = fmaf(U[i * kLuMax + j], vr[j], y);        // padded entries are zero
-            if (i < D) {
-              V[i * RPC + row] = vr[i];
-              Y[i * RPC + row] = y;
-            }
-          }
-        } else if (TPR == 2 || tq == 1) {
-          // dy = dz + L^T dz (strictly lower part)
-          float dzr[kLuMax];
+        if (tq == 1) {
+          const float* U = sm + L.lum;
+          const float* Lw = U + kLuMax * kLuMax;
+          float dzr[kLuMax], dyr[kLuMax];
 #pragma unroll
           for (int i = 0; i < kLuMax; ++i) dzr[i] = (i < D) ? dzs[i * RPC + row] : 0.f;
+          // dy = dz + L^T dz (strictly lower part)
 #pragma unroll
           for (int i = 0; i < kLuMax; ++i) {
             float dy = dzr[i];
@@ -512,84 +610,7 @@ nsf_vjp_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_constant
             for (int j = 0; j < kLuMax; ++j)
               if (j > i) dy = fmaf(Lw[j * kLuMax + i], dzr[j], dy);
             dyr[i] = dy;
-            if (i < D) DY[i * RPC + row] = dy;
           }
-        }
-        if constexpr (UPT == 1) group_sync();
-        else cluster_sync();      // both halves' rows are in their CTA's shared memory
-        SBI_TL(1000 * (li + 1) + 92);
-        // parameter gradients: one (i,j) pair per thread, reduction over the tile rows (order of
-        // lu_backward, nsf.cu); half tiles: CTA 0 of the cluster, rows 64.. from CTA 1
-        if (UPT == 1 || rank == 0) {
-          const float* peer = UPT == 1 ? sm : cluster_peer(sm, 1);
-          // float4 of tile rows [rr, rr + 4) of the feature-major array at p (local address)
-          auto at4 = [&](const float* p, int rr) {
-            return *reinterpret_cast<const float4*>(UPT == 1 || rr < RPC ? p + rr : peer + (p - sm) + (rr - RPC));
-          };
-          const int o_lo = __ldg(v.LT + SBI_L_LU_LOWER), o_up = __ldg(v.LT + SBI_L_LU_UPPER);
-          const int o_dg = __ldg(v.LT + SBI_L_LU_DIAG), o_bi = __ldg(v.LT + SBI_L_LU_BIAS);
-          for (int t = tid; t < D * D + D; t += kThreads) {
-            float a = 0.f;
-            float* dst;
-            // dot products over the 128 tile rows, four independent partial sums; every lane reads a
-            // different feature row (same bank at the same offset), so lane k starts 4k rows in
-            const int rot = 4 * lane;
-            auto dot = [&](const float* p, const float* q) {
-              float a0 = 0.f, a1 = 0.f, a2 = 0.f, a3 = 0.f;
-#pragma unroll 4
-              for (int r = 0; r < kRows; r += 4) {
-                const int rr = (r + rot) & (kRows - 1);
-                const float4 x4 = at4(p, rr);
-                const float4 y4 = at4(q, rr);
-                a0 = fmaf(x4.x, y4.x, a0); a1 = fmaf(x4.y, y4.y, a1);
-                a2 = fmaf(x4.z, y4.z, a2); a3 = fmaf(x4.w, y4.w, a3);
-              }
-              return (a0 + a1) + (a2 + a3);
-            };
-            auto rsum = [&](const float* p) {
-              float a0 = 0.f, a1 = 0.f, a2 = 0.f, a3 = 0.f;
-#pragma unroll 4
-              for (int r = 0; r < kRows; r += 4) {
-                const float4 x4 = at4(p, (r + rot) & (kRows - 1));
-                a0 += x4.x; a1 += x4.y; a2 += x4.z; a3 += x4.w;
-              }
-              return (a0 + a1) + (a2 + a3);
-            };
-            if (t < D * D) {
-              const int i = t / D, j = t % D;
-              if (i > j) {
-                a = dot(dzs + i * RPC, Y + j * RPC);
-                dst = gp + o_lo + i * (i - 1) / 2 + j;
-              } else if (i < j) {
-                a = dot(DY + i * RPC, V + j * RPC);
-                dst = gp + o_up + i * D - i * (i + 1) / 2 + (j - i - 1);
-              } else {
-                a = dot(DY + i * RPC, V + i * RPC);
-                const float gs = rsum(GRs);
-                a = (a + gs / U[i * kLuMax + i]) * sigmoid_f(__ldg(P + o_dg + i));
-                dst = gp + o_dg + i;
-              }
-            } else {
-              const int i = t - D * D;
-              a = rsum(dzs + i * RPC);
-              dst = gp + o_bi + i;
-            }
-            *dst = accum ? (*dst + a) : a;
-          }
-          // the arrays are padded to a multiple of 4 entries: padding takes a zero gradient (every
-          // entry of the slab is written by this kernel or nsf_dw_tc_kernel; nothing is zero-filled beforehand)
-          if (!accum && tid >= kThreads - 4) {
-            const int k = tid - (kThreads - 4);
-            const int ntri = D * (D - 1) / 2;
-            const int o = k == 0 ? o_lo : k == 1 ? o_up : k == 2 ? o_dg : o_bi;
-            const int n = k < 2 ? ntri : D;
-            for (int e = n; e < ((n + 3) & ~3); ++e) gp[o + e] = 0.f;
-          }
-        }
-        if constexpr (UPT == 1) group_sync();
-        else cluster_sync();      // CTA 1's rows have been read
-        SBI_TL(1000 * (li + 1) + 93);
-        if (tq == 1) {
           // dv = U^T dy
 #pragma unroll
           for (int j = 0; j < kLuMax; ++j) {
@@ -603,6 +624,7 @@ nsf_vjp_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_constant
           }
         }
         group_sync();
+        if (l < m.T - 1) publish(svl, SV.lu_unit(), 1);
       }
       if (l > 0) prep_lu(m, l - 1, sm + L.lum);     // next layer's dense factors: first read a whole layer of barriers later
       SBI_TL(1000 * (li + 1) + 1);
@@ -762,6 +784,11 @@ nsf_vjp_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_constant
 #pragma unroll
           for (int j = 0; j < 16; ++j)
             if (j < v.n_id) dzs[__ldg(v.idf + j) * RPC + row] += d[j];
+          // the row's dz at layer l - 1's LULinear output, for the weight-gradient kernel's LULinear unit of that
+          // layer, in this layer's spline parameters, whose last reader is done (nsf_tc_save.cuh).  Before the
+          // barrier: after it, part 1 of the row overwrites dz with dv.  The LU section of layer l - 1
+          // publishes it after its CTA barrier.
+          if (l > 0) tc_save_row16<RPC>(svl + SV.dz_below(), srow, dzs, row, D);
         }
         group_sync();
       }
@@ -851,16 +878,16 @@ static int vjp_tc_launch(const sbi_nsf_model* m, const sbi_nsf_tc* tc_fwd, const
     const bool half_tiles = 2 * grid <= sbi::dev_num_sms();
     if (int rc = tc::launch_forward_save(m, tc_fwd, &rr, d_logp ? d_logp + r0 : nullptr, d_save, half_tiles, s))
       return rc;
-    if (int rc = half_tiles ? launch(tc::nsf_vjp_tc_kernel<50, 64, 10, COND>, Grid(2 * grid, 2), tc::kThreads,
-                                     bwd_bytes_half, s, *m, *tc_bwd, rr, d_gout ? d_gout + r0 : nullptr, g_const,
-                                     d_gpart, d_loss_acc, d_save, r0 > 0 ? 1 : 0, sa,
+    const float* gout = d_gout ? d_gout + r0 : nullptr;
+    if (int rc = half_tiles ? launch(tc::nsf_vjp_tc_kernel<50, 64, 10, COND>, 2 * grid, tc::kThreads, bwd_bytes_half,
+                                     s, *m, *tc_bwd, rr, gout, g_const, d_loss_acc, d_save, sa,
                                      COND ? d_gcond + r0 * m->C : nullptr)
                             : launch(tc::nsf_vjp_tc_kernel<50, tc::kRows, 10, COND>, grid, tc::kThreads, bwd_bytes, s, *m,
-                                     *tc_bwd, rr, d_gout ? d_gout + r0 : nullptr, g_const, d_gpart, d_loss_acc,
-                                     d_save, r0 > 0 ? 1 : 0, sa, COND ? d_gcond + r0 * m->C : nullptr))
+                                     *tc_bwd, rr, gout, g_const, d_loss_acc, d_save, sa,
+                                     COND ? d_gcond + r0 * m->C : nullptr))
       return rc;
-    if (int rc = launch(tc::nsf_dw_tc_kernel<50>, Grid(grid * m->T * tc::dw_units(*m), 1, half_tiles), tc::kThreads,
-                        dw_bytes, s, *m, rr, d_save, d_gpart, r0 > 0 ? 1 : 0, half_tiles ? 2u : 0u))
+    if (int rc = launch(tc::nsf_dw_tc_kernel<50>, Grid(grid * m->T * tc::dw_units(*m), half_tiles), tc::kThreads,
+                        dw_bytes, s, *m, rr, d_save, d_gpart, r0 > 0 ? 1 : 0, half_tiles ? 2u : 0u, gout, g_const))
       return rc;
   }
   return 0;

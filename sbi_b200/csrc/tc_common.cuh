@@ -349,18 +349,6 @@ __device__ __forceinline__ void smem_a8(float* as, uint32_t row, int col, const 
   smem_a4<RPC>(as, row, col + 4, {v[4], v[5], v[6], v[7]});
 }
 __device__ __forceinline__ void group_sync() { asm volatile("bar.sync 1, 256;" ::: "memory"); }
-// barrier of every thread of the CTA's cluster; orders the shared-memory writes before it with the reads
-// of other CTAs after it
-__device__ __forceinline__ void cluster_sync() {
-  asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-// generic address of the same shared-memory location in CTA `rank` of the cluster
-__device__ __forceinline__ const float* cluster_peer(const float* p, uint32_t rank) {
-  uint64_t r;
-  asm("mapa.u64 %0, %1, %2;" : "=l"(r) : "l"(p), "r"(rank));
-  return reinterpret_cast<const float*>(r);
-}
-
 // dense LU factors of NSF layer l, zero-padded to 16x16, into lum = [U | L | bias 16 | diag 16]
 // (all threads; the unit diagonal of L is implicit)
 __device__ __forceinline__ void prep_lu(const sbi_nsf_model& m, int l, float* lum) {
