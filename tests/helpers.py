@@ -1,4 +1,6 @@
 """Shared helpers for the parity tests (oracle side = oracle/, CUDA side = sbi_b200)."""
+from collections import namedtuple
+
 import torch
 
 from oracle import sbi_port
@@ -43,6 +45,69 @@ def nsf_vjp_raw(est, inp, cond, g, save, fill=0.0):
                               L.ptr(gcond), None, L.ptr(save), 0 if save is None else save.numel() * 4,
                               torch.cuda.current_stream().cuda_stream)
     return rc, gpart, ginp, gcond, logp
+
+
+VjpStep = namedtuple("VjpStep", "gpart grad logp loss_acc gcond")
+
+
+def use_vjp_path(monkeypatch, est, tc):
+    """Run the training VJP of `est` on the tensor-core pair (`tc`) or on the SIMT kernel for the rest of the test
+    (SBI_B200_VJP_TC through `monkeypatch`), and drop the estimator's cached verdict."""
+    monkeypatch.setenv("SBI_B200_VJP_TC", "1" if tc else "0")
+    est._cache.pop("tc_train", None)
+
+
+def vjp_step(est, inp, cond, g, *, g_const=0.0, with_cond=False, tc=True, graph=False):
+    """One training step of sum_r g_r log q(inp_r | cond_r) (g_const for every row when `g` is None) through
+    est.vjp, on the tensor-core pair when `tc`, else on the SIMT kernel (asserted either way); with `with_cond`
+    also the condition gradient.  Outputs start as NaN on the tensor-core pair, which writes every entry, and as
+    zero on the SIMT kernel.  Eager, or with `graph` captured once in a CUDA graph (after a warm-up on a side
+    stream) and replayed `int(graph)` times from fresh outputs, every replay bit-identical to the first.
+    Returns CPU copies: VjpStep(partial-gradient slabs, their sum, log-probs, loss statistics, condition gradient
+    or None)."""
+    from sbi_b200 import _lib as L
+    R = inp.shape[0]
+    assert est._vjp_uses_tc(R, True) == tc
+    P, n_part = est.layout.n_params, est.vjp_parts(R)
+    fill = float("nan") if tc else 0.0
+    gpart = torch.full((n_part, P), fill, device="cuda")
+    lp = torch.full((R,), fill, device="cuda")
+    acc = torch.zeros(2, device="cuda")
+    gcond = torch.full((R, cond.shape[1]), fill, device="cuda") if with_cond else None
+    m = est._model(nbuf=3)
+    rows = L.Rows(inp.data_ptr(), cond.data_ptr(), None, R, 0)
+
+    def step():
+        est.vjp(m, rows, R, g, g_const, lp, gpart, None, gcond, acc, cond_tc=with_cond)
+
+    def result():
+        grad = L.reduce_partials(gpart, n_part, P)
+        return VjpStep(gpart.cpu(), grad.cpu(), lp.cpu(), acc.cpu(), None if gcond is None else gcond.cpu())
+
+    if not graph:
+        step()
+        return result()
+    side = torch.cuda.Stream()
+    side.wait_stream(torch.cuda.current_stream())
+    with torch.cuda.stream(side):
+        step()
+    torch.cuda.current_stream().wait_stream(side)
+    cuda_graph = torch.cuda.CUDAGraph()
+    with torch.cuda.graph(cuda_graph):
+        step()
+    outs = []
+    for _ in range(int(graph)):
+        for t in (gpart, lp, gcond):
+            if t is not None:
+                t.fill_(fill)
+        acc.zero_()
+        cuda_graph.replay()
+        outs.append(result())
+    for rep, out in enumerate(outs[1:], 1):
+        for name in ("gpart", "logp", "gcond"):
+            a, b = getattr(out, name), getattr(outs[0], name)
+            assert a is None or torch.equal(a, b), f"replay {rep}: {name} differ from the first replay"
+    return outs[0]
 
 
 def oracle_maf(D=3, C=2, n=2000, seed=0, perturb=0.1, scale_fn="softplus", rqs=False, **kw):

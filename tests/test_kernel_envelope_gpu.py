@@ -19,7 +19,8 @@ import torch
 from torch import nn
 
 from oracle import sbi_port
-from tests.helpers import b200_from_oracle, b200_maf_from_oracle, nsf_vjp_raw, oracle_maf, oracle_nsf
+from tests.helpers import (b200_from_oracle, b200_maf_from_oracle, nsf_vjp_raw, oracle_maf, oracle_nsf, use_vjp_path,
+                           vjp_step)
 
 pytestmark = pytest.mark.gpu
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -462,23 +463,6 @@ def _nsf_lib_tc_ok(est):
     return bool(L.load().sbi_b200_nsf_tc_supported(C.byref(m), C.byref(tc)))
 
 
-def _tc_vjp(est, inp, cond, g):
-    """Parameter gradient of sum g * log q through est.vjp on the tensor-core pair (asserted to be taken)."""
-    from sbi_b200 import _lib as L
-    lib = L.load()
-    R, P = inp.shape[0], est.layout.n_params
-    assert est._vjp_uses_tc(R, True)
-    n_part = est.vjp_parts(R)
-    gpart = torch.full((n_part, P), float("nan"), device="cuda")
-    lp = torch.empty(R, device="cuda")
-    m = est._model(nbuf=3)
-    rows = L.Rows(inp.data_ptr(), cond.data_ptr(), None, R, 0)
-    est.vjp(m, rows, R, g, 0.0, lp, gpart, None, None, torch.zeros(2, device="cuda"))
-    grad = torch.empty(P, device="cuda")
-    L.check(lib.sbi_b200_reduce_partials(L.ptr(gpart), n_part, P, L.ptr(grad), L.stream_ptr()), "reduce")
-    return grad.cpu().double()
-
-
 @pytest.mark.parametrize("D,C,NB", [(2, 14, 1), (2, 14, 3), (16, 12, 1)], ids=["HC64", "HC64_NB3", "D16_C12"])
 def test_nsf_tensor_core_edge_inside(cuda_lib, monkeypatch, D, C, NB):
     """The largest models the wgmma kernels take: H + C = 64, D = 16, and the 112 KB shared-memory budget
@@ -504,9 +488,9 @@ def test_nsf_tensor_core_edge_inside(cuda_lib, monkeypatch, D, C, NB):
         d = (a - b).abs().max().item()
         print(f"D={D} C={C} NB={NB} {name}: |wgmma - SIMT| {d:.3e}")
         assert d <= tol, name
-    monkeypatch.setenv("SBI_B200_VJP_TC", "1")
+    use_vjp_path(monkeypatch, est, True)
     g = torch.randn(R, dtype=torch.float64, generator=torch.Generator().manual_seed(7))
-    got = _tc_vjp(est, inp.cuda(), cond.cuda(), g.float().cuda())
+    got = vjp_step(est, inp.cuda(), cond.cuda(), g.float().cuda()).grad.double()
     r32 = _oracle_grads(flow, est, inp, cond, g, torch.float32)[0]
     r64 = _oracle_grads(flow, est, inp, cond, g, torch.float64)[0]
     assert (got[_padding(est)] == 0).all()
