@@ -379,10 +379,10 @@ enum { SBI_SLICE_BEGIN = 0, SBI_SLICE_LOWER = 1, SBI_SLICE_UPPER = 2, SBI_SLICE_
 typedef struct {
   int32_t C, D;                 /* chains, dimensions */
   int32_t num_samples, tuning;  /* sweeps to record per chain, tuning sweeps before recording */
-  double init_width, max_width;
+  double max_width;
   uint64_t seed;
   double* d_x;                  /* (C, D) current position (in/out) */
-  double* d_width;              /* (C, D) */
+  double* d_width;              /* (C, D) bracket widths: the caller writes the initial widths (in/out) */
   int32_t* d_order;             /* (C, D) */
   int32_t* d_istate;            /* (C, 4): state, i, t, - */
   double* d_fstate;             /* (C, 8): cxi, wi, lx, ux, xi, logu, -, - */

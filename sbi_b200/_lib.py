@@ -122,7 +122,7 @@ F_WI, F_BI, F_WC, F_BC, F_WM, F_BM, F_WT, F_BT, F_WO, F_BO, F_LAYER0 = 0, 1, 2, 
 class SliceChains(C.Structure):
     _fields_ = [
         ("C", C.c_int32), ("D", C.c_int32), ("num_samples", C.c_int32), ("tuning", C.c_int32),
-        ("init_width", C.c_double), ("max_width", C.c_double), ("seed", C.c_uint64),
+        ("max_width", C.c_double), ("seed", C.c_uint64),
         ("d_x", C.c_void_p), ("d_width", C.c_void_p), ("d_order", C.c_void_p), ("d_istate", C.c_void_p),
         ("d_fstate", C.c_void_p), ("d_rng", C.c_void_p), ("d_samples", C.c_void_p),
     ]

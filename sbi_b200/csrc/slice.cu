@@ -3,6 +3,9 @@
 // kernel launch per lock-step.  One thread per chain; chain state (position, bracket, widths,
 // dimension order, Philox RNG) lives in HBM in float64 like the reference's numpy state; the
 // potential is evaluated between steps by the estimator kernels on the (C, D) float32 `params`.
+// The bracket arithmetic is written with explicit round-to-nearest intrinsics so that nvcc does not
+// contract it into FMAs: every bracket end and proposal is then the float64 value numpy computes from
+// the same draws, which lets the tests compare a chain with the reference draw for draw.
 //
 // Reference semantics kept: BEGIN evaluates at the current point and draws the slice height
 // logu = logp + log(1 - u); the bracket is placed randomly, stepped out below then above while the
@@ -49,13 +52,12 @@ __global__ void slice_init_kernel(const sbi_slice_chains s, float* params) {
   curand_init(s.seed, (unsigned long long)c, 0ULL, &r);
   int32_t* ord = s.d_order + (size_t)c * s.D;
   shuffle_order(ord, s.D, &r);
-  for (int d = 0; d < s.D; ++d) s.d_width[(size_t)c * s.D + d] = s.init_width;
   int32_t* is = s.d_istate + (size_t)c * 4;
   is[0] = SBI_SLICE_BEGIN; is[1] = 0; is[2] = 0; is[3] = 0;
   double* fs = s.d_fstate + (size_t)c * 8;
   const int dim = ord[0];
   fs[0] = s.d_x[(size_t)c * s.D + dim];              // cxi
-  fs[1] = s.init_width;                              // wi
+  fs[1] = s.d_width[(size_t)c * s.D + dim];          // wi (the caller's initial widths)
   write_params(s, c, params, dim, fs[0]);
   *rng = r;
 }
@@ -81,7 +83,7 @@ __global__ void slice_step_kernel(const sbi_slice_chains s, const float* __restr
 
   if (state == SBI_SLICE_BEGIN) {
     logu = lp + log(1.0 - rand01(&r));
-    lx = cxi - wi * rand01(&r);
+    lx = __dsub_rn(cxi, __dmul_rn(wi, rand01(&r)));
     ux = lx + wi;
     next = lx;
     state = SBI_SLICE_LOWER;
@@ -98,14 +100,14 @@ __global__ void slice_step_kernel(const sbi_slice_chains s, const float* __restr
       ux += wi;
       next = ux;
     } else {
-      xi = (ux - lx) * rand01(&r) + lx;
+      xi = __dadd_rn(__dmul_rn(ux - lx, rand01(&r)), lx);
       next = xi;
       state = SBI_SLICE_SAMPLE;
     }
   } else {   // SAMPLE_SLICE
     if (lp < logu) {   // rejected: shrink the bracket
       if (xi < cxi) lx = xi; else ux = xi;
-      xi = (ux - lx) * rand01(&r) + lx;
+      xi = __dadd_rn(__dmul_rn(ux - lx, rand01(&r)), lx);
       next = xi;
     } else if (t < s.num_samples + s.tuning) {
       x[dim] = xi;     // accept

@@ -45,7 +45,7 @@ class SliceSamplerVectorized:
         self.thin = 1 if thin is None else thin
         self.tuning = tuning
         self.verbose = verbose
-        self.init_width = float(np.asarray(init_width).reshape(-1)[0])
+        self.init_width = init_width
         self.max_width = max_width
         self._samples = None
         self._device = device
@@ -67,7 +67,8 @@ class SliceSamplerVectorized:
                             dtype=torch.float64).reshape(self.num_chains, -1).to(dev).contiguous()
         Cn, D = x.shape
         seed = int(torch.randint(0, 2 ** 62, (1,)).item()) if self._seed is None else int(self._seed)
-        width = torch.empty(Cn, D, dtype=torch.float64, device=dev)
+        # initial bracket widths per dimension, a scalar broadcast (np.full(n_dims, init_width) in the reference)
+        width = torch.as_tensor(np.asarray(self.init_width, dtype=np.float64)).to(dev).expand(Cn, D).contiguous()
         order = torch.empty(Cn, D, dtype=torch.int32, device=dev)
         istate = torch.zeros(Cn, 4, dtype=torch.int32, device=dev)
         fstate = torch.zeros(Cn, 8, dtype=torch.float64, device=dev)
@@ -75,10 +76,11 @@ class SliceSamplerVectorized:
         samples = torch.empty(Cn, max(int(num_samples), 1), D, dtype=torch.float64, device=dev)
         params = torch.empty(Cn, D, dtype=torch.float32, device=dev)
         n_done = torch.zeros(1, dtype=torch.int32, device=dev)
-        s = L.SliceChains(Cn, D, int(num_samples), int(self.tuning), self.init_width,
-                          float(min(self.max_width, 1e300)), seed, x.data_ptr(), width.data_ptr(),
-                          order.data_ptr(), istate.data_ptr(), fstate.data_ptr(), rng.data_ptr(),
-                          samples.data_ptr())
+        s = L.SliceChains(Cn, D, int(num_samples), int(self.tuning), float(min(self.max_width, 1e300)), seed,
+                          x.data_ptr(), width.data_ptr(), order.data_ptr(), istate.data_ptr(), fstate.data_ptr(),
+                          rng.data_ptr(), samples.data_ptr())
+        # the chains' device state, readable while and after the sampler runs (final widths, state machine)
+        self._chain_state = {"width": width, "order": order, "istate": istate, "fstate": fstate}
         L.check(lib.sbi_b200_slice_init(C.byref(s), L.ptr(params), L.stream_ptr()), "slice_init")
         it = 0
 

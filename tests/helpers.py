@@ -135,6 +135,68 @@ def b200_maf_from_oracle(flow, theta, x, device="cuda", scale_fn="softplus", rqs
     return est.to(device)
 
 
+_M32 = 0xFFFFFFFF
+_PHILOX_M0, _PHILOX_M1 = 0xD2511F53, 0xCD9E8D57      # round multipliers
+_PHILOX_W0, _PHILOX_W1 = 0x9E3779B9, 0xBB67AE85      # key schedule (Weyl) increments
+
+
+def philox4x32_10(ctr, key):
+    """Random123's Philox4x32-10 block function as cuRAND computes it (curand_philox4x32_x.h): ten rounds of
+    two 32x32->64 multiplies on the 4-word counter, the 2-word key bumped by the Weyl constants between rounds.
+    Returns the four output words."""
+    c0, c1, c2, c3 = (int(w) & _M32 for w in ctr)
+    k0, k1 = (int(w) & _M32 for w in key)
+    for rnd in range(10):
+        if rnd:
+            k0, k1 = (k0 + _PHILOX_W0) & _M32, (k1 + _PHILOX_W1) & _M32
+        p0, p1 = _PHILOX_M0 * c0, _PHILOX_M1 * c2
+        c0, c1, c2, c3 = (p1 >> 32) ^ c1 ^ k0, p1 & _M32, (p0 >> 32) ^ c3 ^ k1, p0 & _M32
+    return c0, c1, c2, c3
+
+
+class PhiloxDraws:
+    """The random stream of one slice-sampler chain (csrc/slice.cu), restated on the host.
+
+    Chain `c` of a run with seed `s` draws from `curand_init(s, subsequence=c, offset=0)` on Philox4x32-10: the key
+    is the seed's low and high 32-bit words, the counter starts at (0, 0, low, high) of the subsequence, and
+    `curand()` hands out the four words of each block in order before the counter's low 64 bits step by one.
+    `curand_uniform_double` takes ONE word x and returns x * 2^-32 + 2^-32 in (0, 1].
+
+    On top of that, the kernel's own conventions, so that the object stands in for `np.random` inside the
+    reference sampler: `rand()` is `1 - uniform` in [0, 1) (`rand01`) and `shuffle(list)` is the kernel's
+    Fisher-Yates (`shuffle_order`).  Every value is exact in float64."""
+
+    def __init__(self, seed: int, subsequence: int = 0):
+        self.key = (seed & _M32, (seed >> 32) & _M32)
+        self.ctr = [0, 0, subsequence & _M32, (subsequence >> 32) & _M32]
+        self._block = philox4x32_10(self.ctr, self.key)
+        self._next = 0
+        self.n_words = 0          # words handed out so far
+
+    def word(self) -> int:
+        """curand(): the next 32-bit word."""
+        if self._next == 4:
+            lo = ((self.ctr[1] << 32) | self.ctr[0]) + 1
+            self.ctr[0], self.ctr[1] = lo & _M32, (lo >> 32) & _M32
+            if lo >> 64:              # carry into the high half of the counter
+                hi = (((self.ctr[3] << 32) | self.ctr[2]) + 1) & ((1 << 64) - 1)
+                self.ctr[2], self.ctr[3] = hi & _M32, hi >> 32
+            self._block = philox4x32_10(self.ctr, self.key)
+            self._next = 0
+        w = self._block[self._next]
+        self._next += 1
+        self.n_words += 1
+        return w
+
+    def rand(self) -> float:
+        return 1.0 - (self.word() * 2.0 ** -32 + 2.0 ** -32)
+
+    def shuffle(self, order: list) -> None:
+        for i in range(len(order) - 1, 0, -1):
+            j = min(int(self.rand() * (i + 1)), i)
+            order[i], order[j] = order[j], order[i]
+
+
 def two_moons_simulator(parameters, r_loc=0.1, r_scale=0.01, base_offset=0.25):
     """The two-moons simulator of the reference's mini benchmark, restated
     (/root/reference/tests/mini_sbibm/two_moons.py:15-78): a noisy half circle shifted by
