@@ -4,7 +4,9 @@
 // written, in proposal order, behind the ones already collected, together with their global proposal
 // index; the running count stays on the device.  Three launches (flags + block counts, scan of the block
 // counts, scatter) replace exp / compare / boolean-index (whose `nonzero` synchronises the host) -- the
-// accepted set and its order are exactly those of the reference's boolean indexing.
+// accepted set and its order are exactly those of the reference's boolean indexing.  The accept decision is a
+// predicate functor: the ratio test above (`reject_compact`) or a byte mask computed by the caller
+// (`mask_compact`, the `candidates[accept_reject_fn(candidates)]` of accept_reject_sample, rejection.py:369-384).
 #include <cuda_runtime.h>
 #include <math.h>
 #include <stdint.h>
@@ -19,19 +21,28 @@ constexpr int kThreads = 256;
 constexpr int kPer = 4;                       // consecutive candidates per thread
 constexpr int kTile = kThreads * kPer;        // candidates per block
 
-__device__ __forceinline__ bool keep_flag(const float* lt, const float* ls, const float* u, int64_t i) {
+// Accept predicates of count_kernel / scatter_kernel: keep(i) says whether candidate i is accepted.
+struct RatioAccept {
+  const float* __restrict__ lt;
+  const float* __restrict__ ls;
+  const float* __restrict__ u;
   // same expression as the reference: exp(a - b) > u  (NaN compares false -> rejected)
-  return expf(lt[i] - ls[i]) > u[i];
-}
+  __device__ __forceinline__ bool operator()(int64_t i) const { return expf(lt[i] - ls[i]) > u[i]; }
+};
 
-__global__ void count_kernel(const float* __restrict__ lt, const float* __restrict__ ls,
-                             const float* __restrict__ u, int64_t n, int32_t* __restrict__ block_count) {
+struct MaskAccept {
+  const uint8_t* __restrict__ keep;           // a torch bool tensor's bytes: nonzero = accepted
+  __device__ __forceinline__ bool operator()(int64_t i) const { return keep[i] != 0; }
+};
+
+template <class Accept>
+__global__ void count_kernel(Accept keep_flag, int64_t n, int32_t* __restrict__ block_count) {
   __shared__ int sh[kThreads / 32];
   const int64_t base = (int64_t)blockIdx.x * kTile + (int64_t)threadIdx.x * kPer;
   int c = 0;
 #pragma unroll
   for (int j = 0; j < kPer; ++j)
-    if (base + j < n && keep_flag(lt, ls, u, base + j)) ++c;
+    if (base + j < n && keep_flag(base + j)) ++c;
   for (int o = 16; o > 0; o >>= 1) c += __shfl_xor_sync(0xffffffffu, c, o);
   if ((threadIdx.x & 31) == 0) sh[threadIdx.x >> 5] = c;
   __syncthreads();
@@ -67,9 +78,8 @@ __global__ void scan_kernel(int32_t* __restrict__ block_count, int nb, int32_t* 
   if (threadIdx.x == 0) *count = carry;
 }
 
-__global__ void scatter_kernel(const float* __restrict__ cand, int D, const float* __restrict__ lt,
-                               const float* __restrict__ ls, const float* __restrict__ u, int64_t n,
-                               int64_t index_base, const int32_t* __restrict__ block_off, float* __restrict__ out,
+template <class Accept>
+__global__ void scatter_kernel(const float* __restrict__ cand, int D, Accept keep_flag, int64_t n, int64_t index_base, const int32_t* __restrict__ block_off, float* __restrict__ out,
                                int64_t* __restrict__ out_idx, int64_t cap) {
   __shared__ int sh[kThreads / 32];
   const int64_t base = (int64_t)blockIdx.x * kTile + (int64_t)threadIdx.x * kPer;
@@ -77,7 +87,7 @@ __global__ void scatter_kernel(const float* __restrict__ cand, int D, const floa
   int c = 0;
 #pragma unroll
   for (int j = 0; j < kPer; ++j) {
-    k[j] = base + j < n && keep_flag(lt, ls, u, base + j);
+    k[j] = base + j < n && keep_flag(base + j);
     c += k[j] ? 1 : 0;
   }
   // exclusive prefix of c over the block (threads own consecutive candidates, so thread order = proposal order)
@@ -100,6 +110,20 @@ __global__ void scatter_kernel(const float* __restrict__ cand, int D, const floa
     }
     ++pos;
   }
+}
+
+// count -> scan -> scatter for one batch of n candidates under the accept predicate `keep`
+template <class Accept>
+int compact(Accept keep, const float* cand, int D, int64_t n, int64_t index_base, float* out, int64_t* out_idx,
+            int64_t cap, int32_t* count, int32_t* scratch, cudaStream_t s) {
+  if (n == 0) return 0;
+  const int64_t nb64 = (n + kTile - 1) / kTile;
+  if (nb64 > (1 << 30)) return SBI_EINVAL;
+  const int nb = (int)nb64;
+  count_kernel<<<nb, kThreads, 0, s>>>(keep, n, scratch);
+  scan_kernel<<<1, kThreads, 0, s>>>(scratch, nb, count);
+  scatter_kernel<<<nb, kThreads, 0, s>>>(cand, D, keep, n, index_base, scratch, out, out_idx, cap);
+  return (int)cudaGetLastError();
 }
 
 // ---- sampling-importance-resampling: one categorical draw per group of K candidates ----------------------------
@@ -208,16 +232,17 @@ extern "C" int sbi_b200_reject_compact(const float* d_cand, int32_t D, const flo
   if (!d_cand || !d_log_target || !d_log_scaled || !d_u || !d_out || !d_count || !d_scratch || D < 1 || n < 0 ||
       cap < 0)
     return SBI_EINVAL;
-  if (n == 0) return 0;
-  const int64_t nb64 = (n + compact::kTile - 1) / compact::kTile;
-  if (nb64 > (1 << 30)) return SBI_EINVAL;
-  const int nb = (int)nb64;
-  cudaStream_t s = (cudaStream_t)stream;
-  compact::count_kernel<<<nb, compact::kThreads, 0, s>>>(d_log_target, d_log_scaled, d_u, n, d_scratch);
-  compact::scan_kernel<<<1, compact::kThreads, 0, s>>>(d_scratch, nb, d_count);
-  compact::scatter_kernel<<<nb, compact::kThreads, 0, s>>>(d_cand, D, d_log_target, d_log_scaled, d_u, n, index_base,
-                                                         d_scratch, d_out, d_out_idx, cap);
-  return (int)cudaGetLastError();
+  return compact::compact(compact::RatioAccept{d_log_target, d_log_scaled, d_u}, d_cand, D, n, index_base, d_out,
+                          d_out_idx, cap, d_count, d_scratch, (cudaStream_t)stream);
+}
+
+extern "C" int sbi_b200_mask_compact(const float* d_cand, int32_t D, const uint8_t* d_keep, int64_t n,
+                                     int64_t index_base, float* d_out, int64_t* d_out_idx, int64_t cap,
+                                     int32_t* d_count, int32_t* d_scratch, void* stream) {
+  if (!d_cand || !d_keep || !d_out || !d_count || !d_scratch || D < 1 || n < 0 || cap < 0) return SBI_EINVAL;
+  sbi::DeviceGuard dev_guard_(d_cand);
+  return compact::compact(compact::MaskAccept{d_keep}, d_cand, D, n, index_base, d_out, d_out_idx, cap, d_count,
+                          d_scratch, (cudaStream_t)stream);
 }
 
 // scratch: one count per block of kGroups groups, then the selected index of every group

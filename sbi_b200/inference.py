@@ -332,8 +332,11 @@ class _Trainer:
                            exclude_invalid_x: Optional[bool] = None, data_device: Optional[str] = None):
         """Store simulations (npe_base.py:188-299): float32 only, rows with NaN/Inf in x are
         dropped (user_input_checks.py:708-765, sbiutils.py:491-525)."""
-        # round of this block (npe_base.py:224-241): prior samples are round 0, anything else opens a new round
-        if proposal is None or proposal is self._prior:
+        # round of this block (npe_base.py:224-241): prior samples, and draws of a `RestrictedPrior` of the prior
+        # (TSNPE), are round 0; anything else opens a new round
+        from .restriction import is_restricted_prior
+        restricted = is_restricted_prior(proposal)
+        if proposal is None or proposal is self._prior or (restricted and proposal._prior is self._prior):
             current_round = 0
         elif not self._data_round_index:
             current_round = 1
@@ -349,6 +352,10 @@ class _Trainer:
                     and proposal.posterior_estimator is self._neural_net:
                 raise ValueError("The proposal's posterior_estimator is the same object as the trainer's "
                                  "neural network; use trainer.build_posterior() or a deepcopy.")
+            if restricted:     # npe_base.py:600-609
+                warnings.warn("The proposal you passed is a `RestrictedPrior`, but the proposal distribution it "
+                              "uses is not the prior (it can be accessed via `RestrictedPrior._prior`). We do not "
+                              "recommend to mix the `RestrictedPrior` with multi-round NPE.", stacklevel=2)
         if exclude_invalid_x is None:
             exclude_invalid_x = current_round == 0
         if theta.dtype != torch.float32 or x.dtype != torch.float32:
