@@ -120,7 +120,7 @@ adam_clip_kernel(float* __restrict__ params, const float* __restrict__ grad,
       tot = block_sum((s0 + s1) + (s2 + s3), red) * gscale * gscale;
     }
     const float c = max_norm / (sqrtf(tot) + 1e-6f);
-    clip = c < 1.f ? c : 1.f;
+    clip = c >= 1.f ? 1.f : c;   // a NaN norm gives a NaN clip for every entry, as torch.clamp(max=1) does
   }
   if (threadIdx.x == 0) {
     // bias corrections 1 - beta^t in double like torch (python floats), by repeated squaring: ~2 log2(t)

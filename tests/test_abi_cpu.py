@@ -40,6 +40,13 @@ def test_argument_errors(lib):
     from sbi_b200 import _lib as L
     assert lib.sbi_b200_reduce_partials(None, 1, 4, None, None) == -1
     assert lib.sbi_b200_adam_clip_step(None, None, None, None, None, 4, 1e-3, .9, .999, 1e-8, 5., 1., None) == -1
+    # null pointers are refused before any CUDA call; the length and count checks behind them need device
+    # pointers (tests/test_optim_gpu.py)
+    assert lib.sbi_b200_reduce_partials_norm(None, 1, 4, None, None, None, None) == -1
+    assert lib.sbi_b200_adam_clip_step_norm(None, None, None, None, None, 4, 1e-3, .9, .999, 1e-8, 5., 1., None, 0,
+                                            None) == -1
+    assert lib.sbi_b200_nll_stats(None, 4, None, None) == -1
+    assert lib.sbi_b200_nll_stats(None, -1, None, None) == -1
     assert lib.sbi_b200_nsf_logprob(None, None, None, None, None) == -1
     with pytest.raises(ValueError):
         L.check(-1, "x")

@@ -1,5 +1,5 @@
-"""Training-path parity on the GPU: optimiser kernel vs torch (clip_grad_norm_ + Adam), the
-fused step vs the oracle step, and an end-to-end NPE fit against the analytic posterior."""
+"""Training-path parity on the GPU: the fused step vs the oracle step (the optimiser kernels alone are in
+test_optim_gpu.py), and an end-to-end NPE fit against the analytic posterior."""
 import ctypes as C
 import math
 
@@ -10,49 +10,6 @@ from torch.nn.utils.clip_grad import clip_grad_norm_
 from tests.helpers import b200_from_oracle, oracle_nsf
 
 pytestmark = pytest.mark.gpu
-
-
-def test_adam_clip_kernel_matches_torch(cuda_lib):
-    """Same gradients in -> same parameters out as clip_grad_norm_(5.0) + torch Adam
-    (reference step: trainers/base.py:1181-1187)."""
-    from sbi_b200 import _lib as L
-    torch.manual_seed(0)
-    n = 10_000
-    p0 = torch.randn(n)
-    ref = torch.nn.Parameter(p0.clone())
-    opt = torch.optim.Adam([ref], lr=5e-4)
-    p = p0.clone().cuda()
-    state = torch.zeros(2 * n, device="cuda")
-    step = torch.zeros(2, dtype=torch.int32, device="cuda")
-    for it in range(5):
-        g = torch.randn(n) * (10.0 if it % 2 == 0 else 0.01)   # clipped and unclipped regimes
-        ref.grad = g.clone()
-        clip_grad_norm_([ref], max_norm=5.0)
-        opt.step()
-        gd = g.cuda()
-        L.check(cuda_lib.sbi_b200_adam_clip_step(L.ptr(p), L.ptr(gd), L.ptr(state), L.ptr(step), None, n,
-                                                 5e-4, 0.9, 0.999, 1e-8, 5.0, 1.0, L.stream_ptr()), "adam")
-        err = (p.cpu() - ref.detach()).abs().max().item()
-        assert err <= 2e-7, (it, err)
-    assert int(step[0].item()) == 5
-    # norm taken from the reduction kernel's per-block partials: same update as the self-computed norm
-    gp = torch.randn(3, n, device="cuda") * 4.0
-    outs = []
-    for mode in (0, 1):
-        pp = p0.clone().cuda(); st = torch.zeros(2 * n, device="cuda"); sc = torch.zeros(2, dtype=torch.int32, device="cuda")
-        g = torch.empty(n, device="cuda")
-        if mode == 0:
-            L.check(cuda_lib.sbi_b200_reduce_partials(L.ptr(gp), 3, n, L.ptr(g), L.stream_ptr()), "r")
-            L.check(cuda_lib.sbi_b200_adam_clip_step(L.ptr(pp), L.ptr(g), L.ptr(st), L.ptr(sc), None, n, 5e-4, 0.9, 0.999,
-                                                     1e-8, 5.0, 1.0, L.stream_ptr()), "a")
-        else:
-            ss = torch.zeros(cuda_lib.sbi_b200_sumsq_blocks(n), device="cuda")
-            L.check(cuda_lib.sbi_b200_reduce_partials_norm(L.ptr(gp), 3, n, L.ptr(g), None, L.ptr(ss), L.stream_ptr()), "r")
-            assert abs(ss.sum().item() / (gp.sum(0) ** 2).sum().item() - 1) < 1e-5
-            L.check(cuda_lib.sbi_b200_adam_clip_step_norm(L.ptr(pp), L.ptr(g), L.ptr(st), L.ptr(sc), None, n, 5e-4, 0.9,
-                                                          0.999, 1e-8, 5.0, 1.0, L.ptr(ss), ss.shape[0], L.stream_ptr()), "a")
-        outs.append(pp.cpu())
-    assert (outs[0] - outs[1]).abs().max() <= 1e-7
 
 
 def test_fused_train_step_with_scratch_matches_oracle_step(cuda_lib):
