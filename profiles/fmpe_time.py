@@ -1,4 +1,4 @@
-"""FMPE training epoch time (20-d theta and x, batch 200), per-epoch CUDA graph on/off."""
+"""FMPE training epoch time (20-d theta and x, batch 200), one CUDA graph per epoch."""
 import os, sys, math, torch
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from torch.distributions import MultivariateNormal
@@ -11,5 +11,5 @@ x = theta + math.sqrt(0.1) * torch.randn_like(theta)
 inf = FMPE(prior, device="cuda")
 inf.append_simulations(theta, x).train(training_batch_size=200, max_num_epochs=4)
 d = inf.summary["epoch_durations_sec"]
-print(f"FMPE_GRAPH={os.environ.get('SBI_B200_FMPE_GRAPH','1')}: epoch times {[round(v,3) for v in d]}  "
+print(f"FMPE: epoch times {[round(v,3) for v in d]}  "
       f"val_loss {[round(v,4) for v in inf.summary['validation_loss']]}")

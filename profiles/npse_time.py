@@ -10,12 +10,10 @@ prior = MultivariateNormal(torch.zeros(D), 0.1 * torch.eye(D))
 theta = prior.sample((N,))
 x = theta + math.sqrt(0.1) * torch.randn_like(theta)
 for sde in ("ve", "vp"):
-    for graph in ("1", "0"):
-        os.environ["SBI_B200_NPSE_GRAPH"] = graph
-        inf = NPSE(prior, sde_type=sde, device="cuda")
-        inf.append_simulations(theta, x).train(training_batch_size=B, max_num_epochs=5, stop_after_epochs=100)
-        d = inf.summary["epoch_durations_sec"][1:]
-        n_train = int(0.9 * N)
-        steps = n_train // B
-        print(f"NPSE {sde} graph={graph}: {n_train * len(d) / sum(d) / 1e6:.2f} M samples/s, "
-              f"{1e3 * sum(d) / len(d) / steps:.3f} ms/step incl. validation, loss {inf.summary['training_loss'][-1]:.3f}")
+    inf = NPSE(prior, sde_type=sde, device="cuda")
+    inf.append_simulations(theta, x).train(training_batch_size=B, max_num_epochs=5, stop_after_epochs=100)
+    d = inf.summary["epoch_durations_sec"][1:]
+    n_train = int(0.9 * N)
+    steps = n_train // B
+    print(f"NPSE {sde}: {n_train * len(d) / sum(d) / 1e6:.2f} M samples/s, "
+          f"{1e3 * sum(d) / len(d) / steps:.3f} ms/step incl. validation, loss {inf.summary['training_loss'][-1]:.3f}")

@@ -3,9 +3,13 @@
     python profiles/trainer_trace.py --module sbi_b200.inference --out DIR      # one .pt per case
     python profiles/trainer_trace.py --compare DIR_A DIR_B                      # per-case differences
 
-Each case trains on a seeded linear-Gaussian task for a few epochs and writes the final flat parameters, the
-optimizer state (device Adam, or torch.optim.Adam on the multi-round path) and the summary without the epoch
-durations.  The "short" cases stop early, so the restore of the best weights runs too."""
+Each case trains on a seeded linear-Gaussian task for a few epochs and writes the network's state dict (the flat
+parameters, and the embedding nets' parameters and buffers), the optimizer state (device Adam, or
+torch.optim.Adam on the multi-round path) and the summary without the epoch durations.  The "short" cases stop
+early, so the restore of the best weights runs too.
+
+The NSF / MAF and flow-matching loss kernels sum the loss with float atomics, so the NPE, NLE and FMPE losses in
+the summary can differ in the last bits between two runs of the same code; parameters and optimizer state do not."""
 import argparse
 import glob
 import importlib
@@ -27,17 +31,21 @@ def task(n, D=3, seed=0):
     return prior, theta, theta + math.sqrt(0.1) * torch.randn_like(theta)
 
 
+def fc_embedding(D=3):
+    return torch.nn.Sequential(torch.nn.Linear(D, 16), torch.nn.ReLU(), torch.nn.Linear(16, 4))
+
+
 def cases(m):
+    from sbi_b200.flowmatching import posterior_flow_nn
+    from sbi_b200.neural_nets import posterior_nn
     kw = dict(training_batch_size=200, max_num_epochs=3, stop_after_epochs=1000)
     short = dict(training_batch_size=200, max_num_epochs=25, stop_after_epochs=2)
 
-    def fit(cls, n=4000, env=None, make=None, train=kw, resume=None, **ckw):
+    def fit(cls, n=4000, make=None, train=kw, resume=None, **ckw):
+        """`make()` returns more constructor arguments, built after the task's seed (e.g. an embedding net)."""
         def run():
-            for k in ("SBI_B200_NRE_GRAPH", "SBI_B200_FMPE_GRAPH", "SBI_B200_NPSE_GRAPH"):
-                os.environ.pop(k, None)
-            os.environ.update(env or {})
             prior, theta, x = task(n)
-            t = cls(prior, device="cuda", **ckw)
+            t = cls(prior, device="cuda", **ckw, **(make() if make is not None else {}))
             t.append_simulations(theta, x).train(**train)
             if resume is not None:
                 t.train(resume_training=True, **resume)
@@ -54,31 +62,32 @@ def cases(m):
         return t
 
     calib = dict(kw, calibration_kernel=lambda x: 1.0 / (1.0 + x.pow(2).sum(1)))
+    nsf_embed = lambda: dict(density_estimator=posterior_nn("nsf", embedding_net=fc_embedding()))         # noqa: E731
+    fm_embed = lambda: dict(density_estimator=posterior_flow_nn("mlp", embedding_net=fc_embedding()))     # noqa: E731
     return {
         "npe_nsf_tc_val": fit(m.NPE, n=20000),
+        "npe_nsf_embed": fit(m.NPE, make=nsf_embed),
         "npe_maf": fit(m.NPE, density_estimator="maf"),
         "npe_calibration": fit(m.NPE, train=calib),
         "npe_short": fit(m.NPE, train=short),
         "npe_resume": fit(m.NPE, resume=dict(training_batch_size=200, max_num_epochs=5, stop_after_epochs=1000)),
         "npe_two_rounds": two_rounds,
         "nle": fit(m.NLE),
+        "nle_maf": fit(m.NLE, density_estimator="maf"),
         "nle_short": fit(m.NLE, train=short),
-        "nreb_resnet_graph": fit(m.NRE_B, env={"SBI_B200_NRE_GRAPH": "1"}),
-        "nreb_resnet_eager": fit(m.NRE_B, env={"SBI_B200_NRE_GRAPH": "0"}),
-        "nreb_mlp_graph": fit(m.NRE_B, classifier="mlp", env={"SBI_B200_NRE_GRAPH": "1"}),
-        "nreb_mlp_eager": fit(m.NRE_B, classifier="mlp", env={"SBI_B200_NRE_GRAPH": "0"}),
-        "nreb_short": fit(m.NRE_B, env={"SBI_B200_NRE_GRAPH": "1"}, train=dict(short, stop_after_epochs=1)),
+        "nreb_resnet": fit(m.NRE_B),
+        "nreb_resnet_b5000": fit(m.NRE_B, n=20000, train=dict(kw, training_batch_size=5000)),
+        "nreb_mlp": fit(m.NRE_B, classifier="mlp"),
+        "nreb_short": fit(m.NRE_B, train=dict(short, stop_after_epochs=1)),
         "nreb_resume": fit(m.NRE_B, resume=dict(training_batch_size=200, max_num_epochs=5, stop_after_epochs=1000)),
         "nrea": fit(m.NRE_A),
         "bnre": fit(m.BNRE),
         "nrec": fit(m.NRE_C),
-        "fmpe_graph": fit(m.FMPE, env={"SBI_B200_FMPE_GRAPH": "1"}),
-        "fmpe_eager": fit(m.FMPE, env={"SBI_B200_FMPE_GRAPH": "0"}),
-        "fmpe_graph_noclip": fit(m.FMPE, env={"SBI_B200_FMPE_GRAPH": "1"}, train=dict(kw, clip_max_norm=None)),
-        "fmpe_eager_noclip": fit(m.FMPE, env={"SBI_B200_FMPE_GRAPH": "0"}, train=dict(kw, clip_max_norm=None)),
+        "fmpe": fit(m.FMPE),
+        "fmpe_embed": fit(m.FMPE, make=fm_embed),
+        "fmpe_noclip": fit(m.FMPE, train=dict(kw, clip_max_norm=None)),
         "fmpe_short_noclip": fit(m.FMPE, train=dict(short, clip_max_norm=None, max_num_epochs=40)),
-        "npse_ve_graph": fit(m.NPSE, sde_type="ve", env={"SBI_B200_NPSE_GRAPH": "1"}),
-        "npse_ve_eager": fit(m.NPSE, sde_type="ve", env={"SBI_B200_NPSE_GRAPH": "0"}),
+        "npse_ve": fit(m.NPSE, sde_type="ve"),
         "npse_ve_short": fit(m.NPSE, sde_type="ve", train=dict(short, max_num_epochs=40)),
     }
 
@@ -90,22 +99,27 @@ def dump(t):
     else:
         opt = [t._opt_state, t._opt_step]
     summary = {k: v for k, v in t.summary.items() if k != "epoch_durations_sec"}
-    return {"flat": t._neural_net.flat.data.cpu(), "opt": [v.cpu() for v in opt], "summary": summary}
+    state = {k: v.detach().cpu() for k, v in t._neural_net.state_dict().items()}
+    return {"flat": t._neural_net.flat.data.cpu(), "state": state, "opt": [v.cpu() for v in opt], "summary": summary}
 
 
 def compare(a, b):
     for f in sorted(glob.glob(os.path.join(a, "*.pt"))):
         x, y = torch.load(f), torch.load(os.path.join(b, os.path.basename(f)))
         d = (x["flat"] - y["flat"]).abs()
+        same_state = x["state"].keys() == y["state"].keys() and all(torch.equal(x["state"][k], y["state"][k])
+                                                                    for k in x["state"])
         same_opt = all(torch.equal(u, v) for u, v in zip(x["opt"], y["opt"]))
         sx, sy = x["summary"], y["summary"]
+        same_summary = all(len(sx[k]) == len(sy[k]) and all(u == v or (u != u and v != v) for u, v in zip(sx[k], sy[k]))
+                           for k in sx)
         sdiff = max((abs(u - v) / max(1.0, abs(v)) for k in sx for u, v in zip(sx[k], sy[k])
                      if u == u or v == v), default=0.0)
         same_len = all(len(sx[k]) == len(sy[k]) for k in sx)
-        print(f"{os.path.basename(f)[:-3]:22s} flat {'equal' if torch.equal(x['flat'], y['flat']) else 'DIFF '} "
-              f"opt {'equal' if same_opt else 'DIFF '} max|dflat| {d.max().item():.2e} "
-              f">5e-5 {100 * (d > 5e-5).float().mean().item():.4f}% summary rel {sdiff:.2e} "
-              f"epochs {sx['epochs_trained']} {'' if same_len else 'LENGTHS DIFFER'}")
+        print(f"{os.path.basename(f)[:-3]:22s} state {'equal' if same_state else 'DIFF '} "
+              f"opt {'equal' if same_opt else 'DIFF '} summary {'equal' if same_summary else 'DIFF '} "
+              f"max|dflat| {d.max().item():.2e} >5e-5 {100 * (d > 5e-5).float().mean().item():.4f}% "
+              f"summary rel {sdiff:.2e} epochs {sx['epochs_trained']} {'' if same_len else 'LENGTHS DIFFER'}")
 
 
 if __name__ == "__main__":

@@ -22,7 +22,6 @@ same graph capture (`_capture`); a trainer supplies the body of one epoch.
 from __future__ import annotations
 
 import math
-import os
 import time
 import warnings
 from copy import deepcopy
@@ -430,6 +429,39 @@ class _Trainer:
             self._reset_epochs()
         return _DeviceAdam(net, self._opt_state, self._opt_step, learning_rate, clip_max_norm, self._dp()[1])
 
+    def _rank_rows(self, B: int):
+        """This rank's share of a global batch of `B` rows: (rows it handles, offset of its first row in the
+        batch, rows behind one update).  With partition='global' the ranks split every batch; otherwise every
+        rank draws whole batches of its own."""
+        rank, world, glob = self._dp()
+        if not glob:
+            return B, 0, B * world
+        if B % world:
+            raise ValueError(f"partition='global' needs the batch size ({B}) divisible by the "
+                             f"number of ranks ({world})")
+        return B // world, rank * (B // world), B
+
+    def _epoch_orders(self, B: int, steps: int, Bv: int, vsteps: int):
+        """(perm_buf, vperm_buf, fill): static buffers for the rows of an epoch's `steps` training batches of `B`
+        and `vsteps` validation batches of `Bv`, and `fill()`, which draws the next epoch's orders into them
+        (base.py:499-563: reshuffled every epoch, `drop_last`).  With partition='global' every rank takes rank
+        0's orders."""
+        dev = self._device
+        glob = self._dp()[2]
+        train_idx, val_idx = self.train_indices.to(dev), self.val_indices.to(dev)
+        perm_buf = torch.empty(steps * B, dtype=torch.int64, device=dev)
+        vperm_buf = torch.empty(vsteps * Bv, dtype=torch.int64, device=dev)
+
+        def fill():
+            perm_buf.copy_(train_idx[torch.randperm(train_idx.shape[0], device=dev)[:steps * B]])
+            if vsteps > 0:
+                vperm_buf.copy_(val_idx[torch.randperm(val_idx.shape[0], device=dev)[:vsteps * Bv]])
+            if glob:
+                torch.distributed.broadcast(perm_buf, 0)
+                if vsteps > 0:
+                    torch.distributed.broadcast(vperm_buf, 0)
+        return perm_buf, vperm_buf, fill
+
     def _step_epochs(self, opt: _DeviceAdam, B: int, Bv: int, steps: int, vsteps: int,
                      train_step: Callable, val_step: Callable, graphs: bool) -> Callable:
         """Epochs of per-step launches (NRE, NPSE).  `train_step(idx)` / `val_step(idx)` read the batch rows
@@ -438,15 +470,12 @@ class _Trainer:
         launches that the host cannot issue as fast as the GPU runs them at small batches.  Random draws
         inside a graph use torch's graph-safe Philox offsets.  Returns the function that runs one epoch."""
         dev = self._device
-        train_idx, val_idx = self.train_indices.to(dev), self.val_indices.to(dev)
-        idx_buf = torch.zeros(B, dtype=torch.int64, device=dev)
-        vidx_buf = torch.zeros(max(Bv, 1), dtype=torch.int64, device=dev)
+        perm_buf, vperm_buf, fill = self._epoch_orders(B, steps, Bv, vsteps)
+        # the warm-up and capture run on the first rows of each split
+        idx_buf = self.train_indices[:B].to(dev)
+        vidx_buf = self.val_indices[:Bv].to(dev)
         run_train, run_val = (lambda: train_step(idx_buf)), (lambda: val_step(vidx_buf))
         if graphs and steps > 0 and opt.capturable:
-            idx_buf.copy_(train_idx[:B])
-            if vsteps > 0:
-                vidx_buf.copy_(val_idx[:Bv])
-
             def warmup():
                 for _ in range(3):
                     run_train()
@@ -458,13 +487,8 @@ class _Trainer:
                 run_val = captured[1].replay
 
         def epoch():
-            perm = train_idx[torch.randperm(train_idx.shape[0], device=dev)]
-            vperm = val_idx[torch.randperm(val_idx.shape[0], device=dev)] if vsteps > 0 else None
-            if self._dp()[2]:      # one epoch order for all ranks: rank 0's
-                torch.distributed.broadcast(perm, 0)
-                if vperm is not None:
-                    torch.distributed.broadcast(vperm, 0)
-            for buf, order, n, run in ((idx_buf, perm, steps, run_train), (vidx_buf, vperm, vsteps, run_val)):
+            fill()
+            for buf, order, n, run in ((idx_buf, perm_buf, steps, run_train), (vidx_buf, vperm_buf, vsteps, run_val)):
                 b = buf.shape[0]
                 for s in range(n):
                     buf.copy_(order[s * b:(s + 1) * b])
@@ -608,11 +632,7 @@ class _FlowTrainer(_Trainer):
             raise NotImplementedError("data-parallel training with an embedding net is not implemented")
         # a parameter-free or frozen embedding only transforms the condition: no condition gradient is needed
         train_emb = bool(_embedding_params(net))
-        if glob and B % world:
-            raise ValueError(f"partition='global' needs training_batch_size ({B}) divisible by the "
-                             f"number of ranks ({world})")
-        Bl = B // world if glob else B                 # rows this rank differentiates per step
-        Btot = B if glob else B * world                # rows behind one update
+        Bl, o_t, Btot = self._rank_rows(B)
         # validation rows: every rank evaluates its contiguous share of the epoch's validation order
         from .parallel import shard_range
         v_lo, v_hi = shard_range(vsteps * Bv, rank, world) if glob else (0, vsteps * Bv)
@@ -625,12 +645,7 @@ class _FlowTrainer(_Trainer):
         # Standardize + the user's module in torch; the VJP kernel returns the gradient of the embedded context
         cond_raw = (self._theta if self._swap else self._x) if embed else None
         emb = net.embedding_net
-        train_idx = self.train_indices.to(dev)
-        val_idx = self.val_indices.to(dev)
-        n_train, n_val = train_idx.shape[0], val_idx.shape[0]
-        # static buffers the epoch graph reads
-        perm_buf = torch.empty(steps * B, dtype=torch.int64, device=dev)
-        vperm_buf = torch.empty(max(vsteps * Bv, 1), dtype=torch.int64, device=dev)
+        perm_buf, vperm_buf, fill = self._epoch_orders(B, steps, Bv, vsteps)
         cond_tc = train_emb and net.vjp_cond_uses_tc(Bl)
         n_part = net.vjp_parts(Bl, param_grads_only=cond_tc or not train_emb)
         gpart = net._gpart(n_part)
@@ -656,8 +671,7 @@ class _FlowTrainer(_Trainer):
             if embed:
                 emb.train()
             for s in range(steps):
-                o = s * B + (rank * Bl if glob else 0)
-                idx = perm_buf[o:o + Bl]
+                idx = perm_buf[s * B + o_t:s * B + o_t + Bl]
                 if embed:
                     opt.zero_grad()
                     with torch.set_grad_enabled(train_emb):
@@ -701,25 +715,16 @@ class _FlowTrainer(_Trainer):
                     stats[2] = -(torch.where(fin, vlp, torch.zeros_like(vlp)) * w_all[vrows]).sum()
                     stats[3] = (~fin).sum().float()
 
-        def fill_perms():
-            perm_buf.copy_(train_idx[torch.randperm(n_train, device=dev)[:steps * B]])
-            if vsteps > 0:
-                vperm_buf.copy_(val_idx[torch.randperm(n_val, device=dev)[:vsteps * Bv]])
-            if glob:      # one epoch order for all ranks: rank 0's
-                torch.distributed.broadcast(perm_buf, 0)
-                if vsteps > 0:
-                    torch.distributed.broadcast(vperm_buf, 0)
-
         # warm-up (also sets kernel attributes) on a throw-away copy of the state, then capture
         run = run_epoch
         if opt.capturable:
             rng = torch.cuda.get_rng_state(dev)      # the warm-up's permutation draw leaves no trace:
-            fill_perms()                             # a seed gives the same run with and without graphs
+            fill()                                   # a seed gives the same run with and without graphs
             torch.cuda.set_rng_state(rng, dev)
             run = _capture(opt, run_epoch, run_epoch)[0].replay
 
         def epoch():
-            fill_perms()
+            fill()
             run()
             tl, vl = self._epoch_losses(stats)
             return tl / (steps * Btot), (vl / (vsteps * Bv * (1 if glob else world)) if vsteps > 0 else float("nan"))
@@ -959,7 +964,7 @@ class NRE_B(_PotentialPosterior, _Trainer):
               discard_prior_samples: bool = False, retrain_from_scratch: bool = False,
               show_train_summary: bool = False, dataloader_kwargs: Optional[dict] = None):
         dev = self._device
-        rank, world, glob = self._dp()
+        world = self._dp()[1]
         net, B, Bv, steps, vsteps = self._prepare(validation_fraction, training_batch_size, resume_training,
                                                   retrain_from_scratch)
         embs = net.embedding_nets
@@ -968,12 +973,10 @@ class NRE_B(_PotentialPosterior, _Trainer):
         self._x2d = self._x.reshape(self._x.shape[0], -1).contiguous()
         num_atoms = int(min(max(num_atoms, 2), min(B, Bv)))     # nre_base.py:236-238 (clamp to batch size)
         self._dp_agree(vsteps, "number of validation steps per epoch")
-        if glob and (B % world or Bv % world):
-            raise ValueError(f"partition='global' needs the batch sizes ({B}, {Bv}) divisible by the "
-                             f"number of ranks ({world})")
         # rows of each (global) batch whose loss this rank differentiates / evaluates
-        t_rows = (rank * (B // world), (rank + 1) * (B // world)) if glob else (0, B)
-        v_rows = (rank * (Bv // world), (rank + 1) * (Bv // world)) if glob else (0, Bv)
+        Bl, o_t, _ = self._rank_rows(B)
+        Bvl, o_v, _ = self._rank_rows(Bv)
+        t_rows, v_rows = (o_t, o_t + Bl), (o_v, o_v + Bvl)
         opt = self._optimizer(net, learning_rate, clip_max_norm, resume_training)
         train_sum = torch.zeros((), device=dev)
         val_sum = torch.zeros((), device=dev)
@@ -995,7 +998,7 @@ class NRE_B(_PotentialPosterior, _Trainer):
             with torch.no_grad():
                 val_sum.add_(self._loss_on(net, idx, num_atoms, rows=v_rows) / world)
 
-        graphs = os.environ.get("SBI_B200_NRE_GRAPH", "1") != "0" and B - 1 <= 4096
+        graphs = B - 1 <= 4096      # larger batches draw their contrastive rows with host syncs
         run_steps = self._step_epochs(opt, B, Bv, steps, vsteps, train_step, val_step, graphs)
 
         def epoch():
@@ -1103,7 +1106,7 @@ class FMPE(_Trainer):
               validation_times_nugget: float = 0.05, resume_training: bool = False, **kwargs):
         self._vf_check_rounds(kwargs)
         dev = self._device
-        rank, world, glob = self._dp()
+        world, glob = self._dp()[1:]
         net, B, Bv, steps, vsteps = self._prepare(validation_fraction, training_batch_size, resume_training)
         x2d = self._x.reshape(self._x.shape[0], -1).contiguous()
         D = net.layout.D
@@ -1113,23 +1116,16 @@ class FMPE(_Trainer):
         train_emb = bool(_embedding_params(net))      # False: a parameter-free or frozen embedding
         emb = net.embedding_net
         self._dp_agree(vsteps, "number of validation steps per epoch")
-        if glob and (B % world or Bv % world):
-            raise ValueError(f"partition='global' needs the batch sizes ({B}, {Bv}) divisible by the "
-                             f"number of ranks ({world})")
-        Bl, Bvl = (B // world, Bv // world) if glob else (B, Bv)    # rows of a batch this rank handles
-        o_t, o_v = (rank * Bl, rank * Bvl) if glob else (0, 0)
-        Btot = B if glob else B * world                              # rows behind one update
+        Bl, o_t, Btot = self._rank_rows(B)
+        Bvl, o_v, _ = self._rank_rows(Bv)
         vt = self._validation_times(net, validation_times, validation_times_nugget)
         opt = self._optimizer(net, learning_rate, clip_max_norm, resume_training)
         self._ema_loss_decay = ema_loss_decay
-        train_idx, val_idx = self.train_indices.to(dev), self.val_indices.to(dev)
-        n_train, n_val = train_idx.shape[0], val_idx.shape[0]
         loss_acc = torch.zeros(2, dtype=torch.float32, device=dev)
 
         # One CUDA graph per epoch: every step is [t ~ U, theta_1 ~ N draws, fused loss fwd+bwd kernel,
-        # reduce, clip+Adam]; the epoch's row permutations live in static buffers.
-        perm_buf = torch.zeros(max(steps * B, 1), dtype=torch.int64, device=dev)
-        vperm_buf = torch.zeros(max(vsteps * Bv, 1), dtype=torch.int64, device=dev)
+        # reduce, clip+Adam].
+        perm_buf, vperm_buf, fill = self._epoch_orders(B, steps, Bv, vsteps)
         stats = torch.zeros(4, dtype=torch.float32, device=dev)     # train loss sum, bad, val loss sum, bad
 
         # embedding net: the batch's x rows (event shape) go through Standardize + the user's module in torch; the
@@ -1178,21 +1174,13 @@ class FMPE(_Trainer):
                                      want_loss=False)
             stats[2:4].copy_(loss_acc)
 
-        def fill_perms():
-            perm_buf[:steps * B].copy_(train_idx[torch.randperm(n_train, device=dev)[:steps * B]])
-            if vsteps > 0:
-                vperm_buf[:vsteps * Bv].copy_(val_idx[torch.randperm(n_val, device=dev)[:vsteps * Bv]])
-            if glob:      # one epoch order for all ranks: rank 0's
-                torch.distributed.broadcast(perm_buf, 0)
-                torch.distributed.broadcast(vperm_buf, 0)
-
         run = run_epoch
-        if opt.capturable and os.environ.get("SBI_B200_FMPE_GRAPH", "1") != "0" and steps > 0:
-            fill_perms()
+        if opt.capturable and steps > 0:
+            fill()
             run = _capture(opt, run_epoch, run_epoch)[0].replay
 
         def epoch():
-            fill_perms()
+            fill()
             run()
             tl, vl = self._epoch_losses(stats)
             val_loss = vl / (vsteps * Bv * (1 if glob else world) * vt.shape[0]) if vsteps > 0 else float("nan")
@@ -1323,8 +1311,7 @@ class NPSE(FMPE):
                 stats[2] += ld.sum()
                 stats[3] += (~torch.isfinite(ld)).sum()
 
-        graphs = os.environ.get("SBI_B200_NPSE_GRAPH", "1") != "0"
-        run_steps = self._step_epochs(opt, B, Bv, steps, vsteps, train_step, val_step, graphs)
+        run_steps = self._step_epochs(opt, B, Bv, steps, vsteps, train_step, val_step, True)
 
         def epoch():
             stats.zero_()

@@ -18,7 +18,6 @@ from __future__ import annotations
 
 import ctypes as C
 import logging
-import os
 import time
 import warnings
 from typing import Any, Callable, Optional, Tuple, Union
@@ -54,7 +53,7 @@ class SliceSamplerVectorized:
         # graph=True: `check_every` lock-steps [potential -> state machine] are captured once as a CUDA graph
         # and replayed (the potential must be pure device work without host synchronisation: the estimator
         # potentials of sbi_b200.potentials with a device-resident prior are; a numpy callback is not)
-        self._graph = bool(graph) and os.environ.get("SBI_B200_SLICE_GRAPH", "1") != "0"
+        self._graph = bool(graph)
         self.num_potential_evals = 0
         if num_workers > 1:
             warn("Parallelization of vectorized slice sampling not implement, running serially.", stacklevel=2)

@@ -270,12 +270,11 @@ _graph_ref = {}
 
 @needs_ref
 @pytest.mark.parametrize("check_every", [1, 16])
-def test_graph_replay_equals_eager_equals_reference(cuda_lib, monkeypatch, check_every):
+def test_graph_replay_equals_eager_equals_reference(cuda_lib, check_every):
     """The production path: `check_every` lock-steps captured once as a CUDA graph and replayed, with a potential
     that never synchronises with the host.  Samples are bit-identical to the eager run and to the reference, and
     the host stops at the first check after the slowest chain's last lock-step."""
     from sbi_b200.samplers import SliceSamplerVectorized
-    monkeypatch.delenv("SBI_B200_SLICE_GRAPH", raising=False)
     target, D, Cn, kw, num_samples = _GRAPH_CASE
     seed, x0 = 99, initial_points(target, Cn, D, seed=1)
     runs = {}
