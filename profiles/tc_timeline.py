@@ -1,5 +1,10 @@
 """Phase timeline of CTA 0 of the tensor-core training pair (tuning build -DSBI_TC_TIMELINE).
-    python profiles/tc_timeline.py        # builds sbi_b200/lib/libsbi_b200_tl.so, runs B = 4096, prints deltas"""
+    python profiles/tc_timeline.py [--flush]    # builds sbi_b200/lib/libsbi_b200_tl.so, runs B = 4096, prints deltas
+--flush zeroes a 256 MiB buffer before the traced step, as bench.py does before every timed step, so that the
+prologue's index and row loads come from HBM; without it the traced step runs with a warm L2.
+Prologue markers: forward 1 entry, 2 bias table, 3 ld_const, 4 row gather, 6 first weight stage in; backward
+10 entry, 100 first weight stages requested.  They are thread 0's: work another warp still has in hand shows up at
+the next CTA barrier."""
 import ctypes as C, os, sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
@@ -36,6 +41,8 @@ for _ in range(3):
 torch.cuda.synchronize()
 for name in ("fwd", "bwd"):
     getattr(lib, f"sbi_b200_debug_timeline_{name}")(buf, 4096)          # reset
+if "--flush" in sys.argv:
+    torch.empty(256 << 20, dtype=torch.uint8, device="cuda").zero_()
 run()
 torch.cuda.synchronize()
 for name in ("fwd", "bwd"):

@@ -2,7 +2,7 @@
 tensor-core training step, as the trainer runs it: one step captured in a CUDA graph and replayed, at the bench
 model (cfg2: NSF dim 10) and 4096 / 32768 rows.  One torch.profiler trace (CUDA activities) of the replays;
 per chunk of the step it reports when the dW kernel starts relative to the backward's start and end, and how
-long dW runs on after the backward has ended.  A dW start at or after the backward's end means that the
+long dW runs on after the backward has ended, and when the backward starts relative to the forward's end.  A dW start at or after the backward's end means that the
 programmatic launch edge was lost (results stay correct, the overlap is gone).  The trace goes to OUT_DIR.
     python profiles/vjp_tc_overlap.py [OUT_DIR] [replays]"""
 import json
@@ -62,11 +62,16 @@ for B in (4096, 32768):
     with open(path) as fh:
         ev = [e for e in json.load(fh)["traceEvents"] if e.get("cat") == "kernel"]
     ev.sort(key=lambda e: e["ts"])
-    # pair every backward with the dW kernel that follows it (one pair per chunk of the step)
-    bwd, pairs = None, []
+    # pair every backward with the forward before it and the dW kernel after it (one triple per chunk of the step)
+    fwd, bwd, pairs, fb = None, None, [], []
     for e in ev:
-        if "nsf_vjp_tc_kernel" in e["name"]:
+        if "nsf_logprob_tc_kernel" in e["name"]:
+            fwd = e
+        elif "nsf_vjp_tc_kernel" in e["name"]:
             bwd = e
+            if fwd is not None:
+                fb.append((fwd, e))
+                fwd = None
         elif "nsf_dw_tc_kernel" in e["name"] and bwd is not None:
             pairs.append((bwd, e))
             bwd = None
@@ -81,4 +86,12 @@ for B in (4096, 32768):
         print(f"B={B} chunk {c}: backward {median(b_dur):.1f} us | dW starts {median(start_rel):.1f} us after the "
               f"backward's start, {median(start_vs_end):+.1f} us from its end | dW runs {median(d_dur):.1f} us, "
               f"{median(tail):.1f} us past the backward's end (medians of {len(ps)} replays)", flush=True)
+    # the backward is launched early behind the forward: its grid starts (first CTA resident) before the forward
+    # ends when SMs are free for it (half tiles)
+    for c in range(len(fb) // REPLAYS):
+        ps = fb[c::len(fb) // REPLAYS]
+        f_dur = [f["dur"] for f, _ in ps]
+        b_vs_end = [b["ts"] - (f["ts"] + f["dur"]) for f, b in ps]
+        print(f"B={B} chunk {c}: forward {median(f_dur):.1f} us | backward starts {median(b_vs_end):+.1f} us from "
+              f"the forward's end (medians of {len(ps)} replays)", flush=True)
     print("trace:", path, flush=True)

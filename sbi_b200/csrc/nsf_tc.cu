@@ -124,6 +124,7 @@ nsf_logprob_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_cons
   constexpr int kD = SAVE ? cDs : cD, kG = SAVE ? cGs : cG;
   float* as = sm + L.a;
   float* accs = sm + L.acc;
+  SBI_TL(1);
   IssuerT<kSlots, SAVE, RPC> iss =
       tc_begin<kSlots, SAVE, RPC>(full, sm + L.ring, tc, m.T, nunits, INV, ncols, sa, as, accs);
 
@@ -143,38 +144,77 @@ nsf_logprob_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_cons
 
   // all biases of the conditioners, once per CTA (zero beyond the real widths):
   //   per layer [b0 64 | per block: b1 64, b2 64, bc 64 | bf TRmax*32]
+  // kBatch entries per thread at a time: the layer-table loads of all of them, then their parameter loads, then
+  // the stores, so that a batch waits for two loads rather than two per entry (the evaluation kernels, 128
+  // registers, take one entry at a time)
   {
+    constexpr int kBatch = SAVE ? 8 : 1;
     float* bs = sm + L.bias;
-    for (int e = tid; e < m.T * L.bias_stride; e += kThreads) {
-      const int l = e / L.bias_stride, o = e % L.bias_stride;
-      const int* LT = m.d_layer_tab + l * SBI_NSF_LAYER_STRIDE;
-      float v = 0.f;
-      if (o < 64) {
-        if (o < H) v = __ldg(P + __ldg(LT + SBI_L_B0) + o);
-      } else if (o < 64 + m.NB * 192) {
+    const int n = m.T * L.bias_stride;
+    for (int e0 = tid; e0 < n; e0 += kBatch * kThreads) {
+      int src[kBatch];     // parameter index of the entry, or -1: zero
+#pragma unroll
+      for (int k = 0; k < kBatch; ++k) {
+        const int e = min(e0 + k * kThreads, n - 1);
+        const int l = e / L.bias_stride, o = e % L.bias_stride;
+        const int* LT = m.d_layer_tab + l * SBI_NSF_LAYER_STRIDE;
         const int b = (o - 64) / 192, w = ((o - 64) % 192) / 64, j = (o - 64) % 64;
-        if (j < H) v = __ldg(P + __ldg(LT + SBI_L_BLK0 + 6 * b + 1 + 2 * w) + j);
-      } else {
         const int q = o - 64 - m.NB * 192, f = q / 32, i = q % 32;
-        if (f < __ldg(LT + SBI_L_NTR) && i < 3 * KB - 1) v = __ldg(P + __ldg(LT + SBI_L_BF) + f * m.PR + i);
+        const int slot = o < 64 ? SBI_L_B0 : o < 64 + m.NB * 192 ? SBI_L_BLK0 + 6 * b + 1 + 2 * w : SBI_L_BF;
+        const int base = __ldg(LT + slot), ntr = __ldg(LT + SBI_L_NTR);
+        const bool ok = o < 64 ? o < H : o < 64 + m.NB * 192 ? j < H : f < ntr && i < 3 * KB - 1;
+        const int off = o < 64 ? o : o < 64 + m.NB * 192 ? j : f * m.PR + i;
+        src[k] = ok ? base + off : -1;
       }
-      bs[e] = v;
+      float v[kBatch];
+#pragma unroll
+      for (int k = 0; k < kBatch; ++k) v[k] = src[k] >= 0 ? __ldg(P + src[k]) : 0.f;
+#pragma unroll
+      for (int k = 0; k < kBatch; ++k)
+        if (e0 + k * kThreads < n) bs[e0 + k * kThreads] = v[k];
     }
   }
-  // batch-constant part of the log-density, summed in the order of lu_logdet_total (nsf.cuh)
+  SBI_TL(2);
+  // batch-constant part of the log-density, summed in the order of lu_logdet_total (nsf.cuh).  The training forward
+  // runs one tile per CTA, so this sits on its critical path: each warp of part 1 takes the layer-table entries of
+  // up to 32 layers at once (lane k: layer l0 + k), then per layer lane i < D the term of diagonal entry i, and the
+  // terms are added in feature order, the layer sums in layer order.  The evaluation kernels loop over many tiles
+  // per CTA and keep the serial loop, which needs fewer registers under their 128-register bound.
   float ld_const = 0.f;
   if (tq == 1) {
     float tot = 0.f;
-    for (int l = 0; l < m.T; ++l) {
-      const int* LT = m.d_layer_tab + l * SBI_NSF_LAYER_STRIDE;
-      float sacc = 0.f;
-      if (__ldg(LT + SBI_L_HAS_LU))
-        for (int i = 0; i < D; ++i)
-          sacc += logf(softplus_f(__ldg(P + __ldg(LT + SBI_L_LU_DIAG) + i)) + 1e-3f);
-      tot += sacc;
+    if constexpr (SAVE) {
+      const int lane = tid & 31;
+      for (int l0 = 0; l0 < m.T; l0 += 32) {
+        int has = 0, od = 0;
+        if (l0 + lane < m.T) {
+          const int* LT = m.d_layer_tab + (l0 + lane) * SBI_NSF_LAYER_STRIDE;
+          has = __ldg(LT + SBI_L_HAS_LU);
+          od = __ldg(LT + SBI_L_LU_DIAG);
+        }
+        for (int k = 0; k < 32 && l0 + k < m.T; ++k) {
+          const int hk = __shfl_sync(0xffffffffu, has, k), ok = __shfl_sync(0xffffffffu, od, k);
+          float term = 0.f;
+          if (hk && lane < D) term = logf(softplus_f(__ldg(P + ok + lane)) + 1e-3f);
+          float sacc = 0.f;
+          if (hk)
+            for (int i = 0; i < D; ++i) sacc += __shfl_sync(0xffffffffu, term, i);
+          tot += sacc;
+        }
+      }
+    } else {
+      for (int l = 0; l < m.T; ++l) {
+        const int* LT = m.d_layer_tab + l * SBI_NSF_LAYER_STRIDE;
+        float sacc = 0.f;
+        if (__ldg(LT + SBI_L_HAS_LU))
+          for (int i = 0; i < D; ++i)
+            sacc += logf(softplus_f(__ldg(P + __ldg(LT + SBI_L_LU_DIAG) + i)) + 1e-3f);
+        tot += sacc;
+      }
     }
     ld_const = INV ? (-tot - m.ld_zscore) : (tot + m.ld_zscore - 0.5f * (float)D * 1.8378770664093453f);
   }
+  SBI_TL(3);
 
   auto put_a4 = [&](int col, const float (&a)[4]) {
     if constexpr (SAVE) smem_a4<RPC>(as, row, col, a);
@@ -230,27 +270,59 @@ nsf_logprob_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_cons
     {
       const float* st = m.d_stats;
       const int Dp = m.Dp, Cp = m.Cp;
-      for (int e = tid; e < RPC * Dp; e += kThreads) {
-        const int r = e / Dp, d = e % Dp;
+      if constexpr (SAVE) {
+        // the training forward has one tile per CTA, so the gather sits on its critical path: each thread takes
+        // one row and every TPR-th input and context feature of it (Dp, Cp <= 16: sbi_b200_nsf_tc_supported); the
+        // row's index first, then all of its loads, then the stores.  (The evaluation kernels keep the loop below,
+        // which needs fewer registers under their 128-register bound.)
+        constexpr int kF = 16 / TPR;
+        const int r = tid % RPC, part = tid / RPC;
         const int64_t gr = row0 + r;
-        float val = 0.f;
-        if (d < D && gr < rows.R) {
-          const int64_t src = rows.d_index ? __ldg(rows.d_index + gr) : gr;
-          const float x = __ldg(rows.d_input + src * D + d);
-          val = INV ? x : __fadd_rn(__fmul_rn(x, __ldg(st + Dp + d)), __ldg(st + d));
+        const bool live = gr < rows.R;
+        const int64_t src = live && rows.d_index ? __ldg(rows.d_index + gr) : gr;
+        const int64_t csrc = rows.cond_shared ? 0 : src;
+        float xv[kF], xs[kF], xm[kF], cv[kF], cm[kF], cs[kF];
+#pragma unroll
+        for (int k = 0; k < kF; ++k) {
+          const int d = part + TPR * k;
+          const bool dok = live && d < D, cok = live && d < C;
+          xv[k] = dok ? __ldg(rows.d_input + src * D + d) : 0.f;
+          xs[k] = dok ? __ldg(st + Dp + d) : 0.f;
+          xm[k] = dok ? __ldg(st + d) : 0.f;
+          cv[k] = cok ? __ldg(rows.d_cond + csrc * C + d) : 0.f;
+          cm[k] = cok ? __ldg(st + 2 * Dp + d) : 0.f;
+          cs[k] = cok ? __ldg(st + 2 * Dp + Cp + d) : 1.f;
         }
-        zs[d * RPC + r] = val;
-      }
-      for (int e = tid; e < RPC * Cp; e += kThreads) {
-        const int r = e / Cp, c = e % Cp;
-        const int64_t gr = row0 + r;
-        float val = 0.f;
-        if (c < C && gr < rows.R) {
-          const int64_t src = rows.cond_shared ? 0 : (rows.d_index ? __ldg(rows.d_index + gr) : gr);
-          val = (__ldg(rows.d_cond + src * C + c) - __ldg(st + 2 * Dp + c)) / __ldg(st + 2 * Dp + Cp + c);
+#pragma unroll
+        for (int k = 0; k < kF; ++k) {
+          const int d = part + TPR * k;
+          if (d < Dp) zs[d * RPC + r] = live && d < D ? __fadd_rn(__fmul_rn(xv[k], xs[k]), xm[k]) : 0.f;
+          if (d < Cp) ctx_s[d * RPC + r] = live && d < C ? (cv[k] - cm[k]) / cs[k] : 0.f;
         }
-        ctx_s[c * RPC + r] = val;
+      } else {
+        for (int e = tid; e < RPC * Dp; e += kThreads) {
+          const int r = e / Dp, d = e % Dp;
+          const int64_t gr = row0 + r;
+          float val = 0.f;
+          if (d < D && gr < rows.R) {
+            const int64_t src = rows.d_index ? __ldg(rows.d_index + gr) : gr;
+            const float x = __ldg(rows.d_input + src * D + d);
+            val = INV ? x : __fadd_rn(__fmul_rn(x, __ldg(st + Dp + d)), __ldg(st + d));
+          }
+          zs[d * RPC + r] = val;
+        }
+        for (int e = tid; e < RPC * Cp; e += kThreads) {
+          const int r = e / Cp, c = e % Cp;
+          const int64_t gr = row0 + r;
+          float val = 0.f;
+          if (c < C && gr < rows.R) {
+            const int64_t src = rows.cond_shared ? 0 : (rows.d_index ? __ldg(rows.d_index + gr) : gr);
+            val = (__ldg(rows.d_cond + src * C + c) - __ldg(st + 2 * Dp + c)) / __ldg(st + 2 * Dp + Cp + c);
+          }
+          ctx_s[c * RPC + r] = val;
+        }
       }
+      SBI_TL(4);
       if (INV) prep_lu(m, m.T - 1, sm + L.lum);
       group_sync();
     }
@@ -343,6 +415,7 @@ nsf_logprob_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_cons
       hand_over();
       {
         iss.begin(__ldg(tab + 5 + 4 * stage));
+        if (li == 0) SBI_TL(6);
         uint32_t acc = 0u;
         iss.block(kD, 0, kid8 / 8, 0, 64, acc);
         iss.block(kD, 8 * KC0, nkc, 64 * kid8, 64, acc);

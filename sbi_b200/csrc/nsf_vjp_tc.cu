@@ -460,6 +460,7 @@ nsf_vjp_tc_kernel(const __grid_constant__ sbi_nsf_model m, const __grid_constant
   constexpr int ncols = RPC < kRows ? 0 : kColsDG;
   float* as = sm + L.a;
   float* accs = sm + L.acc;
+  SBI_TL(10);
   IssuerT<kBwdSlots, true, RPC> iss =
       tc_begin<kBwdSlots, true, RPC>(full, sm + L.ring, tcb, m.T, nunits, true, ncols, sa, as, accs);
   // half tiles: the weight-gradient kernel may start once every CTA of this grid is resident (it waits per unit)
