@@ -557,14 +557,6 @@ int sbi_b200_reject_compact(const float* d_cand, int32_t D, const float* d_log_t
                             const float* d_u, int64_t n, int64_t index_base, float* d_out, int64_t* d_out_idx,
                             int64_t cap, int32_t* d_count, int32_t* d_scratch, void* stream);
 
-/* The same compaction with the accept decision given as a byte mask (csrc/compact.cu; reference
- * sbi/samplers/rejection/rejection.py:369-384, `candidates[accept_reject_fn(candidates)]`): candidate i is
- * accepted when d_keep[i] != 0 (a torch bool tensor's bytes).  Same output, index, cap and count rules as
- * sbi_b200_reject_compact; d_scratch: sbi_b200_reject_scratch_ints(n) int32. */
-int sbi_b200_mask_compact(const float* d_cand, int32_t D, const uint8_t* d_keep, int64_t n, int64_t index_base,
-                          float* d_out, int64_t* d_out_idx, int64_t cap, int32_t* d_count, int32_t* d_scratch,
-                          void* stream);
-
 /* ---- sampling-importance-resampling: one categorical draw per group of K proposals (csrc/compact.cu; reference
  * sbi/samplers/importance/sir.py:59-63).  Candidates are (groups*K, D) rows; per group g, lw_k = log_target_k -
  * log_proposal_k (fp32), w = softmax(lw), and the selected candidate is the first k with cumsum(w)_k >= u_g.  A

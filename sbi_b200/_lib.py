@@ -260,8 +260,6 @@ _EXPORTS = {
     "sbi_b200_reject_compact": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64,
                                           C.c_int64, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p,
                                           C.c_void_p]),
-    "sbi_b200_mask_compact": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_int64, C.c_int64, C.c_void_p,
-                                        C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p]),
     "sbi_b200_sir_scratch_ints": (C.c_int64, [C.c_int64]),
     "sbi_b200_sir_select": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64,
                                       C.c_int32, C.c_int64, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p,

@@ -5,8 +5,7 @@
 // index; the running count stays on the device.  Three launches (flags + block counts, scan of the block
 // counts, scatter) replace exp / compare / boolean-index (whose `nonzero` synchronises the host) -- the
 // accepted set and its order are exactly those of the reference's boolean indexing.  The accept decision is a
-// predicate functor: the ratio test above (`reject_compact`) or a byte mask computed by the caller
-// (`mask_compact`, the `candidates[accept_reject_fn(candidates)]` of accept_reject_sample, rejection.py:369-384).
+// predicate functor, the ratio test above.
 #include <cuda_runtime.h>
 #include <math.h>
 #include <stdint.h>
@@ -21,18 +20,13 @@ constexpr int kThreads = 256;
 constexpr int kPer = 4;                       // consecutive candidates per thread
 constexpr int kTile = kThreads * kPer;        // candidates per block
 
-// Accept predicates of count_kernel / scatter_kernel: keep(i) says whether candidate i is accepted.
+// Accept predicate of count_kernel / scatter_kernel: keep(i) says whether candidate i is accepted.
 struct RatioAccept {
   const float* __restrict__ lt;
   const float* __restrict__ ls;
   const float* __restrict__ u;
   // same expression as the reference: exp(a - b) > u  (NaN compares false -> rejected)
   __device__ __forceinline__ bool operator()(int64_t i) const { return expf(lt[i] - ls[i]) > u[i]; }
-};
-
-struct MaskAccept {
-  const uint8_t* __restrict__ keep;           // a torch bool tensor's bytes: nonzero = accepted
-  __device__ __forceinline__ bool operator()(int64_t i) const { return keep[i] != 0; }
 };
 
 template <class Accept>
@@ -234,15 +228,6 @@ extern "C" int sbi_b200_reject_compact(const float* d_cand, int32_t D, const flo
     return SBI_EINVAL;
   return compact::compact(compact::RatioAccept{d_log_target, d_log_scaled, d_u}, d_cand, D, n, index_base, d_out,
                           d_out_idx, cap, d_count, d_scratch, (cudaStream_t)stream);
-}
-
-extern "C" int sbi_b200_mask_compact(const float* d_cand, int32_t D, const uint8_t* d_keep, int64_t n,
-                                     int64_t index_base, float* d_out, int64_t* d_out_idx, int64_t cap,
-                                     int32_t* d_count, int32_t* d_scratch, void* stream) {
-  if (!d_cand || !d_keep || !d_out || !d_count || !d_scratch || D < 1 || n < 0 || cap < 0) return SBI_EINVAL;
-  sbi::DeviceGuard dev_guard_(d_cand);
-  return compact::compact(compact::MaskAccept{d_keep}, d_cand, D, n, index_base, d_out, d_out_idx, cap, d_count,
-                          d_scratch, (cudaStream_t)stream);
 }
 
 // scratch: one count per block of kGroups groups, then the selected index of every group

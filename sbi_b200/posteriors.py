@@ -5,9 +5,10 @@
 mirrors /root/reference/sbi/samplers/rejection/rejection.py:230-457 (same adaptive batch-size
 rule :406-409, same truncation to the first `num_samples` accepted draws, same acceptance
 rate bookkeeping) and `within_support` /root/reference/sbi/utils/sbiutils.py:729-766.
-Proposals come out of the inverse-flow kernel; support checks and compaction are torch
-device ops (no per-iteration host list appends; one host sync per loop iteration for the
-remaining-count, as the loop's data-dependent trip count requires).
+`accept_reject_sample` is the one rejection loop of the direct and vector-field posteriors (one
+observation or a batch of them) and of `restriction.RestrictedPrior`.  Proposals come out of the
+inverse-flow kernel; support checks and the placement of accepted rows are torch device ops, with
+one host read per round, as the loop's data-dependent trip count requires.
 """
 from __future__ import annotations
 
@@ -88,109 +89,71 @@ def accept_reject_sample(
     sample_for_correction_factor: bool = False, max_sampling_batch_size: int = 10_000,
     proposal_sampling_kwargs: Optional[dict] = None, alternative_method: Optional[str] = None,
     max_sampling_time: Optional[float] = None, return_partial_on_timeout: bool = False,
-    **kwargs,
+    device: Optional[Union[str, torch.device]] = None, **kwargs,
 ) -> Tuple[Tensor, Tensor]:
-    """rejection.py:230-457: draw from `proposal`, keep what `accept_reject_fn` accepts, until
-    `num_samples` per observation are collected.  Returns (samples (num_samples, num_xos, D),
-    acceptance rate per observation)."""
+    """rejection.py:230-457: draw from `proposal`, keep what `accept_reject_fn` accepts, until `num_samples` per
+    observation are collected.  Returns (samples (num_samples, num_xos, *event), acceptance rate per observation).
+
+    `proposal(shape, **proposal_sampling_kwargs)` returns (batch, num_xos, D) draws, or (batch, D) for one
+    observation; with `device`, they are moved there before `accept_reject_fn` sees them.  Every accepted row is
+    written to its slot by a cumulative count per observation, so the samples are the first `num_samples` accepted
+    draws of every observation in draw order; rejected rows and those past `num_samples` go to one spare slot.
+    The float32 acceptance rates (accepted over drawn) are computed beside the accept decisions, or on the host when
+    `device` is given (as the reference computes them for its host-side proposals; a CUDA division by the drawn
+    count is not always the correctly rounded one).  One host read per round brings the counts and rates back:
+    `num_samples` minus the smallest count is what remains, and the smallest rate drives the reference's
+    batch-size rule and its low-acceptance warning.
+    After `max_sampling_time`, with `return_partial_on_timeout`, the first rows every observation has filled."""
     if kwargs:
         logging.warning(f"Unused arguments passed to accept_reject_sample: {list(kwargs)}")
     proposal_sampling_kwargs = proposal_sampling_kwargs or {}
-    num_remaining = num_samples
-    accepted = [[] for _ in range(num_xos)]
-    sampling_batch_size = min(num_samples, max_sampling_batch_size)
-    num_sampled_total = None
-    num_samples_possible = 0
+    num_remaining, drawn, batch = num_samples, 0, min(num_samples, max_sampling_batch_size)
     leakage_warning_raised = False
-    acceptance_rate = torch.full((num_xos,), float("nan"))
     start = time.time()
-    candidates = None
     while num_remaining > 0:
-        if max_sampling_time is not None and (time.time() - start) > max_sampling_time:
-            num_collected = min(sum(s.shape[0] for s in accepted[i]) for i in range(num_xos))
+        if drawn and max_sampling_time is not None and (time.time() - start) > max_sampling_time:
+            num_collected = num_samples - num_remaining
             if return_partial_on_timeout and num_collected > 0:
                 warnings.warn(f"Timeout exceeded after collecting {num_collected}/{num_samples}"
                               " samples. Returning partial results.", stacklevel=2)
-                samples = [torch.cat(accepted[i], dim=0)[:num_collected] for i in range(num_xos)]
-                return torch.stack(samples, dim=1), acceptance_rate
+                return out[:num_collected], rate.to(out.device)
             raise RuntimeError(
                 "Sampling aborted early because rejection sampling exceeded max_sampling_time. "
                 "This is likely due to extremely low acceptance.")
-        candidates = proposal(torch.Size((sampling_batch_size,)), **proposal_sampling_kwargs)
-        are_accepted = accept_reject_fn(candidates).reshape(sampling_batch_size, num_xos)
-        cands = candidates.reshape(sampling_batch_size, num_xos, *candidates.shape[candidates.ndim - 1:])
-        for i in range(num_xos):
-            accepted[i].append(cands[are_accepted[:, i], i])
-        num_accepted = are_accepted.sum(dim=0)
-        num_sampled_total = num_accepted.clone() if num_sampled_total is None else num_sampled_total + num_accepted
-        num_samples_possible += sampling_batch_size
-        min_num_accepted = int(num_accepted.min().item())   # the loop's one host sync
-        num_remaining -= min_num_accepted
-        acceptance_rate = num_sampled_total.float() / num_samples_possible
-        min_acceptance_rate = float(acceptance_rate.min().item())
-        sampling_batch_size = min(
-            max_sampling_batch_size,
-            max(int(1.5 * num_remaining / max(min_acceptance_rate, 1e-12)), 100))
-        if (num_samples_possible > (sampling_batch_size - 1) and min_acceptance_rate < warn_acceptance
-                and not leakage_warning_raised):
+        candidates = proposal(torch.Size((batch,)), **proposal_sampling_kwargs)
+        if device is not None:
+            candidates = candidates.to(device)
+        keep = accept_reject_fn(candidates).reshape(batch, num_xos)
+        cands = candidates.reshape(batch, num_xos, candidates.shape[-1])
+        if not drawn:
+            out = cands.new_empty((num_samples + 1, num_xos, cands.shape[-1]))     # row num_samples: the spare slot
+            accepted = torch.zeros(num_xos, dtype=torch.int64, device=keep.device)
+        count = torch.cumsum(keep, dim=0).add_(accepted)           # accepted so far, up to and including each row
+        slot = torch.where(keep, count - 1, num_samples).clamp_(max=num_samples)
+        out.scatter_(0, slot.unsqueeze(-1).expand_as(cands), cands)
+        accepted = count[-1]
+        drawn += batch
+        counts = accepted if device is None else accepted.cpu()
+        rate = counts.float() / drawn
+        stats = torch.cat((counts.double(), rate.double())).tolist()     # the round's one host read
+        num_remaining, min_rate = num_samples - int(min(stats[:num_xos])), min(stats[num_xos:])
+        batch = min(max_sampling_batch_size, max(int(1.5 * num_remaining / max(min_rate, 1e-12)), 100))
+        if drawn > (batch - 1) and min_rate < warn_acceptance and not leakage_warning_raised:
             if sample_for_correction_factor:
                 logging.warning(
                     f"Drawing samples from posterior to estimate the normalizing constant for "
-                    f"`log_prob()`. However, only {min_acceptance_rate:.3%} posterior samples are "
+                    f"`log_prob()`. However, only {min_rate:.3%} posterior samples are "
                     f"within the prior support. It may take a long time to collect the remaining "
                     f"{num_remaining} samples.")
             else:
-                msg = (f"Only {min_acceptance_rate:.3%} proposal samples are accepted. It may take "
+                msg = (f"Only {min_rate:.3%} proposal samples are accepted. It may take "
                        f"a long time to collect the remaining {num_remaining} samples.")
                 if alternative_method is not None:
                     msg += f" Alternatively, consider switching to `{alternative_method}`."
                 logging.warning(msg)
             leakage_warning_raised = True
-    samples = [torch.cat(accepted[i], dim=0)[:num_samples] for i in range(num_xos)]
-    samples = torch.stack(samples, dim=1)
-    samples = samples.reshape(num_samples, *candidates.shape[1:])
-    assert samples.shape[0] == num_samples
-    return samples, acceptance_rate.to(samples.device)
-
-
-@torch.no_grad()
-def accept_reject_batched(propose: Callable[[int], Tensor], prior, num_samples: int, B: int, D: int,
-                          max_sampling_batch_size: int, max_sampling_time: Optional[float] = None,
-                          return_partial_on_timeout: bool = False, device: str = "cuda") -> Tuple[Tensor, Tensor]:
-    """`accept_reject_sample` with `num_xos = B`, resolved on the device: `propose(n)` returns (n, B, D) draws for
-    all observations from one sampling launch; the accepted draws of each observation are placed by a cumulative
-    count, so a round costs one host sync whatever B is.  Returns ((num_samples, B, D) samples, acceptance rate per
-    observation); after a timeout with `return_partial_on_timeout`, the first rows every observation has filled."""
-    out = torch.empty(num_samples, B, D, dtype=torch.float32, device=device)
-    filled = torch.zeros(B, dtype=torch.int64, device=device)
-    drawn, accepted_total = 0, torch.zeros(B, dtype=torch.int64, device=device)
-    batch = min(num_samples, max_sampling_batch_size)
-    start = time.time()
-    while True:
-        cand = propose(batch)
-        ok = within_support(prior, cand.reshape(-1, D)).reshape(batch, B)
-        pos = torch.cumsum(ok.long(), dim=0) - 1 + filled.unsqueeze(0)            # slot of every accepted draw
-        valid = ok & (pos < num_samples)
-        sel = torch.nonzero(valid)                                                # the round's one host sync
-        out[pos[sel[:, 0], sel[:, 1]], sel[:, 1]] = cand[sel[:, 0], sel[:, 1]]
-        acc = ok.sum(0)
-        accepted_total += acc
-        drawn += batch
-        filled = torch.minimum(filled + acc, torch.full_like(filled, num_samples))
-        remaining = int((num_samples - filled).max().item())
-        if remaining <= 0:
-            break
-        if max_sampling_time is not None and (time.time() - start) > max_sampling_time:
-            n_ok = int(filled.min().item())
-            if return_partial_on_timeout and n_ok > 0:
-                warnings.warn(f"Timeout exceeded after collecting {n_ok}/{num_samples} samples. "
-                              "Returning partial results.", stacklevel=3)
-                return out[:n_ok], accepted_total.float() / drawn
-            raise RuntimeError("Sampling aborted early because rejection sampling exceeded max_sampling_time. "
-                               "This is likely due to extremely low acceptance.")
-        rate = float((accepted_total.float() / drawn).min().item())
-        batch = min(max_sampling_batch_size, max(int(1.5 * remaining / max(rate, 1e-12)), 100))
-    return out, accepted_total.float() / drawn
+    samples = out[:num_samples].reshape(num_samples, *candidates.shape[1:])
+    return samples, rate.to(samples.device)
 
 
 class DirectPosterior:
@@ -291,10 +254,12 @@ class DirectPosterior:
             max_sampling_batch_size = max(1, 4_000_000 // B)
         if not (reject_outside_prior and self.prior is not None):
             return est.sample(torch.Size([num_samples]), condition=x).reshape(*torch.Size(sample_shape), B, *est.input_shape)
-        propose = lambda n: est.sample(torch.Size([n]), condition=x).reshape(n, B, D)   # noqa: E731
-        out, self._last_acceptance_rate = accept_reject_batched(
-            propose, self.prior, num_samples, B, D, max_sampling_batch_size, max_sampling_time,
-            return_partial_on_timeout, self._device)
+        out, self._last_acceptance_rate = accept_reject_sample(
+            proposal=lambda shape: est.sample(shape, condition=x).reshape(shape[0], B, D),
+            accept_reject_fn=lambda theta: within_support(self.prior, theta.reshape(-1, D)),
+            num_samples=num_samples, num_xos=B, max_sampling_batch_size=max_sampling_batch_size,
+            alternative_method="build_posterior(..., sample_with='mcmc')", max_sampling_time=max_sampling_time,
+            return_partial_on_timeout=return_partial_on_timeout)
         if out.shape[0] < num_samples:          # partial result after a timeout
             return out
         return out.reshape(*torch.Size(sample_shape), B, *est.input_shape)
@@ -879,7 +844,8 @@ class VectorFieldPosterior:
             max_sampling_batch_size = capped
         eta = (predictor_params or {}).get("eta", 1.0)
 
-        def propose(n: int) -> Tensor:
+        def proposal(shape) -> Tensor:
+            n = shape[0]
             if self.sample_with == "sde":
                 s = sample_sde(est, n, x, steps=steps, ts=ts, eta=eta, corrector=corrector,
                                corrector_params=corrector_params, batched=True)
@@ -890,9 +856,11 @@ class VectorFieldPosterior:
             return s
 
         if not (reject_outside_prior and self.prior is not None):
-            return propose(num_samples).reshape(*torch.Size(sample_shape), B, *est.input_shape)
-        samples, _ = accept_reject_batched(propose, self.prior, num_samples, B, D, max_sampling_batch_size,
-                                           max_sampling_time, return_partial_on_timeout, self._device)
+            return proposal((num_samples,)).reshape(*torch.Size(sample_shape), B, *est.input_shape)
+        samples, _ = accept_reject_sample(
+            proposal=proposal, accept_reject_fn=lambda theta: within_support(self.prior, theta.reshape(-1, D)),
+            num_samples=num_samples, num_xos=B, max_sampling_batch_size=max_sampling_batch_size,
+            max_sampling_time=max_sampling_time, return_partial_on_timeout=return_partial_on_timeout)
         if samples.shape[0] < num_samples:          # partial result after a timeout
             return samples
         return samples.reshape(*torch.Size(sample_shape), B, *est.input_shape)

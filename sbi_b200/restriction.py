@@ -1,23 +1,22 @@
 """Truncated sequential NPE (TSNPE, Deistler et al. 2022): the prior restricted to a posterior's high-density region.
 
 `get_density_thresholder` and `RestrictedPrior` mirror the reference's sbi/utils/restriction_estimator.py:484-521
-and :613-846.  The restricted prior's rejection loop follows `accept_reject_sample`
+and :613-846.  The restricted prior's rejection sampling runs through `posteriors.accept_reject_sample`
 (sbi/samplers/rejection/rejection.py:230-457) for one observation, draw for draw: the user's prior draws each batch
-on its own generator, `accept_reject_fn` decides on the device, and one compaction launch sequence
-(`sbi_b200_mask_compact`, csrc/compact.cu) appends the accepted rows in draw order behind those already collected.  The host reads the running count once per batch; the reference's
-boolean indexing synchronises there too, and keeps a Python list of accepted chunks.
+on its own generator, the draws move to the CUDA device, `accept_reject_fn` decides there and the accepted rows are
+collected there in draw order.  The acceptance rate is computed on the host in the reference's float32 arithmetic,
+wherever the prior draws.
 """
 from __future__ import annotations
 
-import logging
 import sys
-from typing import Any, Callable, Optional, Tuple
+from typing import Any, Callable, Optional
 
 import torch
 from torch import Tensor
 from torch.distributions import Distribution
 
-from . import _lib as L
+from .posteriors import accept_reject_sample
 
 
 def get_density_thresholder(dist: Any, quantile: float = 1e-4,
@@ -45,54 +44,6 @@ def _compute_device(device: str) -> torch.device:
                            "(no CPU fallback)")
     d = torch.device(device)
     return d if d.type == "cuda" and d.index is not None else torch.device("cuda", torch.cuda.current_device())
-
-
-@torch.no_grad()
-def _accept_reject_on_device(draw: Callable[[int], Tensor], accept_reject_fn: Callable, num_samples: int,
-                             max_sampling_batch_size: int, device: torch.device, warn_acceptance: float = 0.01,
-                             alternative_method: Optional[str] = None) -> Tuple[Tensor, float]:
-    """`accept_reject_sample` (rejection.py:230-457) for one observation with the accepted rows collected on
-    `device`: returns the first `num_samples` accepted draws as (num_samples, D) float32, in draw order, and the
-    acceptance rate (accepted over drawn, in the reference's float32 arithmetic, which also drives its batch-size
-    rule).  `draw(n)` returns n candidates; `accept_reject_fn` sees them on `device` and returns one bool each."""
-    if num_samples < 1:
-        raise ValueError(f"num_samples must be positive, got {num_samples}")
-    if num_samples + max_sampling_batch_size > 2 ** 31 - 1:
-        raise ValueError("num_samples + max_sampling_batch_size must stay below 2**31 (the device count is int32)")
-    lib = L.load()
-    out = count = scratch = None
-    num_accepted = torch.zeros(1)           # float32, as the reference accumulates it
-    num_drawn = total = 0
-    warned = False
-    batch = min(num_samples, max_sampling_batch_size)
-    with torch.cuda.device(device):
-        while num_samples - total > 0:
-            cand = draw(batch)
-            cand = cand.reshape(batch, -1).to(device=device, dtype=torch.float32).contiguous()
-            keep = accept_reject_fn(cand).reshape(batch).to(device=device, dtype=torch.bool).contiguous()
-            if out is None:
-                out = torch.empty(num_samples, cand.shape[1], dtype=torch.float32, device=device)
-                count = torch.zeros(1, dtype=torch.int32, device=device)
-                scratch = torch.empty(int(lib.sbi_b200_reject_scratch_ints(max_sampling_batch_size)),
-                                      dtype=torch.int32, device=device)
-            L.check(lib.sbi_b200_mask_compact(cand.data_ptr(), cand.shape[1], keep.data_ptr(), batch, num_drawn,
-                                              out.data_ptr(), None, num_samples, count.data_ptr(),
-                                              scratch.data_ptr(), L.stream_ptr()), "mask_compact")
-            new_total = int(count.item())   # the round's one host sync
-            num_accepted += new_total - total
-            total = new_total
-            num_drawn += batch
-            num_remaining = num_samples - total
-            rate = (num_accepted / num_drawn).item()
-            batch = min(max_sampling_batch_size, max(int(1.5 * num_remaining / max(rate, 1e-12)), 100))
-            if num_drawn > batch - 1 and rate < warn_acceptance and not warned:
-                msg = (f"Only {rate:.3%} proposal samples are accepted. It may take "
-                       f"a long time to collect the remaining {num_remaining} samples.")
-                if alternative_method is not None:
-                    msg += f" Alternatively, consider switching to `{alternative_method}`."
-                logging.warning(msg)
-                warned = True
-    return out, rate
 
 
 def _process_device(device: Optional[str]) -> str:
@@ -137,9 +88,15 @@ class RestrictedPrior(Distribution):
         sample_with = self._sample_with if sample_with is None else sample_with
         dev = _compute_device(self._device)
         if sample_with == "rejection":
-            samples, acceptance_rate = _accept_reject_on_device(
-                lambda n: self._prior.sample((n,)), self._accept_reject_fn, num_samples, max_sampling_batch_size,
-                dev, alternative_method="sample_with='sir'")
+            if num_samples < 1:
+                raise ValueError(f"num_samples must be positive, got {num_samples}")
+            with torch.cuda.device(dev):
+                samples, rate = accept_reject_sample(
+                    lambda shape: self._prior.sample(shape).reshape(shape[0], -1).to(torch.float32),
+                    lambda theta: self._accept_reject_fn(theta).to(device=dev, dtype=torch.bool),
+                    num_samples, max_sampling_batch_size=max_sampling_batch_size,
+                    alternative_method="sample_with='sir'", device=dev)
+            acceptance_rate = rate.item()
             if save_acceptance_rate:
                 self.acceptance_rate = torch.as_tensor(acceptance_rate)
             if print_rejected_frac:

@@ -1,7 +1,7 @@
-"""TSNPE on the GPU: the mask compaction kernel (csrc/compact.cu) against boolean indexing, `RestrictedPrior`
-rejection and SIR sampling against torch restatements of the reference's loops (rejection.py:230-457, sir.py:13-71)
-on the same seed and the same prior object, the density thresholder against its defining expression, and the
-truncated sequential loop on the linear-Gaussian task against the analytic posterior."""
+"""TSNPE on the GPU: `RestrictedPrior` rejection and SIR sampling against torch restatements of the reference's
+loops (rejection.py:230-457, sir.py:13-71) on the same seed and the same prior object, the density thresholder
+against its defining expression, and the truncated sequential loop on the linear-Gaussian task against the analytic
+posterior."""
 import inspect
 import math
 import warnings
@@ -15,51 +15,6 @@ from tests.helpers import b200_from_oracle, oracle_nsf
 pytestmark = pytest.mark.gpu
 D = 3
 MARGIN = 1e-5
-
-
-def _compact(cand, keep, base, out, out_idx, count):
-    from sbi_b200 import _lib as L
-    lib = L.load()
-    n = cand.shape[0]
-    scratch = torch.empty(int(lib.sbi_b200_reject_scratch_ints(n)), dtype=torch.int32, device="cuda")
-    L.check(lib.sbi_b200_mask_compact(cand.data_ptr(), cand.shape[1], keep.data_ptr(), n, base, out.data_ptr(),
-                                      L.ptr(out_idx), out.shape[0], count.data_ptr(), scratch.data_ptr(),
-                                      L.stream_ptr()), "mask_compact")
-
-
-@pytest.mark.parametrize("Dc", [1, 3, 10])
-def test_mask_compact_equals_boolean_indexing(cuda_lib, Dc):
-    """Accepted rows, their order and their global indices equal `cand[keep]` / `nonzero(keep)` over several
-    appended rounds: rounds with nothing accepted, rounds with everything accepted, rounds that are not a multiple
-    of the block tile, and the capacity cut (overflow is counted, not stored)."""
-    g = torch.Generator().manual_seed(Dc)
-    cap = 150_000
-    out = torch.full((cap, Dc), float("nan"), device="cuda")
-    out_idx = torch.full((cap,), -1, dtype=torch.int64, device="cuda")
-    count = torch.zeros(1, dtype=torch.int32, device="cuda")
-    want_rows, want_idx, base = [], [], 0
-    rounds = [(1, 0.0), (1, 1.0), (1023, 0.3), (5000, 0.0), (4097, 1.0), (100_003, 0.01), (300_001, 0.6),
-              (2, 0.0), (777, 0.5)]
-    for n, p in rounds:
-        cand = torch.randn(n, Dc, generator=g).cuda()
-        keep = (torch.rand(n, generator=g) < p).cuda()
-        _compact(cand, keep, base, out, out_idx, count)
-        want_rows.append(cand[keep])
-        want_idx.append(torch.nonzero(keep).reshape(-1) + base)
-        base += n
-        total = sum(r.shape[0] for r in want_rows)
-        assert int(count.item()) == total
-        k = min(total, cap)
-        assert torch.equal(out[:k], torch.cat(want_rows)[:k]) and torch.equal(out_idx[:k], torch.cat(want_idx)[:k])
-    assert int(count.item()) > cap and not out.isnan().any()
-    # without the index output
-    out2 = torch.full((cap, Dc), float("nan"), device="cuda")
-    count2 = torch.zeros(1, dtype=torch.int32, device="cuda")
-    cand = torch.randn(20_000, Dc, generator=g).cuda()
-    keep = (torch.rand(20_000, generator=g) < 0.5).cuda()
-    _compact(cand, keep, 0, out2, None, count2)
-    k = int(count2.item())
-    assert torch.equal(out2[:k], cand[keep]) and out2[k:].isnan().all()
 
 
 def _posterior(prior, x_o, seed=0):
@@ -78,9 +33,17 @@ def _gauss():
     return MultivariateNormal(torch.zeros(D), 4.0 * torch.eye(D))
 
 
+def _box_cuda():
+    return Independent(Uniform(-4 * torch.ones(D, device="cuda"), 4 * torch.ones(D, device="cuda")), 1)
+
+
+def _gauss_cuda():
+    return MultivariateNormal(torch.zeros(D, device="cuda"), 4.0 * torch.eye(D, device="cuda"))
+
+
 def _restated_accept_reject(prior, fn, num_samples, max_batch):
-    """rejection.py:310-457 for one observation: proposal draws on the prior's own generator, boolean indexing,
-    the float32 acceptance bookkeeping and the adaptive batch size."""
+    """rejection.py:310-457 for one observation: proposal draws on the prior's own generator (on the prior's
+    device), boolean indexing, the float32 acceptance bookkeeping on the CPU and the adaptive batch size."""
     accepted = []
     num_sampled_total = torch.zeros(1)
     num_samples_possible = 0
@@ -89,7 +52,7 @@ def _restated_accept_reject(prior, fn, num_samples, max_batch):
     while num_remaining > 0:
         cand = prior.sample((batch,))
         are_accepted = fn(cand).reshape(batch, 1).cpu()
-        accepted.append(cand.reshape(batch, 1, -1)[are_accepted[:, 0], 0])
+        accepted.append(cand.reshape(batch, 1, -1)[are_accepted[:, 0].to(cand.device), 0])
         num_accepted = are_accepted.sum(dim=0)
         num_sampled_total += num_accepted
         num_samples_possible += batch
@@ -99,7 +62,7 @@ def _restated_accept_reject(prior, fn, num_samples, max_batch):
     return torch.cat(accepted)[:num_samples], rate
 
 
-@pytest.mark.parametrize("make_prior", [_box, _gauss])
+@pytest.mark.parametrize("make_prior", [_box, _gauss, _box_cuda, _gauss_cuda])
 def test_rejection_sampling_equals_reference_loop(cuda_lib, make_prior, capsys, caplog):
     from sbi_b200.restriction import RestrictedPrior, get_density_thresholder
     prior = make_prior()
@@ -115,7 +78,7 @@ def test_rejection_sampling_equals_reference_loop(cuda_lib, make_prior, capsys, 
         torch.manual_seed(5)
         want, rate = _restated_accept_reject(prior, thr, n, max_batch)
         assert got.shape == (n, D) and got.device.type == "cuda"
-        assert torch.equal(got.cpu(), want), (n, max_batch)
+        assert torch.equal(got.cpu(), want.cpu()), (n, max_batch)
         assert torch.equal(rp.acceptance_rate, torch.as_tensor(rate)) and 0 < rate < 0.5
         assert thr(got).all()
         printed = capsys.readouterr().out
