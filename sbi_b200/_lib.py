@@ -1,13 +1,15 @@
 """ctypes binding of the C-ABI library (include/sbi_b200.h).
 
 The product path has NO CPU fallback: if the shared library is missing or no sm_90 device
-is present, calls raise.  PyTorch is used only for device memory and streams; kernels are
-launched through the C ABI with raw device pointers on torch's current CUDA stream.
+is present, calls raise.  PyTorch is used only for device memory and streams; every kernel is
+launched through `call`, with raw device pointers, on torch's current stream of the device its
+tensors live on.
 """
 from __future__ import annotations
 
 import ctypes as C
 import os
+from typing import Optional
 
 import torch
 
@@ -197,136 +199,140 @@ class PeerCtx(C.Structure):
     _fields_ = [("h_peer_ptrs", C.c_void_p), ("world", C.c_int), ("rank", C.c_int), ("d_grad_local", C.c_void_p)]
 
 
+class _Stream(C.c_void_p):
+    """The trailing `void* stream` of an entry point that launches kernels (filled in by `call`)."""
+
+
 _EXPORTS = {
     "sbi_b200_abi_version": (C.c_int, []),
     "sbi_b200_device_ok": (C.c_int, []),
     "sbi_b200_nsf_logprob": (C.c_int, [C.POINTER(NsfModel), C.POINTER(Rows), C.c_void_p,
-                                       C.c_void_p, C.c_void_p]),
+                                       C.c_void_p, _Stream]),
     "sbi_b200_nsf_vjp_parts": (C.c_int, [C.c_int64]),
     "sbi_b200_nsf_vjp_save_bytes": (C.c_int64, [C.POINTER(NsfModel), C.c_int64]),
     "sbi_b200_nsf_vjp": (C.c_int, [C.POINTER(NsfModel), C.POINTER(Rows), C.c_void_p, C.c_float,
                                    C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
-                                   C.c_void_p, C.c_int64, C.c_void_p]),
+                                   C.c_void_p, C.c_int64, _Stream]),
     "sbi_b200_nsf_inverse": (C.c_int, [C.POINTER(NsfModel), C.POINTER(Rows), C.c_void_p,
-                                       C.c_void_p, C.c_void_p]),
+                                       C.c_void_p, _Stream]),
     "sbi_b200_nsf_tc_supported": (C.c_int, [C.POINTER(NsfModel), C.POINTER(NsfTc)]),
-    "sbi_b200_nsf_tc_pack": (C.c_int, [C.POINTER(NsfModel), C.POINTER(NsfTc), C.c_void_p]),
+    "sbi_b200_nsf_tc_pack": (C.c_int, [C.POINTER(NsfModel), C.POINTER(NsfTc), _Stream]),
     "sbi_b200_nsf_logprob_tc": (C.c_int, [C.POINTER(NsfModel), C.POINTER(NsfTc), C.POINTER(Rows),
-                                          C.c_void_p, C.c_void_p, C.c_void_p]),
+                                          C.c_void_p, C.c_void_p, _Stream]),
     "sbi_b200_nsf_inverse_tc": (C.c_int, [C.POINTER(NsfModel), C.POINTER(NsfTc), C.POINTER(Rows),
-                                          C.c_void_p, C.c_void_p, C.c_void_p]),
+                                          C.c_void_p, C.c_void_p, _Stream]),
     "sbi_b200_nsf_vjp_tc_supported": (C.c_int, [C.POINTER(NsfModel), C.POINTER(NsfTc), C.POINTER(NsfTc)]),
     "sbi_b200_nsf_vjp_tc_parts": (C.c_int, [C.c_int64]),
     "sbi_b200_nsf_vjp_tc_save_bytes": (C.c_int64, [C.POINTER(NsfModel), C.c_int64]),
     "sbi_b200_nsf_vjp_tc": (C.c_int, [C.POINTER(NsfModel), C.POINTER(NsfTc), C.POINTER(NsfTc), C.POINTER(Rows),
                                       C.c_void_p, C.c_float, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
-                                      C.c_int64, C.c_void_p]),
+                                      C.c_int64, _Stream]),
     "sbi_b200_nsf_vjp_tc_cond": (C.c_int, [C.POINTER(NsfModel), C.POINTER(NsfTc), C.POINTER(NsfTc), C.POINTER(Rows),
                                            C.c_void_p, C.c_float, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
-                                           C.c_void_p, C.c_int64, C.c_void_p]),
+                                           C.c_void_p, C.c_int64, _Stream]),
     "sbi_b200_maf_logprob": (C.c_int, [C.POINTER(MafModel), C.POINTER(Rows), C.c_void_p,
-                                       C.c_void_p, C.c_void_p]),
+                                       C.c_void_p, _Stream]),
     "sbi_b200_maf_vjp_parts": (C.c_int, [C.c_int64]),
     "sbi_b200_maf_vjp": (C.c_int, [C.POINTER(MafModel), C.POINTER(Rows), C.c_void_p, C.c_float,
                                    C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
-                                   C.c_void_p]),
+                                   _Stream]),
     "sbi_b200_maf_inverse": (C.c_int, [C.POINTER(MafModel), C.POINTER(Rows), C.c_void_p,
-                                       C.c_void_p, C.c_void_p]),
-    "sbi_b200_ratio_forward": (C.c_int, [C.POINTER(RatioModel), C.POINTER(Pairs), C.c_void_p, C.c_void_p]),
+                                       C.c_void_p, _Stream]),
+    "sbi_b200_ratio_forward": (C.c_int, [C.POINTER(RatioModel), C.POINTER(Pairs), C.c_void_p, _Stream]),
     "sbi_b200_ratio_tc_supported": (C.c_int, [C.POINTER(RatioModel), C.POINTER(NsfTc)]),
-    "sbi_b200_ratio_tc_pack": (C.c_int, [C.POINTER(RatioModel), C.POINTER(NsfTc), C.c_void_p]),
+    "sbi_b200_ratio_tc_pack": (C.c_int, [C.POINTER(RatioModel), C.POINTER(NsfTc), _Stream]),
     "sbi_b200_ratio_forward_tc": (C.c_int, [C.POINTER(RatioModel), C.POINTER(NsfTc), C.POINTER(Pairs),
-                                            C.c_void_p, C.c_void_p]),
+                                            C.c_void_p, _Stream]),
     "sbi_b200_ratio_vjp_parts": (C.c_int, [C.c_int64]),
     "sbi_b200_ratio_vjp": (C.c_int, [C.POINTER(RatioModel), C.POINTER(Pairs), C.c_void_p, C.c_void_p,
-                                     C.c_void_p, C.c_void_p, C.c_void_p]),
+                                     C.c_void_p, C.c_void_p, _Stream]),
     "sbi_b200_ratio_vjp_inputs": (C.c_int, [C.POINTER(RatioModel), C.POINTER(Pairs), C.c_void_p, C.c_void_p,
-                                            C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+                                            C.c_void_p, C.c_void_p, C.c_void_p, _Stream]),
     "sbi_b200_pair_rows_sum": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p,
-                                         C.c_void_p]),
-    "sbi_b200_ratio_mlp_forward": (C.c_int, [C.POINTER(RatioMlpModel), C.POINTER(Pairs), C.c_void_p, C.c_void_p]),
+                                         _Stream]),
+    "sbi_b200_ratio_mlp_forward": (C.c_int, [C.POINTER(RatioMlpModel), C.POINTER(Pairs), C.c_void_p, _Stream]),
     "sbi_b200_ratio_mlp_vjp_parts": (C.c_int, [C.c_int64]),
     "sbi_b200_ratio_mlp_vjp": (C.c_int, [C.POINTER(RatioMlpModel), C.POINTER(Pairs), C.c_void_p, C.c_void_p,
-                                         C.c_void_p, C.c_void_p, C.c_void_p]),
+                                         C.c_void_p, C.c_void_p, _Stream]),
     "sbi_b200_fm_net_vjp": (C.c_int, [C.POINTER(FmModel), C.POINTER(Rows), C.c_void_p, C.c_void_p, C.c_void_p,
-                                      C.c_void_p]),
+                                      _Stream]),
     "sbi_b200_fm_plan": (C.c_int, [C.POINTER(FmModel), C.c_int32, C.POINTER(C.c_int32)]),
     "sbi_b200_fm_forward_div": (C.c_int, [C.POINTER(FmModel), C.POINTER(Rows), C.c_void_p, C.c_int32, C.c_void_p,
-                                          C.c_void_p, C.c_void_p]),
-    "sbi_b200_made_sample": (C.c_int, [C.POINTER(NsfModel), C.POINTER(Rows), C.c_void_p, C.c_void_p, C.c_void_p]),
+                                          C.c_void_p, _Stream]),
+    "sbi_b200_made_sample": (C.c_int, [C.POINTER(NsfModel), C.POINTER(Rows), C.c_void_p, C.c_void_p, _Stream]),
     "sbi_b200_sde_em_step": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p,
-                                       C.c_float, C.c_float, C.c_float, C.c_void_p]),
+                                       C.c_float, C.c_float, C.c_float, _Stream]),
     "sbi_b200_reject_scratch_ints": (C.c_int64, [C.c_int64]),
     "sbi_b200_reject_compact": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64,
                                           C.c_int64, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p,
-                                          C.c_void_p]),
+                                          _Stream]),
     "sbi_b200_sir_scratch_ints": (C.c_int64, [C.c_int64]),
     "sbi_b200_sir_select": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64,
                                       C.c_int32, C.c_int64, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p,
-                                      C.c_void_p, C.c_void_p]),
+                                      C.c_void_p, _Stream]),
     "sbi_b200_mmd_ws_bytes": (C.c_int64, [C.c_int32]),
     "sbi_b200_mmd": (C.c_int, [C.c_void_p, C.c_int64, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p, C.c_int32,
                                C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p,
-                               C.c_void_p]),
+                               _Stream]),
     "sbi_b200_rbf_matrix": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_int32, C.c_double,
-                                      C.c_void_p, C.c_void_p]),
+                                      C.c_void_p, _Stream]),
     "sbi_b200_lc2st_plan":(C.c_int, [C.POINTER(Lc2stNet), C.POINTER(C.c_int32)]),
     "sbi_b200_lc2st_ws_floats": (C.c_int64, [C.POINTER(Lc2stNet), C.c_int32]),
     "sbi_b200_lc2st_train": (C.c_int, [C.POINTER(Lc2stNet), C.POINTER(Lc2stOpt), C.c_void_p, C.c_int32,
                                        C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p,
                                        C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
-                                       C.c_void_p, C.c_void_p]),
+                                       C.c_void_p, _Stream]),
     "sbi_b200_lc2st_eval_chunks": (C.c_int, [C.POINTER(Lc2stNet), C.c_int64]),
     "sbi_b200_lc2st_eval": (C.c_int, [C.POINTER(Lc2stNet), C.c_void_p, C.c_int32, C.c_int32, C.c_void_p,
                                       C.c_int32, C.c_int64, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p,
-                                      C.c_void_p, C.c_void_p, C.c_void_p]),
+                                      C.c_void_p, C.c_void_p, _Stream]),
     "sbi_b200_ode_red_size": (C.c_int, [C.c_int64]),
     "sbi_b200_ode_stage": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_int32, C.c_void_p,
-                                     C.c_void_p]),
+                                     _Stream]),
     "sbi_b200_ode_error_commit": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p,
-                                            C.c_void_p]),
+                                            _Stream]),
     "sbi_b200_fm_forward": (C.c_int, [C.POINTER(FmModel), C.POINTER(Rows), C.c_void_p, C.c_int32, C.c_void_p,
-                                      C.c_void_p]),
+                                      _Stream]),
     "sbi_b200_fm_vjp_parts": (C.c_int, [C.c_int64]),
     "sbi_b200_fm_loss_vjp": (C.c_int, [C.POINTER(FmModel), C.POINTER(Rows), C.c_void_p, C.c_void_p, C.c_void_p,
-                                       C.c_float, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+                                       C.c_float, C.c_void_p, C.c_void_p, C.c_void_p, _Stream]),
     "sbi_b200_fm_loss_vjp_cond": (C.c_int, [C.POINTER(FmModel), C.POINTER(Rows), C.c_void_p, C.c_void_p,
                                             C.c_void_p, C.c_float, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
-                                            C.c_void_p]),
-    "sbi_b200_slice_init": (C.c_int, [C.POINTER(SliceChains), C.c_void_p, C.c_void_p]),
-    "sbi_b200_slice_step": (C.c_int, [C.POINTER(SliceChains), C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
-    "sbi_b200_hmc_init": (C.c_int, [C.POINTER(HmcChains), C.c_void_p]),
-    "sbi_b200_hmc_step": (C.c_int, [C.POINTER(HmcChains), C.c_void_p, C.c_void_p]),
+                                            _Stream]),
+    "sbi_b200_slice_init": (C.c_int, [C.POINTER(SliceChains), C.c_void_p, _Stream]),
+    "sbi_b200_slice_step": (C.c_int, [C.POINTER(SliceChains), C.c_void_p, C.c_void_p, C.c_void_p, _Stream]),
+    "sbi_b200_hmc_init": (C.c_int, [C.POINTER(HmcChains), _Stream]),
+    "sbi_b200_hmc_step": (C.c_int, [C.POINTER(HmcChains), C.c_void_p, _Stream]),
     "sbi_b200_reduce_partials": (C.c_int, [C.c_void_p, C.c_int, C.c_int64, C.c_void_p,
-                                           C.c_void_p]),
-    "sbi_b200_nll_stats": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p]),
+                                           _Stream]),
+    "sbi_b200_nll_stats": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, _Stream]),
     "sbi_b200_sumsq_blocks": (C.c_int, [C.c_int64]),
     "sbi_b200_reduce_partials_norm": (C.c_int, [C.c_void_p, C.c_int, C.c_int64, C.c_void_p, C.c_void_p,
-                                                C.c_void_p, C.c_void_p]),
+                                                C.c_void_p, _Stream]),
     "sbi_b200_adam_clip_step_norm": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                                C.c_void_p, C.c_int64, C.c_float, C.c_float, C.c_float,
                                                C.c_float, C.c_float, C.c_float, C.c_void_p, C.c_int,
-                                               C.c_void_p]),
+                                               _Stream]),
     "sbi_b200_adam_clip_step": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                           C.c_void_p, C.c_int64, C.c_float, C.c_float, C.c_float,
-                                          C.c_float, C.c_float, C.c_float, C.c_void_p]),
+                                          C.c_float, C.c_float, C.c_float, _Stream]),
     "sbi_b200_nsf_train_step_host": (C.c_int, [C.POINTER(NsfModel), C.POINTER(TrainWs), C.c_void_p,
                                                C.c_void_p, C.c_int64, C.c_float, C.c_float,
                                                C.c_float, C.c_float, C.c_float, C.c_void_p,
-                                               C.c_void_p]),
+                                               _Stream]),
     "sbi_b200_pipe_create": (C.c_void_p, []),
     "sbi_b200_pipe_destroy": (None, [C.c_void_p]),
     "sbi_b200_nsf_train_step_host_async": (C.c_int, [C.POINTER(NsfModel), C.POINTER(TrainWs), C.c_void_p,
                                                      C.c_void_p, C.c_void_p, C.c_int64, C.c_float, C.c_float,
-                                                     C.c_float, C.c_float, C.c_float, C.c_void_p, C.c_void_p]),
+                                                     C.c_float, C.c_float, C.c_float, C.c_void_p, _Stream]),
     "sbi_b200_pipe_drain": (C.c_int, [C.c_void_p, C.c_void_p]),
     "sbi_b200_nsf_train_step_host_async_dp": (C.c_int, [C.POINTER(NsfModel), C.POINTER(TrainWs), C.c_void_p,
                                                         C.POINTER(PeerCtx), C.c_void_p, C.c_void_p, C.c_int64,
                                                         C.c_float, C.c_float, C.c_float, C.c_float, C.c_float,
-                                                        C.c_void_p, C.c_void_p]),
+                                                        C.c_void_p, _Stream]),
     "sbi_b200_nsf_logprob_host": (C.c_int, [C.POINTER(NsfModel), C.POINTER(TrainWs), C.c_void_p,
                                             C.c_void_p, C.c_int64, C.c_int, C.c_void_p,
-                                            C.c_void_p]),
+                                            _Stream]),
     "sbi_b200_peer_bytes": (C.c_int64, [C.c_int64]),
     "sbi_b200_peer_blocks": (C.c_int, [C.c_int64]),
     "sbi_b200_peer_alloc": (C.c_void_p, [C.c_int64]),
@@ -335,14 +341,16 @@ _EXPORTS = {
     "sbi_b200_peer_import": (C.c_void_p, [C.c_void_p]),
     "sbi_b200_peer_close": (C.c_int, [C.c_void_p]),
     "sbi_b200_peer_sum": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int64, C.c_void_p,
-                                    C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+                                    C.c_void_p, C.c_void_p, C.c_void_p, _Stream]),
     "sbi_b200_peer_error": (C.c_int, [C.c_void_p, C.c_int64]),
     "sbi_b200_nsf_logprob_host_tc": (C.c_int, [C.POINTER(NsfModel), C.POINTER(NsfTc), C.POINTER(TrainWs),
                                                C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.c_void_p,
-                                               C.c_void_p]),
+                                               _Stream]),
 }
 
 _lib = None
+# `call`'s names: the entry points whose last parameter is the stream, without the `sbi_b200_` prefix
+_LAUNCH = {name[len("sbi_b200_"):]: name for name, (_, args) in _EXPORTS.items() if args and args[-1] is _Stream}
 
 
 def exported_symbols():
@@ -369,40 +377,73 @@ def load():
     return _lib
 
 
+SBI_EINVAL, SBI_ESMEM = -1, -2
+
+
 class SbiB200Error(RuntimeError):
-    pass
+    """A failed entry point; `rc` is its status (SBI_ESMEM or a CUDA error), None for a check made on the host."""
+
+    def __init__(self, msg: str, rc: Optional[int] = None):
+        super().__init__(msg)
+        self.rc = rc
 
 
 def check(rc: int, what: str):
     if rc == 0:
         return
-    if rc == -1:
+    if rc == SBI_EINVAL:
         raise ValueError(f"{what}: invalid argument (SBI_EINVAL)")
-    if rc == -2:
-        raise SbiB200Error(f"{what}: model does not fit the shared-memory budget (SBI_ESMEM)")
-    raise SbiB200Error(f"{what}: CUDA error {rc}")
+    if rc == SBI_ESMEM:
+        raise SbiB200Error(f"{what}: model does not fit the shared-memory budget (SBI_ESMEM)", rc)
+    raise SbiB200Error(f"{what}: CUDA error {rc}", rc)
 
 
-_active_device = None    # device of the tensors the next kernel launch works on
+def call(name: str, *args, device=None):
+    """Launch `sbi_b200_<name>` on torch's current stream of the device its tensor arguments live on (`device`
+    when it has none, e.g. a struct-only call), and raise on a failed status.  Tensors are passed as their data
+    pointers; None, numbers, ctypes structs (by reference where the prototype takes a pointer) and arrays as they
+    are.  The C side makes that device current for the launch (csrc/device.cuh), so the current device does not
+    matter.  Raises before anything launches for a CPU tensor or for tensors on two devices."""
+    sym = _LAUNCH.get(name)
+    if sym is None:
+        raise ValueError(f"sbi_b200_{name} launches no kernel (its last parameter is not the stream): "
+                         "call it on `load()`")
+    dev = -1
+    if device is not None:
+        device = torch.device(device)
+        if device.type != "cuda":
+            raise RuntimeError(f"sbi_b200: {name} was asked to run on {device}; the kernels only run on a CUDA "
+                               "(sm_90a) device and there is no CPU fallback")
+        dev = torch.cuda.current_device() if device.index is None else device.index
+    argv = []
+    for a in args:
+        if isinstance(a, torch.Tensor):
+            if not a.is_cuda:
+                require_cuda(a, f"a tensor argument of {name}")
+            d = a.get_device()
+            if dev < 0:
+                dev = d
+            elif d != dev:
+                raise ValueError(f"{name}: arguments on cuda:{dev} and cuda:{d}; one launch works on one device")
+            a = a.data_ptr()
+        argv.append(a)
+    if dev < 0:
+        raise ValueError(f"{name}: no tensor argument to take the device from; pass device=")
+    rc = getattr(_lib or load(), sym)(*argv, torch.cuda.current_stream(dev).cuda_stream)
+    if rc:
+        check(rc, name)
 
 
-def stream_ptr() -> int:
-    """torch's current stream ON THE DEVICE OF THE TENSORS last passed to `require_cuda` (every
-    launch path validates its parameters / inputs with it first), not on whatever device happens
-    to be current: an estimator on cuda:1 launches on cuda:1's stream while cuda:0 is current.
-    The C entry points make that device current themselves (csrc/device.cuh)."""
-    if _active_device is None:
-        return torch.cuda.current_stream().cuda_stream
-    return torch.cuda.current_stream(_active_device).cuda_stream
+def stream_ptr(device=None) -> int:
+    """torch's current stream on `device` (default: the current device), for raw calls outside `call`."""
+    return torch.cuda.current_stream(device).cuda_stream
 
 
 def require_cuda(t: torch.Tensor, name: str):
-    global _active_device
     if not t.is_cuda:
         raise RuntimeError(
             f"sbi_b200: `{name}` lives on {t.device}; the kernels only run on a CUDA (sm_90a) "
             "device and there is no CPU fallback")
-    _active_device = t.device
     return t
 
 
@@ -410,8 +451,32 @@ def ptr(t):
     return None if t is None else C.c_void_p(t.data_ptr())
 
 
+def rows(inp: torch.Tensor, cond: torch.Tensor, index: Optional[torch.Tensor] = None, n: Optional[int] = None,
+         shared: bool = False) -> Rows:
+    """`Rows` over the tensors: input rows `inp` and condition rows `cond` (`cond[0]` for every row when `shared`),
+    gathered through the optional int64 row `index`; n rows, by default as many as `index`, else `inp` has.
+    The struct keeps the tensors alive."""
+    if n is None:
+        n = (inp if index is None else index).shape[0]
+    r = Rows(inp.data_ptr(), cond.data_ptr(), None if index is None else index.data_ptr(), n, 1 if shared else 0)
+    r._keep = (inp, cond, index)
+    return r
+
+
+def pairs(theta: torch.Tensor, x: torch.Tensor, ti: Optional[torch.Tensor] = None, xi: Optional[torch.Tensor] = None,
+          n: Optional[int] = None, x_shared: bool = False) -> Pairs:
+    """`Pairs` (theta[ti[r]], x[xi[r]]) over the tensors (row r of each without its index, `x[0]` for every pair
+    when `x_shared`); n pairs, by default as many as `ti`, else `theta` has.  The struct keeps the tensors alive."""
+    if n is None:
+        n = (theta if ti is None else ti).shape[0]
+    p = Pairs(theta.data_ptr(), x.data_ptr(), None if ti is None else ti.data_ptr(),
+              None if xi is None else xi.data_ptr(), n, 1 if x_shared else 0)
+    p._keep = (theta, x, ti, xi)
+    return p
+
+
 def reduce_partials(gpart: torch.Tensor, n_part: int, n_params: int) -> torch.Tensor:
     """The sum of the first `n_part` partial-gradient slabs of `gpart`, as a fresh (n_params,) tensor."""
     g = torch.empty(n_params, dtype=torch.float32, device=gpart.device)
-    check(load().sbi_b200_reduce_partials(ptr(gpart), n_part, n_params, ptr(g), stream_ptr()), "reduce_partials")
+    call("reduce_partials", gpart, n_part, n_params, g)
     return g

@@ -224,15 +224,20 @@ class _PackedEstimator(nn.Module):
         """Family-specific scalars of the model struct."""
 
     def _entry(self, name: str):
-        """The layout's C entry point `sbi_b200_<prefix>_<name>`."""
+        """The layout's query entry point `sbi_b200_<prefix>_<name>` (one that launches nothing, e.g. `vjp_parts`)."""
         return getattr(L.load(), f"sbi_b200_{self._family.prefix}_{name}")
 
-    def _check_rc(self, rc: int, what: str):
-        if rc == -2:
+    def _call(self, name: str, *args):
+        """`L.call` of `sbi_b200_<name>` on the parameters' device; a model that no row tile fits is named in the
+        error."""
+        try:
+            L.call(name, *args, device=self.net.flat.device)
+        except L.SbiB200Error as err:
+            if err.rc != L.SBI_ESMEM:
+                raise
             raise L.SbiB200Error(
-                f"{what}: a row tile of this {self._family.what.format(**vars(self.layout))} needs more than "
-                "the 227 KB of shared memory one CTA can use on sm_90a (SBI_ESMEM)")
-        L.check(rc, what)
+                f"{name}: a row tile of this {self._family.what.format(**vars(self.layout))} needs more than "
+                "the 227 KB of shared memory one CTA can use on sm_90a (SBI_ESMEM)", err.rc) from None
 
     def _gpart(self, n_part: int) -> Tensor:
         """Partial-gradient scratch, (>= n_part, n_params), zeroed when (re)allocated."""
@@ -264,10 +269,9 @@ class _PackedEstimator(nn.Module):
             return None
         desc = L.NsfTc(st["plan"]["n_words"], st["plan"]["stage_cap"], st["src"].data_ptr(),
                        st["tab"].data_ptr(), st["tcw"].data_ptr())
-        lib = L.load()
-        if not getattr(lib, f"sbi_b200_{tc}_tc_supported")(C.byref(m), C.byref(desc)):
+        if not getattr(L.load(), f"sbi_b200_{tc}_tc_supported")(C.byref(m), C.byref(desc)):
             return None
-        L.check(getattr(lib, f"sbi_b200_{tc}_tc_pack")(C.byref(m), C.byref(desc), L.stream_ptr()), f"{tc}_tc_pack")
+        self._call(f"{tc}_tc_pack", m, desc)
         return desc
 
 
@@ -436,7 +440,6 @@ class FlowEstimator(_PackedEstimator):
     def inverse_flow(self, noise: Tensor, condition: Tensor, reps: int = 1):
         """x = T^{-1}(noise | condition); `noise` (B*reps, D) condition-major,
         `condition` (B, *condition_shape).  Returns (x, log|det dx/dnoise|)."""
-        lib = L.load()
         L.require_cuda(noise, "noise")
         Bc = condition.shape[0]
         ctx = self._embed(condition.to(noise.device)).contiguous().float()
@@ -448,15 +451,13 @@ class FlowEstimator(_PackedEstimator):
         out = torch.empty_like(noise)
         lad = torch.empty(R, dtype=torch.float32, device=noise.device)
         m = self._model(nbuf=2)
-        rows = L.Rows(noise.data_ptr(), ctx.data_ptr(), None, R, 1 if shared else 0)
+        rows = L.rows(noise, ctx, shared=shared)
         if R >= self.TC_MIN_ROWS or os.environ.get("SBI_B200_TC", "") == "1":
             tc = self._tc_state(m)
             if tc is not None:
-                L.check(lib.sbi_b200_nsf_inverse_tc(C.byref(m), C.byref(tc), C.byref(rows), L.ptr(out),
-                                                L.ptr(lad), L.stream_ptr()), "nsf_inverse_tc")
+                self._call("nsf_inverse_tc", m, tc, rows, out, lad)
                 return out, lad
-        self._check_rc(self._entry("inverse")(C.byref(m), C.byref(rows), L.ptr(out), L.ptr(lad), L.stream_ptr()),
-                       f"{self.layout.family}_inverse")
+        self._call(f"{self._family.prefix}_inverse", m, rows, out, lad)
         return out, lad
 
     # ---- tensor-core bulk path (nsf only) --------------------------------------------------------
@@ -492,17 +493,16 @@ class FlowEstimator(_PackedEstimator):
             self._cache["tc_train"] = st
         if not st["ok"]:
             return None
-        lib = L.load()
         both = L.NsfTc(st["nf"] + st["nb"], st["cap_f"], st["src"].data_ptr(), st["tab_f"].data_ptr(),
                        st["tcw"].data_ptr())
         tcf = L.NsfTc(st["nf"], st["cap_f"], st["src"].data_ptr(), st["tab_f"].data_ptr(), st["tcw"].data_ptr())
         tcb = L.NsfTc(st["nb"], st["cap_b"], st["src"].data_ptr() + 4 * st["nf"], st["tab_b"].data_ptr(),
                       st["tcw"].data_ptr() + 4 * st["nf"])
-        if not lib.sbi_b200_nsf_vjp_tc_supported(C.byref(m), C.byref(tcf), C.byref(tcb)):
+        if not L.load().sbi_b200_nsf_vjp_tc_supported(C.byref(m), C.byref(tcf), C.byref(tcb)):
             st["ok"] = False
             return None
         if pack:
-            L.check(lib.sbi_b200_nsf_tc_pack(C.byref(m), C.byref(both), L.stream_ptr()), "nsf_tc_pack")
+            self._call("nsf_tc_pack", m, both)
         return tcf, tcb, both
 
     def vjp_parts(self, R: int, param_grads_only: bool = True) -> int:
@@ -553,21 +553,16 @@ class FlowEstimator(_PackedEstimator):
             if tcs is not None:
                 save, nbytes = self._vjp_save(lib.sbi_b200_nsf_vjp_tc_save_bytes(C.byref(m), R))
                 if gcond is not None:
-                    L.check(lib.sbi_b200_nsf_vjp_tc_cond(
-                        C.byref(m), C.byref(tcs[0]), C.byref(tcs[1]), C.byref(rows), L.ptr(gout), g_const, L.ptr(logp),
-                        L.ptr(gpart), L.ptr(loss_acc), L.ptr(gcond), save, nbytes, L.stream_ptr()),
-                        "nsf_vjp_tc_cond")
+                    self._call("nsf_vjp_tc_cond", m, tcs[0], tcs[1], rows, gout, g_const, logp, gpart, loss_acc, gcond,
+                               save, nbytes)
                     return
-                L.check(lib.sbi_b200_nsf_vjp_tc(C.byref(m), C.byref(tcs[0]), C.byref(tcs[1]), C.byref(rows), L.ptr(gout),
-                                                g_const, L.ptr(logp), L.ptr(gpart), L.ptr(loss_acc), save, nbytes,
-                                                L.stream_ptr()), "nsf_vjp_tc")
+                self._call("nsf_vjp_tc", m, tcs[0], tcs[1], rows, gout, g_const, logp, gpart, loss_acc, save, nbytes)
                 return
-        args = (C.byref(m), C.byref(rows), L.ptr(gout), g_const, L.ptr(logp), L.ptr(gpart), L.ptr(ginput),
-                L.ptr(gcond), L.ptr(loss_acc))
-        if self._family.prefix == "nsf":       # `nsf` and `made`: the SIMT kernel spills its activations
-            save, nbytes = self._vjp_save(lib.sbi_b200_nsf_vjp_save_bytes(C.byref(m), R))
-            args += (save, nbytes)
-        self._check_rc(self._entry("vjp")(*args, L.stream_ptr()), f"{self.layout.family}_vjp")
+        prefix = self._family.prefix
+        args = (m, rows, gout, g_const, logp, gpart, ginput, gcond, loss_acc)
+        if prefix == "nsf":       # `nsf` and `made`: the SIMT kernel spills its activations
+            args += self._vjp_save(lib.sbi_b200_nsf_vjp_save_bytes(C.byref(m), R))
+        self._call(f"{prefix}_vjp", *args)
 
     # ---- raw kernel entry (no autograd) --------------------------------------------------------------
     def _logprob_raw(self, inp: Tensor, ctx: Tensor, shared: bool, want_noise=False,
@@ -576,23 +571,19 @@ class FlowEstimator(_PackedEstimator):
         """Log-probs (and with `want_noise` the base-space noise) of R rows, R = n_rows or len(inp), with the
         condition of row r at ctx[r] (ctx[0] when `shared`) and optional row `index`; written into `out` (R,) if
         given.  wgmma kernel from TC_MIN_ROWS rows when the model fits it, else the SIMT kernel."""
-        lib = L.load()
         L.require_cuda(inp, "input")
         L.require_cuda(ctx, "condition")
         R = inp.shape[0] if n_rows is None else n_rows
         lp = torch.empty(R, dtype=torch.float32, device=inp.device) if out is None else out
         noise = torch.empty(R, self.layout.D, dtype=torch.float32, device=inp.device) if want_noise else None
         m = self._model(nbuf=2, raw_condition=raw_condition)
-        rows = L.Rows(inp.data_ptr(), ctx.data_ptr(),
-                      None if index is None else index.data_ptr(), R, 1 if shared else 0)
+        rows = L.rows(inp, ctx, index, R, shared)
         if R >= self.TC_MIN_ROWS or os.environ.get("SBI_B200_TC", "") == "1":
             tc = self._tc_state(m)
             if tc is not None:
-                L.check(lib.sbi_b200_nsf_logprob_tc(C.byref(m), C.byref(tc), C.byref(rows), L.ptr(lp),
-                                                    L.ptr(noise), L.stream_ptr()), "nsf_logprob_tc")
+                self._call("nsf_logprob_tc", m, tc, rows, lp, noise)
                 return lp, noise
-        self._check_rc(self._entry("logprob")(C.byref(m), C.byref(rows), L.ptr(lp), L.ptr(noise), L.stream_ptr()),
-                       f"{self.layout.family}_logprob")
+        self._call(f"{self._family.prefix}_logprob", m, rows, lp, noise)
         return lp, noise
 
 
@@ -615,7 +606,7 @@ class _NsfLogProb(torch.autograd.Function):
         ginp = torch.empty_like(inp) if need_inp else None
         gcond = torch.empty(R, cond.shape[1], dtype=torch.float32, device=inp.device) if need_cond else None
         m = est._model(nbuf=3)
-        rows = L.Rows(inp.data_ptr(), cond.data_ptr(), None, R, 1 if shared else 0)
+        rows = L.rows(inp, cond, shared=shared)
         g = g.contiguous().float()
         est.vjp(m, rows, R, g, 0.0, None, gpart, ginp, gcond, None)
         gflat = L.reduce_partials(gpart, n_part, est.layout.n_params) if need_flat else None
@@ -664,7 +655,6 @@ class MadeEstimator(FlowEstimator):
         (csrc/nsf.cu `made_sample_kernel`); the normal draws and the component-selecting uniforms come from
         torch on the parameter device, condition-major like nflows (`repeat_interleave(context, n)`)."""
         self._check_condition_shape(condition)
-        lib = L.load()
         dev = self.net.flat.device
         Bc = condition.shape[0]
         n = torch.Size(sample_shape).numel()
@@ -678,9 +668,7 @@ class MadeEstimator(FlowEstimator):
             ctx = ctx.repeat_interleave(n, dim=0).contiguous()
         out = torch.empty(R, Dn, dtype=torch.float32, device=dev)
         m = self._model(nbuf=2)
-        rows = L.Rows(noise.data_ptr(), ctx.data_ptr(), None, R, 1 if shared else 0)
-        L.check(lib.sbi_b200_made_sample(C.byref(m), C.byref(rows), unif.data_ptr(), out.data_ptr(), L.stream_ptr()),
-                "made_sample")
+        self._call("made_sample", m, L.rows(noise, ctx, shared=shared), unif, out)
         x = out[:, 1:].reshape(Bc, n, Dn - 1).transpose(0, 1)
         return x.reshape((*sample_shape, Bc, *self.input_shape))
 

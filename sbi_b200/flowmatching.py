@@ -12,7 +12,6 @@ samplers/ode_solvers/zuko_ode.py:29-31, :80-124); every right-hand-side evaluati
 """
 from __future__ import annotations
 
-import ctypes as C
 import math
 import warnings
 from typing import Any, Callable, Optional, Tuple
@@ -81,7 +80,6 @@ class FlowMatchingEstimator(_PackedEstimator):
     def forward(self, input: Tensor, condition: Tensor, time: Tensor) -> Tensor:
         """Velocity in ORIGINAL space (flowmatching_estimator.py:205-268); batch shapes broadcast.  The condition
         is embedded once per distinct condition row, before broadcasting."""
-        lib = L.load()
         L.require_cuda(input, "input")
         bs_in = input.shape[:-len(self.input_shape)]
         bs_c = condition.shape[:-len(self.condition_shape)]
@@ -99,16 +97,13 @@ class FlowMatchingEstimator(_PackedEstimator):
         tt = tt.contiguous()
         v = torch.empty_like(inp)
         m = self._model(nbuf=2)
-        rows = L.Rows(inp.data_ptr(), cond.data_ptr(), None, R, 1 if shared else 0)
-        self._check_rc(lib.sbi_b200_fm_forward(C.byref(m), C.byref(rows), L.ptr(tt), 1 if t_shared else 0, L.ptr(v),
-                                               L.stream_ptr()), "fm_forward")
+        self._call("fm_forward", m, L.rows(inp, cond, shared=shared), tt, 1 if t_shared else 0, v)
         return v.reshape(*bshape, *self.input_shape)
 
     def forward_and_divergence(self, input: Tensor, condition: Tensor, time: Tensor):
         """(v, sum_i dv_i/dtheta_i): the velocity in ORIGINAL space and its exact divergence w.r.t. the
         input, one kernel (csrc/fm.cu `fm_trace_kernel`: forward + D forward-mode tangents).  input (R, D),
         condition (R, *condition_shape) or (1, *condition_shape) (embedded here), time scalar or (R,)."""
-        lib = L.load()
         L.require_cuda(input, "input")
         inp = input.reshape(-1, self.layout.D).contiguous().float()
         R = inp.shape[0]
@@ -120,9 +115,7 @@ class FlowMatchingEstimator(_PackedEstimator):
         v = torch.empty_like(inp)
         div = torch.empty(R, dtype=torch.float32, device=inp.device)
         m = self._model(nbuf=2)
-        rows = L.Rows(inp.data_ptr(), cond.data_ptr(), None, R, 1 if shared else 0)
-        self._check_rc(lib.sbi_b200_fm_forward_div(C.byref(m), C.byref(rows), L.ptr(tt), 1 if t_shared else 0,
-                                                   L.ptr(v), L.ptr(div), L.stream_ptr()), "fm_forward_div")
+        self._call("fm_forward_div", m, L.rows(inp, cond, shared=shared), tt, 1 if t_shared else 0, v, div)
         return v, div
 
     def ode_fn(self, input: Tensor, condition: Tensor, times: Tensor) -> Tensor:
@@ -184,32 +177,25 @@ class FlowMatchingEstimator(_PackedEstimator):
                  want_loss=True, gcond=None):
         """Fused loss forward+backward on (optionally index-gathered) rows; returns the per-row loss.  `gcond`
         (R, C): receives the gradient with respect to the condition rows."""
-        lib = L.load()
         R = (index.shape[0] if index is not None else inp.shape[0]) if R is None else R
         loss = torch.empty(R, dtype=torch.float32, device=inp.device) if want_loss else None
-        n_part = lib.sbi_b200_fm_vjp_parts(R)
+        n_part = L.load().sbi_b200_fm_vjp_parts(R)
         gpart = self._gpart(n_part) if gpart is None else gpart
         m = self._model(nbuf=2)
-        rows = L.Rows(inp.data_ptr(), cond.data_ptr(), None if index is None else index.data_ptr(), R, 0)
-        self._check_rc(lib.sbi_b200_fm_loss_vjp_cond(C.byref(m), C.byref(rows), L.ptr(times), L.ptr(eps), None,
-                                                     g_const, L.ptr(loss), L.ptr(gpart), L.ptr(loss_acc),
-                                                     L.ptr(gcond), L.stream_ptr()), "fm_loss_vjp")
+        self._call("fm_loss_vjp_cond", m, L.rows(inp, cond, index, R), times, eps, None, g_const, loss, gpart,
+                   loss_acc, gcond)
         return loss, gpart, n_part
 
 
 class _FmLoss(torch.autograd.Function):
     @staticmethod
     def forward(ctx, flat, inp, cond, times, eps, est: FlowMatchingEstimator):
-        lib = L.load()
         R = inp.shape[0]
         loss = torch.empty(R, dtype=torch.float32, device=inp.device)
-        n_part = lib.sbi_b200_fm_vjp_parts(R)
-        gpart = est._gpart(n_part)
+        gpart = est._gpart(L.load().sbi_b200_fm_vjp_parts(R))
         m = est._model(nbuf=2)
-        rows = L.Rows(inp.data_ptr(), cond.data_ptr(), None, R, 0)
         # forward value only: g = 0 (the partial gradients written are zeros)
-        est._check_rc(lib.sbi_b200_fm_loss_vjp(C.byref(m), C.byref(rows), L.ptr(times), L.ptr(eps), None, 0.0,
-                                               L.ptr(loss), L.ptr(gpart), None, L.stream_ptr()), "fm_loss")
+        est._call("fm_loss_vjp", m, L.rows(inp, cond), times, eps, None, 0.0, loss, gpart, None)
         ctx.save_for_backward(inp, cond, times, eps)
         ctx.est = est
         return loss
@@ -218,17 +204,12 @@ class _FmLoss(torch.autograd.Function):
     def backward(ctx, g):
         inp, cond, times, eps = ctx.saved_tensors
         est = ctx.est
-        lib = L.load()
-        R = inp.shape[0]
-        n_part = lib.sbi_b200_fm_vjp_parts(R)
+        n_part = L.load().sbi_b200_fm_vjp_parts(inp.shape[0])
         gpart = est._gpart(n_part)
         m = est._model(nbuf=2)
-        rows = L.Rows(inp.data_ptr(), cond.data_ptr(), None, R, 0)
         g = g.contiguous().float()
         gcond = torch.empty_like(cond) if ctx.needs_input_grad[2] else None
-        est._check_rc(lib.sbi_b200_fm_loss_vjp_cond(C.byref(m), C.byref(rows), L.ptr(times), L.ptr(eps), L.ptr(g),
-                                                    0.0, None, L.ptr(gpart), None, L.ptr(gcond), L.stream_ptr()),
-                      "fm_loss_vjp")
+        est._call("fm_loss_vjp_cond", m, L.rows(inp, cond), times, eps, g, 0.0, None, gpart, None, gcond)
         gflat = L.reduce_partials(gpart, n_part, est.layout.n_params) if ctx.needs_input_grad[0] else None
         return gflat, None, gcond, None, None, None
 
@@ -352,13 +333,13 @@ class DeviceDopri5:
 
     def __init__(self, n: int, device, rhs: Callable, atol: float = 1e-6, rtol: float = 1e-5,
                  max_steps: int = 10_000, poll: int = 4, use_graph: bool = True):
-        self.lib = L.load()
+        self.device = torch.device(device)
         self.n, self.rhs, self.atol, self.rtol, self.max_steps, self.poll = n, rhs, atol, rtol, max_steps, poll
         self.y = torch.empty(n, dtype=torch.float32, device=device)
         self.yi = torch.empty(n, dtype=torch.float32, device=device)
         self.y5 = torch.empty(n, dtype=torch.float32, device=device)
         self.k = torch.empty(7, n, dtype=torch.float32, device=device)
-        self.red = torch.empty(self.lib.sbi_b200_ode_red_size(n), dtype=torch.float32, device=device)
+        self.red = torch.empty(L.load().sbi_b200_ode_red_size(n), dtype=torch.float32, device=device)
         self.ctrl = torch.zeros(16, dtype=torch.float32, device=device)
         self.ctrl_i = self.ctrl.view(torch.int32)
         self.t_ptr = self.ctrl.data_ptr() + 4 * self._OFF_TSTAGE
@@ -368,15 +349,13 @@ class DeviceDopri5:
         self.graph = None
 
     def _stage(self, i: int):
-        L.check(self.lib.sbi_b200_ode_stage(L.ptr(self.y), L.ptr(self.k), L.ptr(self.yi), self.n, i,
-                                            self.ctrl.data_ptr(), L.stream_ptr()), "ode_stage")
+        L.call("ode_stage", self.y, self.k, self.yi, self.n, i, self.ctrl)
 
     def _step(self):
         for i in range(1, 7):
             self._stage(i)
             self.rhs(self.yi, self.t_ptr, self.k[i])
-        L.check(self.lib.sbi_b200_ode_error_commit(L.ptr(self.y), L.ptr(self.k), L.ptr(self.y5), L.ptr(self.red),
-                                                   self.n, self.ctrl.data_ptr(), L.stream_ptr()), "ode_error_commit")
+        L.call("ode_error_commit", self.y, self.k, self.y5, self.red, self.n, self.ctrl)
 
     def solve(self, y0: Tensor, t0: float, t1: float):
         """Integrate from t0 to t1 (either direction); returns (y(t1) as a view of the solver's state,
@@ -396,13 +375,13 @@ class DeviceDopri5:
         self.rhs(self.yi, self.t_ptr, self.k[0])         # k_0 (also sets the kernel's attributes before capture)
         if self.use_graph and self.graph is None:
             snap = (self.y.clone(), self.k[0].clone(), self.ctrl.clone())
-            side = torch.cuda.Stream()
-            side.wait_stream(torch.cuda.current_stream())
+            side = torch.cuda.Stream(device=self.device)
+            side.wait_stream(torch.cuda.current_stream(self.device))
             with torch.cuda.stream(side):
                 self._step()                             # warm-up outside capture
-            torch.cuda.current_stream().wait_stream(side)
+            torch.cuda.current_stream(self.device).wait_stream(side)
             self.graph = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(self.graph):
+            with torch.cuda.graph(self.graph, stream=torch.cuda.Stream(device=self.device)):
                 self._step()
             self.y.copy_(snap[0]); self.k[0].copy_(snap[1]); self.ctrl.copy_(snap[2])
         while True:
@@ -412,7 +391,7 @@ class DeviceDopri5:
                 else:
                     self._step()
             self._host.copy_(self.ctrl, non_blocking=True)
-            torch.cuda.current_stream().synchronize()
+            torch.cuda.current_stream(self.device).synchronize()
             hi = self._host.view(torch.int32)
             done = int(hi[self._I_DONE])
             if done:
@@ -425,20 +404,16 @@ class DeviceDopri5:
 def _fm_rhs(est: FlowMatchingEstimator, cond: Tensor, R: int, with_div: bool):
     """Right-hand side launcher for DeviceDopri5: state = theta (R, D) [| log|det| (R)]; `cond` is the embedded
     condition, one row shared by all R rows or one row per state row."""
-    lib = L.load()
     D = est.layout.D
     m = est._model(nbuf=2)
-    keep = (m, cond)
-    shared = 1 if cond.shape[0] == 1 else 0
+    shared = cond.shape[0] == 1
 
     def rhs(y: Tensor, t_ptr: int, out: Tensor):
-        rows = L.Rows(y.data_ptr(), keep[1].data_ptr(), None, R, shared)
+        rows = L.rows(y, cond, n=R, shared=shared)
         if with_div:
-            est._check_rc(lib.sbi_b200_fm_forward_div(C.byref(keep[0]), C.byref(rows), t_ptr, 1, out.data_ptr(),
-                                                      out.data_ptr() + 4 * R * D, L.stream_ptr()), "fm_forward_div")
+            est._call("fm_forward_div", m, rows, t_ptr, 1, out, out.data_ptr() + 4 * R * D)
         else:
-            est._check_rc(lib.sbi_b200_fm_forward(C.byref(keep[0]), C.byref(rows), t_ptr, 1, out.data_ptr(),
-                                                  L.stream_ptr()), "fm_forward")
+            est._call("fm_forward", m, rows, t_ptr, 1, out)
     return rhs
 
 
@@ -616,7 +591,6 @@ def sample_sde(est: FlowMatchingEstimator, num_samples: int, condition: Tensor, 
             if corrector is not None:
                 theta = correct(theta, t0, t1)
         return theta.reshape(num_samples, B, D) if batched else theta
-    lib = L.load()
     theta = theta.contiguous()
     n = theta.numel()
     v = torch.empty_like(theta)
@@ -625,15 +599,12 @@ def sample_sde(est: FlowMatchingEstimator, num_samples: int, condition: Tensor, 
     m = est._model(nbuf=2)
     cond = est._embed(cond)                       # x_o embedded once for all steps
     cond = (cond if B == 1 else cond.repeat(num_samples, 1)).contiguous()
-    rows = L.Rows(theta.data_ptr(), cond.data_ptr(), None, R, 1 if B == 1 else 0)
+    rows = L.rows(theta, cond, shared=B == 1)
 
     def step():
-        est._check_rc(lib.sbi_b200_fm_forward(C.byref(m), C.byref(rows), ctrl.data_ptr(), 1, v.data_ptr(),
-                                              L.stream_ptr()), "fm_forward")
+        est._call("fm_forward", m, rows, ctrl, 1, v)
         z.normal_()
-        L.check(lib.sbi_b200_sde_em_step(theta.data_ptr(), v.data_ptr(), z.data_ptr(), n, ts.data_ptr(),
-                                         ctrl.data_ptr(), float(eta), float(est.noise_scale), 0.99, L.stream_ptr()),
-                "sde_em_step")
+        L.call("sde_em_step", theta, v, z, n, ts, ctrl, float(eta), float(est.noise_scale), 0.99)
 
     nsteps = ts.numel() - 1
     out = theta.reshape(num_samples, B, D) if batched else theta
@@ -643,13 +614,13 @@ def sample_sde(est: FlowMatchingEstimator, num_samples: int, condition: Tensor, 
     if nsteps > 1:
         graph = torch.cuda.CUDAGraph()
         snap = (theta.clone(), ctrl.clone())
-        side = torch.cuda.Stream()
-        side.wait_stream(torch.cuda.current_stream())
+        side = torch.cuda.Stream(device=dev)
+        side.wait_stream(torch.cuda.current_stream(dev))
         with torch.cuda.stream(side):
             step()
-        torch.cuda.current_stream().wait_stream(side)
+        torch.cuda.current_stream(dev).wait_stream(side)
         theta.copy_(snap[0]); ctrl.copy_(snap[1])
-        with torch.cuda.graph(graph):
+        with torch.cuda.graph(graph, stream=torch.cuda.Stream(device=dev)):
             step()
         theta.copy_(snap[0]); ctrl.copy_(snap[1])
         for _ in range(nsteps - 1):

@@ -115,7 +115,6 @@ class HMCSamplerVectorized:
 
     def run(self, num_samples: int) -> np.ndarray:
         assert num_samples >= 0
-        lib = L.load()
         dev = torch.device(self._device)
         z = torch.as_tensor(np.asarray(self.x.detach().cpu() if isinstance(self.x, Tensor) else self.x),
                             dtype=torch.float64).reshape(self.num_chains, -1).to(dev).contiguous()
@@ -146,7 +145,7 @@ class HMCSamplerVectorized:
                         z.data_ptr(), vec.data_ptr(), istate.data_ptr(), fstate.data_ptr(), normal.data_ptr(),
                         uniform.data_ptr(), logp.data_ptr(), grad.data_ptr(), params.data_ptr(),
                         samples.data_ptr(), None if trace is None else trace.data_ptr())
-        L.check(lib.sbi_b200_hmc_init(C.byref(s), L.stream_ptr()), "hmc_init")
+        L.call("hmc_init", s, device=dev)
         self.draws = []
 
         def lock_step():
@@ -163,7 +162,7 @@ class HMCSamplerVectorized:
             uniform.uniform_()
             if self._record:
                 self.draws.append((normal.clone(), uniform.clone()))
-            L.check(lib.sbi_b200_hmc_step(C.byref(s), L.ptr(n_done), L.stream_ptr()), "hmc_step")
+            L.call("hmc_step", s, n_done)
 
         it = 0
         graph = None

@@ -93,7 +93,6 @@ class _DeviceAdam:
     of the matching gradient slice, which autograd accumulates into in place."""
 
     def __init__(self, net, state: Tensor, step: Tensor, lr: float, clip_max_norm: Optional[float], world: int):
-        self.lib = L.load()
         self.flat, self.mask = net.flat, net.net._mask
         self.P = net.layout.n_params
         self.state, self.count = state, step
@@ -111,7 +110,7 @@ class _DeviceAdam:
         self.grad = torch.zeros(self.P, dtype=torch.float32, device=dev)
         # the peer exchange reads this rank's gradient from a buffer of its own
         self.grad_local = torch.zeros(self.P, dtype=torch.float32, device=dev) if self.peer is not None else self.grad
-        n_sumsq = self.peer.n_sumsq if self.peer is not None else self.lib.sbi_b200_sumsq_blocks(self.P)
+        n_sumsq = self.peer.n_sumsq if self.peer is not None else L.load().sbi_b200_sumsq_blocks(self.P)
         self.sumsq = torch.zeros(n_sumsq, dtype=torch.float32, device=dev)
         self.params = None           # the joint parameter vector, with an embedding net
         if self.emb:
@@ -160,36 +159,28 @@ class _DeviceAdam:
         """One update from the `n_part` per-CTA partial gradients of a fused loss kernel (and, with an
         embedding net, the embedding gradients autograd accumulated since `zero_grad`)."""
         if self.emb:                  # the clip+Adam kernel takes the norm over [flat | embedding] itself
-            L.check(self.lib.sbi_b200_reduce_partials(L.ptr(gpart), n_part, self.P, L.ptr(self.grad),
-                                                      L.stream_ptr()), "reduce_partials")
+            L.call("reduce_partials", gpart, n_part, self.P, self.grad)
             self._adam(self.grad, 0)
             return
         if self.world == 1:           # the reduction kernel also emits the sum(g^2) partials
-            L.check(self.lib.sbi_b200_reduce_partials_norm(L.ptr(gpart), n_part, self.P, L.ptr(self.grad),
-                                                           L.ptr(self.mask), L.ptr(self.sumsq), L.stream_ptr()),
-                    "reduce_partials")
+            L.call("reduce_partials_norm", gpart, n_part, self.P, self.grad, self.mask, self.sumsq)
             self._adam(self.grad, self.sumsq.shape[0])
             return
-        L.check(self.lib.sbi_b200_reduce_partials(L.ptr(gpart), n_part, self.P, L.ptr(self.grad_local),
-                                                  L.stream_ptr()), "reduce_partials")
+        L.call("reduce_partials", gpart, n_part, self.P, self.grad_local)
         self.step(self.grad_local)
 
     def _adam(self, grad: Tensor, n_sumsq: int):
         """n_sumsq > 0: `sumsq` already holds that many sum(g^2) partials of `grad`."""
         if self.emb:
-            L.check(self.lib.sbi_b200_adam_clip_step(
-                L.ptr(self.params), L.ptr(grad), L.ptr(self.state), L.ptr(self.count), L.ptr(self.mask), self.n,
-                self.lr, 0.9, 0.999, 1e-8, self.max_norm, 1.0, L.stream_ptr()), "adam_clip_step")
+            L.call("adam_clip_step", self.params, grad, self.state, self.count, self.mask, self.n,
+                   self.lr, 0.9, 0.999, 1e-8, self.max_norm, 1.0)
             return
         if n_sumsq:
-            L.check(self.lib.sbi_b200_adam_clip_step_norm(
-                L.ptr(self.flat.data), L.ptr(grad), L.ptr(self.state), L.ptr(self.count), L.ptr(self.mask), self.P,
-                self.lr, 0.9, 0.999, 1e-8, self.max_norm, 1.0, L.ptr(self.sumsq), n_sumsq, L.stream_ptr()),
-                "adam_clip_step")
+            L.call("adam_clip_step_norm", self.flat.data, grad, self.state, self.count, self.mask, self.P,
+                   self.lr, 0.9, 0.999, 1e-8, self.max_norm, 1.0, self.sumsq, n_sumsq)
         else:
-            L.check(self.lib.sbi_b200_adam_clip_step(
-                L.ptr(self.flat.data), L.ptr(grad), L.ptr(self.state), L.ptr(self.count), L.ptr(self.mask), self.P,
-                self.lr, 0.9, 0.999, 1e-8, self.max_norm, 1.0, L.stream_ptr()), "adam_clip_step")
+            L.call("adam_clip_step", self.flat.data, grad, self.state, self.count, self.mask, self.P,
+                   self.lr, 0.9, 0.999, 1e-8, self.max_norm, 1.0)
 
     def _tensors(self):
         params = self.flat.data if self.params is None else self.params
@@ -220,16 +211,17 @@ def _capture(opt: _DeviceAdam, warmup: Callable, *fns: Callable) -> list:
     attributes); the parameters and the optimizer state are rewound after it and after the capture, so
     neither changes the run."""
     snap = opt.snapshot()
-    side = torch.cuda.Stream()
-    side.wait_stream(torch.cuda.current_stream())
+    dev = opt.flat.device
+    side = torch.cuda.Stream(device=dev)
+    side.wait_stream(torch.cuda.current_stream(dev))
     with torch.cuda.stream(side):
         warmup()
-    torch.cuda.current_stream().wait_stream(side)
+    torch.cuda.current_stream(dev).wait_stream(side)
     opt.restore(snap)
     graphs = []
     for fn in fns:
         graphs.append(torch.cuda.CUDAGraph())
-        with torch.cuda.graph(graphs[-1]):
+        with torch.cuda.graph(graphs[-1], stream=torch.cuda.Stream(device=dev)):
             fn()
     opt.restore(snap)
     return graphs
@@ -619,7 +611,6 @@ class _FlowTrainer(_Trainer):
         if self._round > 0 and discard_prior_samples:
             raise NotImplementedError("discard_prior_samples with the first-round loss is not implemented "
                                       "(append only the rounds to train on)")
-        lib = L.load()
         dev = self._device
         rank, world, glob = self._dp()
         net, B, Bv, steps, vsteps = self._prepare(validation_fraction, training_batch_size, resume_training,
@@ -677,9 +668,9 @@ class _FlowTrainer(_Trainer):
                     with torch.set_grad_enabled(train_emb):
                         ctx = net._embed(cond_raw[idx]).contiguous()
                     inp_b = inp_all[idx]
-                    rows = L.Rows(inp_b.data_ptr(), ctx.data_ptr(), None, Bl, 0)
+                    rows = L.rows(inp_b, ctx, n=Bl)
                 else:
-                    rows = L.Rows(inp_all.data_ptr(), cond_all.data_ptr(), idx.data_ptr(), Bl, 0)
+                    rows = L.rows(inp_all, cond_all, idx, Bl)
                 if w_all is None:
                     net.vjp(m_tr, rows, Bl, None, -1.0 / Btot, None, gpart, None, gcond, loss_acc, cond_tc=cond_tc)
                 else:
@@ -708,8 +699,7 @@ class _FlowTrainer(_Trainer):
                     net._logprob_raw(inp_all, cond_all, False, index=vrows, n_rows=v_hi - v_lo, out=vlp)
                 if w_all is None:
                     # -sum of the finite log-probs and the count of non-finite ones, one fused launch
-                    L.check(lib.sbi_b200_nll_stats(L.ptr(vlp), v_hi - v_lo, L.ptr(stats[2:]), L.stream_ptr()),
-                            "nll_stats")
+                    L.call("nll_stats", vlp, v_hi - v_lo, stats[2:])
                 else:
                     fin = torch.isfinite(vlp)
                     stats[2] = -(torch.where(fin, vlp, torch.zeros_like(vlp)) * w_all[vrows]).sum()

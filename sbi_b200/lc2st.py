@@ -135,10 +135,6 @@ def _device(device: str) -> torch.device:
     return d if d.type == "cuda" else torch.device("cuda", torch.cuda.current_device())
 
 
-def _ptr(t: Optional[Tensor]):
-    return _lib.ptr(t)
-
-
 class TrainedMLP:
     """A trained classifier with sklearn's fitted attributes (`coefs_`, `intercepts_`, `n_iter_`, `loss_curve_`,
     `validation_scores_`, `best_validation_score_`, `best_loss_`) and a `predict_proba` on the device."""
@@ -246,10 +242,8 @@ def _evaluate(clfs: Sequence, theta_blocks: Tensor, group: Optional[Sequence[int
         prob = torch.empty(n, S, dtype=torch.float32, device=dev)
         part = torch.empty(n, nchunk, dtype=torch.float64, device=dev)
         score = torch.empty(n, dtype=torch.float64, device=dev)
-        _lib.require_cuda(params, "classifier parameters")
-        _lib.check(lib.sbi_b200_lc2st_eval(C.byref(net.c), _ptr(params), n, E, _ptr(th) if dt else None, dt, S,
-                                           _ptr(g), _ptr(xo) if xo.numel() else None, xo.numel(), _ptr(prob),
-                                           _ptr(part), _ptr(score), _lib.stream_ptr()), "lc2st_eval")
+        _lib.call("lc2st_eval", net.c, params, n, E, th if dt else None, dt, S, g, xo if xo.numel() else None,
+                  xo.numel(), prob, part, score)
         probs[idx] = prob.cpu().numpy()
         scores[idx] = score.cpu().numpy()
     return probs, scores
@@ -357,11 +351,8 @@ def train_classifiers(theta_table: Tensor, x_table: Tensor, models: List[_Model]
     val_curve = torch.zeros(M, max_iter, dtype=torch.float64, device=device)
     loss_curve = torch.zeros(M, max_iter, dtype=torch.float64, device=device)
     best = torch.empty(M, dtype=torch.float64, device=device)
-    _lib.require_cuda(params, "classifier parameters")
-    _lib.check(lib.sbi_b200_lc2st_train(C.byref(net.c), C.byref(opt), _ptr(d_jobs), M, _ptr(th) if dt else None, dt,
-                                        _ptr(xt) if dx else None, dx, _ptr(d_rows), _ptr(d_lab), _ptr(d_order),
-                                        _ptr(params), _ptr(ws), _ptr(n_iter), _ptr(val_curve), _ptr(loss_curve),
-                                        _ptr(best), _lib.stream_ptr()), "lc2st_train")
+    _lib.call("lc2st_train", net.c, opt, d_jobs, M, th if dt else None, dt, xt if dx else None, dx, d_rows, d_lab,
+              d_order, params, ws, n_iter, val_curve, loss_curve, best)
     n_iter_h, params_h = n_iter.cpu().numpy(), params.cpu().numpy()
     val_h, loss_h, best_h = val_curve.cpu().numpy(), loss_curve.cpu().numpy(), best.cpu().numpy()
     out = []

@@ -14,7 +14,6 @@ CPU path.  `calc_misspecification_logprob` is not provided (it needs zuko-based 
 """
 from __future__ import annotations
 
-import ctypes as C
 import warnings
 from typing import Optional, Tuple
 
@@ -71,12 +70,9 @@ def _mmd_sets(z: Tensor, table: Tensor, nxy: Tensor, mode: Optional[str] = "bias
     if bandwidth is not None:
         bw.fill_(float(bandwidth))
     mmd = None if mode is None else torch.empty(S, dtype=torch.float64, device=dev)
-    lib = _lib.load()
-    ws = torch.empty(max(1, lib.sbi_b200_mmd_ws_bytes(S)), dtype=torch.uint8, device=dev)
-    _lib.require_cuda(z, "z")
-    _lib.check(lib.sbi_b200_mmd(_lib.ptr(z), R, D, _lib.ptr(d_tab), L, _lib.ptr(d_nxy), S, int(nxy[:, 0].max()),
-                                int(nxy[:, 1].max()), int(mode == "unbiased"), int(bandwidth is not None),
-                                _lib.ptr(bw), _lib.ptr(mmd), _lib.ptr(ws), _lib.stream_ptr()), "mmd")
+    ws = torch.empty(max(1, _lib.load().sbi_b200_mmd_ws_bytes(S)), dtype=torch.uint8, device=dev)
+    _lib.call("mmd", z, R, D, d_tab, L, d_nxy, S, int(nxy[:, 0].max()), int(nxy[:, 1].max()), int(mode == "unbiased"),
+              int(bandwidth is not None), bw, mmd, ws)
     return mmd, bw
 
 
@@ -92,8 +88,7 @@ def rbf_kernel(x: Tensor, y: Tensor, bandwidth: float):
     _check_pair(x, y)
     xd, yd = _cuda(x, "x"), _cuda(y, "y")
     out = torch.empty(x.shape[0], y.shape[0], dtype=torch.float32, device=xd.device)
-    _lib.check(_lib.load().sbi_b200_rbf_matrix(_lib.ptr(xd), xd.shape[0], _lib.ptr(yd), yd.shape[0], xd.shape[1],
-                                               float(bandwidth), _lib.ptr(out), _lib.stream_ptr()), "rbf_matrix")
+    _lib.call("rbf_matrix", xd, xd.shape[0], yd, yd.shape[0], xd.shape[1], float(bandwidth), out)
     return out.to(x.device)
 
 

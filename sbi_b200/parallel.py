@@ -143,10 +143,8 @@ class PeerGradientSum:
 
     def sum(self, grad_local: Tensor, grad_out: Tensor, mask: Optional[Tensor], sumsq: Optional[Tensor],
             opt_step: Optional[Tensor] = None) -> None:
-        L, C = self._L, self._C
-        L.check(self.lib.sbi_b200_peer_sum(L.ptr(grad_local), self._ptrs, self.world, self.rank, self.n,
-                                           L.ptr(grad_out), L.ptr(mask), L.ptr(sumsq), L.ptr(opt_step),
-                                           L.stream_ptr()), "peer_sum")
+        self._L.call("peer_sum", grad_local, self._ptrs, self.world, self.rank, self.n, grad_out, mask, sumsq,
+                     opt_step)
 
     def error(self) -> bool:
         return self.lib.sbi_b200_peer_error(self._C.c_void_p(self.own), self.n) != 0

@@ -10,7 +10,6 @@ selects the kernels: `RatioLayout` (resnet) csrc/ratio.cu and csrc/ratio_tc.cu, 
 """
 from __future__ import annotations
 
-import ctypes as C
 import os
 import warnings
 from typing import Any, Callable, Optional, Union
@@ -112,21 +111,17 @@ class RatioEstimator(_PackedEstimator):
     # ---- raw entry (no autograd): pairs given by optional index arrays / shared x
     def logits_raw(self, theta: Tensor, x: Tensor, ti: Optional[Tensor] = None,
                    xi: Optional[Tensor] = None, x_shared: bool = False, R: Optional[int] = None) -> Tensor:
-        lib = L.load()
         L.require_cuda(theta, "theta")
         L.require_cuda(x, "x")
         R = (ti.shape[0] if ti is not None else theta.shape[0]) if R is None else R
         out = torch.empty(R, dtype=torch.float32, device=theta.device)
         m = self._model(nbuf=2)
-        pr = L.Pairs(theta.data_ptr(), x.data_ptr(), None if ti is None else ti.data_ptr(),
-                     None if xi is None else xi.data_ptr(), R, 1 if x_shared else 0)
+        pr = L.pairs(theta, x, ti, xi, R, x_shared)
         tc = self._tc_state(m) if (R >= self.TC_MIN_ROWS or os.environ.get("SBI_B200_TC", "") == "1") else None
         if tc is not None:
-            L.check(lib.sbi_b200_ratio_forward_tc(C.byref(m), C.byref(tc), C.byref(pr), L.ptr(out),
-                                                  L.stream_ptr()), "ratio_forward_tc")
+            self._call("ratio_forward_tc", m, tc, pr, out)
             return out
-        self._check_rc(self._entry("forward")(C.byref(m), C.byref(pr), L.ptr(out), L.stream_ptr()),
-                    f"{self.layout.family}_forward")
+        self._call(f"{self._family.prefix}_forward", m, pr, out)
         return out
 
     #: pairs from which the logits go through the wgmma kernel (csrc/ratio_tc.cu); the crossover against
@@ -160,15 +155,12 @@ class _RatioFn(torch.autograd.Function):
         gth = torch.empty(R, est.layout.Dt, dtype=torch.float32, device=theta.device) if need_th else None
         gx = torch.empty(R, est.layout.Dx, dtype=torch.float32, device=theta.device) if need_x else None
         m = est._model(nbuf=3)
-        pr = L.Pairs(theta.data_ptr(), x.data_ptr(), None if ctx.ti is None else ctx.ti.data_ptr(),
-                     None if ctx.xi is None else ctx.xi.data_ptr(), R, 1 if ctx.x_shared else 0)
+        pr = L.pairs(theta, x, ctx.ti, ctx.xi, R, ctx.x_shared)
         g = g.contiguous().float()
         if resnet:
-            est._check_rc(L.load().sbi_b200_ratio_vjp_inputs(C.byref(m), C.byref(pr), L.ptr(g), None, L.ptr(gpart),
-                                                            L.ptr(gth), L.ptr(gx), L.stream_ptr()), "ratio_vjp")
+            est._call("ratio_vjp_inputs", m, pr, g, None, gpart, gth, gx)
         else:   # per-pair theta gradients, summed onto the gathered rows below
-            est._check_rc(est._entry("vjp")(C.byref(m), C.byref(pr), L.ptr(g), None, L.ptr(gpart), L.ptr(gth),
-                                            L.stream_ptr()), f"{est.layout.family}_vjp")
+            est._call(f"{est._family.prefix}_vjp", m, pr, g, None, gpart, gth)
         gflat = L.reduce_partials(gpart, n_part, est.layout.n_params) if need_flat else None
         if need_th and ctx.ti is not None:
             gth = pair_rows_sum(gth, ctx.ti, theta.shape[0])
@@ -195,9 +187,7 @@ def pair_rows_sum(gpair: Tensor, index: Optional[Tensor], n_rows: int, row_ptr: 
             order = order.contiguous()
         row_ptr = torch.searchsorted(keys, torch.arange(n_rows + 1, dtype=keys.dtype, device=dev))
     out = torch.empty(n_rows, gpair.shape[1], dtype=torch.float32, device=dev)
-    L.check(L.load().sbi_b200_pair_rows_sum(L.ptr(gpair.contiguous()), gpair.shape[1], L.ptr(order),
-                                            L.ptr(row_ptr.contiguous()), n_rows, L.ptr(out), L.stream_ptr()),
-            "pair_rows_sum")
+    L.call("pair_rows_sum", gpair.contiguous(), gpair.shape[1], order, row_ptr.contiguous(), n_rows, out)
     return out
 
 

@@ -16,7 +16,6 @@
 """
 from __future__ import annotations
 
-import ctypes as C
 import logging
 import time
 import warnings
@@ -60,7 +59,6 @@ class SliceSamplerVectorized:
 
     def run(self, num_samples: int) -> np.ndarray:
         assert num_samples >= 0
-        lib = L.load()
         dev = self._device
         x = torch.as_tensor(np.asarray(self.x.cpu() if isinstance(self.x, Tensor) else self.x),
                             dtype=torch.float64).reshape(self.num_chains, -1).to(dev).contiguous()
@@ -80,14 +78,13 @@ class SliceSamplerVectorized:
                           rng.data_ptr(), samples.data_ptr())
         # the chains' device state, readable while and after the sampler runs (final widths, state machine)
         self._chain_state = {"width": width, "order": order, "istate": istate, "fstate": fstate}
-        L.check(lib.sbi_b200_slice_init(C.byref(s), L.ptr(params), L.stream_ptr()), "slice_init")
+        L.call("slice_init", s, params)
         it = 0
 
         def lock_step():
             lp = self._log_prob_fn(params)
             lp = torch.as_tensor(lp, dtype=torch.float32).to(dev).reshape(-1).contiguous()
-            L.check(lib.sbi_b200_slice_step(C.byref(s), L.ptr(lp), L.ptr(params), L.ptr(n_done),
-                                            L.stream_ptr()), "slice_step")
+            L.call("slice_step", s, lp, params, n_done)
 
         graph = None
         while True:
@@ -104,13 +101,13 @@ class SliceSamplerVectorized:
                     break
                 if self._graph and graph is None:
                     # the eager round above warmed everything up; capture the next rounds
-                    side = torch.cuda.Stream()
-                    side.wait_stream(torch.cuda.current_stream())
+                    side = torch.cuda.Stream(device=dev)
+                    side.wait_stream(torch.cuda.current_stream(dev))
                     graph = torch.cuda.CUDAGraph()
                     with torch.cuda.graph(graph, stream=side):
                         for _ in range(self._check_every):
                             lock_step()
-                    torch.cuda.current_stream().wait_stream(side)
+                    torch.cuda.current_stream(dev).wait_stream(side)
         self.num_lock_steps = it
         out = samples[:, :int(num_samples)].cpu().numpy()
         out = out[:, :: self.thin, :]
@@ -267,10 +264,8 @@ def rejection_sample(potential_fn: Callable, proposal: Any, theta_transform: Opt
                 count = torch.zeros(1, dtype=torch.int32, device=dev)
             scratch = torch.empty(int(lib.sbi_b200_reject_scratch_ints(sampling_batch_size)), dtype=torch.int32,
                                   device=dev)
-            L.check(lib.sbi_b200_reject_compact(
-                candidates.data_ptr(), candidates.shape[1], log_target.data_ptr(), log_scaled.data_ptr(),
-                uniform_rand.data_ptr(), sampling_batch_size, num_sampled_total, out.data_ptr(), L.ptr(out_idx),
-                num_samples, count.data_ptr(), scratch.data_ptr(), L.stream_ptr()), "reject_compact")
+            L.call("reject_compact", candidates, candidates.shape[1], log_target, log_scaled, uniform_rand,
+                   sampling_batch_size, num_sampled_total, out, out_idx, num_samples, count, scratch)
             total = int(count.item())
             collected = min(total, num_samples)
             num_sampled_total += sampling_batch_size
@@ -340,10 +335,8 @@ def sampling_importance_resampling(potential_fn: Callable, proposal: Any, num_sa
             lt = log_target.reshape(-1).to(dev).float().contiguous()
             lq = log_proposal.reshape(-1).to(dev).float().contiguous()
             u = uniform_decision.reshape(-1).to(dev).float().contiguous()
-            L.check(lib.sbi_b200_sir_select(
-                cand.data_ptr(), cand.shape[1], lt.data_ptr(), lq.data_ptr(), u.data_ptr(), batch_size, K,
-                groups_done, out.data_ptr(), None, num_samples, count.data_ptr(), scratch.data_ptr(),
-                L.stream_ptr()), "sir_select")
+            L.call("sir_select", cand, cand.shape[1], lt, lq, u, batch_size, K, groups_done, out, None, num_samples,
+                   count, scratch)
             groups_done += batch_size
             total = int(count.item())
             num_remaining = num_samples - total

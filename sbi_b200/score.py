@@ -18,7 +18,6 @@ loss, schedules, drift / diffusion against the UNMODIFIED reference classes exac
 """
 from __future__ import annotations
 
-import ctypes as C
 import math
 import warnings
 from typing import Any, Callable, Optional, Union
@@ -44,15 +43,12 @@ class _RawNet(torch.autograd.Function):
     def backward(ctx, g):
         inp, cond, tenc = ctx.saved_tensors
         est = ctx.est
-        lib = L.load()
         R = inp.shape[0]
-        n_part = lib.sbi_b200_fm_vjp_parts(R)
+        n_part = L.load().sbi_b200_fm_vjp_parts(R)
         gpart = est._gpart(n_part)
         m = est._model(nbuf=2)
-        rows = L.Rows(inp.data_ptr(), cond.data_ptr(), None, R, 1 if cond.shape[0] == 1 and R > 1 else 0)
         g = g.contiguous().float()
-        est._check_rc(lib.sbi_b200_fm_net_vjp(C.byref(m), C.byref(rows), L.ptr(tenc), L.ptr(g), L.ptr(gpart),
-                                              L.stream_ptr()), "fm_net_vjp")
+        est._call("fm_net_vjp", m, L.rows(inp, cond, shared=cond.shape[0] == 1 and R > 1), tenc, g, gpart)
         return L.reduce_partials(gpart, n_part, est.layout.n_params), None, None, None, None
 
 
@@ -86,26 +82,19 @@ class ConditionalScoreEstimator(FlowMatchingEstimator):
         s.raw = 1
 
     def _raw_forward(self, inp: Tensor, cond: Tensor, tenc: Tensor) -> Tensor:
-        lib = L.load()
         L.require_cuda(inp, "input")
-        R = inp.shape[0]
         out = torch.empty_like(inp)
         m = self._model(nbuf=2)
-        rows = L.Rows(inp.data_ptr(), cond.data_ptr(), None, R, 1 if cond.shape[0] == 1 and R > 1 else 0)
-        self._check_rc(lib.sbi_b200_fm_forward(C.byref(m), C.byref(rows), L.ptr(tenc), 0, L.ptr(out),
-                                               L.stream_ptr()), "fm_forward(raw)")
+        self._call("fm_forward", m, L.rows(inp, cond, shared=cond.shape[0] == 1 and inp.shape[0] > 1), tenc, 0, out)
         return out
 
     def _raw_forward_diag(self, inp: Tensor, cond: Tensor, tenc: Tensor):
         """(net(inp), diag of d net / d inp): `sbi_b200_fm_forward_div` in bare-network mode."""
-        lib = L.load()
         L.require_cuda(inp, "input")
-        R = inp.shape[0]
         out, diag = torch.empty_like(inp), torch.empty_like(inp)
         m = self._model(nbuf=2)
-        rows = L.Rows(inp.data_ptr(), cond.data_ptr(), None, R, 1 if cond.shape[0] == 1 and R > 1 else 0)
-        self._check_rc(lib.sbi_b200_fm_forward_div(C.byref(m), C.byref(rows), L.ptr(tenc), 0, L.ptr(out),
-                                                   L.ptr(diag), L.stream_ptr()), "fm_forward_div(raw)")
+        self._call("fm_forward_div", m, L.rows(inp, cond, shared=cond.shape[0] == 1 and inp.shape[0] > 1), tenc, 0,
+                   out, diag)
         return out, diag
 
     def _net_call(self, input_enc: Tensor, condition: Tensor, time_enc: Tensor) -> Tensor:
